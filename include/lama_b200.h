@@ -323,6 +323,57 @@ int lama_dm_coarse_correlate_candidate_scan(lama_dm* dm, const double* ref_pts_x
                                             const double* pts_xyz, int n, const double sensor_origin[3], const double sensor_quat_xyzw[4],
                                             const double ref_xyr[3], const double cand_xyr[3], double between_xyr[3], double* rmse);
 
+/* ---- miniSAM Levenberg-Marquardt over an explicit SE2 factor graph (vendor/minisam/minisam/nonlinear/LevenbergMarquardtOptimizer.cpp:56-332) ----
+ * priors: PriorFactor<SE2> on prior_nodes[i] measured prior_xyr[i]; betweens: BetweenFactor<SE2> between_from_to[2i] -> [2i+1] measured between_xyr[i].
+ * Each factor's loss is loss[4] = {sigma_x, sigma_y, sigma_theta, huber_k}: huber_k <= 0 gives DiagonalLoss::Sigmas (core/LossFunction.cpp:95-114),
+ * huber_k > 0 gives HuberLoss::Huber(huber_k) on the raw error (:190-203; the sigmas are ignored).  Factors enter the graph priors first, then
+ * betweens, in the given order.  *status, report and the SUCCESS-only update of nodes_xyr are those of lama_pgo_optimize.  accepted (may be NULL)
+ * receives one byte per tried lambda, 1 accepted / 0 rejected, at most accepted_cap of them; *n_tries (may be NULL) = the number of tries. */
+int lama_pgo_optimize_graph(int device, double* nodes_xyr, int n_nodes, const int* prior_nodes, const double* prior_xyr, const double* prior_loss, int n_priors,
+                            const int* between_from_to, const double* between_xyr, const double* between_loss, int n_betweens, int* status, double report[6],
+                            uint8_t* accepted, int accepted_cap, int* n_tries);
+
+/* ------------------------------------------------------------------------------------------------
+ * GraphSlam2D -- include/lama/graph_slam2d.h:51-173, src/graph_slam2d.cpp:104-430: key-pose graph SLAM over a transient-map Slam2D,
+ * loop closures by scan correlation against the local map, Huber-robust pose-graph optimisation on the device.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct lama_graph lama_graph;
+typedef struct lama_graph_options { /* GraphSlam2D::Options, graph_slam2d.h:59-87 */
+    lama_slam_options slam;            /* transient_map and truncated_ray are forced to 1 and 1.0 (graph_slam2d.cpp:106-107) */
+    double key_pose_distance;          /* linear distance between key poses */
+    double key_pose_angular_distance;  /* angular distance between key poses */
+    int32_t key_pose_head_delay;       /* the loop search queries the key pose this many keys back */
+    double loop_search_max_distance;   /* search radius max^r min^(1 - r), r = min(accumulated distance, 100) / 100 */
+    double loop_search_min_distance;
+    int32_t loop_max_candidates;       /* candidates correlated per search */
+    double loop_closure_scan_rmse;     /* largest correlation RMSE accepted (twice that after the coarse retry) */
+    int32_t loop_closure_max_candidates; /* declared but unused by the reference; accepted and ignored */
+    int32_t ignore_n_chain_poses;      /* the newest key poses left out of the search */
+} lama_graph_options;
+/* the reference defaults: Slam2D's (lama_slam_options_default) and graph_slam2d.h:62-86 */
+int lama_graph_options_default(lama_graph_options* o);
+int lama_graph_create(const lama_graph_options* o, lama_graph** out);   /* GraphSlam2D::GraphSlam2D, graph_slam2d.cpp:104-111 */
+int lama_graph_destroy(lama_graph* h);
+int lama_graph_set_pose(lama_graph* h, const double xyr[3]);             /* GraphSlam2D::Init, graph_slam2d.cpp:118-121 */
+/* bool GraphSlam2D::update(surface, odometry, timestamp), graph_slam2d.cpp:188-282; *did_update = the bool (may be NULL) */
+int lama_graph_update(lama_graph* h, const double* pts_xyz, int n, const double sensor_origin[3], const double sensor_quat_xyzw[4],
+                      const double odom_xyr[3], double timestamp, int* did_update);
+int lama_graph_get_pose(lama_graph* h, double xyr[3]);                   /* GraphSlam2D::getPose = correction + slam pose, :127-129 */
+/* key_poses: corrected[cap x 3], original[cap x 3], stamps[cap] (each may be NULL); *count = number of key poses (cap = capacity) */
+int lama_graph_get_key_poses(lama_graph* h, double* corrected_xyr, double* original_xyr, double* stamps, int cap, int* count);
+/* the cloud of key pose `key` (its sensor origin / quaternion may be NULL): n x 3 points, *count = n */
+int lama_graph_get_key_cloud(lama_graph* h, int key, double* pts_xyz, int cap, double sensor_origin[3], double sensor_quat_xyzw[4], int* count);
+/* links (graph_slam2d.h:116-117): cap x {candidate key, reference key}, *count = number of links */
+int lama_graph_get_links(lama_graph* h, int32_t* from_to, int cap, int* count);
+/* the candidate ids of the latest update's loop search, nearest first (*count = 0 when that update did not search) */
+int lama_graph_get_last_candidates(lama_graph* h, int32_t* ids, int cap, int* count);
+/* counts[4] = {key poses, loop factors, optimisations run, optimisations that ended in SUCCESS}; last_status and last_report (as
+ * lama_pgo_optimize's) describe the latest optimisation (status -1 before the first); either output may be NULL */
+int lama_graph_get_stats(lama_graph* h, uint64_t counts[4], int* last_status, double last_report[6]);
+/* the inner Slam2D (GraphSlam2D::slam) as a BORROWED handle: the lama_slam_* getters, exports and map writers work on the local map;
+ * lama_slam_destroy on it does nothing, and it dies with the lama_graph */
+int lama_graph_slam(lama_graph* h, lama_slam** slam);
+
 #ifdef __cplusplus
 }
 #endif

@@ -119,6 +119,35 @@ protected:
     lama_slam* h_ = nullptr;
 };
 
+// lama::GraphSlam2D (include/lama/graph_slam2d.h:51-173): key-pose graph SLAM over a transient-map Slam2D
+class GraphSlam2D {
+public:
+    using Options = lama_graph_options;
+    static Options defaults() { Options o; check(lama_graph_options_default(&o)); return o; }
+    explicit GraphSlam2D(const Options& o = defaults()) { check(lama_graph_create(&o, &h_)); }
+    ~GraphSlam2D() { lama_graph_destroy(h_); }
+    GraphSlam2D(const GraphSlam2D&) = delete;
+    GraphSlam2D& operator=(const GraphSlam2D&) = delete;
+    template <typename Pose>
+    void Init(const Pose& prior) { const double xyr[3] = {prior.x(), prior.y(), prior.rotation()}; check(lama_graph_set_pose(h_, xyr)); }   // :118-121
+    template <typename CloudPtr, typename Pose>
+    bool update(const CloudPtr& surface, const Pose& odometry, double timestamp)  // graph_slam2d.h:150
+    {
+        FlatCloud<typename std::remove_reference<decltype(*surface)>::type> f(*surface);
+        const double odom[3] = {odometry.x(), odometry.y(), odometry.rotation()};
+        int did = 0;
+        check(lama_graph_update(h_, f.pts.data(), (int)(f.pts.size() / 3), f.origin, f.quat, odom, timestamp, &did));
+        return did != 0;
+    }
+    void getPose(double xyr[3]) const { check(lama_graph_get_pose(h_, xyr)); }   // :127-129
+    // the inner Slam2D (the public member `slam`), borrowed: valid while this object lives
+    lama_slam* slam() const { lama_slam* s = nullptr; check(lama_graph_slam(h_, &s)); return s; }
+    lama_graph* handle() const { return h_; }
+
+private:
+    lama_graph* h_ = nullptr;
+};
+
 // lama::LidarOdometry2D (include/lama/lidar_odometry_2d.h:45-75): the Slam2D handle in its lidar-odometry mode
 class LidarOdometry2D {
 public:

@@ -50,6 +50,12 @@ class SlamOptions(C.Structure):
                 ("dev", DeviceOptions)]
 
 
+class GraphOptions(C.Structure):
+    _fields_ = [("slam", SlamOptions), ("key_pose_distance", C.c_double), ("key_pose_angular_distance", C.c_double), ("key_pose_head_delay", C.c_int32),
+                ("loop_search_max_distance", C.c_double), ("loop_search_min_distance", C.c_double), ("loop_max_candidates", C.c_int32),
+                ("loop_closure_scan_rmse", C.c_double), ("loop_closure_max_candidates", C.c_int32), ("ignore_n_chain_poses", C.c_int32)]
+
+
 class LocOptions(C.Structure):
     _fields_ = [("trans_thresh", C.c_double), ("rot_thresh", C.c_double), ("l2_max", C.c_double), ("resolution", C.c_double),
                 ("patch_size", C.c_uint32), ("max_iter", C.c_uint32), ("strategy", C.c_int32), ("gloc_particles", C.c_uint32),
@@ -76,6 +82,9 @@ EXPORTED_SYMBOLS = [
     "lama_loc_occupancy_set", "lama_loc_set_seed", "lama_loc_trigger_global_localization", "lama_loc_global_localization_active",
     "lama_dm_create", "lama_dm_destroy", "lama_dm_max_sqdist", "lama_dm_add_obstacles", "lama_dm_remove_obstacles", "lama_dm_update",
     "lama_dm_distance", "lama_dm_bounds", "lama_dm_export", "lama_dm_import", "lama_dm_match_normal_equations", "lama_dm_match_solve",
+    "lama_pgo_optimize_graph", "lama_graph_options_default", "lama_graph_create", "lama_graph_destroy", "lama_graph_set_pose", "lama_graph_update",
+    "lama_graph_get_pose", "lama_graph_get_key_poses", "lama_graph_get_key_cloud", "lama_graph_get_links", "lama_graph_get_last_candidates",
+    "lama_graph_get_stats", "lama_graph_slam",
 ]
 
 
@@ -217,6 +226,39 @@ class SimplePGO:
         self.status = st.value
         self.report = dict(zip(("iterations", "lambda_tries", "cg_iterations", "initial_error", "final_error", "device_ms"), rep.tolist()))
         return st.value == 0
+
+
+_REPORT_KEYS = ("iterations", "lambda_tries", "cg_iterations", "initial_error", "final_error", "device_ms")
+
+
+def diagonal_loss(sigmas):
+    """miniSAM DiagonalLoss::Sigmas(sigmas) as the 4-vector loss of pgo_optimize_graph"""
+    return (float(sigmas[0]), float(sigmas[1]), float(sigmas[2]), 0.0)
+
+
+def huber_loss(k):
+    """miniSAM HuberLoss::Huber(k) as the 4-vector loss of pgo_optimize_graph"""
+    return (1.0, 1.0, 1.0, float(k))
+
+
+def pgo_optimize_graph(nodes, priors=(), betweens=(), device=0):
+    """miniSAM Levenberg-Marquardt over an explicit SE2 factor graph on the device.  nodes (n x 3 xyr), priors [(node, xyr, loss)],
+    betweens [(from, to, xyr, loss)], loss = diagonal_loss(sigmas) or huber_loss(k).  Returns (status, nodes after the call -- optimised only on
+    SUCCESS --, report dict, list of per-lambda-try accept flags)."""
+    x = np.array(nodes, dtype=np.float64).reshape(-1, 3).copy()
+    pn = np.ascontiguousarray([p[0] for p in priors], np.int32)
+    px = np.ascontiguousarray([p[1] for p in priors], np.float64).reshape(-1, 3)
+    pl = np.ascontiguousarray([p[2] for p in priors], np.float64).reshape(-1, 4)
+    bf = np.ascontiguousarray([[b[0], b[1]] for b in betweens], np.int32).reshape(-1, 2)
+    bx = np.ascontiguousarray([b[2] for b in betweens], np.float64).reshape(-1, 3)
+    bl = np.ascontiguousarray([b[3] for b in betweens], np.float64).reshape(-1, 4)
+    st, tries = C.c_int(-1), C.c_int(0)
+    rep = np.zeros(6)
+    acc = np.zeros(4096, np.uint8)
+    _chk(lib().lama_pgo_optimize_graph(C.c_int(device), x.ctypes.data_as(c_dp), C.c_int(len(x)), pn.ctypes.data_as(c_i32p), px.ctypes.data_as(c_dp),
+                                       pl.ctypes.data_as(c_dp), C.c_int(len(pn)), bf.ctypes.data_as(c_i32p), bx.ctypes.data_as(c_dp), bl.ctypes.data_as(c_dp),
+                                       C.c_int(len(bf)), C.byref(st), rep.ctypes.data_as(c_dp), _vp(acc), C.c_int(acc.size), C.byref(tries)))
+    return st.value, x, dict(zip(_REPORT_KEYS, rep.tolist())), acc[:min(tries.value, acc.size)].tolist()
 
 
 def loop_closure_candidates(key_xy, ignore_n_chain_poses, query_xy, radius, max_candidates=5):
@@ -591,6 +633,105 @@ class LidarOdometry2D(Slam2D):
 
     def update(self, pts, timestamp=0.0, origin=_ID3, quat=_IDQ) -> bool:
         return super().update(pts, None, timestamp, origin, quat)
+
+
+class GraphSlam2D:
+    """lama::GraphSlam2D (include/lama/graph_slam2d.h:51-173): key-pose graph SLAM with loop closures over a transient-map Slam2D."""
+
+    @staticmethod
+    def Options(**kw) -> GraphOptions:
+        """the reference defaults; Slam2D fields (and the device knobs) go to .slam, the nine GraphSlam2D fields to the top level"""
+        o = GraphOptions()
+        _chk(lib().lama_graph_options_default(C.byref(o)))
+        for k, v in kw.items():
+            if k in ("device", "dir_dim", "pool_slots", "max_beams", "timing", "stream"):
+                setattr(o.slam.dev, k, v)
+            elif k in dict(SlamOptions._fields_):
+                setattr(o.slam, k, v)
+            else:
+                setattr(o, k, v)
+        return o
+
+    def __init__(self, options: GraphOptions = None):
+        self.options = options if options is not None else GraphSlam2D.Options()
+        self.h = C.c_void_p()
+        _chk(lib().lama_graph_create(C.byref(self.options), C.byref(self.h)))
+
+    def __del__(self):
+        if getattr(self, "h", None) and _lib is not None:
+            _lib.lama_graph_destroy(self.h)
+            self.h = None
+
+    def Init(self, x, y, r):
+        """GraphSlam2D::Init (graph_slam2d.cpp:118-121)"""
+        a, ap = _d([x, y, r])
+        _chk(lib().lama_graph_set_pose(self.h, ap))
+
+    def update(self, pts, odom, timestamp=0.0, origin=_ID3, quat=_IDQ) -> bool:
+        """GraphSlam2D::update (graph_slam2d.cpp:188-282)"""
+        p, pp = _d(pts); o, op = _d(origin); q, qp = _d(quat); od, odp = _d(odom)
+        did = C.c_int(0)
+        _chk(lib().lama_graph_update(self.h, pp, C.c_int(p.size // 3), op, qp, odp, C.c_double(timestamp), C.byref(did)))
+        return bool(did.value)
+
+    def getPose(self):
+        """GraphSlam2D::getPose (graph_slam2d.cpp:127-129): correction + slam pose"""
+        out = np.zeros(3)
+        _chk(lib().lama_graph_get_pose(self.h, out.ctypes.data_as(c_dp)))
+        return out
+
+    def keyPoses(self):
+        """key_poses as (corrected n x 3, original n x 3, timestamps n)"""
+        n = C.c_int(0)
+        _chk(lib().lama_graph_get_key_poses(self.h, None, None, None, C.c_int(0), C.byref(n)))
+        cor, org, st = np.zeros((n.value, 3)), np.zeros((n.value, 3)), np.zeros(n.value)
+        _chk(lib().lama_graph_get_key_poses(self.h, cor.ctypes.data_as(c_dp), org.ctypes.data_as(c_dp), st.ctypes.data_as(c_dp), C.c_int(n.value), C.byref(n)))
+        return cor, org, st
+
+    def keyCloud(self, key):
+        """the cloud of key pose `key`: (points n x 3, sensor origin, sensor quaternion xyzw)"""
+        n = C.c_int(0)
+        _chk(lib().lama_graph_get_key_cloud(self.h, C.c_int(key), None, C.c_int(0), None, None, C.byref(n)))
+        pts, o, q = np.zeros((n.value, 3)), np.zeros(3), np.zeros(4)
+        _chk(lib().lama_graph_get_key_cloud(self.h, C.c_int(key), pts.ctypes.data_as(c_dp), C.c_int(n.value), o.ctypes.data_as(c_dp), q.ctypes.data_as(c_dp),
+                                            C.byref(n)))
+        return pts, o, q
+
+    def _ids(self, fn, width):
+        n = C.c_int(0)
+        _chk(fn(self.h, None, C.c_int(0), C.byref(n)))
+        out = np.zeros((n.value, width), np.int32)
+        if n.value:
+            _chk(fn(self.h, out.ctypes.data_as(c_i32p), C.c_int(n.value), C.byref(n)))
+        return out
+
+    def links(self):
+        """links (graph_slam2d.h:116-117): n x {candidate key, reference key}"""
+        return self._ids(lib().lama_graph_get_links, 2)
+
+    def lastCandidates(self):
+        """candidate ids of the latest update's loop search, nearest first"""
+        return self._ids(lib().lama_graph_get_last_candidates, 1).ravel()
+
+    def stats(self):
+        """{key_poses, loop_factors, optimizations, optimizations_ok, last_status, last_report}"""
+        c = np.zeros(4, np.uint64)
+        st = C.c_int(-1)
+        rep = np.zeros(6)
+        _chk(lib().lama_graph_get_stats(self.h, _vp(c), C.byref(st), rep.ctypes.data_as(c_dp)))
+        out = dict(zip(("key_poses", "loop_factors", "optimizations", "optimizations_ok"), (int(v) for v in c)))
+        out.update(last_status=st.value, last_report=dict(zip(_REPORT_KEYS, rep.tolist())))
+        return out
+
+    @property
+    def slam(self) -> "Slam2D":
+        """the inner Slam2D (the public member `slam`), borrowed: its getters, exports and map writers see the local map"""
+        s = Slam2D.__new__(Slam2D)
+        s.options = self.options.slam
+        s.h = C.c_void_p()
+        _chk(lib().lama_graph_slam(self.h, C.byref(s.h)))
+        s.owner = self        # keeps the graph alive; destroying the borrowed handle is a no-op
+        return s
 
 
 class DynamicDistanceMap:

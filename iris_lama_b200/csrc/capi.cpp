@@ -264,9 +264,10 @@ int export_image(Engine* e, int particle, int kind, bool slam_frontend, uint8_t*
 }  // namespace
 
 struct lama_pf { PFSlam2D* p; };
-struct lama_slam { Slam2D* s; };
+struct lama_slam { Slam2D* s; bool owned = true; };   // borrowed (owned = false): the inner Slam2D of a lama_graph
 struct lama_dm { DistanceMapDev* d; bool owned; };
 struct lama_loc { Loc2D* l; lama_dm dm; };
+struct lama_graph { GraphSlam2D* g; lama_slam slam; };
 
 extern "C" {
 
@@ -592,6 +593,17 @@ try {
 LAMA_CATCH
 
 // ---- Slam2D ---------------------------------------------------------------------------------------------
+namespace {
+SlamOptions slam_from(const lama_slam_options* o)
+{
+    SlamOptions s;
+    s.trans_thresh = o->trans_thresh; s.rot_thresh = o->rot_thresh; s.l2_max = o->l2_max; s.truncated_ray = o->truncated_ray;
+    s.transient_map = o->transient_map != 0; s.lidar_odometry = o->lidar_odometry != 0;
+    s.truncated_range = o->truncated_range; s.resolution = o->resolution; s.patch_size = o->patch_size; s.max_iter = o->max_iter;
+    s.strategy = o->strategy; s.occupancy = o->occupancy; s.dev = dev_from(o->dev);
+    return s;
+}
+}  // namespace
 int lama_slam_options_default(lama_slam_options* o)
 try {
     if (!o) return set_err("null options", LAMA_ERR_ARG);
@@ -605,11 +617,7 @@ LAMA_CATCH
 int lama_slam_create(const lama_slam_options* o, lama_slam** out)
 try {
     if (!o || !out) return set_err("null argument", LAMA_ERR_ARG);
-    SlamOptions s;
-    s.trans_thresh = o->trans_thresh; s.rot_thresh = o->rot_thresh; s.l2_max = o->l2_max; s.truncated_ray = o->truncated_ray;
-    s.transient_map = o->transient_map != 0; s.lidar_odometry = o->lidar_odometry != 0;
-    s.truncated_range = o->truncated_range; s.resolution = o->resolution; s.patch_size = o->patch_size; s.max_iter = o->max_iter;
-    s.strategy = o->strategy; s.occupancy = o->occupancy; s.dev = dev_from(o->dev);
+    const SlamOptions s = slam_from(o);
     std::string err;
     Slam2D* sl = Slam2D::create(s, err);
     if (!sl) return set_err(err, lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_ARG);
@@ -619,7 +627,7 @@ try {
 LAMA_CATCH
 int lama_slam_destroy(lama_slam* h)
 try {
-    if (!h) return LAMA_OK;
+    if (!h || !h->owned) return LAMA_OK;
     delete h->s;
     delete h;
     return LAMA_OK;
@@ -956,6 +964,41 @@ try {
 }
 LAMA_CATCH
 
+// ---- LevenbergMarquardtOptimizer over an explicit factor graph (GraphSlam2D's graph goes through the same pgo_optimize_graph) -------------------
+int lama_pgo_optimize_graph(int device, double* nodes_xyr, int n_nodes, const int* prior_nodes, const double* prior_xyr, const double* prior_loss, int n_priors,
+                            const int* between_from_to, const double* between_xyr, const double* between_loss, int n_betweens, int* status, double report[6],
+                            uint8_t* accepted, int accepted_cap, int* n_tries)
+try {
+    if (!nodes_xyr || n_nodes < 1 || n_priors < 0 || n_betweens < 0 || (n_priors && (!prior_nodes || !prior_xyr || !prior_loss)) ||
+        (n_betweens && (!between_from_to || !between_xyr || !between_loss)) || (accepted && accepted_cap < 0))
+        return set_err("bad argument", LAMA_ERR_ARG);
+    auto loss_of = [](const double* l) { return PgoLoss{{l[0], l[1], l[2]}, l[3]}; };
+    std::vector<SE2> nodes((size_t)n_nodes);
+    for (int i = 0; i < n_nodes; ++i) nodes[(size_t)i] = se2_from_xyr(nodes_xyr[3 * i], nodes_xyr[3 * i + 1], nodes_xyr[3 * i + 2]);
+    std::vector<PgoPrior> priors((size_t)n_priors);
+    for (int f = 0; f < n_priors; ++f)
+        priors[(size_t)f] = PgoPrior{prior_nodes[f], se2_from_xyr(prior_xyr[3 * f], prior_xyr[3 * f + 1], prior_xyr[3 * f + 2]), loss_of(prior_loss + 4 * f)};
+    std::vector<PgoBetween> betweens((size_t)n_betweens);
+    for (int f = 0; f < n_betweens; ++f)
+        betweens[(size_t)f] = PgoBetween{between_from_to[2 * f], between_from_to[2 * f + 1],
+                                         se2_from_xyr(between_xyr[3 * f], between_xyr[3 * f + 1], between_xyr[3 * f + 2]), loss_of(between_loss + 4 * f)};
+    PgoReport rep;
+    std::string err;
+    const int rc = pgo_optimize_graph(device, nodes, priors, betweens, rep, err);
+    if (rc != LAMA_OK) return set_err(err, rc);
+    if (status) *status = rep.status;
+    if (report) {
+        report[0] = rep.iterations; report[1] = rep.lambda_tries; report[2] = (double)rep.cg_iterations;
+        report[3] = rep.initial_error; report[4] = rep.final_error; report[5] = rep.device_ms;
+    }
+    if (accepted) std::copy_n(rep.accepted.begin(), std::min<size_t>(rep.accepted.size(), (size_t)accepted_cap), accepted);
+    if (n_tries) *n_tries = (int)rep.accepted.size();
+    if (rep.status == 0)
+        for (int i = 0; i < n_nodes; ++i) xyr_of(nodes[(size_t)i], nodes_xyr + 3 * i);
+    return LAMA_OK;
+}
+LAMA_CATCH
+
 // ---- GraphSlam2D loop-closure front end (src/graph_slam2d.cpp:283-392) ---------------------------------------------------------------------
 namespace {
 int correlate_on(Engine* e, const DeviceOptions* coarse_dev, const double* ref_pts, int ref_n, const double* ref_origin, const double* ref_quat, const double* pts, int n,
@@ -1180,6 +1223,135 @@ try {
     if (!h || !stats) return set_err("null argument", LAMA_ERR_ARG);
     stats[0] = h->l->iterations();
     stats[1] = h->l->evals();
+    return LAMA_OK;
+}
+LAMA_CATCH
+
+// ---- GraphSlam2D (src/graph_slam2d.cpp:104-430) ------------------------------------------------------------------------------------------------
+int lama_graph_options_default(lama_graph_options* o)
+try {
+    if (!o) return set_err("null options", LAMA_ERR_ARG);
+    std::memset(o, 0, sizeof(*o));
+    int rc = lama_slam_options_default(&o->slam);   // Options : Slam2D::Options (graph_slam2d.h:59-60)
+    if (rc != LAMA_OK) return rc;
+    o->key_pose_distance = 1.0; o->key_pose_angular_distance = 0.5 * M_PI; o->key_pose_head_delay = 5;   // graph_slam2d.h:62-86
+    o->loop_search_max_distance = 10.0; o->loop_search_min_distance = 2.0; o->loop_max_candidates = 5;
+    o->loop_closure_scan_rmse = 0.05; o->loop_closure_max_candidates = 10; o->ignore_n_chain_poses = 20;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_create(const lama_graph_options* o, lama_graph** out)
+try {
+    if (!o || !out) return set_err("null argument", LAMA_ERR_ARG);
+    GraphOptions g;
+    g.slam = slam_from(&o->slam);
+    g.key_pose_distance = o->key_pose_distance; g.key_pose_angular_distance = o->key_pose_angular_distance; g.key_pose_head_delay = o->key_pose_head_delay;
+    g.loop_search_max_distance = o->loop_search_max_distance; g.loop_search_min_distance = o->loop_search_min_distance;
+    g.loop_max_candidates = o->loop_max_candidates; g.loop_closure_scan_rmse = o->loop_closure_scan_rmse;
+    g.loop_closure_max_candidates = o->loop_closure_max_candidates; g.ignore_n_chain_poses = o->ignore_n_chain_poses;
+    if (g.key_pose_head_delay < 0 || g.ignore_n_chain_poses < 0 || g.loop_max_candidates < 0) return set_err("GraphSlam2D: negative count in the options", LAMA_ERR_ARG);
+    std::string err;
+    GraphSlam2D* gs = GraphSlam2D::create(g, err);
+    if (!gs) return set_err(err, lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_ARG);
+    *out = new lama_graph{gs, lama_slam{gs->slam(), false}};
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_destroy(lama_graph* h)
+try {
+    if (!h) return LAMA_OK;
+    delete h->g;
+    delete h;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_set_pose(lama_graph* h, const double xyr[3])
+try {
+    if (!h || !xyr) return set_err("null argument", LAMA_ERR_ARG);
+    h->g->init(xyr[0], xyr[1], xyr[2]);
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_update(lama_graph* h, const double* pts, int n, const double* origin, const double* quat, const double* odom, double stamp, int* did_update)
+try {
+    if (!h || !pts || !odom || n < 1) return set_err("null argument or empty scan", LAMA_ERR_ARG);
+    bool did = false;
+    int rc = h->g->update(pts, n, origin, quat, odom, stamp, &did);
+    if (did_update) *did_update = did ? 1 : 0;
+    return rc == LAMA_OK ? rc : set_err(h->g->error(), rc);
+}
+LAMA_CATCH
+int lama_graph_get_pose(lama_graph* h, double xyr[3])
+try {
+    if (!h || !xyr) return set_err("null argument", LAMA_ERR_ARG);
+    xyr_of(h->g->pose(), xyr);
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_get_key_poses(lama_graph* h, double* corrected_xyr, double* original_xyr, double* stamps, int cap, int* count)
+try {
+    if (!h || !count || cap < 0) return set_err("null argument", LAMA_ERR_ARG);
+    const auto& k = h->g->key_poses();
+    const int m = std::min(cap, (int)k.size());
+    for (int i = 0; i < m; ++i) {
+        if (corrected_xyr) xyr_of(k[(size_t)i].pose, corrected_xyr + 3 * i);
+        if (original_xyr) xyr_of(k[(size_t)i].original, original_xyr + 3 * i);
+        if (stamps) stamps[i] = k[(size_t)i].stamp;
+    }
+    *count = (int)k.size();
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_get_key_cloud(lama_graph* h, int key, double* pts, int cap, double* origin, double* quat, int* count)
+try {
+    if (!h || !count || cap < 0) return set_err("null argument", LAMA_ERR_ARG);
+    const auto& k = h->g->key_poses();
+    if (key < 0 || key >= (int)k.size()) return set_err("no such key pose", LAMA_ERR_ARG);
+    const auto& kp = k[(size_t)key];
+    const int n = (int)(kp.pts.size() / 3);
+    if (pts) std::copy_n(kp.pts.begin(), 3 * (size_t)std::min(cap, n), pts);
+    if (origin) std::copy_n(kp.origin, 3, origin);
+    if (quat) std::copy_n(kp.quat, 4, quat);
+    *count = n;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_get_links(lama_graph* h, int32_t* from_to, int cap, int* count)
+try {
+    if (!h || !count || cap < 0 || (cap > 0 && !from_to)) return set_err("null argument", LAMA_ERR_ARG);
+    const auto& l = h->g->links();
+    const int m = std::min(cap, (int)l.size());
+    for (int i = 0; i < m; ++i) { from_to[2 * i] = l[(size_t)i].first; from_to[2 * i + 1] = l[(size_t)i].second; }
+    *count = (int)l.size();
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_get_last_candidates(lama_graph* h, int32_t* ids, int cap, int* count)
+try {
+    if (!h || !count || cap < 0 || (cap > 0 && !ids)) return set_err("null argument", LAMA_ERR_ARG);
+    const auto& c = h->g->last_candidates();
+    std::copy_n(c.begin(), std::min<size_t>(c.size(), (size_t)cap), ids);
+    *count = (int)c.size();
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_get_stats(lama_graph* h, uint64_t counts[4], int* last_status, double last_report[6])
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    const GraphSlam2D::Stats& s = h->g->stats();
+    if (counts) { counts[0] = h->g->key_poses().size(); counts[1] = s.loop_factors; counts[2] = s.optimizations; counts[3] = s.optimizations_ok; }
+    if (last_status) *last_status = s.last.status;
+    if (last_report) {
+        last_report[0] = s.last.iterations; last_report[1] = s.last.lambda_tries; last_report[2] = (double)s.last.cg_iterations;
+        last_report[3] = s.last.initial_error; last_report[4] = s.last.final_error; last_report[5] = s.last.device_ms;
+    }
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_graph_slam(lama_graph* h, lama_slam** slam)
+try {
+    if (!h || !slam) return set_err("null argument", LAMA_ERR_ARG);
+    *slam = &h->slam;
     return LAMA_OK;
 }
 LAMA_CATCH

@@ -868,6 +868,123 @@ int coarse_correlate_candidate_scan(Engine* e, int particle, const DeviceOptions
 }
 
 // =====================================================================================================
+// GraphSlam2D (src/graph_slam2d.cpp:104-430)
+// =====================================================================================================
+GraphSlam2D* GraphSlam2D::create(const GraphOptions& o, std::string& err)
+{
+    if (o.slam.lidar_odometry || o.slam.occupancy != 0) { err = "GraphSlam2D: the inner Slam2D runs on a FrequencyOccupancyMap without lidar odometry"; return nullptr; }
+    GraphOptions g = o;
+    g.slam.transient_map = true;   // :106-107
+    g.slam.truncated_ray = 1.0;
+    Slam2D* s = Slam2D::create(g.slam, err);
+    if (!s) return nullptr;
+    GraphSlam2D* gs = new GraphSlam2D();
+    gs->opt_ = g;
+    gs->slam_.reset(s);
+    return gs;
+}
+
+int GraphSlam2D::update(const double* pts, int n, const double* origin, const double* quat, const double odom_xyr[3], double stamp, bool* did_update)
+{
+    *did_update = false;
+    last_candidates_.clear();
+    bool did = false;
+    int rc = slam_->update(pts, n, origin, quat, odom_xyr, stamp, &did);   // 1. the transient slam (:193-195)
+    if (rc != LAMA_OK) { err_ = slam_->error(); return rc; }
+    if (!did) return LAMA_OK;
+    *did_update = true;
+
+    // 2. key pose test (:200-207): diff = slam pose - prev = pose^-1 prev
+    const SE2 sp = slam_->pose();
+    const SE2 diff = se2_mul(se2_inv(sp), prev_);
+    if (xy_norm(diff) < opt_.key_pose_distance && std::fabs(se2_rotation(diff)) < opt_.key_pose_angular_distance) return LAMA_OK;
+    prev_ = sp;
+
+    // 4. the key pose and its factor (:210-228)
+    int keyid = (int)keys_.size();
+    const SE2 corrected = se2_mul(correction_, sp);
+    if (keyid == 0) {
+        priors_.push_back(PgoPrior{0, sp, PgoLoss{{0.01, 0.01, 0.01}, 0.0}});
+    } else {
+        accdist_ += xy_norm(diff);
+        factors_.push_back(PgoBetween{keyid - 1, keyid, se2_mul(se2_inv(keys_.back().pose), corrected), PgoLoss{{0.25, 0.25, 0.15}, 0.0}});
+    }
+    KeyPose kp;
+    kp.id = keyid;
+    kp.pose = corrected;
+    kp.original = sp;
+    kp.pts.assign(pts, pts + 3 * (size_t)n);
+    for (int k = 0; k < 3; ++k) kp.origin[k] = origin ? origin[k] : 0.0;
+    for (int k = 0; k < 4; ++k) kp.quat[k] = quat ? quat[k] : (k == 3 ? 1.0 : 0.0);
+    kp.stamp = stamp;
+    keys_.push_back(std::move(kp));
+    if (keyid < opt_.key_pose_head_delay || keyid < opt_.ignore_n_chain_poses) return LAMA_OK;   // :230-232
+
+    // 5. loop closure search (:236-273): radius max^r min^(1 - r), query = the key pose head_delay keys back
+    const double r = std::min(accdist_, 100.0) / 100.0;
+    const double radius = std::pow(opt_.loop_search_max_distance, r) * std::pow(opt_.loop_search_min_distance, 1.0 - r);
+    keyid -= opt_.key_pose_head_delay;
+    std::vector<double> key_xy(keys_.size() * 2);
+    for (size_t i = 0; i < keys_.size(); ++i) { key_xy[2 * i] = keys_[i].pose.tx; key_xy[2 * i + 1] = keys_[i].pose.ty; }
+    const double query[2] = {keys_[(size_t)keyid].pose.tx, keys_[(size_t)keyid].pose.ty};
+    last_candidates_ = find_loop_closure_candidates(key_xy.data(), (int)keys_.size(), opt_.ignore_n_chain_poses, query, radius, opt_.loop_max_candidates);
+    factordist_ += xy_norm(diff);
+
+    const SE2 cinv = se2_inv(correction_);
+    const KeyPose& ref = keys_[(size_t)keyid];
+    const SE2 ref_pose = se2_mul(cinv, ref.pose);   // Pose2D(correction.state.inverse()) + pose (:319-320)
+    Engine* e = slam_->engine();
+    for (size_t i = 0; i < last_candidates_.size(); ++i) {
+        const int idx = last_candidates_[i];
+        const KeyPose& cand = keys_[(size_t)idx];
+        const SE2 cand_pose = se2_mul(cinv, cand.pose);
+        SE2 between{1, 0, 0, 0};
+        double rmse = 0.0;
+        rc = correlate_candidate_scan(e, 0, cand.pts.data(), (int)(cand.pts.size() / 3), cand.origin, cand.quat, ref_pose, cand_pose, &between, &rmse);
+        if (rc != LAMA_OK) { err_ = e->last_error(); return rc; }
+        if (rmse > opt_.loop_closure_scan_rmse) {
+            if (i != 0) continue;
+            // one more chance, only for the closest candidate (:254-258)
+            rc = coarse_correlate_candidate_scan(e, 0, slam_->device_options(), ref.pts.data(), (int)(ref.pts.size() / 3), ref.origin, ref.quat, cand.pts.data(),
+                                                 (int)(cand.pts.size() / 3), cand.origin, cand.quat, ref_pose, cand_pose, &between, &rmse, err_);
+            if (rc != LAMA_OK) return rc;
+            if (rmse > opt_.loop_closure_scan_rmse * 2.0) continue;
+        }
+        links_.push_back({idx, keyid});                                              // :266-268, HuberLoss::Huber(0.1)
+        queue_.push_back(PgoBetween{idx, keyid, between, PgoLoss{{1.0, 1.0, 1.0}, 0.1}});
+        ++stats_.loop_factors;
+        factordist_ = 0.0;
+        break;   // only one factor per update
+    }
+    if (queue_.empty() || (queue_.size() <= 5 && factordist_ <= 15.0)) return LAMA_OK;   // :275-276
+    rc = optimize_pose_graph();
+    factordist_ = 0.0;
+    return rc;
+}
+
+int GraphSlam2D::optimize_pose_graph()
+{
+    if (queue_.empty()) return LAMA_OK;
+    factors_.insert(factors_.end(), queue_.begin(), queue_.end());   // :399-402
+    queue_.clear();
+    std::vector<SE2> nodes(keys_.size());
+    for (size_t i = 0; i < keys_.size(); ++i) nodes[i] = keys_[i].pose;   // :408-411
+    PgoReport rep;
+    std::string e;
+    int rc = pgo_optimize_graph(opt_.slam.dev.device, nodes, priors_, factors_, rep, e);   // LevenbergMarquardtOptimizer, default parameters (:404-413)
+    if (rc != LAMA_OK) { err_ = e; return rc; }
+    ++stats_.optimizations;
+    if (rep.status == 0) {   // :414-426: propagate the corrections, correction = (B A^-1)^-1
+        ++stats_.optimizations_ok;
+        for (size_t i = 0; i < keys_.size(); ++i) keys_[i].pose = nodes[i];
+        correction_ = se2_inv(se2_mul(slam_->pose(), se2_inv(keys_.back().pose)));
+    }
+    stats_.last = std::move(rep);
+    accdist_ = 0.0;   // :428-429
+    return LAMA_OK;
+}
+
+// =====================================================================================================
 // Slam2D
 // =====================================================================================================
 Slam2D* Slam2D::create(const SlamOptions& o, std::string& err)

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "engine.h"
+#include "pgo.h"
 
 namespace lama_b200 {
 
@@ -227,6 +228,65 @@ int correlate_candidate_scan(Engine* e, int particle, const double* pts, int n, 
 int coarse_correlate_candidate_scan(Engine* e, int particle, const DeviceOptions& dev, const double* ref_pts, int ref_n, const double* ref_origin, const double* ref_quat,
                                     const double* pts, int n, const double* origin, const double* quat, const SE2& ref_pose, const SE2& cand_pose, SE2* between,
                                     double* rmse, std::string& err);
+
+// ---- GraphSlam2D (include/lama/graph_slam2d.h:51-173, src/graph_slam2d.cpp:104-430) ----------------------------------------------------------
+struct GraphOptions {  // GraphSlam2D::Options, graph_slam2d.h:59-87
+    SlamOptions slam;
+    double key_pose_distance = 1.0, key_pose_angular_distance = 0.5 * M_PI;
+    int key_pose_head_delay = 5;
+    double loop_search_max_distance = 10.0, loop_search_min_distance = 2.0;
+    int loop_max_candidates = 5;
+    double loop_closure_scan_rmse = 0.05;
+    int loop_closure_max_candidates = 10;   // declared but read nowhere in the reference; accepted and ignored
+    int ignore_n_chain_poses = 20;
+};
+
+class GraphSlam2D {
+public:
+    struct KeyPose {   // GraphSlam2D::KeyPose (graph_slam2d.h:97-104); `odom` is read nowhere in the reference and is not kept
+        int id;
+        SE2 pose, original;               // corrected (optimised) and as the inner Slam2D estimated it
+        std::vector<double> pts;          // host copy of the cloud, n x 3
+        double origin[3], quat[4];
+        double stamp;
+    };
+    struct Stats {
+        uint64_t loop_factors = 0, optimizations = 0, optimizations_ok = 0;
+        PgoReport last;                   // of the latest optimisation
+    };
+
+    static GraphSlam2D* create(const GraphOptions& o, std::string& err);
+    void init(double x, double y, double r) { slam_->set_pose(x, y, r); }   // Init (:118-121)
+    // bool update(surface, odometry, timestamp) (:188-282); returns a LAMA_* status
+    int update(const double* pts, int n, const double* origin, const double* quat, const double odom_xyr[3], double stamp, bool* did_update);
+    SE2 pose() const { return se2_mul(correction_, slam_->pose()); }        // getPose (:127-129)
+    Slam2D* slam() { return slam_.get(); }
+    const std::vector<KeyPose>& key_poses() const { return keys_; }
+    const std::vector<std::pair<int, int>>& links() const { return links_; }
+    const std::vector<int>& last_candidates() const { return last_candidates_; }   // of the latest loop search (empty when there was none)
+    const Stats& stats() const { return stats_; }
+    const std::string& error() const { return err_; }
+
+private:
+    GraphOptions opt_;
+    std::unique_ptr<Slam2D> slam_;
+    std::vector<KeyPose> keys_;
+    std::vector<std::pair<int, int>> links_;
+    std::vector<PgoPrior> priors_;            // the persistent graph (graph_slam2d.cpp:110): the prior on key 0,
+    std::vector<PgoBetween> factors_;         // then chain and loop factors in graph->add order
+    std::vector<PgoBetween> queue_;           // factor_queue: loop factors not yet in the graph
+    std::vector<int> last_candidates_;
+    SE2 correction_{1, 0, 0, 0};
+    double accdist_ = 0.0;
+    // the function-local statics of update() (:197, :200, :244) kept per instance: the reference shares them across every
+    // GraphSlam2D of a process; for a single instance the behaviour is the same
+    SE2 prev_ = se2_from_xyr(1e10, 1e10, 0.0);
+    double factordist_ = 0.0;
+    Stats stats_;
+    std::string err_;
+    GraphSlam2D() = default;
+    int optimize_pose_graph();                 // optimizePoseGraph (:394-430)
+};
 
 // SimpleOccupancyMap (src/sdm/simple_occupancy_map.cpp:36-149): Loc2D's static tri-state map.  It is only consulted by
 // the host-side rejection sampling of globalLocalization, so it lives on the host.
