@@ -177,6 +177,9 @@ struct RayShared {
     uint32_t log_count, event_count, cells, err;
     uint32_t work[2];       // work-item counters of the two passes
     uint32_t any_pending, n_cand;
+#ifdef LAMA_PHASE_TIMING
+    uint32_t walk_cells[2];  // planar walk cells of the first pass in y-major / x-major beam groups
+#endif
 };
 
 // In-place ascending bitonic sort of n (power of two) 64-bit keys in shared memory by the whole block.
@@ -245,9 +248,14 @@ __device__ __forceinline__ int next_pow2(int v)
 // the z axis of the reference's loop never moves: delta_z = 0 and 2 * err_z = 0 < n).  Its state after i steps has
 // the closed form   k = floor((2 i d + n) / (2 n)),  coord = from + s k,  err = i d - k n,
 // so a walk can start anywhere: work items are (group of 32 adjacent beams, segment of kSegSteps steps), handed to
-// warps through a shared counter.  Lanes of a warp walk angularly adjacent beams in lock step (their atomics fall
-// into the same sectors) and every warp gets the same amount of work, whatever the ray lengths.
+// warps through a shared counter.  Lanes of a warp walk angularly adjacent beams in lock step (in y-major groups their
+// atomics fall into the same sectors; x-major groups walk several steps of fewer beams per instruction, see raycast_pass)
+// and every warp gets the same amount of work, whatever the ray lengths.
 constexpr int kSegSteps = 64;
+// x-major groups: consecutive steps of one beam per reduction instruction (see raycast_pass).  8 = 4 beams x 8 steps; on the H100
+// 4 was slower and 16 no faster (DESIGN.md §5)
+constexpr int kXStride = 8;
+static_assert(32 % kXStride == 0, "the lanes of a warp split evenly over the beams of a round");
 
 struct BeamEnds {      // 16 bytes; WINDOW-RELATIVE cell coordinates (< 2^16)
     uint32_t fx, fy;   // from cell; bit 31 of fx: mark_hit, bit 31 of fy: non-planar (generic 3-axis walk)
@@ -301,6 +309,9 @@ struct RayCtx {
     int log2dim;
     bool mark;                 // first pass: note the patches that are not writable yet
     int last_di;               // kProb
+#ifdef LAMA_PHASE_TIMING
+    bool no_red = false;       // RayParams::debug: skip the reductions of the current touches
+#endif
 
     __device__ __forceinline__ uint32_t dir_of_cell(uint32_t P) const { return packed_dir_index(P, log2dim); }
 
@@ -329,7 +340,7 @@ struct RayCtx {
             lo |= off;
             asm("mov.b64 %0, {%1, %2};" : "=l"(addr) : "r"(lo), "r"(hi));
 #ifdef LAMA_PHASE_TIMING
-            if (rp.debug & 1) { if (addr == 1) sh.err = lo; } else
+            if (no_red) { if (addr == 1) sh.err = lo; } else
 #endif
             asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(addr), "r"(hit ? kOccHitInc : run * kOccMissInc) : "memory");
         }
@@ -361,6 +372,9 @@ __device__ __forceinline__ void raycast_pass(RayCtx<kProb>& c, const BeamEnds* b
 {
     const int tid = threadIdx.x, lane = tid & 31;
     c.last_di = -1;
+#ifdef LAMA_PHASE_TIMING
+    c.no_red = c.rp.debug & 1;
+#endif
     // hits (setOccupied, pf_slam2d.cpp:493-498)
     for (int b = tid; b < n_beams; b += blockDim.x) {
         const BeamEnds be = beams[b];
@@ -382,9 +396,20 @@ __device__ __forceinline__ void raycast_pass(RayCtx<kProb>& c, const BeamEnds* b
         const int seg = (int)(item - seg_prefix[g]);
         const int b = g * 32 + lane;
         const BeamEnds be = beams[b];   // the cache is padded to whole groups (padding lanes are flagged non-planar)
-        SegWalk w;
-        w.init(be.fx & ~kBeamFlag, be.fy & ~kBeamFlag, be.tx, be.ty, seg * kSegSteps, (be.fy & kBeamFlag) ? 0 : kSegSteps);
+        // the group is x-major when most of its planar beams are (SegWalk::init: dx >= dy)
+        const bool planar = !(be.fy & kBeamFlag);
+        const int adx = abs((int)(be.tx - (be.fx & ~kBeamFlag))), ady = abs((int)(be.ty - (be.fy & ~kBeamFlag)));
+        const unsigned planar_lanes = __ballot_sync(0xffffffffu, planar), xmajor_lanes = __ballot_sync(0xffffffffu, planar && adx >= ady);
+        const bool xgroup = 2 * __popc(xmajor_lanes) > __popc(planar_lanes);
+#ifdef LAMA_PHASE_TIMING
+        c.no_red = (c.rp.debug & 1) || (c.rp.debug & (xgroup ? 4 : 8));
+        const int seg_cells = planar ? min(max(adx, ady) - 1, (seg + 1) * kSegSteps) - seg * kSegSteps : 0;
+        const uint32_t cells = __reduce_add_sync(0xffffffffu, (uint32_t)max(seg_cells, 0));
+        if (c.mark && lane == 0) atomicAdd(&c.sh.walk_cells[xgroup], cells);
+#endif
         if (seg == 0) {
+            SegWalk w;
+            w.init(be.fx & ~kBeamFlag, be.fy & ~kBeamFlag, be.tx, be.ty, 0, planar ? kSegSteps : 0);
             // Lanes walk angularly adjacent beams in lock step, so close to the sensor neighbouring lanes sit on the
             // same cell: runs of equal cells are merged into ONE reduction carrying the run length (counter additions
             // commute; the visited half-word wraps like the reference's uint16).  The ordered-path log stays per touch.
@@ -402,27 +427,40 @@ __device__ __forceinline__ void raycast_pass(RayCtx<kProb>& c, const BeamEnds* b
                 }
             }
         } else {
-            // software pipeline: the patch-info word of the NEXT cell is fetched from shared memory before the current cell is
-            // processed, so the load latency overlaps the address arithmetic and the reduction of the current cell.  The lane counts
-            // its steps itself (no end test inside the walk); the step taken past the last cell of the segment lands on a cell of the
-            // same beam (at most its end cell), so its directory index is valid and its patch-info word is simply not used.
-            int rem = w.iend - w.i;
-            if (rem > 0) {
-                w.step();
-                uint32_t P = w.P, di = c.dir_of_cell(P);
+            // Issue order.  In a y-major group the lanes of one step share a row, so one reduction instruction falls into a few
+            // sectors: lane = beam, one step at a time.  In an x-major group the lanes of one step share a COLUMN (up to 32 lines);
+            // there kXStride lanes walk one beam at consecutive offsets with stride kXStride, so that one instruction covers
+            // 32 / kXStride beams x kXStride consecutive steps along their rows, and the group's beams take kXStride rounds.
+            // The cells touched are the same (counter additions commute, the log is sorted), only the order of the reductions changes.
+            const int S = xgroup ? kXStride : 1;
+            for (int round = 0; round < S; ++round) {
+                const int bb = xgroup ? g * 32 + round * (32 / kXStride) + lane / kXStride : b;
+                const BeamEnds e = xgroup ? beams[bb] : be;
+                StrideWalk sw;
+                sw.init(e.fx & ~kBeamFlag, e.fy & ~kBeamFlag, e.tx, e.ty, seg * kSegSteps + 1 + (xgroup ? lane % kXStride : 0),
+                        (e.fy & kBeamFlag) ? 0 : (seg + 1) * kSegSteps, S);
+                if (sw.i > sw.iend) continue;
+                // software pipeline: the patch-info word of the NEXT cell is fetched from shared memory before the current cell is
+                // processed, so the load latency overlaps the address arithmetic and the reduction of the current cell.  The walk never
+                // steps past the lane's last cell, so every directory index it forms lies inside the beam's bounding box.
+                uint32_t P = sw.P, di = c.dir_of_cell(P);
                 uint32_t info = c.pinfo[di];
-                for (;;) {
-                    const uint32_t pos = (uint32_t)w.i;
-                    w.step();
-                    const uint32_t Pn = w.P, din = c.dir_of_cell(Pn);
+                const int last_prefetch = sw.iend - S;
+                while (sw.i <= last_prefetch) {
+                    const uint32_t pos = (uint32_t)sw.i;
+                    sw.step();
+                    const uint32_t Pn = sw.P, din = c.dir_of_cell(Pn);
                     const uint32_t infon = c.pinfo[din];
-                    c.cell(P, info, di, (uint32_t)b, pos, false, 1u);
-                    if (--rem == 0) break;
+                    c.cell(P, info, di, (uint32_t)bb, pos, false, 1u);
                     P = Pn; di = din; info = infon;
                 }
+                c.cell(P, info, di, (uint32_t)bb, (uint32_t)sw.i, false, 1u);
             }
         }
     }
+#ifdef LAMA_PHASE_TIMING
+    c.no_red = c.rp.debug & 1;
+#endif
     // non-planar beams (tilted sensor): the reference's 3-axis walk, one thread per beam
     for (int b = tid; b < n_beams; b += blockDim.x) {
         if (!(beams[b].fy & kBeamFlag)) continue;
@@ -490,6 +528,9 @@ k_raycast(StoreView s, RayParams rp, const SE2* __restrict__ states, uint64_t* _
         sh.work[0] = sh.work[1] = 0;
         sh.any_pending = 0;
         sh.n_cand = 0;
+#ifdef LAMA_PHASE_TIMING
+        sh.walk_cells[0] = sh.walk_cells[1] = 0;
+#endif
     }
     for (int i = tid; i < 2 * nwords; i += blockDim.x) hotmap[i] = 0u;  // hotmap + pending are contiguous
     for (int i = tid; i < dim2; i += blockDim.x) pinfo[i] = 0xFFFFFFFFu;  // kCandNone, not writable
@@ -754,8 +795,8 @@ k_raycast(StoreView s, RayParams rp, const SE2* __restrict__ states, uint64_t* _
     __syncthreads();
     RAY_MARK(5);
     if (tid == 0 && (blockIdx.x == 0 || blockIdx.x == 200))
-        printf("ray cta %d: setup %lld walk %lld sort %lld replay %lld events %lld | log %u events %u\n", blockIdx.x, ph[1] - ph[0], ph[2] - ph[1], ph[3] - ph[2],
-               ph[4] - ph[3], ph[5] - ph[4], sh.log_count, sh.event_count);
+        printf("ray cta %d debug %d: setup %lld walk %lld sort %lld replay %lld events %lld | log %u events %u | walk cells y-major %u x-major %u\n", blockIdx.x,
+               rp.debug, ph[1] - ph[0], ph[2] - ph[1], ph[3] - ph[2], ph[4] - ph[3], ph[5] - ph[4], sh.log_count, sh.event_count, sh.walk_cells[0], sh.walk_cells[1]);
 #endif
     if (tid == 0) {
         MapUpdateStats& st = stats[blockIdx.x];

@@ -59,7 +59,8 @@ struct RayParams {
     int state_stride;        // bytes between the poses handed to k_raycast (sizeof(SE2), or sizeof(MatchResult) when it reads k_match's output)
     int log_cap, event_cap;  // powers of two
     int cand_cap;            // candidate bitmaps (patches with hit cells or distance-map obstacles), <= 253
-    int debug;               // developer experiments (LAMA_RAY_DEBUG, only honoured by LAMA_PHASE_TIMING builds): 1 no RED, 2 no LDS
+    int debug;               // developer experiments (LAMA_RAY_DEBUG, only honoured by LAMA_PHASE_TIMING builds): 1 no RED, 2 no LDS,
+                             // 4 no RED in the walk of x-major beam groups, 8 no RED in the walk of y-major beam groups
     int prob_mode;           // 1: log-odds occupancy (ProbabilisticOccupancyMap), counts go to the scratch map first
     int pull_fallback;       // 1: k_raycast only handles the particles k_ray_setup left to it (RayPullHeader::ok == 0)
     ProbParams prob;

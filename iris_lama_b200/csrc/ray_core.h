@@ -180,6 +180,37 @@ struct SegWalk {
     }
 };
 
+// The planar walk taken S steps at a time: it visits the cells SegWalk visits at steps first, first + S, first + 2 S, ... up to
+// iend.  With S d = q n + r (0 <= r < n), a stride moves the major axis S times and the minor axis q or q + 1 times: the
+// state after step j has e in [-n/2, n/2), so e + r < 3n/2 and one test decides the extra move, as in the unit step
+//   e += r;  minor coordinate += q;  if (2 e >= n) { minor coordinate moves once more; e -= n; }
+// and a stride costs what a step costs.  k_raycast lets S lanes walk one x-major beam at consecutive offsets: the cells of one
+// reduction instruction then lie along a row of each beam's patch instead of down a column.
+struct StrideWalk {
+    int e2, r2, n2, i, iend, S;   // e2 = 2 e - n as in SegWalk, r2 = 2 r
+    int MS, N;                    // packed vector of one stride without the extra minor move / of the extra minor move
+    uint32_t P;
+    // first >= 1; the walk ends at step min(end, n - 1), the last interior cell; i > iend: nothing to visit
+    LAMA_HD void init(uint32_t fx, uint32_t fy, uint32_t tx, uint32_t ty, int first, int end, int stride)
+    {
+        SegWalk w;
+        w.init(fx, fy, tx, ty, first, end - first);
+        const int n = w.n2 >> 1, d = w.d2 >> 1;
+        const int q = n ? (int)((uint32_t)(stride * d) / (uint32_t)n) : 0;
+        e2 = w.e2; r2 = 2 * (stride * d - q * n); n2 = w.n2;
+        i = first; iend = w.iend; S = stride;
+        MS = stride * w.M + q * w.N; N = w.N;
+        P = w.P;
+    }
+    LAMA_HD void step()
+    {
+        i += S;
+        e2 += r2;
+        P += (uint32_t)MS;
+        if (e2 >= 0) { P += (uint32_t)N; e2 -= n2; }
+    }
+};
+
 // ---- event log ---------------------------------------------------------------------------------------
 // log record: [cell key : 32][beam : 16][pos : 15][kind : 1], kind 1 = hit, 0 = miss.  Sorting the
 // 64-bit records groups touches by cell and orders them by beam (a beam touches a cell at most once).
