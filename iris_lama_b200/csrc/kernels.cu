@@ -263,6 +263,26 @@ struct BeamEnds {      // 16 bytes; WINDOW-RELATIVE cell coordinates (< 2^16)
 };
 constexpr uint32_t kBeamFlag = 0x80000000u;
 
+// The class of a group, decided by the warp that holds its 32 cached beams: x-major when most of its planar beams are (SegWalk::init:
+// dx >= dy).  Phase 1a (segment counts) and raycast_pass (segment partition) both decide it here, from the same cache entries.
+__device__ __forceinline__ bool group_is_xmajor(const BeamEnds& be)
+{
+    const bool planar = !(be.fy & kBeamFlag);
+    const int adx = abs((int)(be.tx - (be.fx & ~kBeamFlag))), ady = abs((int)(be.ty - (be.fy & ~kBeamFlag)));
+    const unsigned planar_lanes = __ballot_sync(0xffffffffu, planar), xmajor_lanes = __ballot_sync(0xffffffffu, planar && adx >= ady);
+    return 2 * __popc(xmajor_lanes) > __popc(planar_lanes);
+}
+// Sector alignment of the strided walk (see raycast_pass): an x-major beam of an x-major group starts segment s >= 1 at step
+// s * kSegSteps + 1 - delta (xmajor_seg_shift), so each of its kXStride-step octets covers one aligned 32-byte run of counters along
+// its row.  Segment 0 ends at step kSegSteps - delta.  All other beams have delta = 0.
+static_assert(kSegSteps % kXStride == 0 && kXStride == 8, "one octet of 4-byte counters = one 32-byte sector");
+__device__ __forceinline__ int seg_shift(const BeamEnds& be, bool xgroup)
+{
+    const uint32_t fx = be.fx & ~kBeamFlag;
+    const int adx = abs((int)(be.tx - fx)), ady = abs((int)(be.ty - (be.fy & ~kBeamFlag)));
+    return xgroup && !(be.fy & kBeamFlag) && adx >= ady ? xmajor_seg_shift(fx, be.tx) : 0;
+}
+
 constexpr uint32_t kCandNone = 0xFF, kCandOverflow = 0xFE;
 constexpr uint32_t kInfoSlotMask = 0x00FFFFFFu;   // slot field of a patch-info word; all ones = not writable in this pass
 
@@ -396,23 +416,25 @@ __device__ __forceinline__ void raycast_pass(RayCtx<kProb>& c, const BeamEnds* b
         const int seg = (int)(item - seg_prefix[g]);
         const int b = g * 32 + lane;
         const BeamEnds be = beams[b];   // the cache is padded to whole groups (padding lanes are flagged non-planar)
-        // the group is x-major when most of its planar beams are (SegWalk::init: dx >= dy)
         const bool planar = !(be.fy & kBeamFlag);
-        const int adx = abs((int)(be.tx - (be.fx & ~kBeamFlag))), ady = abs((int)(be.ty - (be.fy & ~kBeamFlag)));
-        const unsigned planar_lanes = __ballot_sync(0xffffffffu, planar), xmajor_lanes = __ballot_sync(0xffffffffu, planar && adx >= ady);
-        const bool xgroup = 2 * __popc(xmajor_lanes) > __popc(planar_lanes);
+        const bool xgroup = group_is_xmajor(be);
+        const int shift = seg_shift(be, xgroup);
 #ifdef LAMA_PHASE_TIMING
         c.no_red = (c.rp.debug & 1) || (c.rp.debug & (xgroup ? 4 : 8));
-        const int seg_cells = planar ? min(max(adx, ady) - 1, (seg + 1) * kSegSteps) - seg * kSegSteps : 0;
+        const int adx = abs((int)(be.tx - (be.fx & ~kBeamFlag))), ady = abs((int)(be.ty - (be.fy & ~kBeamFlag)));
+        const int seg_cells = planar ? min(max(adx, ady) - 1, (seg + 1) * kSegSteps - shift) - max(seg * kSegSteps - shift, 0) : 0;
         const uint32_t cells = __reduce_add_sync(0xffffffffu, (uint32_t)max(seg_cells, 0));
         if (c.mark && lane == 0) atomicAdd(&c.sh.walk_cells[xgroup], cells);
 #endif
-        if (seg == 0) {
+        if (seg == 0 || !xgroup) {
+            // Issue order of segment 0 and of y-major groups: lane = beam, one step at a time.  In a y-major group the lanes of one step
+            // share a row, so one reduction instruction falls into a few sectors.  Lanes walk angularly adjacent beams in lock step, so
+            // neighbouring lanes often sit on the same cell (everywhere close to the sensor, in y-major groups for several segments):
+            // runs of equal cells are merged into ONE reduction carrying the run length (counter additions commute; the visited
+            // half-word wraps like the reference's uint16).  The ordered-path log stays per touch.
+            const int i0 = max(seg * kSegSteps - shift, 0);
             SegWalk w;
-            w.init(be.fx & ~kBeamFlag, be.fy & ~kBeamFlag, be.tx, be.ty, 0, planar ? kSegSteps : 0);
-            // Lanes walk angularly adjacent beams in lock step, so close to the sensor neighbouring lanes sit on the
-            // same cell: runs of equal cells are merged into ONE reduction carrying the run length (counter additions
-            // commute; the visited half-word wraps like the reference's uint16).  The ordered-path log stays per touch.
+            w.init(be.fx & ~kBeamFlag, be.fy & ~kBeamFlag, be.tx, be.ty, i0, planar ? (seg + 1) * kSegSteps - shift - i0 : 0);
             for (;;) {
                 const bool v = w.next();
                 const unsigned valid = __ballot_sync(0xffffffffu, v);
@@ -427,25 +449,26 @@ __device__ __forceinline__ void raycast_pass(RayCtx<kProb>& c, const BeamEnds* b
                 }
             }
         } else {
-            // Issue order.  In a y-major group the lanes of one step share a row, so one reduction instruction falls into a few
-            // sectors: lane = beam, one step at a time.  In an x-major group the lanes of one step share a COLUMN (up to 32 lines);
-            // there kXStride lanes walk one beam at consecutive offsets with stride kXStride, so that one instruction covers
-            // 32 / kXStride beams x kXStride consecutive steps along their rows, and the group's beams take kXStride rounds.
-            // The cells touched are the same (counter additions commute, the log is sorted), only the order of the reductions changes.
-            const int S = xgroup ? kXStride : 1;
-            for (int round = 0; round < S; ++round) {
-                const int bb = xgroup ? g * 32 + round * (32 / kXStride) + lane / kXStride : b;
-                const BeamEnds e = xgroup ? beams[bb] : be;
+            // Issue order of the later segments of an x-major group.  The lanes of one step share a COLUMN (up to 32 lines), so
+            // kXStride lanes walk one beam at consecutive offsets with stride kXStride: one instruction covers 32 / kXStride beams x
+            // kXStride consecutive steps along their rows, and the group's beams take kXStride rounds.  The segments of x-major beams
+            // are shifted back by seg_shift, so those kXStride cells of a beam fill one 32-byte sector whenever the minor axis does not
+            // move among them.  The cells touched are the same (counter additions commute, the log is sorted), only the order of the
+            // reductions changes.
+            for (int round = 0; round < kXStride; ++round) {
+                const int bb = g * 32 + round * (32 / kXStride) + lane / kXStride;
+                const BeamEnds e = beams[bb];
+                const int first = seg * kSegSteps + 1 - seg_shift(e, true);
                 StrideWalk sw;
-                sw.init(e.fx & ~kBeamFlag, e.fy & ~kBeamFlag, e.tx, e.ty, seg * kSegSteps + 1 + (xgroup ? lane % kXStride : 0),
-                        (e.fy & kBeamFlag) ? 0 : (seg + 1) * kSegSteps, S);
+                sw.init(e.fx & ~kBeamFlag, e.fy & ~kBeamFlag, e.tx, e.ty, first + lane % kXStride,
+                        (e.fy & kBeamFlag) ? 0 : first + kSegSteps - 1, kXStride);
                 if (sw.i > sw.iend) continue;
                 // software pipeline: the patch-info word of the NEXT cell is fetched from shared memory before the current cell is
                 // processed, so the load latency overlaps the address arithmetic and the reduction of the current cell.  The walk never
                 // steps past the lane's last cell, so every directory index it forms lies inside the beam's bounding box.
                 uint32_t P = sw.P, di = c.dir_of_cell(P);
                 uint32_t info = c.pinfo[di];
-                const int last_prefetch = sw.iend - S;
+                const int last_prefetch = sw.iend - kXStride;
                 while (sw.i <= last_prefetch) {
                     const uint32_t pos = (uint32_t)sw.i;
                     sw.step();
@@ -549,7 +572,7 @@ k_raycast(StoreView s, RayParams rp, const SE2* __restrict__ states, uint64_t* _
     }
     for (int b = tid; b < n_groups * 32; b += blockDim.x) {
         BeamEnds be{0u, 0u | kBeamFlag, 0u, 0u};  // padding lanes: flagged non-planar, never walked (b >= n)
-        int segs = 0;
+        int walk = 0;   // interior cells of a planar beam
         if (b < n) {
             const double pt[3] = {__ldg(rp.points + 3 * (size_t)b), __ldg(rp.points + 3 * (size_t)b + 1), __ldg(rp.points + 3 * (size_t)b + 2)};
             const BeamCells bc = beam_cells(tf, rp.scan, pt);
@@ -568,11 +591,14 @@ k_raycast(StoreView s, RayParams rp, const SE2* __restrict__ states, uint64_t* _
                 const int nn = max(max(ddx < 0 ? -ddx : ddx, ddy < 0 ? -ddy : ddy), ddz < 0 ? -ddz : ddz);
                 my_cells += nn > 1 ? (uint32_t)(nn - 1) : 0u;
                 if (ddz != 0) be.fy |= kBeamFlag;
-                else segs = nn > 1 ? (nn - 1 + kSegSteps - 1) / kSegSteps : 0;
+                else walk = nn - 1;
             }
         }
         beams[b] = be;
-        segs = __reduce_max_sync(0xffffffffu, segs);  // segments of a group = those of its longest beam
+        // one warp holds one group: steps 1 .. walk in segments shifted back by seg_shift; a group has the segments of its longest beam
+        const bool xgroup = group_is_xmajor(be);   // warp-collective: every lane of the warp, before any lane-dependent branch
+        int segs = walk > 0 ? (walk + seg_shift(be, xgroup) + kSegSteps - 1) / kSegSteps : 0;
+        segs = __reduce_max_sync(0xffffffffu, segs);
         if (lane == 0) seg_prefix[b >> 5] = (uint32_t)segs;
     }
     __syncthreads();

@@ -211,6 +211,11 @@ struct StrideWalk {
     }
 };
 
+// Sector alignment of an x-major beam's strided segments: the delta in 0 .. 7 for which step 8 m + 1 - delta (m >= 1) is the first cell of an
+// aligned octet of x in walk direction, x = 0 mod 8 when tx >= fx and x = 7 mod 8 when tx < fx (the major axis moves on every step).
+// Window-relative x has the alignment of the cell's offset in its patch row, so the octet is one 32-byte sector of counters.
+LAMA_HD int xmajor_seg_shift(uint32_t fx, uint32_t tx) { return (int)((tx < fx ? 0u - fx : fx + 1u) & 7u); }
+
 // ---- event log ---------------------------------------------------------------------------------------
 // log record: [cell key : 32][beam : 16][pos : 15][kind : 1], kind 1 = hit, 0 = miss.  Sorting the
 // 64-bit records groups touches by cell and orders them by beam (a beam touches a cell at most once).
