@@ -374,6 +374,42 @@ int lama_graph_get_stats(lama_graph* h, uint64_t counts[4], int* last_status, do
  * lama_slam_destroy on it does nothing, and it dies with the lama_graph */
 int lama_graph_slam(lama_graph* h, lama_slam** slam);
 
+/* ------------------------------------------------------------------------------------------------
+ * FrequencyOccupancyMap -- include/lama/sdm/frequency_occupancy_map.h: a device-resident {occupied, visited} map with its own
+ * 'known' plane (a pruned cell is {0, 0} and still known).  Cells outside the directory window make a call fail with
+ * LAMA_ERR_WINDOW; the map is then partly updated.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct lama_om lama_om;
+/* FrequencyOccupancyMap(resolution, patch_size), window of dev->dir_dim^2 patches centred on center_xy (NULL: origin); dev->pool_slots
+ * 0 = dir_dim^2 patches, so a full window cannot run out */
+int lama_om_create(double resolution, uint32_t patch_size, const double center_xy[2], const lama_device_options* dev, lama_om** out);
+int lama_om_destroy(lama_om* om);   /* does nothing on a borrowed handle */
+/* the loop of GraphSlam2D::generateOccupancyMap (graph_slam2d.cpp:135-160) for any posed scans: scan k = points [offsets[k],
+ * offsets[k + 1]) of pts_xyz (offsets[0] = 0), sensor origins + 3k / quats_xyzw + 4k (either may be NULL: identity), base pose
+ * states + 4k as SE2 {cos, sin, x, y}.  In point order: setOccupied(tf * p), and with `full` setFree on every cell of
+ * computeRay(w2m(tf.translation()), w2m(tf * p)) (both ends excluded).  *cells (may be NULL) = cell updates.  No prune. */
+int lama_om_insert_scans(lama_om* om, const double* pts_xyz, const int64_t* offsets, int n_scans, const double* origins, const double* quats_xyzw,
+                         const double* states, int full, uint64_t* cells);
+int lama_om_prune(lama_om* om);   /* FrequencyOccupancyMap::prune, frequency_occupancy_map.cpp:149-158 */
+int lama_om_resolution(lama_om* om, double* resolution);
+int lama_om_bounds(lama_om* om, uint32_t mn[2], uint32_t mx[2], int* patches);   /* Map::bounds in cells, map.cpp:139-157 */
+/* flags bit 0 isFree, bit 1 isOccupied, bit 2 isUnknown; prob = getProbability (as lama_pf_occupancy_query) */
+int lama_om_query(lama_om* om, const uint32_t* cells_xy, int n, double* prob, uint8_t* flags);
+int lama_om_export(lama_om* om, uint32_t x0, uint32_t y0, int w, int hgt, uint16_t* occupied, uint16_t* visited, uint8_t* known);
+int lama_om_write(lama_om* om, const char* path);                                   /* Map::write, map.cpp:490-529 */
+int lama_om_export_image(lama_om* om, uint8_t* pixels, size_t cap, int dims[2]);   /* sdm::export_to_png(OccupancyMap), export.cpp:46-73 */
+/* with dev->timing: ms[1] = device time of the casts (lama_om_insert_scans), launches as lama_slam_kernel_times */
+int lama_om_kernel_times(lama_om* om, double ms[4], uint64_t launches[5]);
+/* GraphSlam2D::generateOccupancyMap(full) (graph_slam2d.cpp:131-164): after an optimisation (or on the first call) a new map at
+ * (full ? resolution : 0.1 m), then the key scans not yet cast, at their corrected poses, then prune over the whole map.  The handle
+ * is BORROWED: owned by the lama_graph, and the map behind it is replaced in place when it is recreated (possibly at another
+ * resolution), where the reference hands out a new shared_ptr. */
+int lama_graph_generate_occupancy_map(lama_graph* h, int full, lama_om** om);
+/* GraphSlam2D::generateCoarseDistanceMap (graph_slam2d.cpp:166-186): a new 0.1 m distance map with a 5 m reach and an obstacle at
+ * every occupied cell of the inner Slam2D, visited in ascending directory index, then cell index (x fastest); *processed (may be
+ * NULL) = its update() return value.  BORROWED like the occupancy map. */
+int lama_graph_generate_coarse_distance_map(lama_graph* h, lama_dm** dm, uint32_t* processed);
+
 #ifdef __cplusplus
 }
 #endif

@@ -142,6 +142,10 @@ public:
     void getPose(double xyr[3]) const { check(lama_graph_get_pose(h_, xyr)); }   // :127-129
     // the inner Slam2D (the public member `slam`), borrowed: valid while this object lives
     lama_slam* slam() const { lama_slam* s = nullptr; check(lama_graph_slam(h_, &s)); return s; }
+    // generateOccupancyMap (:131-164) / generateCoarseDistanceMap (:166-186): BORROWED maps, owned by this object and replaced in
+    // place when it recreates them (the reference returns a fresh shared_ptr instead)
+    lama_om* generateOccupancyMap(bool full = false) { lama_om* m = nullptr; check(lama_graph_generate_occupancy_map(h_, full ? 1 : 0, &m)); return m; }
+    lama_dm* generateCoarseDistanceMap() { lama_dm* d = nullptr; check(lama_graph_generate_coarse_distance_map(h_, &d, nullptr)); return d; }
     lama_graph* handle() const { return h_; }
 
 private:

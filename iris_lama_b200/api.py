@@ -84,7 +84,9 @@ EXPORTED_SYMBOLS = [
     "lama_dm_distance", "lama_dm_bounds", "lama_dm_export", "lama_dm_import", "lama_dm_match_normal_equations", "lama_dm_match_solve",
     "lama_pgo_optimize_graph", "lama_graph_options_default", "lama_graph_create", "lama_graph_destroy", "lama_graph_set_pose", "lama_graph_update",
     "lama_graph_get_pose", "lama_graph_get_key_poses", "lama_graph_get_key_cloud", "lama_graph_get_links", "lama_graph_get_last_candidates",
-    "lama_graph_get_stats", "lama_graph_slam",
+    "lama_graph_get_stats", "lama_graph_slam", "lama_graph_generate_occupancy_map", "lama_graph_generate_coarse_distance_map",
+    "lama_om_create", "lama_om_destroy", "lama_om_insert_scans", "lama_om_prune", "lama_om_resolution", "lama_om_bounds", "lama_om_query",
+    "lama_om_export", "lama_om_write", "lama_om_export_image", "lama_om_kernel_times",
 ]
 
 
@@ -732,6 +734,101 @@ class GraphSlam2D:
         _chk(lib().lama_graph_slam(self.h, C.byref(s.h)))
         s.owner = self        # keeps the graph alive; destroying the borrowed handle is a no-op
         return s
+
+    def generateOccupancyMap(self, full=False) -> "FrequencyOccupancyMap":
+        """GraphSlam2D::generateOccupancyMap (graph_slam2d.cpp:131-164).  The map is BORROWED: owned by this graph and replaced in
+        place when the graph recreates it (after a pose-graph optimisation), so an earlier returned object sees the newest map."""
+        h = C.c_void_p()
+        _chk(lib().lama_graph_generate_occupancy_map(self.h, C.c_int(1 if full else 0), C.byref(h)))
+        return FrequencyOccupancyMap(handle=h, owner=self)
+
+    def generateCoarseDistanceMap(self) -> "DynamicDistanceMap":
+        """GraphSlam2D::generateCoarseDistanceMap (graph_slam2d.cpp:166-186): a borrowed 0.1 m DynamicDistanceMap with a 5 m reach;
+        .processed holds its update() return value"""
+        h = C.c_void_p()
+        n = C.c_uint32(0)
+        _chk(lib().lama_graph_generate_coarse_distance_map(self.h, C.byref(h), C.byref(n)))
+        dm = DynamicDistanceMap(handle=h, owner=self)
+        dm.processed = n.value
+        return dm
+
+
+class FrequencyOccupancyMap:
+    """Device-resident lama::FrequencyOccupancyMap (include/lama/sdm/frequency_occupancy_map.h), stand-alone or borrowed from a
+    GraphSlam2D (handle= / owner=, as DynamicDistanceMap)."""
+
+    def __init__(self, resolution=0.05, patch_size=32, center=(0.0, 0.0), handle=None, owner=None, **dev):
+        self.owner = owner
+        if handle is not None:
+            self.h = handle
+            self.owned = False
+            return
+        d = DeviceOptions(device=0, dir_dim=64, pool_slots=0, max_beams=2048, timing=0, stream=0)
+        for k, v in dev.items():
+            setattr(d, k, v)
+        c, cp = _d(center)
+        self.h = C.c_void_p()
+        self.owned = True
+        _chk(lib().lama_om_create(C.c_double(resolution), C.c_uint32(patch_size), cp, C.byref(d), C.byref(self.h)))
+
+    def __del__(self):
+        if getattr(self, "owned", False) and getattr(self, "h", None) and _lib is not None:
+            _lib.lama_om_destroy(self.h)
+            self.h = None
+
+    @property
+    def resolution(self) -> float:
+        r = C.c_double(0)
+        _chk(lib().lama_om_resolution(self.h, C.byref(r)))
+        return r.value
+
+    def insertScans(self, scans, states, full=True, origins=None, quats=None) -> int:
+        """the loop of generateOccupancyMap (graph_slam2d.cpp:135-160) for posed scans: `scans` a list of (n_k, 3) clouds, `states`
+        (S, 4) SE2 {cos, sin, x, y}, origins (S, 3) / quats (S, 4) xyzw or None (identity).  Returns the number of cell updates."""
+        scans = [np.ascontiguousarray(s, np.float64).reshape(-1, 3) for s in scans]
+        offsets = np.zeros(len(scans) + 1, np.int64)
+        offsets[1:] = np.cumsum([len(s) for s in scans])
+        p, pp = _d(np.concatenate(scans) if scans else np.zeros((0, 3)))
+        s, sp = _d(np.asarray(states, np.float64).reshape(-1, 4))
+        o, op = (None, None) if origins is None else _d(np.asarray(origins, np.float64).reshape(-1, 3))
+        q, qp = (None, None) if quats is None else _d(np.asarray(quats, np.float64).reshape(-1, 4))
+        cells = C.c_uint64(0)
+        _chk(lib().lama_om_insert_scans(self.h, pp, offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int(len(scans)), op, qp, sp,
+                                        C.c_int(1 if full else 0), C.byref(cells)))
+        return cells.value
+
+    def prune(self):
+        """FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158)"""
+        _chk(lib().lama_om_prune(self.h))
+
+    def bounds(self):
+        return _bounds(lib().lama_om_bounds, (self.h,))
+
+    def export(self, x0, y0, w, h):
+        o = _occ_arrays(w, h)
+        _chk(lib().lama_om_export(self.h, C.c_uint32(x0), C.c_uint32(y0), C.c_int(w), C.c_int(h), _vp(o["occupied"]), _vp(o["visited"]), _vp(o["known"])))
+        return o
+
+    def query(self, cells):
+        """(getProbability, flags bit 0 isFree / bit 1 isOccupied / bit 2 isUnknown) of cells (n, 2)"""
+        c, cp = _u32(cells)
+        n = c.size // 2
+        prob, flags = np.zeros(n), np.zeros(n, np.uint8)
+        _chk(lib().lama_om_query(self.h, cp, C.c_int(n), prob.ctypes.data_as(c_dp), _vp(flags)))
+        return prob, flags
+
+    def write(self, path):
+        """Map::write (map.cpp:490-529): a reference .sdm file"""
+        _chk(lib().lama_om_write(self.h, str(path).encode()))
+
+    def exportImage(self):
+        return _image(lib().lama_om_export_image, (self.h,))
+
+    def saveImage(self, path):
+        write_png(path, self.exportImage())
+
+    def kernelTimes(self):
+        return _times(lib().lama_om_kernel_times, self.h)
 
 
 class DynamicDistanceMap:

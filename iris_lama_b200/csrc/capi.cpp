@@ -85,6 +85,10 @@ int export_occ(Engine* e, int particle, uint32_t x0, uint32_t y0, int w, int h, 
         if (visited) visited[i] = (uint16_t)occ_visited(wd);
         if (known) known[i] = wd != 0;  // every mutable access counts a visit
     }
+    if (known && e->config().known_plane) {   // a pruned cell is {0, 0} and still known: read the known plane
+        rc = e->export_bits(particle, 1, x0, y0, w, h, known);
+        if (rc != LAMA_OK) return set_err(e->last_error(), rc);
+    }
     return LAMA_OK;
 }
 int export_dm(Engine* e, int particle, bool with_occ, uint32_t x0, uint32_t y0, int w, int h, uint16_t* sqdist, uint8_t* valid, uint8_t* known,
@@ -204,7 +208,7 @@ int occupancy_query(Engine* e, int particle, const uint32_t* cells, int n, doubl
             prob[i]  = known ? prob_of(l) : prob_of((float)thr);
             flags[i] = (uint8_t)((known && (double)l < thr ? 1 : 0) | (known && (double)l > thr ? 2 : 0) | (!known || (double)l == thr ? 4 : 0));
         } else {
-            const bool known = words[i] != 0;   // every mutable access counts a visit
+            const bool known = e->config().known_plane ? (fl[i] & 2) != 0 : words[i] != 0;   // every mutable access counts a visit
             const uint32_t occ = occ_occupied(words[i]), vis = occ_visited(words[i]);
             const double p = vis == 0 ? 0.25 : ((double)occ) / ((double)vis);   // frequency_occupancy_map.cpp:40-45
             prob[i]  = known ? p : 0.25;
@@ -266,8 +270,11 @@ int export_image(Engine* e, int particle, int kind, bool slam_frontend, uint8_t*
 struct lama_pf { PFSlam2D* p; };
 struct lama_slam { Slam2D* s; bool owned = true; };   // borrowed (owned = false): the inner Slam2D of a lama_graph
 struct lama_dm { DistanceMapDev* d; bool owned; };
+struct lama_om { OccupancyMapDev* m; bool owned; };
 struct lama_loc { Loc2D* l; lama_dm dm; };
-struct lama_graph { GraphSlam2D* g; lama_slam slam; };
+// om / coarse: the borrowed handles of the generated maps; the graph recreates a map in place, so a handle it returned earlier
+// follows the newest map
+struct lama_graph { GraphSlam2D* g; lama_slam slam; lama_om om{nullptr, false}; lama_dm coarse{nullptr, false}; };
 
 extern "C" {
 
@@ -1253,7 +1260,7 @@ try {
     std::string err;
     GraphSlam2D* gs = GraphSlam2D::create(g, err);
     if (!gs) return set_err(err, lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_ARG);
-    *out = new lama_graph{gs, lama_slam{gs->slam(), false}};
+    *out = new lama_graph{gs, lama_slam{gs->slam(), false}, lama_om{nullptr, false}, lama_dm{nullptr, false}};
     return LAMA_OK;
 }
 LAMA_CATCH
@@ -1353,6 +1360,129 @@ try {
     if (!h || !slam) return set_err("null argument", LAMA_ERR_ARG);
     *slam = &h->slam;
     return LAMA_OK;
+}
+LAMA_CATCH
+// GraphSlam2D::generateOccupancyMap (graph_slam2d.cpp:131-164)
+int lama_graph_generate_occupancy_map(lama_graph* h, int full, lama_om** om)
+try {
+    if (!h || !om) return set_err("null argument", LAMA_ERR_ARG);
+    OccupancyMapDev* m = nullptr;
+    int rc = h->g->generate_occupancy_map(full != 0, &m);
+    h->om.m = h->g->occupancy_map();   // null until the first successful call
+    if (rc != LAMA_OK) return set_err(h->g->error(), rc);
+    *om = &h->om;
+    return LAMA_OK;
+}
+LAMA_CATCH
+// GraphSlam2D::generateCoarseDistanceMap (graph_slam2d.cpp:166-186)
+int lama_graph_generate_coarse_distance_map(lama_graph* h, lama_dm** dm, uint32_t* processed)
+try {
+    if (!h || !dm) return set_err("null argument", LAMA_ERR_ARG);
+    DistanceMapDev* d = nullptr;
+    int rc = h->g->generate_coarse_distance_map(&d, processed);
+    h->coarse.d = h->g->coarse_distance_map();
+    if (rc != LAMA_OK) return set_err(h->g->error(), rc);
+    *dm = &h->coarse;
+    return LAMA_OK;
+}
+LAMA_CATCH
+
+// ---- FrequencyOccupancyMap (include/lama/sdm/frequency_occupancy_map.h) -------------------------------------------------------------
+namespace {
+Engine* om_engine(lama_om* om) { return om && om->m ? om->m->engine() : nullptr; }
+}
+// FrequencyOccupancyMap(resolution, patch_size) (frequency_occupancy_map.cpp:47-49) on the device, window centred on center_xy
+int lama_om_create(double resolution, uint32_t patch_size, const double center_xy[2], const lama_device_options* dev, lama_om** out)
+try {
+    if (!out) return set_err("null argument", LAMA_ERR_ARG);
+    if (!(resolution > 0)) return set_err("resolution must be positive", LAMA_ERR_ARG);
+    lama_device_options d;
+    if (dev) d = *dev; else dev_default(&d);
+    std::string err;
+    OccupancyMapDev* m = OccupancyMapDev::create(resolution, patch_size, center_xy ? center_xy[0] : 0.0, center_xy ? center_xy[1] : 0.0, dev_from(d), err);
+    if (!m) return set_err(err, lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_ARG);
+    *out = new lama_om{m, true};
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_om_destroy(lama_om* om)
+try {
+    if (!om || !om->owned) return LAMA_OK;   // a borrowed handle belongs to its lama_graph
+    delete om->m;
+    delete om;
+    return LAMA_OK;
+}
+LAMA_CATCH
+// the loop of graph_slam2d.cpp:135-160 for any posed scans: setOccupied(tf * p) and, with full, setFree along computeRay(so, hit)
+int lama_om_insert_scans(lama_om* om, const double* pts_xyz, const int64_t* offsets, int n_scans, const double* origins, const double* quats_xyzw,
+                         const double* states, int full, uint64_t* cells)
+try {
+    if (!om || (n_scans > 0 && (!offsets || !states))) return set_err("null argument", LAMA_ERR_ARG);
+    if (!om->m) return set_err("no map yet (generateOccupancyMap has not been called)", LAMA_ERR_STATE);
+    if (n_scans < 0) return set_err("negative number of scans", LAMA_ERR_ARG);
+    std::vector<SE2> st((size_t)n_scans);
+    for (int k = 0; k < n_scans; ++k) st[k] = SE2{states[4 * k], states[4 * k + 1], states[4 * k + 2], states[4 * k + 3]};
+    int rc = om->m->insert_scans(pts_xyz, offsets, n_scans, origins, quats_xyzw, st.data(), full != 0, cells);
+    return rc == LAMA_OK ? rc : set_err(om->m->error(), rc);
+}
+LAMA_CATCH
+// FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158)
+int lama_om_prune(lama_om* om)
+try {
+    if (!om) return set_err("null handle", LAMA_ERR_ARG);
+    if (!om->m) return set_err("no map yet (generateOccupancyMap has not been called)", LAMA_ERR_STATE);
+    int rc = om->m->prune();
+    return rc == LAMA_OK ? rc : set_err(om->m->error(), rc);
+}
+LAMA_CATCH
+int lama_om_resolution(lama_om* om, double* resolution)
+try {
+    if (!om || !resolution) return set_err("null argument", LAMA_ERR_ARG);
+    Engine* e = om_engine(om);
+    if (!e) return set_err("no map yet (generateOccupancyMap has not been called)", LAMA_ERR_STATE);
+    *resolution = e->config().resolution;
+    return LAMA_OK;
+}
+LAMA_CATCH
+// Map::bounds (map.cpp:139-157) in cells, patch granular
+int lama_om_bounds(lama_om* om, uint32_t mn[2], uint32_t mx[2], int* patches)
+try {
+    if (!om || !mn || !mx) return set_err("null argument", LAMA_ERR_ARG);
+    return bounds_out(om_engine(om), 0, 0, mn, mx, patches);
+}
+LAMA_CATCH
+// getProbability / isFree / isOccupied / isUnknown (frequency_occupancy_map.cpp:110-172), flags as lama_pf_occupancy_query
+int lama_om_query(lama_om* om, const uint32_t* cells_xy, int n, double* prob, uint8_t* flags)
+try {
+    if (!om) return set_err("null handle", LAMA_ERR_ARG);
+    return occupancy_query(om_engine(om), 0, cells_xy, n, prob, flags);
+}
+LAMA_CATCH
+int lama_om_export(lama_om* om, uint32_t x0, uint32_t y0, int w, int hgt, uint16_t* occupied, uint16_t* visited, uint8_t* known)
+try {
+    if (!om) return set_err("null handle", LAMA_ERR_ARG);
+    if (w < 1 || hgt < 1) return set_err("empty window", LAMA_ERR_ARG);
+    return export_occ(om_engine(om), 0, x0, y0, w, hgt, occupied, visited, known);
+}
+LAMA_CATCH
+// Map::write (map.cpp:490-529)
+int lama_om_write(lama_om* om, const char* path)
+try {
+    if (!om || !path) return set_err("null argument", LAMA_ERR_ARG);
+    return write_map(om_engine(om), 0, 0, false, path);
+}
+LAMA_CATCH
+// the grey image of sdm::export_to_png (export.cpp:46-96); pixels == NULL: only the dimensions
+int lama_om_export_image(lama_om* om, uint8_t* pixels, size_t cap, int dims[2])
+try {
+    if (!om || !dims) return set_err("null argument", LAMA_ERR_ARG);
+    return export_image(om_engine(om), 0, 0, false, pixels, cap, dims);
+}
+LAMA_CATCH
+int lama_om_kernel_times(lama_om* om, double ms[4], uint64_t launches[5])
+try {
+    if (!om) return set_err("null handle", LAMA_ERR_ARG);
+    return times_out(om_engine(om), ms, launches);
 }
 LAMA_CATCH
 

@@ -24,6 +24,9 @@ struct EngineConfig {
     double center_y   = 0.0;
     uint64_t stream   = 0;      // external cudaStream_t (0 = own non-blocking stream)
     int occupancy_kind = 0;     // 0 = FrequencyOccupancyMap (PFSlam2D, Slam2D), 1 = ProbabilisticOccupancyMap (log-odds)
+    int event_cap      = 0;     // obstacle events one brushfire takes (0 = auto: max_beams rounded up to a power of two, at least 2 048)
+    bool known_plane   = false; // a frequency map that keeps the Container 'known' bits in their own plane (render_scans / prune_frequency):
+                                // after a prune, `known` can no longer be derived from a non-zero cell
 };
 
 struct HostMatchResult {
@@ -114,6 +117,15 @@ public:
     int pack_size(int particle, size_t* bytes);
     int pack(int particle, void* buf, size_t cap, size_t* used);
     int unpack(int particle, const void* buf, size_t bytes);
+
+    // Posed scans cast into particle 0's frequency map (GraphSlam2D::generateOccupancyMap's loop, graph_slam2d.cpp:136-160; needs
+    // known_plane): scan k = points [offsets[k], offsets[k + 1]) of pts (xyz), sensor origin / quaternion xyzw origins + 3k / quats + 4k
+    // (null: identity), base pose states[k].  Every hit cell gets setOccupied and, with `full`, every interior ray cell setFree;
+    // *cells = number of cell updates.
+    int render_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states, bool full,
+                     uint64_t* cells);
+    // FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158) of particle 0's map
+    int prune_frequency();
 
     // Direct DynamicDistanceMap::addObstacle / removeObstacle calls in list order, then update().
     int dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_add, int n, uint32_t* processed);

@@ -11,6 +11,7 @@
 #include <cmath>
 #include <cstring>
 #include <limits>
+#include <unordered_set>
 
 namespace lama_b200 {
 
@@ -980,7 +981,108 @@ int GraphSlam2D::optimize_pose_graph()
         correction_ = se2_inv(se2_mul(slam_->pose(), se2_inv(keys_.back().pose)));
     }
     stats_.last = std::move(rep);
-    accdist_ = 0.0;   // :428-429
+    mapping_keyid_ = 0;   // :428-429
+    accdist_ = 0.0;
+    return LAMA_OK;
+}
+
+// the inner Slam2D's window centre (its engine is created at the first update, centred on the pose of that moment)
+static void slam_window_center(Slam2D* s, double c[2])
+{
+    if (s->engine()) {
+        c[0] = s->engine()->config().center_x;
+        c[1] = s->engine()->config().center_y;
+    } else {
+        c[0] = s->pose().tx;
+        c[1] = s->pose().ty;
+    }
+}
+
+int GraphSlam2D::generate_occupancy_map(bool full, OccupancyMapDev** out)
+{
+    if (mapping_keyid_ == 0 || !occ_) {   // :132-133
+        double c[2];
+        slam_window_center(slam_.get(), c);
+        OccupancyMapDev* m = OccupancyMapDev::create(full ? opt_.slam.resolution : 0.1, 32, c[0], c[1], slam_->device_options(), err_);
+        if (!m) return LAMA_ERR_CUDA;
+        occ_.reset(m);   // borrowed handles never see a null map
+        mapping_keyid_ = 0;
+    }
+    const size_t n_scans = keys_.size() - mapping_keyid_;
+    std::vector<double> pts, origins, quats;
+    std::vector<int64_t> offsets(1, 0);
+    std::vector<SE2> states;
+    for (size_t i = mapping_keyid_; i < keys_.size(); ++i) {   // :135-160, the key's CURRENT (corrected) pose
+        const KeyPose& k = keys_[i];
+        pts.insert(pts.end(), k.pts.begin(), k.pts.end());
+        offsets.push_back(offsets.back() + (int64_t)(k.pts.size() / 3));
+        origins.insert(origins.end(), k.origin, k.origin + 3);
+        quats.insert(quats.end(), k.quat, k.quat + 4);
+        states.push_back(k.pose);
+    }
+    int rc = occ_->insert_scans(pts.data(), offsets.data(), (int)n_scans, origins.data(), quats.data(), states.data(), full, nullptr);
+    if (rc == LAMA_OK) rc = occ_->prune();   // :162
+    if (rc != LAMA_OK) { err_ = occ_->error(); return rc; }
+    mapping_keyid_ = keys_.size();           // :163
+    *out = occ_.get();
+    return LAMA_OK;
+}
+
+int GraphSlam2D::generate_coarse_distance_map(DistanceMapDev** out, uint32_t* processed)
+{
+    Engine* e = slam_->engine();
+    if (!e) { err_ = "no map yet (update() has not been called)"; return LAMA_ERR_STATE; }
+    double c[2];
+    slam_window_center(slam_.get(), c);
+    // visit_all_cells of the inner distance map (:171): its known cells are those of its own patches and, for a frequency map, every
+    // touched occupancy cell (see unpack_distance_words); both maps are read over the union of their patches
+    uint32_t a0[2], a1[2], b0[2], b1[2];
+    const int nd = e->bounds(0, 1, a0, a1), no = e->bounds(0, 0, b0, b1);
+    if (nd < 0 || no < 0) { err_ = e->last_error(); return LAMA_ERR_ARG; }
+    std::vector<uint32_t> cells;
+    std::unordered_set<uint64_t> seen;
+    if (nd + no > 0) {
+        uint32_t mn[2], mx[2];
+        for (int k = 0; k < 2; ++k) {
+            mn[k] = nd && no ? std::min(a0[k], b0[k]) : (nd ? a0[k] : b0[k]);
+            mx[k] = nd && no ? std::max(a1[k], b1[k]) : (nd ? a1[k] : b1[k]);
+        }
+        const int w = (int)(mx[0] - mn[0]), h = (int)(mx[1] - mn[1]);
+        std::vector<uint32_t> dw((size_t)w * h), ow((size_t)w * h);
+        int rc = e->export_window(0, 1, mn[0], mn[1], w, h, dw.data(), nullptr);
+        if (rc == LAMA_OK) rc = e->export_window(0, 0, mn[0], mn[1], w, h, ow.data(), nullptr);
+        if (rc != LAMA_OK) { err_ = e->last_error(); return rc; }
+        const double fine = 1.0 / opt_.slam.resolution, coarse = 1.0 / 0.1;
+        // ascending directory index = patch rows bottom up, patches left to right; then cells in container order (x fastest)
+        for (int py = 0; py < h; py += kPatchLen)
+            for (int px = 0; px < w; px += kPatchLen)
+                for (int y = py; y < py + kPatchLen; ++y)
+                    for (int x = px; x < px + kPatchLen; ++x) {
+                        const size_t i = (size_t)y * w + x;
+                        const bool known = (dw[i] & kDmKnown) || ow[i] != 0;
+                        if (!known || !occ_is_occupied(occ_occupied(ow[i]), occ_visited(ow[i]))) continue;   // isOccupied (:173-174)
+                        uint32_t m[2];
+                        for (int k = 0; k < 2; ++k) {
+                            const double wpos = ((double)((k ? mn[1] + (uint32_t)y : mn[0] + (uint32_t)x)) - (double)kMapOffsetCells) / fine;   // m2w (map.h:147-148)
+                            m[k] = w2m(wpos, coarse);                                                                                      // w2m (:176)
+                        }
+                        // a repeated addObstacle of a cell is a no-op (dynamic_distance_map.cpp:217-218): only the first call is kept, so the
+                        // list stays within one brushfire batch
+                        if (!seen.insert((uint64_t)m[0] << 32 | m[1]).second) continue;
+                        cells.push_back(m[0]);
+                        cells.push_back(m[1]);
+                    }
+    }
+    // :168-169; the whole list goes through one brushfire, as the reference's single update() (lists beyond 8 192 cells are applied in
+    // batches, DESIGN.md 10)
+    const int n = (int)(cells.size() / 2);
+    DistanceMapDev* dm = DistanceMapDev::create(0.1, 32, 5.0, c[0], c[1], slam_->device_options(), err_, std::min(n, 8192));
+    if (!dm) return LAMA_ERR_CUDA;
+    coarse_dm_.reset(dm);   // borrowed handles never see a null map
+    int rc = dm->add(cells.data(), n, true);
+    if (rc == LAMA_OK) rc = dm->update(processed);   // :183
+    if (rc != LAMA_OK) { err_ = dm->error(); return rc; }
+    *out = dm;
     return LAMA_OK;
 }
 
@@ -1115,11 +1217,13 @@ int Slam2D::update(const double* pts, int n, const double* origin, const double*
 // DistanceMapDev + Loc2D
 // =====================================================================================================
 DistanceMapDev* DistanceMapDev::create(double resolution, uint32_t patch_size, double l2_max, double cx, double cy, const DeviceOptions& dev,
-                                       std::string& err)
+                                       std::string& err, int event_cap)
 {
     if (patch_size != 32) { err = "DynamicDistanceMap: only patch_size 32 is supported on the device"; return nullptr; }
     if (cuda_device_count() < 1) { err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
-    Engine* en = Engine::create(engine_config(dev, 1, resolution, l2_max, cx, cy), err);
+    EngineConfig cfg = engine_config(dev, 1, resolution, l2_max, cx, cy);
+    cfg.event_cap = event_cap;
+    Engine* en = Engine::create(cfg, err);
     if (!en) return nullptr;
     DistanceMapDev* d = new DistanceMapDev();
     d->eng_.reset(en);
@@ -1156,6 +1260,36 @@ int DistanceMapDev::flush_if_pending()
     // Reads of a map with queued-but-unpropagated obstacle changes see the marked cells in the
     // reference; here the marks are applied lazily, so bring the device up to date first.
     return update(nullptr);
+}
+
+OccupancyMapDev* OccupancyMapDev::create(double resolution, uint32_t patch_size, double cx, double cy, const DeviceOptions& dev, std::string& err)
+{
+    if (patch_size != 32) { err = "FrequencyOccupancyMap: only patch_size 32 is supported on the device"; return nullptr; }
+    if (cuda_device_count() < 1) { err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
+    EngineConfig cfg = engine_config(dev, 1, resolution, resolution, cx, cy);   // no distance map is kept: the smallest reach
+    if (cfg.pool_slots <= 0) cfg.pool_slots = cfg.dir_dim * cfg.dir_dim;
+    cfg.known_plane = true;
+    Engine* en = Engine::create(cfg, err);
+    if (!en) return nullptr;
+    OccupancyMapDev* m = new OccupancyMapDev();
+    m->eng_.reset(en);
+    en->enable_timing(dev.timing != 0);
+    return m;
+}
+
+int OccupancyMapDev::insert_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states,
+                                  bool full, uint64_t* cells)
+{
+    int rc = eng_->render_scans(pts, offsets, n_scans, origins, quats, states, full, cells);
+    if (rc != LAMA_OK) err_ = eng_->last_error();
+    return rc;
+}
+
+int OccupancyMapDev::prune()
+{
+    int rc = eng_->prune_frequency();
+    if (rc != LAMA_OK) err_ = eng_->last_error();
+    return rc;
 }
 
 // ---- SimpleOccupancyHost ---------------------------------------------------------------------------------------

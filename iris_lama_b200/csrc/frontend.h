@@ -199,8 +199,9 @@ private:
 // ---- device DynamicDistanceMap + Loc2D -------------------------------------------------------------------
 class DistanceMapDev {
 public:
+    // event_cap: addObstacle / removeObstacle calls one update() applies in a single brushfire (0 = the engine's default)
     static DistanceMapDev* create(double resolution, uint32_t patch_size, double l2_max, double cx, double cy, const DeviceOptions& dev,
-                                  std::string& err);
+                                  std::string& err, int event_cap = 0);
     int add(const uint32_t* cells_xy, int n, bool is_add);
     int update(uint32_t* processed);
     Engine* engine() { return eng_.get(); }
@@ -211,6 +212,23 @@ private:
     std::unique_ptr<Engine> eng_;
     std::vector<uint32_t> pend_cells_;
     std::vector<uint8_t> pend_kind_;
+    std::string err_;
+};
+
+// ---- device FrequencyOccupancyMap that keeps its own known plane: GraphSlam2D's global map ---------------------------------------------
+class OccupancyMapDev {
+public:
+    // one-particle engine; dev.pool_slots 0 = dir_dim^2 slots, so a full window cannot run out of patches
+    static OccupancyMapDev* create(double resolution, uint32_t patch_size, double cx, double cy, const DeviceOptions& dev, std::string& err);
+    // GraphSlam2D::generateOccupancyMap's loop body (graph_slam2d.cpp:136-160) for any posed scans (Engine::render_scans)
+    int insert_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states, bool full,
+                     uint64_t* cells);
+    int prune();   // FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158)
+    Engine* engine() { return eng_.get(); }
+    const std::string& error() const { return err_; }
+
+private:
+    std::unique_ptr<Engine> eng_;
     std::string err_;
 };
 
@@ -266,10 +284,21 @@ public:
     const std::vector<int>& last_candidates() const { return last_candidates_; }   // of the latest loop search (empty when there was none)
     const Stats& stats() const { return stats_; }
     const std::string& error() const { return err_; }
+    // generateOccupancyMap (:131-164): a new map at (full ? resolution : 0.1) when mapping_keyid is 0, the key scans from mapping_keyid on
+    // cast at their corrected poses, prune, mapping_keyid = number of keys.  The map is owned here and replaced on the next recreation.
+    int generate_occupancy_map(bool full, OccupancyMapDev** out);
+    // generateCoarseDistanceMap (:166-186): a new 0.1 m distance map (reach 5 m) with an obstacle at every occupied cell of the inner
+    // Slam2D, visited in ascending directory index, then cell index; *processed = its update() return value
+    int generate_coarse_distance_map(DistanceMapDev** out, uint32_t* processed);
+    OccupancyMapDev* occupancy_map() { return occ_.get(); }
+    DistanceMapDev* coarse_distance_map() { return coarse_dm_.get(); }
 
 private:
     GraphOptions opt_;
     std::unique_ptr<Slam2D> slam_;
+    size_t mapping_keyid_ = 0;                      // graph_slam2d.h: the first key not yet cast into occ_
+    std::unique_ptr<OccupancyMapDev> occ_;
+    std::unique_ptr<DistanceMapDev> coarse_dm_;
     std::vector<KeyPose> keys_;
     std::vector<std::pair<int, int>> links_;
     std::vector<PgoPrior> priors_;            // the persistent graph (graph_slam2d.cpp:110): the prior on key 0,

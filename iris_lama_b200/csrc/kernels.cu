@@ -1762,6 +1762,134 @@ __global__ void k_distance(StoreView s, int set, int particle, const double* __r
     }
 }
 
+// ==================================================================================================
+// k_render_scans: posed scans cast into ONE frequency map (GraphSlam2D::generateOccupancyMap, graph_slam2d.cpp:131-164)
+// ==================================================================================================
+// One CTA per scan, lane = beam: the lanes of a warp walk angularly adjacent beams in lock step, so the reductions of one
+// step fall into neighbouring cells.  Every update of a render is a counter increment, so there is no ordered path: no log,
+// no replay, no candidate bitmaps.  kMark: the first pass only marks the directory entries of the touched cells (one byte
+// each, written when the walk enters another patch), so that exactly the reference's patch set gets allocated before the
+// counting pass; the counting pass walks the same cells and adds fire-and-forget reductions.
+constexpr int kRenderThreads = 256;
+
+template <bool kMark>
+__global__ void __launch_bounds__(kRenderThreads) k_render_scans(StoreView s, int set, RenderParams p)
+{
+    __shared__ Affine tf;
+    if (threadIdx.x == 0) tf = compose_tf(p.states[blockIdx.x], p.moving[blockIdx.x]);   // the transform of Slam2D's map update
+    __syncthreads();
+    const int32_t* dir = dir_of(s, set, 0, kMapOcc);
+    const DirWindow win = s.window;
+    const uint32_t bx0 = (uint32_t)win.base_px << kPatchLog2, by0 = (uint32_t)win.base_py << kPatchLog2;
+    const uint32_t side = (uint32_t)win.dim << kPatchLog2;
+    int log2dim = 0;
+    while ((1 << (log2dim + 1)) <= win.dim) ++log2dim;
+    ScanParams sp{};   // no truncation, no lidar-odometry rays: hit = tf * p, ray start = tf.translation()
+    sp.scale = p.scale;
+    uint32_t err = 0;
+    unsigned long long cells = 0;
+    int last_di = -1;
+    uint32_t* base = nullptr;   // patch of last_di (counting pass); null: not allocated (the pool ran dry, reported)
+    auto touch = [&](uint32_t P, uint32_t inc) {
+        const int di = (int)packed_dir_index(P, log2dim);
+        if (di != last_di) {
+            last_di = di;
+            if (kMark) {
+                if (!p.marks[di]) p.marks[di] = 1;
+            } else {
+                const int e = __ldg(dir + di);
+                base = e < 0 ? nullptr : patch_ptr(s, e & kDirSlotMask);
+            }
+        }
+        if (kMark || !base) return;
+        uint32_t* cell = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(base) + packed_cell_offset(P));
+        asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(cell), "r"(inc) : "memory");
+        ++cells;
+    };
+    const int64_t b0 = p.offsets[blockIdx.x], b1 = p.offsets[blockIdx.x + 1];
+    for (int64_t b = b0 + threadIdx.x; b < b1; b += blockDim.x) {
+        const double pt[3] = {__ldg(p.points + 3 * b), __ldg(p.points + 3 * b + 1), __ldg(p.points + 3 * b + 2)};
+        const BeamCells bc = beam_cells(tf, sp, pt);
+        const uint32_t fx = bc.from[0] - bx0, fy = bc.from[1] - by0, tx = bc.to[0] - bx0, ty = bc.to[1] - by0;
+        if ((fx | fy | tx | ty) >= side) {   // the beam leaves the directory window: reported, nothing is written
+            err |= kErrWindow;
+            continue;
+        }
+        touch(tx | (ty << 16), kOccHitInc);   // setOccupied(tf * p)
+        if (!p.full) continue;
+        if (bc.from[2] == bc.to[2]) {          // planar beam: the 2-axis form of computeRay (every 2-D scan)
+            SegWalk w;
+            w.init(fx, fy, tx, ty, 0, 1 << 30);
+            while (w.next()) touch(w.P, kOccMissInc);
+        } else {                               // tilted sensor: the 3-axis walk
+            RayWalk3 w(bc);
+            while (w.next()) touch((w.x - bx0) | ((w.y - by0) << 16), kOccMissInc);
+        }
+    }
+    err = __reduce_or_sync(0xffffffffu, err);
+    if ((threadIdx.x & 31) == 0 && err) atomicOr(s.status, err);
+    if (!kMark) {
+        for (int o = 16; o > 0; o >>= 1) cells += __shfl_xor_sync(0xffffffffu, cells, o);
+        if ((threadIdx.x & 31) == 0 && cells) atomicAdd(p.cells, cells);
+    }
+}
+
+// one warp per directory entry: a zeroed patch for every marked entry that has none (Map::get mutable, map.cpp:400-408)
+__global__ void k_render_alloc(StoreView s, int set, const uint8_t* __restrict__ marks)
+{
+    const int lane = threadIdx.x & 31;
+    const int di   = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (di >= s.window.dim * s.window.dim || !marks[di]) return;
+    int32_t* dir = dir_of(s, set, 0, kMapOcc);
+    if (dir[di] >= 0) return;
+    int ns = 0;
+    if (lane == 0) {
+        ns = alloc_slot(s);
+        if (ns >= 0) atomicAdd((unsigned long long*)&s.counters[0], 1ull);
+    }
+    ns = __shfl_sync(0xffffffffu, ns, 0);
+    if (ns < 0) return;
+    warp_zero_patch(patch_ptr(s, ns), lane);
+    fbits_ptr(s, ns)[lane] = 0u;
+    kbits_ptr(s, ns)[lane] = 0u;
+    if (lane == 0) dir[di] = ns | kDirOwn;
+}
+
+// one warp per directory entry touched by the render: known |= (word != 0) (every touch went through Map::get, which sets the
+// Container bit; counters only grow within a render), then the mark is cleared for the next render
+__global__ void k_render_known(StoreView s, int set, uint8_t* __restrict__ marks)
+{
+    const int lane = threadIdx.x & 31;
+    const int di   = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (di >= s.window.dim * s.window.dim || !marks[di]) return;
+    const int e = dir_of(s, set, 0, kMapOcc)[di];
+    if (e >= 0) {
+        const uint32_t* cells = patch_ptr(s, e & kDirSlotMask);
+        uint32_t* kb = kbits_ptr(s, e & kDirSlotMask);
+        for (int row = 0; row < kPatchLen; ++row) {
+            const uint32_t known = __ballot_sync(0xffffffffu, __ldcg(cells + row * kPatchLen + lane) != 0u);
+            if (lane == 0 && known) kb[row] |= known;
+        }
+    }
+    if (lane == 0) marks[di] = 0;
+}
+
+// FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158) over every patch: cells visited once and occupied at most
+// once go back to {0, 0}; their known bit stays
+__global__ void k_prune_freq(StoreView s, int set)
+{
+    const int lane = threadIdx.x & 31;
+    const int di   = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (di >= s.window.dim * s.window.dim) return;
+    const int e = dir_of(s, set, 0, kMapOcc)[di];
+    if (e < 0) return;
+    uint32_t* cells = patch_ptr(s, e & kDirSlotMask);
+    for (int row = 0; row < kPatchLen; ++row) {
+        const uint32_t w = cells[row * kPatchLen + lane];
+        if (occ_visited(w) == 1u && occ_occupied(w) <= 1u) cells[row * kPatchLen + lane] = 0u;
+    }
+}
+
 }  // namespace
 
 // ==================================================================================================
@@ -1786,21 +1914,33 @@ size_t brushfire_smem_bytes(int dir_dim, const BrushParams& bp)
     return (size_t)dim2 * 4 + (size_t)(bp.lower_cap + bp.raise_cap + 4 + bp.event_cap) * 8 + 32 * 4 + 16 + 16;
 }
 
+// The dynamic shared-memory limit of a kernel is process-wide state, while engines of different configurations live side by side (a
+// GraphSlam2D's inner Slam2D next to its global maps, a Loc2D next to a PFSlam2D): an engine only ever raises it.
+template <typename Kernel>
+static cudaError_t raise_smem_limit(Kernel* k, size_t bytes)
+{
+    cudaFuncAttributes a;
+    cudaError_t e = cudaFuncGetAttributes(&a, k);
+    if (e != cudaSuccess) return e;
+    if ((size_t)a.maxDynamicSharedSizeBytes >= bytes) return cudaSuccess;
+    return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+}
+
 cudaError_t configure_kernels(int dir_dim, uint32_t max_sqdist_limit, const RayParams& rp, const BrushParams& bp)
 {
     cudaError_t e;
-    e = cudaFuncSetAttribute(k_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)match_smem_bytes(dir_dim, max_sqdist_limit));
+    e = raise_smem_limit(k_match, match_smem_bytes(dir_dim, max_sqdist_limit));
     if (e != cudaSuccess) return e;
-    if (rp.prob_mode) e = cudaFuncSetAttribute(k_raycast<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)raycast_smem_bytes(dir_dim, rp));
-    else e = cudaFuncSetAttribute(k_raycast<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)raycast_smem_bytes(dir_dim, rp));
+    if (rp.prob_mode) e = raise_smem_limit(k_raycast<true>, raycast_smem_bytes(dir_dim, rp));
+    else e = raise_smem_limit(k_raycast<false>, raycast_smem_bytes(dir_dim, rp));
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_brushfire, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)brushfire_smem_bytes(dir_dim, bp));
+    e = raise_smem_limit(k_brushfire, brushfire_smem_bytes(dir_dim, bp));
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_ray_setup, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ray_setup_smem_bytes(dir_dim, rp.scan.n_beams > 4096 ? 4096 : rp.scan.n_beams));
+    e = raise_smem_limit(k_ray_setup, ray_setup_smem_bytes(dir_dim, rp.scan.n_beams > 4096 ? 4096 : rp.scan.n_beams));
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_ray_pull<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ray_pull_smem_bytes(rp.scan.n_beams > 4096 ? 4096 : rp.scan.n_beams));
+    e = raise_smem_limit(k_ray_pull<false>, ray_pull_smem_bytes(rp.scan.n_beams > 4096 ? 4096 : rp.scan.n_beams));
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_ray_pull<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ray_pull_smem_bytes(rp.scan.n_beams > 4096 ? 4096 : rp.scan.n_beams));
+    e = raise_smem_limit(k_ray_pull<true>, ray_pull_smem_bytes(rp.scan.n_beams > 4096 ? 4096 : rp.scan.n_beams));
     return e;
 }
 
@@ -1920,6 +2060,20 @@ void launch_distance(const StoreView& s, int set, int particle, const double* d_
     int blocks = (n + 255) / 256;
     if (blocks > 1184) blocks = 1184;
     k_distance<<<blocks, 256, 0, st>>>(s, set, particle, d_pts, n, resolution, max_sqdist, d_dist, d_grad);
+}
+void launch_render_scans(const StoreView& s, int set, const RenderParams& p, int n_scans, cudaStream_t st)
+{
+    if (n_scans <= 0) return;
+    const int dim2 = s.window.dim * s.window.dim, blocks = (dim2 + 7) / 8;   // one warp per directory entry
+    k_render_scans<true><<<n_scans, kRenderThreads, 0, st>>>(s, set, p);
+    k_render_alloc<<<blocks, 256, 0, st>>>(s, set, p.marks);
+    k_render_scans<false><<<n_scans, kRenderThreads, 0, st>>>(s, set, p);
+    k_render_known<<<blocks, 256, 0, st>>>(s, set, p.marks);
+}
+void launch_prune_freq(const StoreView& s, int set, cudaStream_t st)
+{
+    const int dim2 = s.window.dim * s.window.dim;
+    k_prune_freq<<<(dim2 + 7) / 8, 256, 0, st>>>(s, set);
 }
 
 }  // namespace lama_b200

@@ -132,4 +132,20 @@ void launch_match_error(const StoreView& s, int set, int particle0, bool shared_
 void launch_distance(const StoreView& s, int set, int particle, const double* d_pts, int n, double resolution, uint32_t max_sqdist, double* d_dist,
                      double* d_grad, cudaStream_t st);
 
+// GraphSlam2D::generateOccupancyMap's cast of posed scans into particle 0's frequency map (the map needs the `known` plane)
+struct RenderParams {
+    const double* points;       // xyz of all scans
+    const int64_t* offsets;     // [n_scans + 1]: the points of scan k are [offsets[k], offsets[k + 1])
+    const MovingTf* moving;     // [n_scans] sensor pose in the base frame
+    const SE2* states;          // [n_scans] base pose
+    double scale;               // 1 / resolution
+    int full;                   // 1: hits and free rays, 0: hits only
+    uint8_t* marks;             // [dim^2] zero on entry, zero again on exit
+    unsigned long long* cells;  // += cell updates (hits + ray cells)
+};
+// mark pass -> allocation of the marked patches -> counting pass -> known bits of the touched patches
+void launch_render_scans(const StoreView& s, int set, const RenderParams& p, int n_scans, cudaStream_t st);
+// FrequencyOccupancyMap::prune over the whole map of particle 0
+void launch_prune_freq(const StoreView& s, int set, cudaStream_t st);
+
 }  // namespace lama_b200
