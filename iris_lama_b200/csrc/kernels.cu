@@ -755,7 +755,9 @@ k_raycast(StoreView s, RayParams rp, const SE2* __restrict__ states, uint64_t* _
             patch_ptr(s, dir_s[di] & kDirSlotMask)[ci] = 0u;
             atomicOr(kbits_ptr(s, dir[di] & kDirSlotMask) + (ci >> 5), 1u << (ci & 31));
         } else {
-            obstacle = replay_cell(log, i, end, final_word, before, emit);
+            uint32_t word = final_word;
+            obstacle = replay_cell(log, i, end, word, before, emit);
+            if (word != final_word) *cell = word;   // the replay is the only writer of a logged cell after the barrier
         }
         if (obstacle != before) {
             if (obstacle) {
@@ -1769,7 +1771,7 @@ __global__ void k_distance(StoreView s, int set, int particle, const double* __r
 // step fall into neighbouring cells.  Every update of a render is a counter increment, so there is no ordered path: no log,
 // no replay, no candidate bitmaps.  kMark: the first pass only marks the directory entries of the touched cells (one byte
 // each, written when the walk enters another patch), so that exactly the reference's patch set gets allocated before the
-// counting pass; the counting pass walks the same cells and adds fire-and-forget reductions.
+// counting pass; the counting pass walks the same cells and adds fire-and-forget reductions (hits: a returning add, see touch).
 constexpr int kRenderThreads = 256;
 
 template <bool kMark>
@@ -1803,7 +1805,14 @@ __global__ void __launch_bounds__(kRenderThreads) k_render_scans(StoreView s, in
         }
         if (kMark || !base) return;
         uint32_t* cell = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(base) + packed_cell_offset(P));
-        asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(cell), "r"(inc) : "memory");
+        if (inc == kOccHitInc) {
+            // a hit (one touch in a few hundred) returns the old word: the hit that finds `occupied` at 0xFFFF wraps it, and its
+            // carry into `visited` is taken back (adding 0xFFFF0000 leaves the low half alone; the adds of a cell commute)
+            if (occ_occupied(atomicAdd(cell, kOccHitInc)) == 0xFFFFu)
+                asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(cell), "r"(0u - kOccMissInc) : "memory");
+        } else {
+            asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(cell), "r"(inc) : "memory");
+        }
         ++cells;
     };
     const int64_t b0 = p.offsets[blockIdx.x], b1 = p.offsets[blockIdx.x + 1];
@@ -1856,7 +1865,8 @@ __global__ void k_render_alloc(StoreView s, int set, const uint8_t* __restrict__
 }
 
 // one warp per directory entry touched by the render: known |= (word != 0) (every touch went through Map::get, which sets the
-// Container bit; counters only grow within a render), then the mark is cleared for the next render
+// Container bit; a touched cell's word is 0 only when both counters wrapped back to 0, DESIGN.md §10), then the mark is cleared for
+// the next render
 __global__ void k_render_known(StoreView s, int set, uint8_t* __restrict__ marks)
 {
     const int lane = threadIdx.x & 31;

@@ -36,8 +36,9 @@ constexpr uint32_t kMapOffsetCells = kUniversalHalf * kPatchLen;  // 42 275 904
 
 // ---- occupancy cell: FrequencyOccupancyMap {uint16 occupied; uint16 visited} packed in one word so
 // that a hit is ONE atomicAdd(+0x00010001) and a miss ONE atomicAdd(+0x00010000); `visited` (high half)
-// wraps at 2^16 exactly like the reference's uint16.  (A carry out of `occupied` would need 65 536 hits on
-// one cell while visited, which counts the same hits, has wrapped as well.)
+// wraps at 2^16 exactly like the reference's uint16.  The reference's two counters are independent, but in the
+// packed word the 65 536th hit of a cell carries out of `occupied` into `visited`: every writer that adds hits
+// takes that carry back (occ_drop_carry in the ray-cast replay, a returning add in the render).
 // Whether a cell is currently an obstacle of the distance map (valid_obstacle && sqdist == 0) -- which
 // decides if a miss can trigger removeObstacle -- is mirrored in a separate bit plane of 32 words per patch
 // (StoreView::fbits), so that the ray-cast kernel never needs the value returned by an atomic.
@@ -45,6 +46,9 @@ constexpr uint32_t kOccHitInc   = 0x00010001u;
 constexpr uint32_t kOccMissInc  = 0x00010000u;
 LAMA_HD uint32_t occ_occupied(uint32_t w) { return w & 0xFFFFu; }
 LAMA_HD uint32_t occ_visited(uint32_t w) { return w >> 16; }
+// `word` after `hits` (< 2^16) packed hits and any number of misses: `occupied` carried into `visited` at most once, and it did
+// exactly when the final `occupied` is below `hits`.  Returns the word with that carry taken back.
+LAMA_HD uint32_t occ_drop_carry(uint32_t word, uint32_t hits) { return occ_occupied(word) < hits ? word - kOccMissInc : word; }
 // prob() < 0.25 / > 0.25 of frequency_occupancy_map.cpp:40-45 in exact integer arithmetic
 // (occupied/visited == 0.25 exactly iff 4*occupied == visited; unvisited cells read 0.25).
 LAMA_HD bool occ_is_free(uint32_t occupied, uint32_t visited) { return visited != 0 && 4u * occupied < visited; }

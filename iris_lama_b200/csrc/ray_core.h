@@ -229,22 +229,25 @@ LAMA_HD bool log_is_hit(uint64_t r) { return (r & 1u) != 0; }
 // push record: [seq : 32][cell key : 32]; sorting by it orders obstacle events like the reference.
 LAMA_HD uint64_t push_record(uint32_t seq, uint32_t key) { return ((uint64_t)seq << 32) | key; }
 
-// Replays the sorted touches log[first, last) of ONE cell.  `final_word` is the occupancy word after
-// all of this scan's atomics, `obstacle` the cell's obstacle-mirror bit before the scan; returns the new
-// mirror bit and emits obstacle events through `emit(kind_is_add, seq)` in call order.
+// Replays the sorted touches log[first, last) of ONE cell.  `word` is the occupancy word after all of this
+// scan's atomics; it comes back with the carry of a wrapped `occupied` taken out (occ_drop_carry: every hit
+// of the cell is in the log), and the caller stores it when it changed.  `obstacle` is the cell's
+// obstacle-mirror bit before the scan; returns the new mirror bit and emits obstacle events through
+// `emit(kind_is_add, seq)` in call order.
 //   setFree     frequency_occupancy_map.cpp:65-74   setOccupied :81-91
 //   addObstacle / removeObstacle no-op rules: dynamic_distance_map.cpp:217-218,233-234
 template <typename Emit>
-LAMA_HD bool replay_cell(const uint64_t* log, int first, int last, uint32_t final_word, bool obstacle, Emit&& emit)
+LAMA_HD bool replay_cell(const uint64_t* log, int first, int last, uint32_t& word, bool obstacle, Emit&& emit)
 {
     uint32_t hits = 0, misses = 0;
     for (int i = first; i < last; ++i) {
         if (log_is_hit(log[i])) ++hits;
         else ++misses;
     }
+    word = occ_drop_carry(word, hits);
     // counters before this scan (uint16 wrap-around arithmetic like the reference's cells)
-    uint32_t occupied = (occ_occupied(final_word) - hits) & 0xFFFFu;
-    uint32_t visited  = (occ_visited(final_word) - hits - misses) & 0xFFFFu;
+    uint32_t occupied = (occ_occupied(word) - hits) & 0xFFFFu;
+    uint32_t visited  = (occ_visited(word) - hits - misses) & 0xFFFFu;
     for (int i = first; i < last; ++i) {
         const uint64_t r = log[i];
         if (log_is_hit(r)) {

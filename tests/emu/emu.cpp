@@ -685,6 +685,22 @@ uint32_t emu_dm_apply(void* h, const uint32_t* cells_xy, const uint8_t* is_add, 
     }
     return bf.update();
 }
+// replay_cell (ray_core.h) on one frequency cell as k_raycast runs it: the touches kinds[i] (1 hit / 0 miss, beam order) are first
+// added to the packed word {visited, occupied} = word_in (packed adds carry from occupied into visited; they commute, so their
+// order does not matter), then replayed; returns the word the replay stores.  events_out[i] = 1 add, 2 remove, 0 none
+uint32_t emu_freq_replay(const uint8_t* kinds, int n, uint32_t word_in, int obstacle_in, uint8_t* events_out, int* obstacle_out)
+{
+    std::vector<uint64_t> log((size_t)n);
+    uint32_t word = word_in;
+    for (int i = 0; i < n; ++i) {
+        word += kinds[i] ? kOccHitInc : kOccMissInc;
+        log[i] = log_record(7u, (uint32_t)i, kinds[i] ? 0u : 1u, kinds[i] != 0);
+        events_out[i] = 0;
+    }
+    const bool obstacle = replay_cell(log.data(), 0, n, word, obstacle_in != 0, [&](bool add, uint32_t seq) { events_out[seq >> 15] = add ? 1 : 2; });
+    *obstacle_out = obstacle;
+    return word;
+}
 // replay_cell_prob (ray_core.h) on one cell: kinds[i] = 1 hit / 0 miss in beam order; events_out[i] = 1 add, 2 remove, 0 none
 float emu_prob_replay(const uint8_t* kinds, int n, const double* constants, int obstacle_in, uint8_t* events_out, int* obstacle_out)
 {

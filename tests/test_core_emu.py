@@ -19,8 +19,9 @@ def emu():
     L.emu_create.argtypes = [C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_uint32, C.c_int]
     L.emu_dm_apply.restype = C.c_uint32
     L.emu_prob_replay.restype = C.c_float
+    L.emu_freq_replay.restype = C.c_uint32
     for f in ("emu_destroy", "emu_set_pose", "emu_get_state", "emu_counters", "emu_slam_update", "emu_export_dm", "emu_export_occ", "emu_dm_apply", "emu_set_pull",
-              "emu_pull_fallbacks"):
+              "emu_pull_fallbacks", "emu_freq_replay"):
         getattr(L, f).argtypes = None
     return L
 
@@ -171,6 +172,57 @@ def test_emulated_slam_equals_oracle(emu, po, synth, name, beams, T, shuffle):
         emu.emu_pull_fallbacks.restype = C.c_uint32
         assert emu.emu_pull_fallbacks(C.c_void_p(h)) == 0   # every scan went through the pull path
     emu.emu_destroy(C.c_void_p(h))
+
+
+def _frequency_cell(occ, vis, kinds, obstacle):
+    """FrequencyOccupancyMap::setOccupied / setFree (frequency_occupancy_map.cpp:65-91) on two independent uint16 counters, and the
+    no-op rules of addObstacle / removeObstacle (dynamic_distance_map.cpp:217-218,233-234): the final counters, the obstacle flag and
+    the event of every touch (1 add, 2 remove, 0 none)"""
+    ev = np.zeros(len(kinds), np.uint8)
+    for i, k in enumerate(kinds):
+        if k:
+            was = vis != 0 and 4 * occ > vis
+            occ, vis = (occ + 1) & 0xFFFF, (vis + 1) & 0xFFFF
+            if not was and vis != 0 and 4 * occ > vis and not obstacle:
+                obstacle, ev[i] = True, 1
+        else:
+            was = vis != 0 and 4 * occ < vis
+            vis = (vis + 1) & 0xFFFF
+            if not was and vis != 0 and 4 * occ < vis and obstacle:
+                obstacle, ev[i] = False, 2
+    return occ, vis, obstacle, ev
+
+
+def test_frequency_replay_takes_back_the_carry_of_a_wrapped_occupied_count(emu):
+    """replay_cell (ray_core.h) on packed words whose `occupied` half wraps in this scan: a packed hit carries into `visited`, the
+    reference's separate uint16 does not.  The stored word, the pre-scan state the replay starts from (seen through its events) and
+    the obstacle flag must follow the two independent counters; the plain packed sum must differ wherever occupied wrapped."""
+    rng = np.random.default_rng(21)
+    cases = [(0xFFFF, 0xFFFF, [1]), (0xFFFF, 0x0000, [1]), (0xFFFE, 0x0010, [1, 1, 1]), (0x0000, 0x0000, [1] * 65535),
+             (0xFFF0, 0x4000, [0] * 60000 + [1] * 16), (0x3FFF, 0xFFFF, [0, 1]), (0xFFFF, 0xFFFF, [0] * 3)]
+    for _ in range(300):
+        occ, vis = int(rng.choice([0xFFFF, 0xFFFE, 0xFF80, 0xC000, 0x4000, 0, 7])), int(rng.integers(0, 0x10000))
+        n = int(rng.integers(1, 600))
+        cases.append((occ, vis, (rng.random(n) < rng.choice([0.05, 0.3, 0.6, 1.0])).astype(np.uint8).tolist()))
+    wrapped = 0
+    for occ, vis, kinds in cases:
+        k = np.ascontiguousarray(kinds, np.uint8)
+        hits = int(k.sum())
+        assert hits < 0x10000                                    # a cell takes at most one hit per beam and scan
+        for obstacle_in in (0, 1):
+            ev = np.zeros(len(k), np.uint8)
+            ob = C.c_int(0)
+            word = emu.emu_freq_replay(_vp(k), C.c_int(len(k)), C.c_uint32((vis << 16) | occ), C.c_int(obstacle_in), _vp(ev), C.byref(ob))
+            o2, v2, flag, want = _frequency_cell(occ, vis, kinds, bool(obstacle_in))
+            assert word == (v2 << 16) | o2, (occ, vis, hits, len(k))
+            assert (ev == want).all() and bool(ob.value) == flag
+            packed = (((vis << 16) | occ) + hits * 0x10001 + (len(k) - hits) * 0x10000) & 0xFFFFFFFF
+            if occ + hits >= 0x10000:
+                wrapped += 1
+                assert packed >> 16 == (v2 + 1) & 0xFFFF             # without the correction visited is one ahead
+            else:
+                assert packed == word
+    assert wrapped >= 20
 
 
 def test_logodds_replay_equals_probabilistic_occupancy_map(emu, po):
