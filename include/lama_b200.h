@@ -410,6 +410,41 @@ int lama_graph_generate_occupancy_map(lama_graph* h, int full, lama_om** om);
  * NULL) = its update() return value.  BORROWED like the occupancy map. */
 int lama_graph_generate_coarse_distance_map(lama_graph* h, lama_dm** dm, uint32_t* processed);
 
+/* ------------------------------------------------------------------------------------------------
+ * TruncatedSignedDistanceMap -- include/lama/sdm/truncated_signed_distance_map.h, src/sdm/truncated_signed_distance_map.cpp:
+ * cells {float distance; float weight} and an "on" bit, in a dense window of window[0] x window[1] x window[2] patches of 32 x 32
+ * (x 32 in 3-D) cells.  Cells are absolute map coordinates (x, y, z) as Map::w2m gives them; in 2-D, z is not addressed.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct lama_tsdm lama_tsdm;
+/* TruncatedSignedDistanceMap(resolution, patch_size, is3d) (:41-49); patch_size must be 32.  The window is centred on center_xyz
+ * (NULL: origin); window_patches NULL = (dev->dir_dim, dev->dir_dim, 1) in 2-D and (8, 8, 4) in 3-D, at most 2048 per axis.
+ * dev->pool_slots 0 = one patch per window entry (a 3-D patch is 260 KiB, so the 3-D default takes 65 MiB). */
+int lama_tsdm_create(double resolution, uint32_t patch_size, int is3d, const double center_xyz[3], const int32_t window_patches[3],
+                     const lama_device_options* dev, lama_tsdm** out);
+int lama_tsdm_destroy(lama_tsdm* h);
+int lama_tsdm_set_max_distance(lama_tsdm* h, double distance);   /* setMaxDistance (:210-213): truncate_size_ */
+int lama_tsdm_max_distance(lama_tsdm* h, double* distance);      /* maxDistance (:215-218) */
+/* n_clouds calls of insertPointCloud (:141-158) in order: cloud k = points [offsets[k], offsets[k + 1]) of pts_xyz (offsets[0] = 0),
+ * sensor origins + 3k / quats_xyzw + 4k in world coordinates (either may be NULL: zero / identity); inserted[k] (may be NULL) = its
+ * return value, the number of distinct hit cells.  A hit or a ray cell outside the window fails with LAMA_ERR_WINDOW (in 2-D also a
+ * hit more than 2^15 cells from world z = 0), a full pool with LAMA_ERR_POOL; the map is then unchanged. */
+int lama_tsdm_insert_point_clouds(lama_tsdm* h, const double* pts_xyz, const int64_t* offsets, int n_clouds, const double* origins,
+                                  const double* quats_xyzw, uint64_t* inserted);
+/* distance(Vector3d, gradient) (:59-130) of n world points: bilinear in 2-D, trilinear in 3-D; gradient (n x 3) may be NULL */
+int lama_tsdm_distance(lama_tsdm* h, const double* pts_xyz, int n, double* distance, double* gradient);
+/* Map::bounds (map.cpp:139-157) in cells, all three axes; *patches (may be NULL) = allocated patches */
+int lama_tsdm_bounds(lama_tsdm* h, uint32_t mn[3], uint32_t mx[3], int* patches);
+/* the cells of the box lo + [0, size) (x fastest, then y, then z); cells that are off read 0; any output may be NULL */
+int lama_tsdm_export(lama_tsdm* h, const uint32_t lo[3], const int32_t size[3], float* distance, float* weight, uint8_t* on);
+/* toMesh (:220-272): 3 unshared vertices (x, y, z floats) per triangle, PolygonMesh::index[i] = i.  *n_vertices = the vertex count;
+ * the vertices are written when vertices != NULL and cap (in vertices) >= *n_vertices.  Cells are visited in ascending window
+ * entry, then cell index, where the reference iterates an unordered_map. */
+int lama_tsdm_to_mesh(lama_tsdm* h, float* vertices, size_t cap, size_t* n_vertices);
+/* sdm::export_to_ply (export.cpp:112-143): ASCII PLY of toMesh, faces written as 3 i+2 i+1 i */
+int lama_tsdm_write_ply(lama_tsdm* h, const char* path);
+/* with dev->timing: ms = device time of [0] insert_point_clouds, [1] distance, [2] to_mesh; launches likewise */
+int lama_tsdm_kernel_times(lama_tsdm* h, double ms[3], uint64_t launches[3]);
+
 #ifdef __cplusplus
 }
 #endif

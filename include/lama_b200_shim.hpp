@@ -214,4 +214,41 @@ private:
     lama_loc* h_ = nullptr;
 };
 
+// lama::TruncatedSignedDistanceMap (include/lama/sdm/truncated_signed_distance_map.h) on the device; toMesh gives the vertices
+// (3 per triangle, index[i] = i), writePly is sdm::export_to_ply
+class TruncatedSignedDistanceMap {
+public:
+    explicit TruncatedSignedDistanceMap(double resolution, uint32_t patch_size = 32, bool is3d = false)
+    {
+        check(lama_tsdm_create(resolution, patch_size, is3d ? 1 : 0, nullptr, nullptr, nullptr, &h_));
+    }
+    ~TruncatedSignedDistanceMap() { lama_tsdm_destroy(h_); }
+    TruncatedSignedDistanceMap(const TruncatedSignedDistanceMap&) = delete;
+    TruncatedSignedDistanceMap& operator=(const TruncatedSignedDistanceMap&) = delete;
+    template <typename CloudPtr>
+    size_t insertPointCloud(const CloudPtr& cloud)   // truncated_signed_distance_map.cpp:141-158
+    {
+        FlatCloud<typename std::remove_reference<decltype(*cloud)>::type> f(*cloud);
+        const int64_t offsets[2] = {0, (int64_t)(f.pts.size() / 3)};
+        uint64_t n = 0;
+        check(lama_tsdm_insert_point_clouds(h_, f.pts.data(), offsets, 1, f.origin, f.quat, &n));
+        return (size_t)n;
+    }
+    double distance(const double xyz[3], double gradient[3] = nullptr) const { double d = 0; check(lama_tsdm_distance(h_, xyz, 1, &d, gradient)); return d; }
+    void setMaxDistance(double d) { check(lama_tsdm_set_max_distance(h_, d)); }
+    double maxDistance() const { double d = 0; check(lama_tsdm_max_distance(h_, &d)); return d; }
+    std::vector<float> toMesh() const   // x, y, z per vertex
+    {
+        size_t n = 0;
+        check(lama_tsdm_to_mesh(h_, nullptr, 0, &n));
+        std::vector<float> v(n * 3);
+        if (n) check(lama_tsdm_to_mesh(h_, v.data(), n, &n));
+        return v;
+    }
+    void writePly(const std::string& path) const { check(lama_tsdm_write_ply(h_, path.c_str())); }
+
+private:
+    lama_tsdm* h_ = nullptr;
+};
+
 }  // namespace lama_b200_shim

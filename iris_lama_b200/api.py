@@ -87,6 +87,8 @@ EXPORTED_SYMBOLS = [
     "lama_graph_get_stats", "lama_graph_slam", "lama_graph_generate_occupancy_map", "lama_graph_generate_coarse_distance_map",
     "lama_om_create", "lama_om_destroy", "lama_om_insert_scans", "lama_om_prune", "lama_om_resolution", "lama_om_bounds", "lama_om_query",
     "lama_om_export", "lama_om_write", "lama_om_export_image", "lama_om_kernel_times",
+    "lama_tsdm_create", "lama_tsdm_destroy", "lama_tsdm_set_max_distance", "lama_tsdm_max_distance", "lama_tsdm_insert_point_clouds",
+    "lama_tsdm_distance", "lama_tsdm_bounds", "lama_tsdm_export", "lama_tsdm_to_mesh", "lama_tsdm_write_ply", "lama_tsdm_kernel_times",
 ]
 
 
@@ -829,6 +831,94 @@ class FrequencyOccupancyMap:
 
     def kernelTimes(self):
         return _times(lib().lama_om_kernel_times, self.h)
+
+
+def _clouds(clouds):
+    clouds = [np.ascontiguousarray(c, np.float64).reshape(-1, 3) for c in clouds]
+    offsets = np.zeros(len(clouds) + 1, np.int64)
+    offsets[1:] = np.cumsum([len(c) for c in clouds])
+    return np.ascontiguousarray(np.concatenate(clouds) if clouds else np.zeros((0, 3))), offsets
+
+
+class TruncatedSignedDistanceMap:
+    """Device-resident lama::TruncatedSignedDistanceMap (include/lama/sdm/truncated_signed_distance_map.h).  `window` = patches per
+    axis (None: dir_dim x dir_dim x 1 in 2-D, 8 x 8 x 4 in 3-D), centred on `center`."""
+
+    def __init__(self, resolution, patch_size=32, is3d=False, center=(0.0, 0.0, 0.0), window=None, **dev):
+        d = DeviceOptions(device=0, dir_dim=64, pool_slots=0, max_beams=2048, timing=0, stream=0)
+        for k, v in dev.items():
+            setattr(d, k, v)
+        c, cp = _d(center)
+        win = None if window is None else (C.c_int32 * 3)(*[int(x) for x in window])
+        self.is3d = bool(is3d)
+        self.h = C.c_void_p()
+        _chk(lib().lama_tsdm_create(C.c_double(resolution), C.c_uint32(patch_size), C.c_int(1 if is3d else 0), cp, win, C.byref(d), C.byref(self.h)))
+
+    def __del__(self):
+        if getattr(self, "h", None) and _lib is not None:
+            _lib.lama_tsdm_destroy(self.h)
+            self.h = None
+
+    def setMaxDistance(self, distance):
+        _chk(lib().lama_tsdm_set_max_distance(self.h, C.c_double(distance)))
+
+    def maxDistance(self) -> float:
+        r = C.c_double(0)
+        _chk(lib().lama_tsdm_max_distance(self.h, C.byref(r)))
+        return r.value
+
+    def insertPointClouds(self, clouds, origins=None, quats=None):
+        """insertPointCloud on each (n_k, 3) cloud in order; origins (S, 3) / quats (S, 4) xyzw world sensor poses or None (zero /
+        identity).  Returns the (S,) return values: distinct hit cells per cloud."""
+        p, offsets = _clouds(clouds)
+        o = None if origins is None else np.ascontiguousarray(origins, np.float64).reshape(-1, 3)
+        q = None if quats is None else np.ascontiguousarray(quats, np.float64).reshape(-1, 4)
+        out = np.zeros(len(offsets) - 1, np.uint64)
+        _chk(lib().lama_tsdm_insert_point_clouds(self.h, _vp(p), offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int(len(offsets) - 1), _vp(o), _vp(q),
+                                                 _vp(out)))
+        return out
+
+    def insertPointCloud(self, points, origin=None, quat=None) -> int:
+        """insertPointCloud (truncated_signed_distance_map.cpp:141-158)"""
+        return int(self.insertPointClouds([points], None if origin is None else [origin], None if quat is None else [quat])[0])
+
+    def distance(self, points, gradient=False):
+        """distance(Vector3d, gradient) of (n, 3) world points: (n,) distances, and (n, 3) gradients with gradient=True"""
+        p, pp = _d(np.asarray(points, np.float64).reshape(-1, 3))
+        n = p.size // 3
+        dist, grad = np.zeros(n), np.zeros((n, 3))
+        _chk(lib().lama_tsdm_distance(self.h, pp, C.c_int(n), dist.ctypes.data_as(c_dp), grad.ctypes.data_as(c_dp) if gradient else None))
+        return (dist, grad) if gradient else dist
+
+    def bounds(self):
+        """(allocated patches, min cell (3,), max cell (3,)) as Map::bounds"""
+        mn, mx, n = np.zeros(3, np.uint32), np.zeros(3, np.uint32), C.c_int(0)
+        _chk(lib().lama_tsdm_bounds(self.h, mn.ctypes.data_as(c_u32p), mx.ctypes.data_as(c_u32p), C.byref(n)))
+        return n.value, mn, mx
+
+    def export(self, lo, size):
+        """cells of the box lo + [0, size): dict(distance, weight, on) shaped (size z, size y, size x)"""
+        lo = np.ascontiguousarray(lo, np.uint32)
+        sz = np.ascontiguousarray(size, np.int32)
+        shape = (int(sz[2]), int(sz[1]), int(sz[0]))
+        o = dict(distance=np.zeros(shape, np.float32), weight=np.zeros(shape, np.float32), on=np.zeros(shape, np.uint8))
+        _chk(lib().lama_tsdm_export(self.h, _vp(lo), _vp(sz), _vp(o["distance"]), _vp(o["weight"]), _vp(o["on"])))
+        return o
+
+    def toMesh(self):
+        """toMesh (:220-272): (vertices (n, 3) float32, index (n,) uint32 = 0..n-1), 3 vertices per triangle"""
+        n = C.c_size_t(0)
+        _chk(lib().lama_tsdm_to_mesh(self.h, None, C.c_size_t(0), C.byref(n)))
+        v = np.zeros((n.value, 3), np.float32)
+        if n.value:
+            _chk(lib().lama_tsdm_to_mesh(self.h, _vp(v), C.c_size_t(n.value), C.byref(n)))
+        return v, np.arange(n.value, dtype=np.uint32)
+
+    def kernelTimes(self):
+        ms, ln = np.zeros(3), np.zeros(3, np.uint64)
+        _chk(lib().lama_tsdm_kernel_times(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
+        keys = ("insert", "distance", "mesh")
+        return dict(zip(keys, ms.tolist())), dict(zip(keys, ln.tolist()))
 
 
 class DynamicDistanceMap:

@@ -1,6 +1,7 @@
 // capi.cpp -- the extern "C" boundary declared in include/lama_b200.h.
 #include <algorithm>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <new>
 #include <stdexcept>
@@ -13,6 +14,7 @@
 #include "sdm_io.h"
 #include "shard_comm.h"
 #include "pgo.h"
+#include "tsdm.h"
 
 #include "../../include/lama_b200.h"
 
@@ -1483,6 +1485,115 @@ int lama_om_kernel_times(lama_om* om, double ms[4], uint64_t launches[5])
 try {
     if (!om) return set_err("null handle", LAMA_ERR_ARG);
     return times_out(om_engine(om), ms, launches);
+}
+LAMA_CATCH
+
+// ---- TruncatedSignedDistanceMap (include/lama/sdm/truncated_signed_distance_map.h) -------------------------------------------------
+struct lama_tsdm { TsdmDev* t; };
+// TruncatedSignedDistanceMap(resolution, patch_size, is3d) (truncated_signed_distance_map.cpp:41-49) on the device
+int lama_tsdm_create(double resolution, uint32_t patch_size, int is3d, const double center_xyz[3], const int32_t window_patches[3],
+                     const lama_device_options* dev, lama_tsdm** out)
+try {
+    if (!out) return set_err("null argument", LAMA_ERR_ARG);
+    lama_device_options d;
+    if (dev) d = *dev; else dev_default(&d);
+    std::string err;
+    TsdmDev* t = TsdmDev::create(resolution, patch_size, is3d != 0, center_xyz, window_patches, dev_from(d), err);
+    if (!t) {
+        const bool bad_arg = !(resolution > 0) || patch_size != 32 || err.find("window") != std::string::npos;
+        return set_err(err, !bad_arg && lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : (bad_arg ? LAMA_ERR_ARG : LAMA_ERR_CUDA));
+    }
+    *out = new lama_tsdm{t};
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_tsdm_destroy(lama_tsdm* h)
+try {
+    if (!h) return LAMA_OK;
+    delete h->t;
+    delete h;
+    return LAMA_OK;
+}
+LAMA_CATCH
+// setMaxDistance (:210-213)
+int lama_tsdm_set_max_distance(lama_tsdm* h, double distance)
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    h->t->set_max_distance(distance);
+    return LAMA_OK;
+}
+LAMA_CATCH
+// maxDistance (:215-218)
+int lama_tsdm_max_distance(lama_tsdm* h, double* distance)
+try {
+    if (!h || !distance) return set_err("null argument", LAMA_ERR_ARG);
+    *distance = h->t->max_distance();
+    return LAMA_OK;
+}
+LAMA_CATCH
+// insertPointCloud (:141-158), n_clouds of them in order
+int lama_tsdm_insert_point_clouds(lama_tsdm* h, const double* pts_xyz, const int64_t* offsets, int n_clouds, const double* origins,
+                                  const double* quats_xyzw, uint64_t* inserted)
+try {
+    if (!h || (n_clouds > 0 && !offsets)) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->t->insert_point_clouds(pts_xyz, offsets, n_clouds, origins, quats_xyzw, inserted);
+    return rc == LAMA_OK ? rc : set_err(h->t->error(), rc);
+}
+LAMA_CATCH
+// distance(Vector3d, gradient) (:59-130)
+int lama_tsdm_distance(lama_tsdm* h, const double* pts_xyz, int n, double* distance, double* gradient)
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    int rc = h->t->distance(pts_xyz, n, distance, gradient);
+    return rc == LAMA_OK ? rc : set_err(h->t->error(), rc);
+}
+LAMA_CATCH
+// Map::bounds (map.cpp:139-157)
+int lama_tsdm_bounds(lama_tsdm* h, uint32_t mn[3], uint32_t mx[3], int* patches)
+try {
+    if (!h || !mn || !mx) return set_err("null argument", LAMA_ERR_ARG);
+    return h->t->bounds(mn, mx, patches);
+}
+LAMA_CATCH
+int lama_tsdm_export(lama_tsdm* h, const uint32_t lo[3], const int32_t size[3], float* distance, float* weight, uint8_t* on)
+try {
+    if (!h || !lo || !size) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->t->export_box(lo, size, distance, weight, on);
+    return rc == LAMA_OK ? rc : set_err(h->t->error(), rc);
+}
+LAMA_CATCH
+// toMesh (:220-272)
+int lama_tsdm_to_mesh(lama_tsdm* h, float* vertices, size_t cap, size_t* n_vertices)
+try {
+    if (!h || !n_vertices) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->t->to_mesh(vertices, cap, n_vertices);
+    return rc == LAMA_OK ? rc : set_err(h->t->error(), rc);
+}
+LAMA_CATCH
+// sdm::export_to_ply (export.cpp:112-143)
+int lama_tsdm_write_ply(lama_tsdm* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    size_t n = 0;
+    int rc = h->t->to_mesh(nullptr, 0, &n);
+    std::vector<float> v(n * 3);
+    if (rc == LAMA_OK && n) rc = h->t->to_mesh(v.data(), n, &n);
+    if (rc != LAMA_OK) return set_err(h->t->error(), rc);
+    FILE* f = std::fopen(path, "w");
+    if (!f) return set_err(std::string("cannot open file '") + path + "'", LAMA_ERR_ARG);
+    std::fprintf(f, "ply\nformat ascii 1.0\nelement vertex %zu\nproperty float x\nproperty float y\nproperty float z\nelement face %zu\n"
+                    "property list uchar int vertex_index\nend_header\n", n, n / 3);
+    for (size_t i = 0; i < n; ++i) std::fprintf(f, "%f %f %f\n", (double)v[3 * i], (double)v[3 * i + 1], (double)v[3 * i + 2]);
+    for (size_t i = 0; i + 2 < n; i += 3) std::fprintf(f, "3 %d %d %d\n", (int)(i + 2), (int)(i + 1), (int)i);
+    const bool ok = std::fclose(f) == 0;
+    return ok ? LAMA_OK : set_err(std::string("cannot write file '") + path + "'", LAMA_ERR_ARG);
+}
+LAMA_CATCH
+int lama_tsdm_kernel_times(lama_tsdm* h, double ms[3], uint64_t launches[3])
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    h->t->kernel_times(ms, launches);
+    return LAMA_OK;
 }
 LAMA_CATCH
 

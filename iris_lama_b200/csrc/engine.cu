@@ -311,7 +311,7 @@ int Engine::synchronize()
 }
 
 // Translation3d(sensor_origin) * Quaterniond  (match_surface_2d.cpp:49; Eigen quaternion -> matrix); null = identity
-static MovingTf moving_tf(const double origin[3], const double quat[4])
+MovingTf moving_tf(const double origin[3], const double quat[4])
 {
     MovingTf m;
     const double x = quat ? quat[0] : 0, y = quat ? quat[1] : 0, z = quat ? quat[2] : 0, w = quat ? quat[3] : 1;

@@ -201,4 +201,7 @@ enum : int {
     LAMA_ERR_STATE     = -7,
 };
 
+// Translation3d(origin) * Quaterniond(quat xyzw) of a PointCloudXYZ (types.h:111-120); NULL = zero / identity
+MovingTf moving_tf(const double origin[3], const double quat[4]);
+
 }  // namespace lama_b200

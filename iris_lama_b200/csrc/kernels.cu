@@ -286,32 +286,6 @@ __device__ __forceinline__ int seg_shift(const BeamEnds& be, bool xgroup)
 constexpr uint32_t kCandNone = 0xFF, kCandOverflow = 0xFE;
 constexpr uint32_t kInfoSlotMask = 0x00FFFFFFu;   // slot field of a patch-info word; all ones = not writable in this pass
 
-// Map::computeRay's 3-axis walk in 32-bit arithmetic (cell coordinates and deltas are < 2^27): tilted sensors only
-struct RayWalk3 {
-    int e0, e1, e2, d0, d1, d2, s0, s1, s2, n, i;
-    uint32_t x, y, z;
-    __device__ __forceinline__ explicit RayWalk3(const BeamCells& b)
-    {
-        x = b.from[0]; y = b.from[1]; z = b.from[2];
-        const int a0 = (int)(b.to[0] - b.from[0]), a1 = (int)(b.to[1] - b.from[1]), a2 = (int)(b.to[2] - b.from[2]);
-        s0 = a0 < 0 ? -1 : 1; s1 = a1 < 0 ? -1 : 1; s2 = a2 < 0 ? -1 : 1;
-        d0 = a0 < 0 ? -a0 : a0; d1 = a1 < 0 ? -a1 : a1; d2 = a2 < 0 ? -a2 : a2;
-        n = max(d0, max(d1, d2));
-        e0 = e1 = e2 = 0;
-        i = 0;
-    }
-    __device__ __forceinline__ bool next()
-    {
-        if (i >= n - 1) return false;
-        ++i;
-        e0 += d0; e1 += d1; e2 += d2;
-        if (2 * e0 >= n) { x += s0; e0 -= n; }
-        if (2 * e1 >= n) { y += s1; e1 -= n; }
-        if (2 * e2 >= n) { z += s2; e2 -= n; }
-        return true;
-    }
-};
-
 // The inner loop of the ray cast: everything it needs to know about a patch is ONE shared-memory word
 //   pinfo[directory index] = [candidate bitmap index : 8][slot the counters go to : 24]
 // (slot all ones: the patch cannot be written in this pass), so a step is walk + index + LDS + RED with no

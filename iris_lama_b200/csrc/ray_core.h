@@ -124,6 +124,34 @@ struct RayWalk {
     }
 };
 
+// Map::computeRay's 3-axis walk in 32-bit arithmetic (cell coordinates and deltas are < 2^27): tilted sensors in the ray cast and
+// the render, every ray of the truncated signed distance map (tsdm.cu)
+struct RayWalk3 {
+    int e0, e1, e2, d0, d1, d2, s0, s1, s2, n, i;
+    uint32_t x, y, z;
+    LAMA_HD explicit RayWalk3(const BeamCells& b)
+    {
+        x = b.from[0]; y = b.from[1]; z = b.from[2];
+        const int a0 = (int)(b.to[0] - b.from[0]), a1 = (int)(b.to[1] - b.from[1]), a2 = (int)(b.to[2] - b.from[2]);
+        s0 = a0 < 0 ? -1 : 1; s1 = a1 < 0 ? -1 : 1; s2 = a2 < 0 ? -1 : 1;
+        d0 = a0 < 0 ? -a0 : a0; d1 = a1 < 0 ? -a1 : a1; d2 = a2 < 0 ? -a2 : a2;
+        n = d0 > d1 ? d0 : d1;
+        n = n > d2 ? n : d2;
+        e0 = e1 = e2 = 0;
+        i = 0;
+    }
+    LAMA_HD bool next()
+    {
+        if (i >= n - 1) return false;
+        ++i;
+        e0 += d0; e1 += d1; e2 += d2;
+        if (2 * e0 >= n) { x += s0; e0 -= n; }
+        if (2 * e1 >= n) { y += s1; e1 -= n; }
+        if (2 * e2 >= n) { z += s2; e2 -= n; }
+        return true;
+    }
+};
+
 // ---- packed cells: P = yr << 16 | xr, window-relative coordinates (each < 2^13) -------------------------------------------
 // directory index of the patch of P in a window of (1 << log2dim)^2 patches
 LAMA_HD uint32_t packed_dir_index(uint32_t P, int log2dim) { return ((P >> 21) << log2dim) | ((P >> kPatchLog2) & 0xFFu); }

@@ -45,6 +45,14 @@ def read_sdm(path, n_params=None):
     return dict(header=hdr, params=raw[32:32 + n_params].tobytes(), patches=patches)
 
 
+def export_to_ply(tsdm, filename):
+    """sdm::export_to_ply (export.cpp:112-143): ASCII PLY of a TruncatedSignedDistanceMap's toMesh, faces written as 3 i+2 i+1 i"""
+    import ctypes as C
+    from . import api
+    api._chk(api.lib().lama_tsdm_write_ply(tsdm.h, C.c_char_p(str(filename).encode())))
+    return True
+
+
 def patch_origin(pid, patch_length=32):
     """Map::p2m (map.h:166-177): the absolute cell coordinates of a patch's first cell"""
     return (pid // UNIVERSAL_CONSTANT) * patch_length, (pid % UNIVERSAL_CONSTANT) * patch_length

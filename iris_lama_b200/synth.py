@@ -233,3 +233,74 @@ def make_pose_graph(n_nodes, n_loops, seed=7, step=0.1, odom_sigma=(0.02, 0.02, 
         a, b = (a, b) if a < b else (b, a)
         edges.append((int(a), int(b), xyr(np.linalg.inv(T[a]) @ T[b]) + rng.normal(0, loop_sigma)))
     return truth, np.array(nodes), edges
+
+
+# ---- 3-D scenes for the truncated signed distance map ----------------------------------------------------------------------------
+def make_scene_3d():
+    """A 10 x 10 x 3 m room (the inside of an axis-aligned box) with a box standing on the floor and a sphere in the air."""
+    return dict(room=(np.array([-5.0, -5.0, 0.0]), np.array([5.0, 5.0, 3.0])),
+                boxes=[(np.array([1.0, -2.0, 0.0]), np.array([2.0, -1.0, 1.2]))],
+                spheres=[(np.array([-1.5, 1.5, 1.0]), 0.6)])
+
+
+def cast_3d(scene, origin, dirs, max_range=30.0):
+    """Ranges along unit world directions (n, 3) from `origin`: the nearest of the room's walls (exit of its box), the obstacle boxes
+    (slab entry) and the spheres."""
+    o = np.asarray(origin, np.float64)
+    d = np.asarray(dirs, np.float64)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        inv = 1.0 / d
+        lo, hi = scene["room"]
+        t_exit = np.maximum((lo - o) * inv, (hi - o) * inv)
+        t = np.minimum(np.nanmin(np.where(np.isfinite(t_exit), t_exit, np.inf), axis=1), max_range)
+        for blo, bhi in scene["boxes"]:
+            t1, t2 = (blo - o) * inv, (bhi - o) * inv
+            tmin = np.nanmax(np.minimum(t1, t2), axis=1)
+            tmax = np.nanmin(np.maximum(t1, t2), axis=1)
+            hit = (tmax >= tmin) & (tmin > 0)
+            t = np.where(hit, np.minimum(t, tmin), t)
+    for c, r in scene["spheres"]:
+        oc = o - c
+        b = d @ oc
+        disc = b * b - (oc @ oc - r * r)
+        ts = -b - np.sqrt(np.maximum(disc, 0.0))
+        t = np.where((disc >= 0) & (ts > 0), np.minimum(t, ts), t)
+    return t
+
+
+def ring_lidar_dirs(n_rings=32, n_az=900, fov_down_deg=-15.0, fov_up_deg=15.0):
+    """Unit beam directions (n_rings * n_az, 3) of a spinning ring lidar in its own frame, ring-major."""
+    el = np.deg2rad(np.linspace(fov_down_deg, fov_up_deg, n_rings))
+    az = np.arange(n_az) * (2 * np.pi / n_az)
+    e, a = np.meshgrid(el, az, indexing="ij")
+    return np.stack([np.cos(e) * np.cos(a), np.cos(e) * np.sin(a), np.sin(e)], axis=-1).reshape(-1, 3)
+
+
+def quat_xyzw(yaw, pitch=0.0, roll=0.0):
+    """Quaternion (x, y, z, w) of Rz(yaw) Ry(pitch) Rx(roll)."""
+    cy, sy, cp, sp, cr, sr = np.cos(yaw / 2), np.sin(yaw / 2), np.cos(pitch / 2), np.sin(pitch / 2), np.cos(roll / 2), np.sin(roll / 2)
+    return np.array([sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy, cr * cp * cy + sr * sp * sy])
+
+
+def quat_matrix(q):
+    x, y, z, w = q
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+
+def make_clouds_3d(n_clouds, n_rings=32, n_az=900, seed=5, range_sigma=0.005, max_range=30.0):
+    """Seeded 3-D lidar sequence in make_scene_3d(): a sensor 1 m above the floor on a 2.5 m circle, slightly pitched.
+    Returns (clouds: list of (n, 3) points in the sensor frame, origins (S, 3), quats (S, 4) xyzw) -- world sensor poses."""
+    scene = make_scene_3d()
+    dirs = ring_lidar_dirs(n_rings, n_az)
+    rng = np.random.Generator(np.random.PCG64(seed))
+    clouds, origins, quats = [], np.zeros((n_clouds, 3)), np.zeros((n_clouds, 4))
+    for k in range(n_clouds):
+        a = 2 * np.pi * k / max(1, n_clouds)
+        origins[k] = (2.5 * np.cos(a), 2.5 * np.sin(a), 1.0)
+        quats[k] = quat_xyzw(a + np.pi / 2, 0.05 * np.sin(3 * a))
+        r = cast_3d(scene, origins[k], dirs @ quat_matrix(quats[k]).T, max_range)
+        r = r + rng.normal(0.0, range_sigma, size=r.shape)
+        clouds.append(dirs * r[:, None])
+    return clouds, origins, quats
