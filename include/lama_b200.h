@@ -445,6 +445,53 @@ int lama_tsdm_write_ply(lama_tsdm* h, const char* path);
 /* with dev->timing: ms = device time of [0] insert_point_clouds, [1] distance, [2] to_mesh; launches likewise */
 int lama_tsdm_kernel_times(lama_tsdm* h, double ms[3], uint64_t launches[3]);
 
+/* ------------------------------------------------------------------------------------------------
+ * 3-D occupancy maps -- FrequencyOccupancyMap / ProbabilisticOccupancyMap(resolution, patch_size, is3d = true)
+ * (include/lama/sdm/frequency_occupancy_map.h, probabilistic_occupancy_map.h, src/sdm/map.cpp:42-48): cells {uint16 occupied;
+ * uint16 visited} (kind 0, frequency) or a float log-odds (kind 1), and a known bit, in a dense window of window[0] x window[1] x
+ * window[2] patches of 32 x 32 x 32 cells.  Cells are absolute map coordinates (x, y, z) as Map::w2m gives them (lama_w2m3).
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct lama_om3 lama_om3;
+/* ops of lama_om3_apply */
+#define LAMA_OM3_SET_FREE 0
+#define LAMA_OM3_SET_OCCUPIED 1
+#define LAMA_OM3_SET_UNKNOWN 2
+/* the map of `kind` (0 frequency, 1 log-odds) with is3d = true; patch_size must be 32.  The window is centred on center_xyz (NULL:
+ * origin); window_patches NULL = (8, 8, 4), at most 2048 per axis and 65 536 entries in all.  dev->pool_slots 0 = one patch per
+ * window entry (a patch is 132 KiB, so the default takes 33 MiB). */
+int lama_om3_create(double resolution, uint32_t patch_size, int kind, const double center_xyz[3], const int32_t window_patches[3],
+                    const lama_device_options* dev, lama_om3** out);
+int lama_om3_destroy(lama_om3* h);
+/* the loop body of GraphSlam2D::generateOccupancyMap (graph_slam2d.cpp:146-158) for every point of n_clouds clouds in order:
+ * setOccupied(tf * p), then with `full` setFree on computeRay(w2m(tf.translation()), w2m(tf * p)), tf = Translation(origin) * quat.
+ * Clouds as lama_tsdm_insert_point_clouds.  *cells (may be NULL) = the cell updates made.  A cell outside the window fails with
+ * LAMA_ERR_WINDOW, a full pool with LAMA_ERR_POOL; the map is then unchanged. */
+int lama_om3_insert_point_clouds(lama_om3* h, const double* pts_xyz, const int64_t* offsets, int n_clouds, const double* origins,
+                                 const double* quats_xyzw, int full, uint64_t* cells);
+/* setFree / setOccupied / setUnknown (LAMA_OM3_SET_*) of n cells in list order (frequency_occupancy_map.cpp:65-108,
+ * probabilistic_occupancy_map.cpp:82-123); changed[i] (may be NULL) = what op i returns.  Errors as insert. */
+int lama_om3_apply(lama_om3* h, const uint32_t* cells_xyz, const uint8_t* ops, int n, uint8_t* changed);
+/* getProbability (prob, may be NULL) and flags (may be NULL) bit 0 isFree, bit 1 isOccupied, bit 2 isUnknown of n cells */
+int lama_om3_query(lama_om3* h, const uint32_t* cells_xyz, int n, double* prob, uint8_t* flags);
+/* FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158); LAMA_ERR_ARG on a log-odds map */
+int lama_om3_prune(lama_om3* h);
+/* Map::bounds (map.cpp:139-157) in cells, all three axes; *patches (may be NULL) = allocated patches */
+int lama_om3_bounds(lama_om3* h, uint32_t mn[3], uint32_t mx[3], int* patches);
+/* the box lo + [0, size) (x fastest, then y, then z): cell words ({occupied | visited << 16} or the float bits) and known bits;
+ * either output may be NULL */
+int lama_om3_export(lama_om3* h, const uint32_t lo[3], const int32_t size[3], uint32_t* cells, uint8_t* known);
+/* Map::write (map.cpp:490-529) with is_3d = 1: patches in ascending window entry, where the reference iterates an unordered_map */
+int lama_om3_write(lama_om3* h, const char* path);
+/* Map::read (map.cpp:531-575) into an empty map: a 4-byte-cell 3-D file, whose resolution the map takes */
+int lama_om3_read(lama_om3* h, const char* path);
+/* the z-slice image of sdm::export_to_png(occ, file, zed) (export.cpp:46-72): dims = {width, height} from the x / y bounds, slice
+ * z = w2m((0, 0, zed)).z; pixels (row-major, width per row) written when cap >= width * height */
+int lama_om3_export_image(lama_om3* h, double zed, uint8_t* pixels, size_t cap, int dims[2]);
+/* with dev->timing: ms = device time of [0] insert_point_clouds, [1] apply, [2] query; launches likewise */
+int lama_om3_kernel_times(lama_om3* h, double ms[3], uint64_t launches[3]);
+/* Map::w2m (map.h:125-126) on all three axes: world points (n x 3) -> cells (n x 3) */
+int lama_w2m3(double resolution, const double* pts_xyz, int n, uint32_t* cells_xyz);
+
 #ifdef __cplusplus
 }
 #endif

@@ -251,4 +251,41 @@ private:
     lama_tsdm* h_ = nullptr;
 };
 
+// lama::FrequencyOccupancyMap (kind 0) / lama::ProbabilisticOccupancyMap (kind 1) with is3d = true on the device.  Cells are map
+// coordinates {x, y, z}; insertPointCloud is the loop body of GraphSlam2D::generateOccupancyMap for every point of the cloud.
+class OccupancyMap3D {
+public:
+    explicit OccupancyMap3D(double resolution, int kind = 0, uint32_t patch_size = 32)
+    {
+        check(lama_om3_create(resolution, patch_size, kind, nullptr, nullptr, nullptr, &h_));
+    }
+    ~OccupancyMap3D() { lama_om3_destroy(h_); }
+    OccupancyMap3D(const OccupancyMap3D&) = delete;
+    OccupancyMap3D& operator=(const OccupancyMap3D&) = delete;
+    template <typename CloudPtr>
+    uint64_t insertPointCloud(const CloudPtr& cloud, bool full = true)   // graph_slam2d.cpp:146-158; returns the cell updates
+    {
+        FlatCloud<typename std::remove_reference<decltype(*cloud)>::type> f(*cloud);
+        const int64_t offsets[2] = {0, (int64_t)(f.pts.size() / 3)};
+        uint64_t n = 0;
+        check(lama_om3_insert_point_clouds(h_, f.pts.data(), offsets, 1, f.origin, f.quat, full ? 1 : 0, &n));
+        return n;
+    }
+    bool setFree(const uint32_t xyz[3]) { return set(xyz, LAMA_OM3_SET_FREE); }
+    bool setOccupied(const uint32_t xyz[3]) { return set(xyz, LAMA_OM3_SET_OCCUPIED); }
+    bool setUnknown(const uint32_t xyz[3]) { return set(xyz, LAMA_OM3_SET_UNKNOWN); }
+    bool isFree(const uint32_t xyz[3]) const { return (flags(xyz) & 1) != 0; }
+    bool isOccupied(const uint32_t xyz[3]) const { return (flags(xyz) & 2) != 0; }
+    bool isUnknown(const uint32_t xyz[3]) const { return (flags(xyz) & 4) != 0; }
+    double getProbability(const uint32_t xyz[3]) const { double p = 0; uint8_t f = 0; check(lama_om3_query(h_, xyz, 1, &p, &f)); return p; }
+    void prune() { check(lama_om3_prune(h_)); }
+    bool write(const std::string& path) const { check(lama_om3_write(h_, path.c_str())); return true; }
+    bool read(const std::string& path) { check(lama_om3_read(h_, path.c_str())); return true; }
+
+private:
+    bool set(const uint32_t xyz[3], uint8_t op) { uint8_t c = 0; check(lama_om3_apply(h_, xyz, &op, 1, &c)); return c != 0; }
+    uint8_t flags(const uint32_t xyz[3]) const { double p = 0; uint8_t f = 0; check(lama_om3_query(h_, xyz, 1, &p, &f)); return f; }
+    lama_om3* h_ = nullptr;
+};
+
 }  // namespace lama_b200_shim

@@ -89,6 +89,8 @@ EXPORTED_SYMBOLS = [
     "lama_om_export", "lama_om_write", "lama_om_export_image", "lama_om_kernel_times",
     "lama_tsdm_create", "lama_tsdm_destroy", "lama_tsdm_set_max_distance", "lama_tsdm_max_distance", "lama_tsdm_insert_point_clouds",
     "lama_tsdm_distance", "lama_tsdm_bounds", "lama_tsdm_export", "lama_tsdm_to_mesh", "lama_tsdm_write_ply", "lama_tsdm_kernel_times",
+    "lama_om3_create", "lama_om3_destroy", "lama_om3_insert_point_clouds", "lama_om3_apply", "lama_om3_query", "lama_om3_prune",
+    "lama_om3_bounds", "lama_om3_export", "lama_om3_write", "lama_om3_read", "lama_om3_export_image", "lama_om3_kernel_times", "lama_w2m3",
 ]
 
 
@@ -170,6 +172,15 @@ def w2m(resolution, pts):
     n = p.size // 3
     out = np.zeros((n, 2), np.uint32)
     _chk(lib().lama_w2m(C.c_double(resolution), pp, C.c_int(n), _vp(out)))
+    return out
+
+
+def w2m3(resolution, pts):
+    """Map::w2m (map.h:125-126) on all three axes: world points (n, 3) -> cells (n, 3)"""
+    p, pp = _d(pts)
+    n = p.size // 3
+    out = np.zeros((n, 3), np.uint32)
+    _chk(lib().lama_w2m3(C.c_double(resolution), pp, C.c_int(n), _vp(out)))
     return out
 
 
@@ -918,6 +929,130 @@ class TruncatedSignedDistanceMap:
         ms, ln = np.zeros(3), np.zeros(3, np.uint64)
         _chk(lib().lama_tsdm_kernel_times(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
         keys = ("insert", "distance", "mesh")
+        return dict(zip(keys, ms.tolist())), dict(zip(keys, ln.tolist()))
+
+
+class OccupancyMap3D:
+    """Device-resident lama::FrequencyOccupancyMap (kind="frequency") or lama::ProbabilisticOccupancyMap (kind="logodds") with
+    is3d = true (include/lama/sdm/*_occupancy_map.h).  `window` = patches per axis (None: 8 x 8 x 4), centred on `center`.
+
+    Cells are (n, 3) integer map coordinates; floating-point arrays are world points and go through Map::w2m (w2m3), as the
+    reference's Vector3d overloads do."""
+
+    KINDS = {"frequency": 0, "logodds": 1}
+    SET_FREE, SET_OCCUPIED, SET_UNKNOWN = 0, 1, 2
+
+    def __init__(self, resolution, kind="frequency", patch_size=32, center=(0.0, 0.0, 0.0), window=None, **dev):
+        d = DeviceOptions(device=0, dir_dim=64, pool_slots=0, max_beams=2048, timing=0, stream=0)
+        for k, v in dev.items():
+            setattr(d, k, v)
+        c, cp = _d(center)
+        win = None if window is None else (C.c_int32 * 3)(*[int(x) for x in window])
+        self.kind = kind
+        self.resolution = float(resolution)
+        self.h = C.c_void_p()
+        _chk(lib().lama_om3_create(C.c_double(resolution), C.c_uint32(patch_size), C.c_int(self.KINDS[kind]), cp, win, C.byref(d), C.byref(self.h)))
+
+    def __del__(self):
+        if getattr(self, "h", None) and _lib is not None:
+            _lib.lama_om3_destroy(self.h)
+            self.h = None
+
+    def _cells(self, cells):
+        a = np.asarray(cells)
+        if np.issubdtype(a.dtype, np.floating):
+            return np.ascontiguousarray(w2m3(self.resolution, a.reshape(-1, 3)))
+        return np.ascontiguousarray(a, np.uint32).reshape(-1, 3)
+
+    def insertPointClouds(self, clouds, origins=None, quats=None, full=True) -> int:
+        """generateOccupancyMap's loop body (graph_slam2d.cpp:146-158) for every point of every (n_k, 3) cloud in order: setOccupied
+        of the hit and, with full, setFree along the ray from the sensor origin.  origins (S, 3) / quats (S, 4) xyzw world sensor poses
+        or None (zero / identity).  Returns the number of cell updates."""
+        p, offsets = _clouds(clouds)
+        o = None if origins is None else np.ascontiguousarray(origins, np.float64).reshape(-1, 3)
+        q = None if quats is None else np.ascontiguousarray(quats, np.float64).reshape(-1, 4)
+        n = C.c_uint64(0)
+        _chk(lib().lama_om3_insert_point_clouds(self.h, _vp(p), offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int(len(offsets) - 1), _vp(o), _vp(q),
+                                                C.c_int(1 if full else 0), C.byref(n)))
+        return n.value
+
+    def apply(self, cells, ops):
+        """the setters in list order: ops (n,) of SET_FREE / SET_OCCUPIED / SET_UNKNOWN.  Returns what each call returns, (n,) bool."""
+        c = self._cells(cells)
+        o = np.ascontiguousarray(np.broadcast_to(np.asarray(ops, np.uint8), (len(c),)))
+        changed = np.zeros(len(c), np.uint8)
+        _chk(lib().lama_om3_apply(self.h, _vp(c), _vp(o), C.c_int(len(c)), _vp(changed)))
+        return changed.astype(bool)
+
+    def setFree(self, cells):
+        return self.apply(cells, self.SET_FREE)
+
+    def setOccupied(self, cells):
+        return self.apply(cells, self.SET_OCCUPIED)
+
+    def setUnknown(self, cells):
+        return self.apply(cells, self.SET_UNKNOWN)
+
+    def query(self, cells):
+        """(getProbability (n,), flags (n,) bit 0 isFree / bit 1 isOccupied / bit 2 isUnknown)"""
+        c = self._cells(cells)
+        prob, flags = np.zeros(len(c)), np.zeros(len(c), np.uint8)
+        _chk(lib().lama_om3_query(self.h, _vp(c), C.c_int(len(c)), prob.ctypes.data_as(c_dp), _vp(flags)))
+        return prob, flags
+
+    def getProbability(self, cells):
+        return self.query(cells)[0]
+
+    def isFree(self, cells):
+        return (self.query(cells)[1] & 1) != 0
+
+    def isOccupied(self, cells):
+        return (self.query(cells)[1] & 2) != 0
+
+    def isUnknown(self, cells):
+        return (self.query(cells)[1] & 4) != 0
+
+    def prune(self):
+        """FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158)"""
+        _chk(lib().lama_om3_prune(self.h))
+
+    def bounds(self):
+        """(allocated patches, min cell (3,), max cell (3,)) as Map::bounds"""
+        mn, mx, n = np.zeros(3, np.uint32), np.zeros(3, np.uint32), C.c_int(0)
+        _chk(lib().lama_om3_bounds(self.h, mn.ctypes.data_as(c_u32p), mx.ctypes.data_as(c_u32p), C.byref(n)))
+        return n.value, mn, mx
+
+    def export(self, lo, size):
+        """cells of the box lo + [0, size), shaped (size z, size y, size x): dict(occupied, visited, known) for a frequency map,
+        dict(prob (float32 log-odds), known) for a log-odds map, and `word`, the raw 32-bit cells"""
+        lo = np.ascontiguousarray(lo, np.uint32)
+        sz = np.ascontiguousarray(size, np.int32)
+        shape = (int(sz[2]), int(sz[1]), int(sz[0]))
+        w, k = np.zeros(shape, np.uint32), np.zeros(shape, np.uint8)
+        _chk(lib().lama_om3_export(self.h, _vp(lo), _vp(sz), _vp(w), _vp(k)))
+        if self.kind == "frequency":
+            return dict(word=w, occupied=(w & 0xFFFF).astype(np.uint16), visited=(w >> 16).astype(np.uint16), known=k)
+        return dict(word=w, prob=w.view(np.float32), known=k)
+
+    def write(self, path):
+        """Map::write (map.cpp:490-529): a 3-D .sdm file"""
+        _chk(lib().lama_om3_write(self.h, str(path).encode()))
+
+    def read(self, path):
+        """Map::read (map.cpp:531-575) into this (empty) map"""
+        _chk(lib().lama_om3_read(self.h, str(path).encode()))
+
+    def exportImage(self, zed=0.0):
+        """the z-slice image of sdm::export_to_png(occ, file, zed) (export.cpp:46-72), (height, width) uint8"""
+        return _image(lib().lama_om3_export_image, (self.h, C.c_double(zed)))
+
+    def saveImage(self, path, zed=0.0):
+        write_png(path, self.exportImage(zed))
+
+    def kernelTimes(self):
+        ms, ln = np.zeros(3), np.zeros(3, np.uint64)
+        _chk(lib().lama_om3_kernel_times(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
+        keys = ("insert", "apply", "query")
         return dict(zip(keys, ms.tolist())), dict(zip(keys, ln.tolist()))
 
 

@@ -15,6 +15,7 @@
 #include "shard_comm.h"
 #include "pgo.h"
 #include "tsdm.h"
+#include "om3d.h"
 
 #include "../../include/lama_b200.h"
 
@@ -1593,6 +1594,123 @@ int lama_tsdm_kernel_times(lama_tsdm* h, double ms[3], uint64_t launches[3])
 try {
     if (!h) return set_err("null handle", LAMA_ERR_ARG);
     h->t->kernel_times(ms, launches);
+    return LAMA_OK;
+}
+LAMA_CATCH
+
+// ---- 3-D occupancy maps (include/lama/sdm/frequency_occupancy_map.h, probabilistic_occupancy_map.h with is3d) ----------------------
+struct lama_om3 { OccMap3Dev* m; };
+// FrequencyOccupancyMap / ProbabilisticOccupancyMap(resolution, patch_size, true) (frequency_occupancy_map.cpp:47-49,
+// probabilistic_occupancy_map.cpp:48-60, map.cpp:42-48) on the device
+int lama_om3_create(double resolution, uint32_t patch_size, int kind, const double center_xyz[3], const int32_t window_patches[3],
+                    const lama_device_options* dev, lama_om3** out)
+try {
+    if (!out) return set_err("null argument", LAMA_ERR_ARG);
+    lama_device_options d;
+    if (dev) d = *dev; else dev_default(&d);
+    std::string err;
+    OccMap3Dev* m = OccMap3Dev::create(resolution, patch_size, kind, center_xyz, window_patches, dev_from(d), err);
+    if (!m) {
+        const bool bad_arg = !(resolution > 0) || patch_size != 32 || (kind != 0 && kind != 1) || err.find("window") != std::string::npos;
+        return set_err(err, !bad_arg && lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : (bad_arg ? LAMA_ERR_ARG : LAMA_ERR_CUDA));
+    }
+    *out = new lama_om3{m};
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_om3_destroy(lama_om3* h)
+try {
+    if (!h) return LAMA_OK;
+    delete h->m;
+    delete h;
+    return LAMA_OK;
+}
+LAMA_CATCH
+// the loop body of GraphSlam2D::generateOccupancyMap (graph_slam2d.cpp:146-158) over every point of every cloud
+int lama_om3_insert_point_clouds(lama_om3* h, const double* pts_xyz, const int64_t* offsets, int n_clouds, const double* origins,
+                                 const double* quats_xyzw, int full, uint64_t* cells)
+try {
+    if (!h || (n_clouds > 0 && !offsets)) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->insert_point_clouds(pts_xyz, offsets, n_clouds, origins, quats_xyzw, full != 0, cells);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// setFree / setOccupied / setUnknown (frequency_occupancy_map.cpp:65-108, probabilistic_occupancy_map.cpp:82-123) in list order
+int lama_om3_apply(lama_om3* h, const uint32_t* cells_xyz, const uint8_t* ops, int n, uint8_t* changed)
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    int rc = h->m->apply(cells_xyz, ops, n, changed);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// getProbability / isFree / isOccupied / isUnknown (frequency_occupancy_map.cpp:110-172, probabilistic_occupancy_map.cpp:125-175)
+int lama_om3_query(lama_om3* h, const uint32_t* cells_xyz, int n, double* prob, uint8_t* flags)
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    int rc = h->m->query(cells_xyz, n, prob, flags);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158)
+int lama_om3_prune(lama_om3* h)
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    int rc = h->m->prune();
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// Map::bounds (map.cpp:139-157)
+int lama_om3_bounds(lama_om3* h, uint32_t mn[3], uint32_t mx[3], int* patches)
+try {
+    if (!h || !mn || !mx) return set_err("null argument", LAMA_ERR_ARG);
+    return h->m->bounds(mn, mx, patches);
+}
+LAMA_CATCH
+// the cells of a box, as Map::get (map.cpp:414-455) reads them
+int lama_om3_export(lama_om3* h, const uint32_t lo[3], const int32_t size[3], uint32_t* cells, uint8_t* known)
+try {
+    if (!h || !lo || !size) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->export_box(lo, size, cells, known);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// Map::write (map.cpp:490-529)
+int lama_om3_write(lama_om3* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->write(path);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// Map::read (map.cpp:531-575)
+int lama_om3_read(lama_om3* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->read(path);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// sdm::export_to_png(occ, file, zed) (export.cpp:46-72,98-103): the grey image
+int lama_om3_export_image(lama_om3* h, double zed, uint8_t* pixels, size_t cap, int dims[2])
+try {
+    if (!h || !dims) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->export_image(zed, pixels, cap, dims);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+int lama_om3_kernel_times(lama_om3* h, double ms[3], uint64_t launches[3])
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    h->m->kernel_times(ms, launches);
+    return LAMA_OK;
+}
+LAMA_CATCH
+// Map::w2m (map.h:125-126), all three axes
+int lama_w2m3(double resolution, const double* pts_xyz, int n, uint32_t* cells_xyz)
+try {
+    if (!(resolution > 0) || n < 0 || (n > 0 && (!pts_xyz || !cells_xyz))) return set_err("bad argument", LAMA_ERR_ARG);
+    const double scale = 1.0 / resolution;
+    for (int i = 0; i < 3 * n; ++i) cells_xyz[i] = w2m(pts_xyz[i], scale);
     return LAMA_OK;
 }
 LAMA_CATCH

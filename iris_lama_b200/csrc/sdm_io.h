@@ -45,7 +45,8 @@ struct SdmFrequencyCell {  // frequency_occupancy_map.h:43-46
 #pragma pack(pop)
 static_assert(sizeof(SdmDistanceCell) == 10 && sizeof(SdmFrequencyCell) == 4, "cell layout");
 
-// A map as the file holds it: patches in file order, `cells` = num_patches * 1024 * cell_size bytes, 16 mask words per patch.
+// A map as the file holds it: patches in file order, `cells` = num_patches * volume * cell_size bytes, volume / 64 mask words per
+// patch; volume = 1024 cells, or 32 768 when header.is_3d.
 struct SdmFile {
     SdmHeader header{};
     std::vector<uint8_t> params;   // what writeParameters emitted
@@ -61,7 +62,8 @@ struct SdmWindow {
 };
 
 bool sdm_write(const std::string& path, const SdmFile& f, std::string& err);
-bool sdm_read(const std::string& path, uint32_t expect_cell_size, size_t n_params, SdmFile& f, std::string& err);
+// expect_3d: the file must hold a 3-D map (is_3d = 1, 32 x 32 x 32 patches); otherwise a 2-D one
+bool sdm_read(const std::string& path, uint32_t expect_cell_size, size_t n_params, SdmFile& f, std::string& err, bool expect_3d = false);
 
 // planes -> file: one patch per 32x32 block that holds a known cell (a reference patch always has one: Map::get marks
 // the touched cell, map.cpp:400-411)

@@ -3,6 +3,7 @@
 Layout (src/sdm/map.cpp:490-575): IOHeader (include/lama/sdm/map.h:95-103, 32 bytes with natural padding), the concrete
 map's parameters (DynamicDistanceMap: uint32 max_sqdist_, dynamic_distance_map.cpp:200-208; the occupancy maps: none), then
 per patch: uint64 id = (x >> 5) * 2642244 + (y >> 5) (map.h:153-161), 1024 cells, 16 uint64 mask words (container.cpp:143-176).
+3-D maps (is_3d = 1): id = ((x >> 5) * 2642244 + (y >> 5)) * 2642244 + (z >> 5), 32 768 cells, 512 mask words per patch.
 The files are written by lama_*_write_map / lama_dm_write (include/lama_b200.h) and by the reference's Map::write.
 """
 import numpy as np
@@ -23,7 +24,8 @@ CELL_TYPES = {
 
 
 def read_sdm(path, n_params=None):
-    """-> dict(header=..., params=bytes, patches={id: (cells[1024], mask[16])}); n_params defaults to 4 for 10-byte cells"""
+    """-> dict(header=..., params=bytes, patches={id: (cells[volume], mask[volume // 64])}); volume = 1024, or 32 768 in a 3-D
+    file; n_params defaults to 4 for 10-byte cells"""
     raw = np.fromfile(path, np.uint8)
     hdr = raw[:32].view(HEADER)[0]
     if hdr["magic"] != MAGIC or hdr["version"] != IO_VERSION:
@@ -31,7 +33,7 @@ def read_sdm(path, n_params=None):
     cs = int(hdr["cell_size"])
     if n_params is None:
         n_params = 4 if cs == 10 else 0
-    vol = int(hdr["patch_length"]) ** 2
+    vol = int(hdr["patch_length"]) ** (3 if hdr["is_3d"] else 2)
     rec = 8 + vol * cs + (vol // 64) * 8
     body = raw[32 + n_params:]
     n = int(hdr["num_patches"])
@@ -51,6 +53,12 @@ def export_to_ply(tsdm, filename):
     from . import api
     api._chk(api.lib().lama_tsdm_write_ply(tsdm.h, C.c_char_p(str(filename).encode())))
     return True
+
+
+def patch_origin3(pid, patch_length=32):
+    """Map::p2m (map.h:166-177) of a 3-D map: the absolute cell coordinates (x, y, z) of a patch's first cell"""
+    u = UNIVERSAL_CONSTANT
+    return (pid // (u * u)) * patch_length, ((pid % (u * u)) // u) * patch_length, (pid % u) * patch_length
 
 
 def patch_origin(pid, patch_length=32):
