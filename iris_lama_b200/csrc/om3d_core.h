@@ -9,7 +9,8 @@
 // the log-odds for a probabilistic map.  The two uint16 counters wrap independently, as the reference's do.
 #pragma once
 
-#include "tsdm_core.h"
+#include "patch_window.h"
+#include "ray_core.h"
 
 namespace lama_b200 {
 

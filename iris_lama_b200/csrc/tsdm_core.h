@@ -12,6 +12,7 @@
 
 #include "ray_core.h"
 #include "match_core.h"
+#include "patch_window.h"
 
 namespace lama_b200 {
 
@@ -98,28 +99,6 @@ LAMA_HD void tsdm_fold(float& cd, float& cw, float d, float w, float max_weight)
     const float sum = fadd_rn(cw, w);
     cd = fdiv_rn(fadd_rn(fmul_rn(cw, cd), fmul_rn(w, d)), sum);
     cw = max_weight < sum ? max_weight : sum;
-}
-
-// ---- directory window of the device store ----------------------------------------------------------------------------------
-// dim[0] x dim[1] x dim[2] patches from patch coordinates base (cell >> 5); dim[2] == 1 and z ignored in 2-D (MASK3D, map.h:182-189)
-struct TsdmWindow {
-    int32_t base[3];
-    int32_t dim[3];
-    int is3d;
-};
-// directory index (x fastest, then y, then z), or -1 outside the window
-LAMA_HD int tsdm_dir_index(const TsdmWindow& w, uint32_t x, uint32_t y, uint32_t z)
-{
-    const int px = (int)(x >> kPatchLog2) - w.base[0], py = (int)(y >> kPatchLog2) - w.base[1];
-    const int pz = w.is3d ? (int)(z >> kPatchLog2) - w.base[2] : 0;
-    if ((unsigned)px >= (unsigned)w.dim[0] || (unsigned)py >= (unsigned)w.dim[1] || (unsigned)pz >= (unsigned)w.dim[2]) return -1;
-    return (pz * w.dim[1] + py) * w.dim[0] + px;
-}
-// Map::m2c (map.h:182-189)
-LAMA_HD uint32_t tsdm_cell_index(uint32_t x, uint32_t y, uint32_t z, int is3d)
-{
-    const uint32_t m = kPatchLen - 1;
-    return (x & m) | ((y & m) << kPatchLog2) | (is3d ? (z & m) << (2 * kPatchLog2) : 0u);
 }
 
 // ---- queries ---------------------------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
 // tsdm_emu.cpp -- host build of the device fusion core (iris_lama_b200/csrc/tsdm_core.h): the same tsdm_ray / RayWalk3 /
-// tsdm_sample / tsdm_fold calls as k_tsdm_walk and k_tsdm_fold, run sequentially on a plain host store, for comparison with the
+// tsdm_sample / tsdm_fold calls as k_tsdm_walk and k_fold_runs, run sequentially on a plain host store, for comparison with the
 // oracle (tsdm_oracle.cpp).  TEST INFRASTRUCTURE ONLY: compiled by tests/tsdm_oracle.py, -ffp-contract=off.
 #include "../../iris_lama_b200/csrc/mc_table.h"
 #include "../../iris_lama_b200/csrc/tsdm_core.h"
