@@ -492,6 +492,27 @@ int lama_om3_kernel_times(lama_om3* h, double ms[3], uint64_t launches[3]);
 /* Map::w2m (map.h:125-126) on all three axes: world points (n x 3) -> cells (n x 3) */
 int lama_w2m3(double resolution, const double* pts_xyz, int n, uint32_t* cells_xyz);
 
+/* ------------------------------------------------------------------------------------------------
+ * Checkpoints (no counterpart in the reference): save a PFSlam2D or Slam2D session to a file and continue it later, in another
+ * process or on another device, bit for bit as if it had not stopped.  The file holds the options, the front end's state (poses,
+ * weights, trajectories, the mt19937 state, counters, the Summary buckets) and the device maps with their copy-on-write sharing;
+ * DESIGN.md section 13 gives the layout.  Saving settles the pending map update first and does not change the handle.  Kernel times,
+ * traffic counters and staged scans start empty on a loaded handle (lama_pf_update_staged needs a new lama_pf_stage_scans).
+ * Loading checks the whole file (size, checksum, version, kind, every count, directory entry and reference count) before it touches
+ * CUDA: a bad file gives LAMA_ERR_ARG and no handle; a valid file on a host without a device gives LAMA_ERR_NO_DEVICE.
+ * From `dev` (may be NULL: device 0) only device, stream and timing are taken; dir_dim, pool_slots and max_beams must be 0 or the
+ * saved values.  A sharded PFSlam2D (shard_count > 1) cannot be saved (LAMA_ERR_STATE).  A LidarOdometry2D-mode Slam2D loads back in
+ * that mode; the inner Slam2D of a lama_graph (lama_graph_slam) can be saved and loads back as a standalone Slam2D.
+ * ------------------------------------------------------------------------------------------------ */
+int lama_pf_save_state(lama_pf* h, const char* path);
+int lama_pf_load_state(const char* path, const lama_device_options* dev, lama_pf** out);
+int lama_slam_save_state(lama_slam* h, const char* path);
+int lama_slam_load_state(const char* path, const lama_device_options* dev, lama_slam** out);
+/* what the last save or load on this thread took and moved.  ms = {count, compaction, gather (device, CUDA events; save only), slot
+ * copy (chunked through pinned buffers), engine creation, tables (directories, reference counts, free stack; load only), encode
+ * (serialisation / parsing, checks and checksum), file I/O, total}; sizes = {slots in use, per-particle patch references, file bytes} */
+int lama_checkpoint_last_stats(double ms[9], uint64_t sizes[3]);
+
 #ifdef __cplusplus
 }
 #endif

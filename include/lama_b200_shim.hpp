@@ -85,8 +85,18 @@ public:
         return img;
     }
     lama_pf* handle() const { return h_; }
+    // checkpoints (no counterpart in the reference): the whole session to a file, and a filter that continues it bit for bit
+    void saveState(const std::string& path) const { check(lama_pf_save_state(h_, path.c_str())); }
+    static std::unique_ptr<PFSlam2D> loadState(const std::string& path, int device = 0)
+    {
+        lama_device_options dev = {device, 0, 0, 0, 0, 0};
+        lama_pf* h = nullptr;
+        check(lama_pf_load_state(path.c_str(), &dev, &h));
+        return std::unique_ptr<PFSlam2D>(new PFSlam2D(h));
+    }
 
 private:
+    explicit PFSlam2D(lama_pf* h) : h_(h) {}
     lama_pf* h_ = nullptr;
 };
 
@@ -114,8 +124,18 @@ public:
     uint32_t getNumberOfProcessedCells() const { uint32_t n = 0; check(lama_slam_get_processed_cells(h_, &n)); return n; }
     void writeMap(int kind, const std::string& path) const { check(lama_slam_write_map(h_, kind, path.c_str())); }
     lama_slam* handle() const { return h_; }
+    // checkpoints (no counterpart in the reference), as PFSlam2D::saveState / loadState
+    void saveState(const std::string& path) const { check(lama_slam_save_state(h_, path.c_str())); }
+    static std::unique_ptr<Slam2D> loadState(const std::string& path, int device = 0)
+    {
+        lama_device_options dev = {device, 0, 0, 0, 0, 0};
+        lama_slam* h = nullptr;
+        check(lama_slam_load_state(path.c_str(), &dev, &h));
+        return std::unique_ptr<Slam2D>(new Slam2D(h));
+    }
 
 protected:
+    explicit Slam2D(lama_slam* h) : h_(h) {}
     lama_slam* h_ = nullptr;
 };
 

@@ -91,6 +91,7 @@ EXPORTED_SYMBOLS = [
     "lama_tsdm_distance", "lama_tsdm_bounds", "lama_tsdm_export", "lama_tsdm_to_mesh", "lama_tsdm_write_ply", "lama_tsdm_kernel_times",
     "lama_om3_create", "lama_om3_destroy", "lama_om3_insert_point_clouds", "lama_om3_apply", "lama_om3_query", "lama_om3_prune",
     "lama_om3_bounds", "lama_om3_export", "lama_om3_write", "lama_om3_read", "lama_om3_export_image", "lama_om3_kernel_times", "lama_w2m3",
+    "lama_pf_save_state", "lama_pf_load_state", "lama_slam_save_state", "lama_slam_load_state", "lama_checkpoint_last_stats",
 ]
 
 
@@ -304,6 +305,38 @@ def shard_unique_id() -> bytes:
     buf = (C.c_uint8 * 128)()
     _chk(lib().lama_shard_unique_id(buf))
     return bytes(buf)
+
+
+# ---- checkpoints ------------------------------------------------------------------------------------------------
+CKPT_PFSLAM2D, CKPT_SLAM2D, CKPT_LIDAR_ODOMETRY2D = 1, 2, 3   # handle kind in the checkpoint header (u32 at byte 12)
+
+
+def checkpoint_kind(path) -> tuple:
+    """(handle kind, first options word) of a checkpoint file's header -- the particle count of a PFSlam2D checkpoint.  Only the header is
+    read here; loading checks the whole file."""
+    with open(path, "rb") as f:
+        head = f.read(36)
+    if len(head) < 36 or head[:8] != b"LAMACKPT":
+        raise LamaError(-1, f"{path} is not a checkpoint")
+    return int.from_bytes(head[12:16], "little"), int.from_bytes(head[32:36], "little")
+
+
+def _load_state(fn, path, device, stream, timing):
+    d = DeviceOptions(device=device, dir_dim=0, pool_slots=0, max_beams=0, timing=int(timing), stream=stream)
+    h = C.c_void_p()
+    _chk(fn(str(path).encode(), C.byref(d), C.byref(h)))
+    return h
+
+
+def checkpoint_stats():
+    """what the last saveState / loadState on this thread took: dict of ms and sizes (lama_checkpoint_last_stats)"""
+    ms = np.zeros(9)
+    sz = np.zeros(3, np.uint64)
+    _chk(lib().lama_checkpoint_last_stats(ms.ctypes.data_as(c_dp), _vp(sz)))
+    keys = ("count_ms", "compact_ms", "gather_ms", "copy_ms", "create_ms", "tables_ms", "encode_ms", "io_ms", "total_ms")
+    out = dict(zip(keys, ms.tolist()))
+    out.update(used_slots=int(sz[0]), references=int(sz[1]), file_bytes=int(sz[2]))
+    return out
 
 
 class PFSlam2D:
@@ -523,6 +556,22 @@ class PFSlam2D:
         buf = np.ascontiguousarray(buf, np.uint8)
         _chk(lib().lama_pf_particle_unpack(self.h, C.c_int(slot), _vp(buf), C.c_size_t(buf.size)))
 
+    # ---- checkpoints -----------------------------------------------------------------------------------------
+    def saveState(self, path):
+        """writes the whole session (options, filter state, device maps) to `path`; the handle is not changed"""
+        _chk(lib().lama_pf_save_state(self.h, str(path).encode()))
+
+    @classmethod
+    def loadState(cls, path, device=0, stream=0, timing=False) -> "PFSlam2D":
+        """a PFSlam2D that continues the saved session bit for bit, on `device` / `stream`"""
+        h = _load_state(lib().lama_pf_load_state, path, device, stream, timing)
+        _, particles = checkpoint_kind(path)
+        self = cls.__new__(cls)
+        self.h = h
+        self.options = cls.Options(particles, device=device, stream=stream, timing=int(timing))
+        self.P = particles
+        return self
+
 
 class Slam2D:
     """lama::Slam2D (include/lama/slam2d.h:128-161)."""
@@ -638,6 +687,21 @@ class Slam2D:
 
     def saveOccImage(self, path):
         write_png(path, self.exportImage(0))
+
+    def saveState(self, path):
+        """writes the whole session (options, state, device maps) to `path`; the handle is not changed"""
+        _chk(lib().lama_slam_save_state(self.h, str(path).encode()))
+
+    @staticmethod
+    def loadState(path, device=0, stream=0, timing=False) -> "Slam2D":
+        """the saved Slam2D, continuing bit for bit; a LidarOdometry2D checkpoint comes back as a LidarOdometry2D"""
+        h = _load_state(lib().lama_slam_load_state, path, device, stream, timing)
+        kind, _ = checkpoint_kind(path)
+        lo = kind == CKPT_LIDAR_ODOMETRY2D
+        self = (LidarOdometry2D if lo else Slam2D).__new__(LidarOdometry2D if lo else Slam2D)
+        self.h = h
+        self.options = Slam2D.Options(lidar_odometry=int(lo), device=device, stream=stream, timing=int(timing))
+        return self
 
 
 class LidarOdometry2D(Slam2D):

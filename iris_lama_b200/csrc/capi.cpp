@@ -10,6 +10,7 @@
 
 // engine.h declares the status codes as an enum; the C header re-states them as macros, so the C++
 // headers must come first.
+#include "checkpoint.h"
 #include "frontend.h"
 #include "sdm_io.h"
 #include "shard_comm.h"
@@ -1711,6 +1712,70 @@ try {
     if (!(resolution > 0) || n < 0 || (n > 0 && (!pts_xyz || !cells_xyz))) return set_err("bad argument", LAMA_ERR_ARG);
     const double scale = 1.0 / resolution;
     for (int i = 0; i < 3 * n; ++i) cells_xyz[i] = w2m(pts_xyz[i], scale);
+    return LAMA_OK;
+}
+LAMA_CATCH
+
+// ---- checkpoints (no counterpart in the reference) -----------------------------------------------------------
+namespace {
+thread_local CheckpointStats g_ckpt;
+DeviceOptions load_dev(const lama_device_options* d)   // only device, stream and timing are taken; the geometry fields are checked
+{
+    DeviceOptions o;
+    o.device = d ? d->device : 0;
+    o.dir_dim = d ? d->dir_dim : 0;
+    o.pool_slots = d ? d->pool_slots : 0;
+    o.max_beams = d ? d->max_beams : 0;
+    o.timing = d ? d->timing : 0;
+    o.stream = d ? d->stream : 0;
+    return o;
+}
+}  // namespace
+int lama_pf_save_state(lama_pf* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    const int rc = h->p->save(path, &g_ckpt);
+    return rc == LAMA_OK ? rc : set_err(h->p->error(), rc);
+}
+LAMA_CATCH
+int lama_pf_load_state(const char* path, const lama_device_options* dev, lama_pf** out)
+try {
+    if (!path || !out) return set_err("null argument", LAMA_ERR_ARG);
+    *out = nullptr;
+    std::string err;
+    int rc = LAMA_OK;
+    PFSlam2D* p = PFSlam2D::load(path, load_dev(dev), err, &rc, &g_ckpt);
+    if (!p) return set_err(err, rc == LAMA_OK ? LAMA_ERR_ARG : rc);
+    *out = new lama_pf{p};
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_slam_save_state(lama_slam* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    const int rc = h->s->save(path, &g_ckpt);
+    return rc == LAMA_OK ? rc : set_err(h->s->error(), rc);
+}
+LAMA_CATCH
+int lama_slam_load_state(const char* path, const lama_device_options* dev, lama_slam** out)
+try {
+    if (!path || !out) return set_err("null argument", LAMA_ERR_ARG);
+    *out = nullptr;
+    std::string err;
+    int rc = LAMA_OK;
+    Slam2D* s = Slam2D::load(path, load_dev(dev), err, &rc, &g_ckpt);
+    if (!s) return set_err(err, rc == LAMA_OK ? LAMA_ERR_ARG : rc);
+    *out = new lama_slam{s};
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_checkpoint_last_stats(double ms[9], uint64_t sizes[3])
+try {
+    if (!ms || !sizes) return set_err("null argument", LAMA_ERR_ARG);
+    const CheckpointStats& s = g_ckpt;
+    const double v[9] = {s.dev.count_ms, s.dev.compact_ms, s.dev.gather_ms, s.dev.copy_ms, s.dev.create_ms, s.dev.tables_ms, s.encode_ms, s.io_ms, s.total_ms};
+    std::copy(v, v + 9, ms);
+    sizes[0] = s.used_slots; sizes[1] = s.references; sizes[2] = s.file_bytes;
     return LAMA_OK;
 }
 LAMA_CATCH

@@ -39,9 +39,7 @@ enum MapKind : int { kMapOcc = 0, kMapDm = 1, kMapScratch = 2 };
 //   kDirOwn   persistent: this particle is the ONLY owner of the slot (reference count verified to be 1), so the
 //             patch can be written in place without looking at the count.  Set on allocation, on copy-on-write
 //             detach and when a count of 1 is observed; cleared on every entry that k_copy_dirs shares.
-constexpr int32_t kDirSlotMask = 0x00FFFFFF;
-constexpr int32_t kDirHot      = 1 << 28;
-constexpr int32_t kDirOwn      = 1 << 29;
+// (kDirSlotMask, kDirHot and kDirOwn live in lama_core.h, where the host-side checkpoint reader checks entries too)
 
 __device__ __forceinline__ int32_t* dir_of(const StoreView& s, int set, int particle, int kind)
 {

@@ -2,8 +2,10 @@
 #include "engine.h"
 
 #include <algorithm>
+#include <chrono>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 
 #include "kernels.cuh"
 
@@ -1062,7 +1064,7 @@ int Engine::pack_device(int particle, DeviceBlob* out)
         int32_t* d_slots = (int32_t*)(base + out->bytes);                              // scratch behind the blob
         CU_TRY(cudaMemcpyAsync(base, entries.data(), n * 4, cudaMemcpyHostToDevice, d_->stream));
         CU_TRY(cudaMemcpyAsync(d_slots, slots.data(), n * 4, cudaMemcpyHostToDevice, d_->stream));
-        launch_gather_patches(d_->view, d_slots, (int)n, d_out, d_fb, d_->stream);
+        launch_gather_patches(d_->view, d_slots, (int)n, d_out, d_fb, nullptr, d_->stream);
         CU_TRY(cudaGetLastError());   // no synchronisation: `entries` / `slots` are pageable, the runtime has staged them when cudaMemcpyAsync returns
         times_.misc_launches += 1;
     }
@@ -1235,6 +1237,199 @@ int Engine::memory_usage(int kind, uint32_t cell_bytes, uint64_t* out)
         out[p] = (uint64_t)total;
     }
     return 0;
+}
+
+// ---- checkpoints --------------------------------------------------------------------------------------------------------------------
+constexpr size_t kCkptChunk = (size_t)8 << 20;   // bytes per pinned buffer of the chunked copies (two of them)
+
+namespace {
+struct PinnedPair {   // two pinned chunk buffers and their completion events, released on every exit path
+    char* buf[2] = {nullptr, nullptr};
+    cudaEvent_t done[2] = {nullptr, nullptr};
+    cudaError_t init()
+    {
+        for (int b = 0; b < 2; ++b) {
+            cudaError_t e = cudaMallocHost((void**)&buf[b], kCkptChunk);
+            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming);
+            if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+    }
+    ~PinnedPair()
+    {
+        for (int b = 0; b < 2; ++b) {
+            if (done[b]) cudaEventSynchronize(done[b]), cudaEventDestroy(done[b]);
+            if (buf[b]) cudaFreeHost(buf[b]);
+        }
+    }
+};
+struct DeviceAllocs {
+    std::vector<void*> p;
+    cudaError_t alloc(void** out, size_t bytes)
+    {
+        cudaError_t e = cudaMalloc(out, bytes ? bytes : 16);
+        if (e == cudaSuccess) p.push_back(*out);
+        return e;
+    }
+    ~DeviceAllocs() { for (void* q : p) cudaFree(q); }
+};
+double host_ms(std::chrono::steady_clock::time_point a) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count(); }
+}  // namespace
+
+int Engine::snapshot(EngineImage* out, CheckpointTimes* t)
+{
+    { int rc = settle(nullptr); if (rc != LAMA_OK) return rc; }
+    CU_TRY(cudaSetDevice(cfg_.device));
+    const StoreView& v = d_->view;
+    const size_t n_slots = (size_t)v.n_slots, n_dir = (size_t)cfg_.particles * v.n_kinds * cfg_.dir_dim * cfg_.dir_dim;
+    DeviceAllocs mem;
+    CkptScratch c{};
+    c.temp_bytes = ckpt_scan_temp_bytes(v.n_slots);
+    CU_TRY(mem.alloc((void**)&c.cnt, n_slots * 4));
+    CU_TRY(mem.alloc((void**)&c.used, n_slots * 4));
+    CU_TRY(mem.alloc((void**)&c.new_id, n_slots * 4));
+    CU_TRY(mem.alloc((void**)&c.list, n_slots * 4));
+    CU_TRY(mem.alloc((void**)&c.ref, n_slots * 4));
+    CU_TRY(mem.alloc((void**)&c.dirs, n_dir * 4));
+    CU_TRY(mem.alloc((void**)&c.bad, 16));
+    CU_TRY(mem.alloc(&c.temp, c.temp_bytes));
+    cudaEvent_t ev[4] = {};
+    struct Events { cudaEvent_t* e; ~Events() { for (int k = 0; k < 4; ++k) if (e[k]) cudaEventDestroy(e[k]); } } ev_guard{ev};
+    for (int k = 0; k < 4; ++k) CU_TRY(cudaEventCreate(&ev[k]));
+    CU_TRY(cudaMemsetAsync(c.cnt, 0, n_slots * 4, d_->stream));
+    CU_TRY(cudaMemsetAsync(c.bad, 0, 4, d_->stream));
+    CU_TRY(cudaEventRecord(ev[0], d_->stream));
+    launch_ckpt_compact(v, cur_set_, c, d_->stream, ev[1]);
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaEventRecord(ev[2], d_->stream));
+    uint32_t bad = 0;
+    int32_t last[2] = {0, 0};
+    CU_TRY(cudaMemcpyAsync(&bad, c.bad, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(&last[0], c.new_id + n_slots - 1, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(&last[1], c.used + n_slots - 1, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaStreamSynchronize(d_->stream));
+    times_.misc_launches += 6;
+    if (bad) return fail(bad & 1u ? "snapshot: a directory entry points outside the patch pool" : "snapshot: a patch's reference count differs from its directory references",
+                         LAMA_ERR_STATE);
+    const uint32_t K = (uint32_t)(last[0] + last[1]);
+
+    EngineImage& img = *out;
+    img.particles = cfg_.particles; img.dir_dim = cfg_.dir_dim; img.pool_slots = cfg_.pool_slots; img.max_beams = cfg_.max_beams;
+    img.occupancy_kind = cfg_.occupancy_kind; img.known_plane = cfg_.known_plane; img.resolution = cfg_.resolution; img.l2_max = cfg_.l2_max;
+    img.window = window_;
+    img.used = K;
+    const size_t stride = img.slot_stride(), bytes = (size_t)K * stride;
+    char* stage = nullptr;
+    CU_TRY(mem.alloc((void**)&stage, bytes));
+    uint32_t* cells = (uint32_t*)stage;
+    uint32_t* fb = (uint32_t*)(stage + (size_t)K * kPatchBytes);
+    uint32_t* kb = img.has_kbits() ? (uint32_t*)(stage + (size_t)K * (kPatchBytes + 128)) : nullptr;
+    launch_gather_patches(v, c.list, (int)K, cells, fb, kb, d_->stream);
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaEventRecord(ev[3], d_->stream));
+    if (K) times_.misc_launches += 1;
+    img.refcount.resize(K);
+    img.dirs.resize(n_dir);
+    uint64_t cnt[3];
+    CU_TRY(cudaMemcpyAsync(img.refcount.data(), c.ref, (size_t)K * 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(img.dirs.data(), c.dirs, n_dir * 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(cnt, v.counters, sizeof(cnt), cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaStreamSynchronize(d_->stream));
+    for (int k = 0; k < 3; ++k) img.counters[k] = cnt[k];
+
+    // copy-out of the slots through two pinned chunk buffers: chunk i lands while the host copies chunk i - 1 away
+    const auto t0 = std::chrono::steady_clock::now();
+    img.slot_store.resize(bytes);
+    img.slot_bytes = img.slot_store.data();
+    PinnedPair pin;
+    CU_TRY(pin.init());
+    const size_t n_chunks = (bytes + kCkptChunk - 1) / kCkptChunk;
+    for (size_t i = 0; i <= n_chunks; ++i) {
+        if (i < n_chunks) {
+            const size_t off = i * kCkptChunk, len = std::min(kCkptChunk, bytes - off);
+            CU_TRY(cudaMemcpyAsync(pin.buf[i & 1], stage + off, len, cudaMemcpyDeviceToHost, d_->stream));
+            CU_TRY(cudaEventRecord(pin.done[i & 1], d_->stream));
+        }
+        if (i > 0) {
+            const size_t j = i - 1, off = j * kCkptChunk, len = std::min(kCkptChunk, bytes - off);
+            CU_TRY(cudaEventSynchronize(pin.done[j & 1]));
+            std::memcpy(img.slot_store.data() + off, pin.buf[j & 1], len);
+        }
+    }
+    d2h_bytes_ += bytes + n_dir * 4 + (uint64_t)K * 4;
+    if (t) {
+        float a = 0, b = 0, g = 0;
+        CU_TRY(cudaEventElapsedTime(&a, ev[0], ev[1]));
+        CU_TRY(cudaEventElapsedTime(&b, ev[1], ev[2]));
+        CU_TRY(cudaEventElapsedTime(&g, ev[2], ev[3]));
+        t->count_ms = a; t->compact_ms = b; t->gather_ms = g;
+        t->copy_ms = host_ms(t0);
+    }
+    return LAMA_OK;
+}
+
+Engine* Engine::restore(const EngineImage& img, int device, uint64_t stream, std::string& err, CheckpointTimes* t)
+{
+    const auto t0 = std::chrono::steady_clock::now();
+    EngineConfig cfg;
+    cfg.device = device; cfg.particles = img.particles; cfg.resolution = img.resolution; cfg.l2_max = img.l2_max; cfg.dir_dim = img.dir_dim;
+    cfg.pool_slots = img.pool_slots; cfg.max_beams = img.max_beams; cfg.stream = stream; cfg.occupancy_kind = img.occupancy_kind;
+    cfg.known_plane = img.known_plane;
+    std::unique_ptr<Engine> e(create(cfg, err));
+    if (!e) return nullptr;
+    if (e->cfg_.pool_slots != img.pool_slots || img.used > (uint32_t)img.pool_slots) { err = "restore: pool size differs from the image"; return nullptr; }
+    const double create_ms = host_ms(t0);
+    // the saved window base, not one recomputed from a centre
+    e->window_ = img.window;
+    Impl* d = e->d_;
+    StoreView& v = d->view;
+    v.window = img.window;
+    const uint32_t K = img.used;
+    auto cu = [&](cudaError_t r, const char* what) {
+        if (r != cudaSuccess) err = std::string("restore: ") + what + ": " + cudaGetErrorString(r);
+        return r == cudaSuccess;
+    };
+    // k_init_store left every directory at -1, every count at 0 and the free stack as n_slots-1 .. 0 with slot 0 on top: the slots K ..
+    // n_slots-1 are its lowest n_slots - K entries, the lowest slot on top
+    const auto t1 = std::chrono::steady_clock::now();
+    const int32_t free_count = v.n_slots - (int32_t)K;
+    if (!cu(cudaMemcpyAsync(v.refcount, img.refcount.data(), (size_t)K * 4, cudaMemcpyHostToDevice, d->stream), "reference counts") ||
+        !cu(cudaMemcpyAsync(v.dirs, img.dirs.data(), img.dirs.size() * 4, cudaMemcpyHostToDevice, d->stream), "directories") ||
+        !cu(cudaMemcpyAsync(v.counters, img.counters, 3 * sizeof(uint64_t), cudaMemcpyHostToDevice, d->stream), "store counters") ||
+        !cu(cudaMemcpyAsync(v.free_count, &free_count, 4, cudaMemcpyHostToDevice, d->stream), "free stack") ||
+        !cu(cudaStreamSynchronize(d->stream), "synchronize"))
+        return nullptr;
+    const double tables_ms = host_ms(t1);
+    // the slots straight into pool slots 0 .. K-1 and the planes behind them, through two pinned chunk buffers
+    const auto t2 = std::chrono::steady_clock::now();
+    const size_t bytes = (size_t)K * img.slot_stride();
+    struct Region { char* dst; size_t len; } regions[3] = {{(char*)v.pool, (size_t)K * kPatchBytes}, {(char*)v.fbits, (size_t)K * 128},
+                                                          {img.has_kbits() ? (char*)v.kbits : nullptr, img.has_kbits() ? (size_t)K * 128 : 0}};
+    PinnedPair pin;
+    if (!cu(pin.init(), "pinned buffers")) return nullptr;
+    const size_t n_chunks = (bytes + kCkptChunk - 1) / kCkptChunk;
+    for (size_t i = 0; i < n_chunks; ++i) {
+        const size_t off = i * kCkptChunk, len = std::min(kCkptChunk, bytes - off);
+        if (i >= 2 && !cu(cudaEventSynchronize(pin.done[i & 1]), "copy")) return nullptr;   // chunk i - 2 has left this buffer
+        std::memcpy(pin.buf[i & 1], img.slot_bytes + off, len);
+        size_t base = 0;
+        for (const Region& r : regions) {   // the chunk may straddle the cells and the planes
+            const size_t lo = std::max(off, base), hi = std::min(off + len, base + r.len);
+            if (lo < hi && !cu(cudaMemcpyAsync(r.dst + (lo - base), pin.buf[i & 1] + (lo - off), hi - lo, cudaMemcpyHostToDevice, d->stream), "copy"))
+                return nullptr;
+            base += r.len;
+        }
+        if (!cu(cudaEventRecord(pin.done[i & 1], d->stream), "copy")) return nullptr;
+    }
+    if (!cu(cudaStreamSynchronize(d->stream), "synchronize")) return nullptr;
+    e->h2d_bytes_ = 0;
+    e->settled_counters_[0] = img.counters[0]; e->settled_counters_[1] = img.counters[1]; e->settled_counters_[2] = img.counters[2];
+    e->settled_counters_[3] = (uint64_t)free_count;
+    if (t) {
+        *t = CheckpointTimes();
+        t->create_ms = create_ms; t->tables_ms = tables_ms; t->copy_ms = host_ms(t2);
+    }
+    return e.release();
 }
 
 }  // namespace lama_b200

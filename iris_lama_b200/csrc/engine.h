@@ -39,6 +39,32 @@ struct HostMapStats {
     uint32_t ray_cells, log_records, events, dm_pops;
 };
 
+// The device state of an engine in a self-contained form (checkpoint.h writes and reads it).  The K slots in use are renumbered
+// 0 .. K-1 in ascending order of their old slot; directory entries keep their flag bits.
+struct EngineImage {
+    int particles = 1, dir_dim = 64, pool_slots = 0, max_beams = 2048, occupancy_kind = 0;
+    bool known_plane = false;
+    double resolution = 0.05, l2_max = 0.5;
+    DirWindow window{};
+    uint64_t counters[3] = {0, 0, 0};      // patches allocated, detached, freed
+    uint32_t used = 0;                     // K
+    std::vector<int32_t> refcount;         // [K]
+    std::vector<int32_t> dirs;             // [particles][n_kinds][dir_dim^2] of the current set
+    // K x 4 KiB of cells, then K x 128 B of obstacle-mirror bits, then (known plane) K x 128 B of known bits
+    const uint8_t* slot_bytes = nullptr;
+    std::vector<uint8_t> slot_store;       // owns slot_bytes after a snapshot
+    int n_kinds() const { return occupancy_kind == 1 ? 3 : 2; }
+    bool has_kbits() const { return occupancy_kind == 1 || known_plane; }
+    size_t slot_stride() const { return (size_t)kPatchBytes + 128 + (has_kbits() ? 128 : 0); }
+};
+
+// where the time of a snapshot / restore went (ms).  Snapshot: count, compaction, gather = CUDA events; copy = host clock of the chunked
+// device -> host copy.  Restore: create = engine creation, tables = directories, reference counts, free stack and counters; copy = the
+// chunked host -> device copy of the slots.
+struct CheckpointTimes {
+    double count_ms = 0, compact_ms = 0, gather_ms = 0, copy_ms = 0, create_ms = 0, tables_ms = 0;
+};
+
 struct KernelTimes {  // accumulated CUDA-event durations (ms) and launch counts since reset
     double match_ms = 0, raycast_ms = 0, brushfire_ms = 0, resample_ms = 0;
     uint64_t match_launches = 0, raycast_launches = 0, brushfire_launches = 0, resample_launches = 0, misc_launches = 0;
@@ -146,6 +172,14 @@ public:
     // Map::memory() (src/sdm/map.cpp:115-125) of one map kind of every particle: per patch 72 bytes of table entry (key, COWPtr = shared_ptr + mutex, pointer)
     // plus the container's cell bytes divided by its use count; out[particle] truncated to an integer like the reference's return value
     int memory_usage(int kind, uint32_t cell_bytes, uint64_t* out);
+
+    // Checkpoints.  snapshot() settles, checks that every slot's reference count equals its directory references (LAMA_ERR_STATE when
+    // not), and copies the slots in use, renumbered, with the directories of the current set into `out`; the engine is not changed.
+    // restore() creates an engine with the image's geometry and window on `device` / `stream`: the K slots become 0 .. K-1, the
+    // directories set 0, the free stack holds K .. n_slots-1 with the lowest on top (as a fresh engine).  The image must be valid
+    // (checkpoint.h checks it).
+    int snapshot(EngineImage* out, CheckpointTimes* t = nullptr);
+    static Engine* restore(const EngineImage& img, int device, uint64_t stream, std::string& err, CheckpointTimes* t = nullptr);
 
     // sticky device error bits (lama_core.h) -- reads the device word; 0 = ok
     uint32_t device_status();

@@ -1,5 +1,6 @@
 // frontend.cpp -- host orchestration of PFSlam2D / Slam2D / Loc2D over the device Engine.
 #include "frontend.h"
+#include "checkpoint.h"
 #include "rng_skip.h"
 
 #include <cuda_runtime.h>
@@ -11,6 +12,7 @@
 #include <cmath>
 #include <cstring>
 #include <limits>
+#include <sstream>
 #include <unordered_set>
 
 namespace lama_b200 {
@@ -1534,6 +1536,303 @@ void unpack_distance_words(const uint32_t* words, const uint8_t* occ_known, size
         if (oy) oy[i] = (int16_t)dm_oy(w);
         if (queued) queued[i] = (w & kDmQueued) ? 1 : 0;
     }
+}
+
+// =====================================================================================================
+// Checkpoints (format: checkpoint.h, DESIGN.md §13)
+// =====================================================================================================
+namespace {
+using clk = std::chrono::steady_clock;
+double ms_since(clk::time_point a) { return std::chrono::duration<double, std::milli>(clk::now() - a).count(); }
+
+void put_counters(CkptWriter& w, const Counters& c)
+{
+    w.u64(c.evals); w.u64(c.ray_cells); w.u64(c.dm_pops); w.u64(c.detached); w.u64(c.gn_iters); w.u64(c.resampled);
+}
+Counters get_counters(CkptReader& r)
+{
+    Counters c;
+    c.evals = r.u64("counters"); c.ray_cells = r.u64("counters"); c.dm_pops = r.u64("counters");
+    c.detached = r.u64("counters"); c.gn_iters = r.u64("counters"); c.resampled = r.u64("counters");
+    return c;
+}
+void put_geometry(CkptWriter& w, const DeviceOptions& d) { w.i32(d.dir_dim); w.i32(d.pool_slots); w.i32(d.max_beams); }
+void get_geometry(CkptReader& r, DeviceOptions& d) { d.dir_dim = r.i32("dir_dim"); d.pool_slots = r.i32("pool_slots"); d.max_beams = r.i32("max_beams"); }
+// the caller's dir_dim / pool_slots / max_beams: 0, or the file's (its options, or the engine it holds)
+bool geometry_matches(const DeviceOptions& call, const DeviceOptions& file, const EngineImage* img, std::string& err)
+{
+    auto ok = [](int v, int opt, int eng) { return v == 0 || v == opt || v == eng; };
+    if (ok(call.dir_dim, file.dir_dim, img ? img->dir_dim : file.dir_dim) && ok(call.pool_slots, file.pool_slots, img ? img->pool_slots : file.pool_slots) &&
+        ok(call.max_beams, file.max_beams, img ? img->max_beams : file.max_beams))
+        return true;
+    err = "device options differ from the checkpoint's geometry (dir_dim, pool_slots and max_beams must be 0 or the saved values)";
+    return false;
+}
+bool finite_se2(const SE2& s) { return std::isfinite(s.c) && std::isfinite(s.s) && std::isfinite(s.tx) && std::isfinite(s.ty); }
+uint64_t sum_refs(const EngineImage& img)
+{
+    uint64_t n = 0;
+    for (int32_t v : img.refcount) n += (uint64_t)v;
+    return n;
+}
+}  // namespace
+
+int PFSlam2D::save(const std::string& path, CheckpointStats* st)
+{
+    const auto t0 = clk::now();
+    CheckpointStats local;
+    CheckpointStats& s = st ? *st : local;
+    s = CheckpointStats();
+    if (opt_.shard_count > 1) return fail("saveState: a sharded handle cannot be saved (each rank holds only its part of the filter)", LAMA_ERR_STATE);
+    EngineImage img;
+    if (eng_) {
+        int rc = settle_counters();   // the pending map update and its counters, as the getters would book them
+        if (rc != LAMA_OK) return rc;
+        rc = eng_->snapshot(&img, &s.dev);
+        if (rc != LAMA_OK) return engine_fail(rc);
+    }
+    const auto t1 = clk::now();
+    CkptWriter w;
+    // options
+    w.u32(opt_.particles);
+    for (double v : {opt_.srr, opt_.str, opt_.stt, opt_.srt, opt_.meas_sigma, opt_.meas_sigma_gain, opt_.trans_thresh, opt_.rot_thresh, opt_.l2_max,
+                     opt_.truncated_ray, opt_.truncated_range, opt_.resolution})
+        w.f64(v);
+    w.u32(opt_.patch_size); w.u32(opt_.max_iter); w.i32(opt_.strategy); w.i32(opt_.threads); w.u32(opt_.seed);
+    put_geometry(w, opt_.dev);
+    // front-end state
+    w.se2(prior_); w.se2(odom_); w.u8(has_first_);
+    w.f64(acc_trans_); w.f64(acc_rot_); w.f64(neff_);
+    for (uint32_t i = 0; i < P_; ++i) w.se2(pose_[i]);
+    for (const std::vector<double>* v : {&weight_, &nweight_, &wsum_}) w.bytes(v->data(), (size_t)P_ * 8);
+    w.u32((uint32_t)last_idx_.size());
+    w.bytes(last_idx_.data(), last_idx_.size() * 4);
+    w.u64(resample_count_); w.u64(resample_hash_); w.u64(scans_seen_);
+    w.u32((uint32_t)timestamps_.size());
+    w.bytes(timestamps_.data(), timestamps_.size() * 8);
+    put_counters(w, last_); put_counters(w, total_);
+    w.u64(detached_seen_);
+    w.f64(t_sample_); w.f64(t_solve_); w.f64(t_norm_); w.f64(t_resample_);
+    // the trajectory nodes reachable from the particles, renumbered in their old order (a parent precedes its children)
+    std::vector<int> renum(nodes_.size(), -1);
+    for (uint32_t i = 0; i < P_; ++i)
+        for (int n = node_of_[i]; n >= 0 && renum[(size_t)n] < 0; n = nodes_[(size_t)n].parent) renum[(size_t)n] = 0;
+    uint32_t kept = 0;
+    for (int& v : renum)
+        if (v == 0) v = (int)kept++;
+    w.u32(kept);
+    for (size_t n = 0; n < nodes_.size(); ++n)
+        if (renum[n] >= 0) {
+            w.se2(nodes_[n].pose);
+            w.i32(nodes_[n].parent < 0 ? -1 : renum[(size_t)nodes_[n].parent]);
+        }
+    for (uint32_t i = 0; i < P_; ++i) w.i32(node_of_[i] < 0 ? -1 : renum[(size_t)node_of_[i]]);
+    std::ostringstream rng;
+    rng << gen_;
+    w.str(rng.str());
+    ckpt_put_engine(w, eng_ ? &img : nullptr);
+    s.encode_ms = ms_since(t1);
+    std::string err;
+    const int rc = ckpt_write_file(path, kCkptPFSlam2D, w, img.slot_bytes, (size_t)img.used * img.slot_stride(), err, &s);
+    if (rc != LAMA_OK) return fail(err, rc);
+    s.used_slots = img.used;
+    s.references = sum_refs(img);
+    s.total_ms   = ms_since(t0);
+    return LAMA_OK;
+}
+
+PFSlam2D* PFSlam2D::load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st)
+{
+    const auto t0 = clk::now();
+    CheckpointStats local;
+    CheckpointStats& s = st ? *st : local;
+    s = CheckpointStats();
+    std::vector<uint8_t> file;
+    uint32_t kind = 0;
+    *code = ckpt_read_file(path, file, &kind, err, &s);
+    if (*code != LAMA_OK) return nullptr;
+    *code = LAMA_ERR_ARG;
+    if (kind != kCkptPFSlam2D) {
+        err = kind == kCkptSlam2D || kind == kCkptLidarOdometry2D ? "the checkpoint holds a Slam2D, not a PFSlam2D" : "unknown checkpoint handle kind";
+        return nullptr;
+    }
+    const auto t1 = clk::now();
+    CkptReader r(file.data() + kCkptHeaderBytes, file.size() - kCkptHeaderBytes);
+    PFOptions o;
+    o.particles = r.u32("options");
+    double* f[] = {&o.srr, &o.str, &o.stt, &o.srt, &o.meas_sigma, &o.meas_sigma_gain, &o.trans_thresh, &o.rot_thresh, &o.l2_max, &o.truncated_ray,
+                   &o.truncated_range, &o.resolution};
+    for (double* v : f) *v = r.f64("options");
+    o.patch_size = r.u32("options"); o.max_iter = r.u32("options"); o.strategy = r.i32("options"); o.threads = r.i32("options"); o.seed = r.u32("options");
+    get_geometry(r, o.dev);
+    if (r.ok() && (o.particles < 1 || o.patch_size != 32 || !(o.resolution > 0) || o.dev.dir_dim < 8 || o.dev.max_beams < 1 || o.dev.pool_slots < 0))
+        r.fail("bad options");
+    const uint32_t P = r.ok() ? o.particles : 0;
+    // front-end state
+    const SE2 prior = r.se2("state"), odom = r.se2("state");
+    const bool has_first = r.u8("state");
+    const double acc_trans = r.f64("state"), acc_rot = r.f64("state"), neff = r.f64("state");
+    std::vector<SE2> pose(r.count(P, 4 * 8, "poses"));
+    for (SE2& p : pose) p = r.se2("poses");
+    std::vector<double> weight, nweight, wsum;
+    r.array(weight, P, "weights");
+    r.array(nweight, P, "weights");
+    r.array(wsum, P, "weights");
+    std::vector<int32_t> last_idx;
+    r.array(last_idx, r.u32("resample indices"), "resample indices");
+    const uint64_t rs_count = r.u64("resample digest"), rs_hash = r.u64("resample digest"), scans_seen = r.u64("resample digest");
+    std::vector<double> stamps;
+    r.array(stamps, r.u32("timestamps"), "timestamps");
+    const Counters last = get_counters(r), total = get_counters(r);
+    const uint64_t detached_seen = r.u64("counters");
+    double summary[4];
+    for (double& v : summary) v = r.f64("summary");
+    std::vector<Node> nodes(r.count(r.u32("nodes"), 4 * 8 + 4, "nodes"));
+    for (size_t n = 0; n < nodes.size(); ++n) {
+        nodes[n].pose   = r.se2("nodes");
+        nodes[n].parent = r.i32("nodes");
+        if (r.ok() && (nodes[n].parent < -1 || nodes[n].parent >= (int)n)) r.fail("a trajectory node does not follow its parent");
+    }
+    std::vector<int32_t> node_of;
+    r.array(node_of, P, "trajectory heads");
+    const std::string rng = r.str("random generator");
+    if (r.ok()) {
+        for (int32_t v : last_idx)
+            if (v < 0 || v >= (int32_t)P) r.fail("resample index out of range");
+        if (!last_idx.empty() && last_idx.size() != P) r.fail("resample indices of the wrong length");
+        for (int32_t v : node_of)
+            if (v < -1 || v >= (int32_t)nodes.size() || (has_first && v < 0)) r.fail("trajectory head out of range");
+        if (!ckpt_check_rng(rng)) r.fail("malformed random generator state");
+        if (!finite_se2(prior) || !finite_se2(odom)) r.fail("non-finite pose");
+    }
+    EngineImage img;
+    bool present = false;
+    if (r.ok()) ckpt_get_engine(r, &present, img, (int)P, 0);
+    if (r.ok() && has_first && !present) r.fail("a filter past its first scan without device state");
+    if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
+    if (!r.ok()) { err = r.error(); return nullptr; }
+    if (!geometry_matches(dev, o.dev, present ? &img : nullptr, err)) return nullptr;
+    s.encode_ms += ms_since(t1);
+    // the file is valid: from here on the device
+    if (cuda_device_count() < 1) { *code = LAMA_ERR_NO_DEVICE; err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
+    o.dev.device = dev.device; o.dev.stream = dev.stream; o.dev.timing = dev.timing;
+    std::unique_ptr<PFSlam2D> p(create(o, err));
+    if (!p) return nullptr;
+    p->prior_ = prior; p->odom_ = odom; p->has_first_ = has_first;
+    p->acc_trans_ = acc_trans; p->acc_rot_ = acc_rot; p->neff_ = neff;
+    p->pose_ = pose; p->weight_ = weight; p->nweight_ = nweight; p->wsum_ = wsum;
+    p->last_idx_ = last_idx;
+    p->resample_count_ = rs_count; p->resample_hash_ = rs_hash; p->scans_seen_ = scans_seen;
+    p->timestamps_ = stamps;
+    p->last_ = last; p->total_ = total; p->detached_seen_ = detached_seen;
+    p->t_sample_ = summary[0]; p->t_solve_ = summary[1]; p->t_norm_ = summary[2]; p->t_resample_ = summary[3];
+    p->nodes_ = nodes; p->node_of_.assign(node_of.begin(), node_of.end());
+    std::istringstream in(rng);
+    in >> p->gen_;
+    if (present) {
+        Engine* e = Engine::restore(img, dev.device, dev.stream, err, &s.dev);
+        if (!e) { *code = LAMA_ERR_CUDA; return nullptr; }
+        p->eng_.reset(e);
+        e->enable_timing(dev.timing != 0);
+    }
+    s.used_slots = img.used;
+    s.references = sum_refs(img);
+    s.total_ms   = ms_since(t0);
+    *code = LAMA_OK;
+    return p.release();
+}
+
+int Slam2D::save(const std::string& path, CheckpointStats* st)
+{
+    const auto t0 = clk::now();
+    CheckpointStats local;
+    CheckpointStats& s = st ? *st : local;
+    s = CheckpointStats();
+    EngineImage img;
+    if (eng_) {
+        const int rc = eng_->snapshot(&img, &s.dev);
+        if (rc != LAMA_OK) { err_ = eng_->last_error(); return rc; }
+    }
+    const auto t1 = clk::now();
+    CkptWriter w;
+    for (double v : {opt_.trans_thresh, opt_.rot_thresh, opt_.l2_max, opt_.truncated_ray, opt_.truncated_range, opt_.resolution}) w.f64(v);
+    w.u32(opt_.patch_size); w.u32(opt_.max_iter); w.i32(opt_.strategy); w.i32(opt_.occupancy);
+    w.u8(opt_.transient_map); w.u8(opt_.lidar_odometry);
+    put_geometry(w, opt_.dev);
+    w.se2(pose_); w.se2(odom_); w.se2(map_update_pose_);
+    w.u8(has_first_); w.u8(engine_ready_);
+    w.u32(processed_); w.u64(removed_); w.u64(map_updates_);
+    put_counters(w, last_); put_counters(w, total_);
+    ckpt_put_engine(w, eng_ ? &img : nullptr);
+    s.encode_ms = ms_since(t1);
+    std::string err;
+    const int rc = ckpt_write_file(path, opt_.lidar_odometry ? kCkptLidarOdometry2D : kCkptSlam2D, w, img.slot_bytes, (size_t)img.used * img.slot_stride(), err, &s);
+    if (rc != LAMA_OK) { err_ = err; return rc; }
+    s.used_slots = img.used;
+    s.references = sum_refs(img);
+    s.total_ms   = ms_since(t0);
+    return LAMA_OK;
+}
+
+Slam2D* Slam2D::load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st)
+{
+    const auto t0 = clk::now();
+    CheckpointStats local;
+    CheckpointStats& s = st ? *st : local;
+    s = CheckpointStats();
+    std::vector<uint8_t> file;
+    uint32_t kind = 0;
+    *code = ckpt_read_file(path, file, &kind, err, &s);
+    if (*code != LAMA_OK) return nullptr;
+    *code = LAMA_ERR_ARG;
+    if (kind != kCkptSlam2D && kind != kCkptLidarOdometry2D) {
+        err = kind == kCkptPFSlam2D ? "the checkpoint holds a PFSlam2D, not a Slam2D" : "unknown checkpoint handle kind";
+        return nullptr;
+    }
+    const auto t1 = clk::now();
+    CkptReader r(file.data() + kCkptHeaderBytes, file.size() - kCkptHeaderBytes);
+    SlamOptions o;
+    for (double* v : {&o.trans_thresh, &o.rot_thresh, &o.l2_max, &o.truncated_ray, &o.truncated_range, &o.resolution}) *v = r.f64("options");
+    o.patch_size = r.u32("options"); o.max_iter = r.u32("options"); o.strategy = r.i32("options"); o.occupancy = r.i32("options");
+    o.transient_map = r.u8("options"); o.lidar_odometry = r.u8("options");
+    get_geometry(r, o.dev);
+    if (r.ok() && (o.patch_size != 32 || !(o.resolution > 0) || o.occupancy < 0 || o.occupancy > 1 || o.dev.dir_dim < 8 || o.dev.max_beams < 1 ||
+                   o.dev.pool_slots < 0 || o.lidar_odometry != (kind == kCkptLidarOdometry2D)))
+        r.fail("bad options");
+    const SE2 pose = r.se2("state"), odom = r.se2("state"), mu = r.se2("state");
+    const bool has_first = r.u8("state"), engine_ready = r.u8("state");
+    const uint32_t processed = r.u32("state");
+    const uint64_t removed = r.u64("state"), map_updates = r.u64("state");
+    const Counters last = get_counters(r), total = get_counters(r);
+    if (r.ok() && (!finite_se2(pose) || !finite_se2(odom) || !finite_se2(mu))) r.fail("non-finite pose");
+    EngineImage img;
+    bool present = false;
+    if (r.ok()) ckpt_get_engine(r, &present, img, 1, o.occupancy == 1 ? 1 : 0);
+    if (r.ok() && has_first && !present) r.fail("a Slam2D past its first scan without device state");
+    if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
+    if (!r.ok()) { err = r.error(); return nullptr; }
+    if (!geometry_matches(dev, o.dev, present ? &img : nullptr, err)) return nullptr;
+    s.encode_ms += ms_since(t1);
+    if (cuda_device_count() < 1) { *code = LAMA_ERR_NO_DEVICE; err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
+    o.dev.device = dev.device; o.dev.stream = dev.stream; o.dev.timing = dev.timing;
+    std::unique_ptr<Slam2D> p(create(o, err));
+    if (!p) return nullptr;
+    p->pose_ = pose; p->odom_ = odom; p->map_update_pose_ = mu;
+    p->has_first_ = has_first; p->engine_ready_ = engine_ready;
+    p->processed_ = processed; p->removed_ = removed; p->map_updates_ = map_updates;
+    p->last_ = last; p->total_ = total;
+    if (present) {
+        Engine* e = Engine::restore(img, dev.device, dev.stream, err, &s.dev);
+        if (!e) { *code = LAMA_ERR_CUDA; return nullptr; }
+        p->eng_.reset(e);
+        e->enable_timing(dev.timing != 0);
+        e->set_lidar_odometry_rays(o.lidar_odometry);
+    }
+    s.used_slots = img.used;
+    s.references = sum_refs(img);
+    s.total_ms   = ms_since(t0);
+    *code = LAMA_OK;
+    return p.release();
 }
 
 }  // namespace lama_b200

@@ -17,6 +17,7 @@
 namespace lama_b200 {
 
 struct ShardComm;
+struct CheckpointStats;
 
 struct DeviceOptions {
     int device = 0, dir_dim = 64, pool_slots = 0, max_beams = 2048, timing = 0;
@@ -96,6 +97,12 @@ public:
     Engine* engine() { return eng_.get(); }
     const std::string& error() const { return err_; }
     bool has_first_scan() const { return has_first_; }
+    // Checkpoints (format: checkpoint.h).  save() settles the pending map update and counters, then writes the whole session without
+    // changing it; a sharded handle is refused (LAMA_ERR_STATE).  load() checks the whole file before it touches CUDA (LAMA_ERR_ARG with
+    // the reason in `err`), then restores on dev.device / dev.stream with dev.timing; dev.dir_dim / pool_slots / max_beams must be 0 or
+    // the file's.  Kernel times, traffic counters and staged scans start empty on the loaded handle.
+    int save(const std::string& path, CheckpointStats* st = nullptr);
+    static PFSlam2D* load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st = nullptr);
     bool maps_enqueued_ = false;   // sharded ranks: this scan's map update was enqueued together with its match
     int settle_counters();
     int pipelined_begin(const double* pts, int n, const double* origin, const double* quat, bool moved, bool* did_update, double* local_out);
@@ -181,6 +188,10 @@ public:
     Engine* engine() { return eng_.get(); }
     const DeviceOptions& device_options() const { return opt_.dev; }
     const std::string& error() const { return err_; }
+    bool lidar_odometry() const { return opt_.lidar_odometry; }
+    // checkpoints, as PFSlam2D::save / load; a handle saved before its first scan has no engine section
+    int save(const std::string& path, CheckpointStats* st = nullptr);
+    static Slam2D* load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st = nullptr);
 
 private:
     SlamOptions opt_;

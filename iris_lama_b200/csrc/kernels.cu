@@ -6,12 +6,16 @@
 //                atomics + ordered replay of threshold crossings (see ray_core.h)
 //   k_brushfire  one warp per particle: DynamicDistanceMap::update() in exact heap order (ddm_core.h)
 //   k_copy_dirs / k_release / k_merge_free   resampling = directory copies with COW reference counts
+//   k_ckpt_*     checkpoints: reference counts checked, used slots compacted, directories renumbered
 //
 // All of them are memory/latency bound integer + fp64 work: no tensor cores.  Directories are staged
 // into shared memory with TMA bulk copies (cp.async.bulk + mbarrier).
 #include "kernels.cuh"
 
+#include <algorithm>
 #include <cstdio>
+
+#include <cub/device/device_scan.cuh>
 
 #include "brushfire_warp.cuh"
 
@@ -1615,14 +1619,64 @@ __global__ void k_import(StoreView s, int set, int particle, int kind, uint32_t 
     }
 }
 
-// gather the patches listed in `slots` into a contiguous buffer (particle migration between GPUs)
-__global__ void k_gather_patches(StoreView s, const int32_t* __restrict__ slots, int n, uint32_t* __restrict__ out, uint32_t* __restrict__ out_fbits)
+// gather the patches listed in `slots` into a contiguous buffer (particle migration between GPUs, checkpoints); out_kbits (may be null)
+// also takes the known plane of a store that has one
+__global__ void k_gather_patches(StoreView s, const int32_t* __restrict__ slots, int n, uint32_t* __restrict__ out, uint32_t* __restrict__ out_fbits,
+                                 uint32_t* __restrict__ out_kbits)
 {
     const int lane = threadIdx.x & 31;
     const int pi = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (pi >= n) return;
-    warp_copy_patch(out + (size_t)pi * kPatchCells, patch_ptr(s, slots[pi] & kDirSlotMask), lane);
-    out_fbits[(size_t)pi * 32 + lane] = __ldcg(fbits_ptr(s, slots[pi] & kDirSlotMask) + lane);
+    const int slot = slots[pi] & kDirSlotMask;
+    warp_copy_patch(out + (size_t)pi * kPatchCells, patch_ptr(s, slot), lane);
+    out_fbits[(size_t)pi * 32 + lane] = __ldcg(fbits_ptr(s, slot) + lane);
+    if (out_kbits && s.kbits) out_kbits[(size_t)pi * 32 + lane] = __ldcg(kbits_ptr(s, slot) + lane);
+}
+
+// ---- checkpoint: count the references of every slot, compact the slots in use, rewrite the directories ---------------------------------
+// one thread per directory entry of `set` (every particle, every kind incl. the log-odds scratch kind): cnt[slot] += 1 per reference.
+// bad bit 0: an entry whose slot lies outside the pool
+__global__ void k_ckpt_count(StoreView s, int set, int32_t* __restrict__ cnt, uint32_t* __restrict__ bad)
+{
+    const size_t n = (size_t)s.n_particles * s.n_kinds * s.window.dim * s.window.dim;
+    const int32_t* d = dir_of(s, set, 0, 0);
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const int32_t e = d[i];
+        if (e < 0) continue;
+        const int32_t slot = e & kDirSlotMask;
+        if (slot >= s.n_slots) { atomicOr(bad, 1u); continue; }
+        atomicAdd(&cnt[slot], 1);
+    }
+}
+// one thread per slot: used[slot] = 1 when a directory references it.  bad bit 1: the count differs from the slot's reference count
+// (a store that is not self-consistent is never written)
+__global__ void k_ckpt_mark(StoreView s, const int32_t* __restrict__ cnt, int32_t* __restrict__ used, uint32_t* __restrict__ bad)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < s.n_slots; i += gridDim.x * blockDim.x) {
+        const int32_t c = cnt[i];
+        used[i] = c > 0 ? 1 : 0;
+        if (c != s.refcount[i]) atomicOr(bad, 2u);
+    }
+}
+// after the exclusive scan (new_id = number of used slots below): list[new_id] = old slot, ref[new_id] = its reference count
+__global__ void k_ckpt_list(StoreView s, const int32_t* __restrict__ used, const int32_t* __restrict__ new_id, int32_t* __restrict__ list,
+                            int32_t* __restrict__ ref)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < s.n_slots; i += gridDim.x * blockDim.x)
+        if (used[i]) {
+            list[new_id[i]] = i;
+            ref[new_id[i]]  = s.refcount[i];
+        }
+}
+// one thread per directory entry of `set`: out = new id | the entry's flags (kDirHot and kDirOwn kept exactly); the store is not written
+__global__ void k_ckpt_remap(StoreView s, int set, const int32_t* __restrict__ new_id, int32_t* __restrict__ out)
+{
+    const size_t n = (size_t)s.n_particles * s.n_kinds * s.window.dim * s.window.dim;
+    const int32_t* d = dir_of(s, set, 0, 0);
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const int32_t e = d[i];
+        out[i] = e < 0 ? -1 : (new_id[e & kDirSlotMask] | (e & ~kDirSlotMask));
+    }
 }
 // allocate a patch per listed directory entry of (set, particle, kind) and fill it from `in`
 __global__ void k_scatter_patches(StoreView s, int set, int particle, int kind, const int32_t* __restrict__ entries, int n, const uint32_t* __restrict__ in,
@@ -2014,10 +2068,29 @@ void launch_import(const StoreView& s, int set, int particle, int kind, uint32_t
     if (patches <= 0) return;
     k_import<<<(patches + 3) / 4, 128, 0, st>>>(s, set, particle, kind, x0, y0, w, h, d_in);
 }
-void launch_gather_patches(const StoreView& s, const int32_t* d_slots, int n, uint32_t* d_out, uint32_t* d_out_fbits, cudaStream_t st)
+void launch_gather_patches(const StoreView& s, const int32_t* d_slots, int n, uint32_t* d_out, uint32_t* d_out_fbits, uint32_t* d_out_kbits,
+                           cudaStream_t st)
 {
     if (n <= 0) return;
-    k_gather_patches<<<(n + 3) / 4, 128, 0, st>>>(s, d_slots, n, d_out, d_out_fbits);
+    k_gather_patches<<<(n + 3) / 4, 128, 0, st>>>(s, d_slots, n, d_out, d_out_fbits, d_out_kbits);
+}
+size_t ckpt_scan_temp_bytes(int n_slots)
+{
+    size_t bytes = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const int32_t*)nullptr, (int32_t*)nullptr, n_slots);
+    return bytes;
+}
+void launch_ckpt_compact(const StoreView& s, int set, const CkptScratch& c, cudaStream_t st, cudaEvent_t after_count)
+{
+    const size_t n_dir = (size_t)s.n_particles * s.n_kinds * s.window.dim * s.window.dim;
+    const int dir_blocks = (int)std::min<size_t>((n_dir + 255) / 256, 4736), slot_blocks = std::min((s.n_slots + 255) / 256, 4736);
+    k_ckpt_count<<<dir_blocks, 256, 0, st>>>(s, set, c.cnt, c.bad);
+    if (after_count) cudaEventRecord(after_count, st);
+    k_ckpt_mark<<<slot_blocks, 256, 0, st>>>(s, c.cnt, c.used, c.bad);
+    size_t temp = c.temp_bytes;
+    cub::DeviceScan::ExclusiveSum(c.temp, temp, c.used, c.new_id, s.n_slots, st);
+    k_ckpt_list<<<slot_blocks, 256, 0, st>>>(s, c.used, c.new_id, c.list, c.ref);
+    k_ckpt_remap<<<dir_blocks, 256, 0, st>>>(s, set, c.new_id, c.dirs);
 }
 void launch_scatter_patches(const StoreView& s, int set, int particle, int kind, const int32_t* d_entries, int n, const uint32_t* d_in,
                             const uint32_t* d_in_fbits, cudaStream_t st)

@@ -119,7 +119,21 @@ void launch_export(const StoreView& s, int set, int particle, int kind, uint32_t
 // dense, patch-aligned window import (x0,y0 multiples of 32; w,h multiples of 32); all-zero patches are skipped
 void launch_import(const StoreView& s, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, const uint32_t* d_in,
                    cudaStream_t st);
-void launch_gather_patches(const StoreView& s, const int32_t* d_slots, int n, uint32_t* d_out, uint32_t* d_out_fbits, cudaStream_t st);
+// one warp per listed slot: 4 KiB of cells to d_out, 128 B of obstacle-mirror bits to d_out_fbits and, when d_out_kbits is not null and the
+// store has a known plane, 128 B of known bits to d_out_kbits
+void launch_gather_patches(const StoreView& s, const int32_t* d_slots, int n, uint32_t* d_out, uint32_t* d_out_fbits, uint32_t* d_out_kbits,
+                           cudaStream_t st);
+// device scratch of a checkpoint snapshot: cnt / used / new_id / list / ref are n_slots entries, dirs the directories of one set
+struct CkptScratch {
+    int32_t *cnt, *used, *new_id, *list, *ref, *dirs;
+    uint32_t* bad;      // bit 0: a directory entry points outside the pool, bit 1: a reference count differs from the directory references
+    void* temp;         // CUB scan temporary storage
+    size_t temp_bytes;
+};
+size_t ckpt_scan_temp_bytes(int n_slots);
+// k_ckpt_count (cnt must be zero) -> [after_count recorded] -> k_ckpt_mark -> exclusive scan of `used` -> k_ckpt_list -> k_ckpt_remap;
+// the used slots in ascending order get the ids 0 .. K-1, K = new_id[n_slots - 1] + used[n_slots - 1]
+void launch_ckpt_compact(const StoreView& s, int set, const CkptScratch& c, cudaStream_t st, cudaEvent_t after_count);
 void launch_scatter_patches(const StoreView& s, int set, int particle, int kind, const int32_t* d_entries, int n, const uint32_t* d_in,
                             const uint32_t* d_in_fbits, cudaStream_t st);
 // Loc2D::addSamplingCovariance likelihoods: out[i] for offset i (offsets = n x 2 doubles)

@@ -79,6 +79,10 @@ struct DirWindow {
     int32_t base_px, base_py;  // patch coordinates (cell >> 5) of directory entry (0,0)
     int32_t dim;               // entries per side (power of two)
 };
+// a directory entry is -1 or slot | flags (the flags are described in device_store.cuh)
+constexpr int32_t kDirSlotMask = 0x00FFFFFF;
+constexpr int32_t kDirHot      = 1 << 28;
+constexpr int32_t kDirOwn      = 1 << 29;
 // directory index of the patch holding cell (x, y), or -1 when outside the window.
 LAMA_HD int dir_index(const DirWindow& w, uint32_t x, uint32_t y)
 {
