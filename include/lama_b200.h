@@ -493,24 +493,31 @@ int lama_om3_kernel_times(lama_om3* h, double ms[3], uint64_t launches[3]);
 int lama_w2m3(double resolution, const double* pts_xyz, int n, uint32_t* cells_xyz);
 
 /* ------------------------------------------------------------------------------------------------
- * Checkpoints (no counterpart in the reference): save a PFSlam2D or Slam2D session to a file and continue it later, in another
- * process or on another device, bit for bit as if it had not stopped.  The file holds the options, the front end's state (poses,
+ * Checkpoints (no counterpart in the reference): save a PFSlam2D, Slam2D or GraphSlam2D session to a file and continue it later, in
+ * another process or on another device, bit for bit as if it had not stopped.  The file holds the options, the front end's state (poses,
  * weights, trajectories, the mt19937 state, counters, the Summary buckets) and the device maps with their copy-on-write sharing;
- * DESIGN.md section 13 gives the layout.  Saving settles the pending map update first and does not change the handle.  Kernel times,
+ * a GraphSlam2D file also holds its key poses with their clouds, links, pose graph, loop-factor queue and correction, the inner Slam2D
+ * and the global occupancy map when the next lama_graph_generate_occupancy_map would add to it (the coarse distance map is rebuilt by
+ * every call and is not saved).  DESIGN.md section 13 gives the layout.  Saving settles the pending map update first and does not
+ * change the handle.  Kernel times,
  * traffic counters and staged scans start empty on a loaded handle (lama_pf_update_staged needs a new lama_pf_stage_scans).
  * Loading checks the whole file (size, checksum, version, kind, every count, directory entry and reference count) before it touches
  * CUDA: a bad file gives LAMA_ERR_ARG and no handle; a valid file on a host without a device gives LAMA_ERR_NO_DEVICE.
  * From `dev` (may be NULL: device 0) only device, stream and timing are taken; dir_dim, pool_slots and max_beams must be 0 or the
  * saved values.  A sharded PFSlam2D (shard_count > 1) cannot be saved (LAMA_ERR_STATE).  A LidarOdometry2D-mode Slam2D loads back in
- * that mode; the inner Slam2D of a lama_graph (lama_graph_slam) can be saved and loads back as a standalone Slam2D.
+ * that mode.  Each loader refuses the other kinds' files (LAMA_ERR_ARG); the inner Slam2D of a lama_graph (lama_graph_slam) can still
+ * be saved on its own and loads back as a standalone Slam2D.
  * ------------------------------------------------------------------------------------------------ */
 int lama_pf_save_state(lama_pf* h, const char* path);
 int lama_pf_load_state(const char* path, const lama_device_options* dev, lama_pf** out);
 int lama_slam_save_state(lama_slam* h, const char* path);
 int lama_slam_load_state(const char* path, const lama_device_options* dev, lama_slam** out);
+int lama_graph_save_state(lama_graph* h, const char* path);
+int lama_graph_load_state(const char* path, const lama_device_options* dev, lama_graph** out);
 /* what the last save or load on this thread took and moved.  ms = {count, compaction, gather (device, CUDA events; save only), slot
  * copy (chunked through pinned buffers), engine creation, tables (directories, reference counts, free stack; load only), encode
- * (serialisation / parsing, checks and checksum), file I/O, total}; sizes = {slots in use, per-particle patch references, file bytes} */
+ * (serialisation / parsing, checks and checksum), file I/O, total}; sizes = {slots in use, per-particle patch references, file bytes}.
+ * For a GraphSlam2D, device times, slots and references are the sums over its two engines (inner Slam2D and global map). */
 int lama_checkpoint_last_stats(double ms[9], uint64_t sizes[3]);
 
 #ifdef __cplusplus

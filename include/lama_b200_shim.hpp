@@ -167,8 +167,18 @@ public:
     lama_om* generateOccupancyMap(bool full = false) { lama_om* m = nullptr; check(lama_graph_generate_occupancy_map(h_, full ? 1 : 0, &m)); return m; }
     lama_dm* generateCoarseDistanceMap() { lama_dm* d = nullptr; check(lama_graph_generate_coarse_distance_map(h_, &d, nullptr)); return d; }
     lama_graph* handle() const { return h_; }
+    // checkpoints (no counterpart in the reference), as PFSlam2D::saveState / loadState
+    void saveState(const std::string& path) const { check(lama_graph_save_state(h_, path.c_str())); }
+    static std::unique_ptr<GraphSlam2D> loadState(const std::string& path, int device = 0)
+    {
+        lama_device_options dev = {device, 0, 0, 0, 0, 0};
+        lama_graph* h = nullptr;
+        check(lama_graph_load_state(path.c_str(), &dev, &h));
+        return std::unique_ptr<GraphSlam2D>(new GraphSlam2D(h));
+    }
 
 private:
+    explicit GraphSlam2D(lama_graph* h) : h_(h) {}
     lama_graph* h_ = nullptr;
 };
 

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import struct
 
 import numpy as np
 
@@ -92,6 +93,7 @@ EXPORTED_SYMBOLS = [
     "lama_om3_create", "lama_om3_destroy", "lama_om3_insert_point_clouds", "lama_om3_apply", "lama_om3_query", "lama_om3_prune",
     "lama_om3_bounds", "lama_om3_export", "lama_om3_write", "lama_om3_read", "lama_om3_export_image", "lama_om3_kernel_times", "lama_w2m3",
     "lama_pf_save_state", "lama_pf_load_state", "lama_slam_save_state", "lama_slam_load_state", "lama_checkpoint_last_stats",
+    "lama_graph_save_state", "lama_graph_load_state",
 ]
 
 
@@ -308,7 +310,7 @@ def shard_unique_id() -> bytes:
 
 
 # ---- checkpoints ------------------------------------------------------------------------------------------------
-CKPT_PFSLAM2D, CKPT_SLAM2D, CKPT_LIDAR_ODOMETRY2D = 1, 2, 3   # handle kind in the checkpoint header (u32 at byte 12)
+CKPT_PFSLAM2D, CKPT_SLAM2D, CKPT_LIDAR_ODOMETRY2D, CKPT_GRAPHSLAM2D = 1, 2, 3, 4   # handle kind in the checkpoint header (u32 at byte 12)
 
 
 def checkpoint_kind(path) -> tuple:
@@ -828,6 +830,37 @@ class GraphSlam2D:
         dm = DynamicDistanceMap(handle=h, owner=self)
         dm.processed = n.value
         return dm
+
+    # ---- checkpoints -----------------------------------------------------------------------------------------
+    def saveState(self, path):
+        """writes the whole session (options, inner Slam2D, key poses and clouds, pose graph, device maps) to `path`; the handle is not
+        changed"""
+        _chk(lib().lama_graph_save_state(self.h, str(path).encode()))
+
+    @classmethod
+    def loadState(cls, path, device=0, stream=0, timing=False) -> "GraphSlam2D":
+        """a GraphSlam2D that continues the saved session bit for bit, on `device` / `stream`; `.options` (and `.slam.options`) are the
+        saved session's, with the device, stream and timing of this call"""
+        h = _load_state(lib().lama_graph_load_state, path, device, stream, timing)
+        self = cls.__new__(cls)
+        self.h = h
+        self.options = _graph_options_of_checkpoint(path, device, stream, timing)
+        return self
+
+
+def _graph_options_of_checkpoint(path, device, stream, timing) -> GraphOptions:
+    """the graph options and inner Slam2D options at the start of a kind-4 checkpoint's body (DESIGN.md §13); the loader has checked it"""
+    with open(path, "rb") as f:
+        f.seek(32)
+        b = f.read(56 + 78)
+    o = GraphSlam2D.Options()
+    (o.key_pose_distance, o.key_pose_angular_distance, o.key_pose_head_delay, o.loop_search_max_distance, o.loop_search_min_distance,
+     o.loop_max_candidates, o.loop_closure_scan_rmse, o.loop_closure_max_candidates, o.ignore_n_chain_poses) = struct.unpack_from("<ddiddidii", b)
+    s = o.slam
+    (s.trans_thresh, s.rot_thresh, s.l2_max, s.truncated_ray, s.truncated_range, s.resolution, s.patch_size, s.max_iter, s.strategy,
+     s.occupancy, s.transient_map, s.lidar_odometry, s.dev.dir_dim, s.dev.pool_slots, s.dev.max_beams) = struct.unpack_from("<6dIIii2B3i", b, 56)
+    s.dev.device, s.dev.stream, s.dev.timing = device, stream, int(timing)
+    return o
 
 
 class FrequencyOccupancyMap:

@@ -1769,6 +1769,25 @@ try {
     return LAMA_OK;
 }
 LAMA_CATCH
+int lama_graph_save_state(lama_graph* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    const int rc = h->g->save(path, &g_ckpt);
+    return rc == LAMA_OK ? rc : set_err(h->g->error(), rc);
+}
+LAMA_CATCH
+int lama_graph_load_state(const char* path, const lama_device_options* dev, lama_graph** out)
+try {
+    if (!path || !out) return set_err("null argument", LAMA_ERR_ARG);
+    *out = nullptr;
+    std::string err;
+    int rc = LAMA_OK;
+    GraphSlam2D* g = GraphSlam2D::load(path, load_dev(dev), err, &rc, &g_ckpt);
+    if (!g) return set_err(err, rc == LAMA_OK ? LAMA_ERR_ARG : rc);
+    *out = new lama_graph{g, lama_slam{g->slam(), false}, lama_om{g->occupancy_map(), false}, lama_dm{nullptr, false}};
+    return LAMA_OK;
+}
+LAMA_CATCH
 int lama_checkpoint_last_stats(double ms[9], uint64_t sizes[3])
 try {
     if (!ms || !sizes) return set_err("null argument", LAMA_ERR_ARG);

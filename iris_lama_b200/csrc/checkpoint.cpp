@@ -24,13 +24,16 @@ uint64_t fnv1a64(const uint8_t* p, size_t n, uint64_t h)
     return h;
 }
 
-int ckpt_write_file(const std::string& path, uint32_t kind, CkptWriter& w, const uint8_t* tail, size_t tail_bytes, std::string& err, CheckpointStats* st)
+int ckpt_write_file(const std::string& path, uint32_t kind, CkptWriter& w, const std::vector<CkptSegment>& tail, std::string& err, CheckpointStats* st)
 {
     const auto t0 = std::chrono::steady_clock::now();
     uint8_t* h = w.buf.data();
-    const uint64_t total = (uint64_t)w.buf.size() + tail_bytes;
+    uint64_t total = (uint64_t)w.buf.size();
     uint64_t sum = fnv1a64(h + kCkptHeaderBytes, w.buf.size() - kCkptHeaderBytes);
-    sum = fnv1a64(tail, tail_bytes, sum);
+    for (const CkptSegment& s : tail) {
+        total += s.n;
+        sum = fnv1a64(s.p, s.n, sum);
+    }
     std::memcpy(h, &kCkptMagic, 8);
     std::memcpy(h + 8, &kCkptVersion, 4);
     std::memcpy(h + 12, &kind, 4);
@@ -39,8 +42,9 @@ int ckpt_write_file(const std::string& path, uint32_t kind, CkptWriter& w, const
     const auto t1 = std::chrono::steady_clock::now();
     File f{std::fopen(path.c_str(), "wb")};
     if (!f.f) { err = "cannot open " + path + " for writing"; return LAMA_ERR_ARG; }
-    if (std::fwrite(w.buf.data(), 1, w.buf.size(), f.f) != w.buf.size() || (tail_bytes && std::fwrite(tail, 1, tail_bytes, f.f) != tail_bytes) ||
-        std::fflush(f.f) != 0) {
+    bool ok = std::fwrite(w.buf.data(), 1, w.buf.size(), f.f) == w.buf.size();
+    for (const CkptSegment& s : tail) ok = ok && (s.n == 0 || std::fwrite(s.p, 1, s.n, f.f) == s.n);
+    if (!ok || std::fflush(f.f) != 0) {
         err = "write error on " + path;
         return LAMA_ERR_ARG;
     }
@@ -99,7 +103,7 @@ void ckpt_put_engine(CkptWriter& w, const EngineImage* img)
     w.bytes(img->dirs.data(), img->dirs.size() * 4);
 }
 
-bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particles, int occupancy_kind)
+bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particles, int occupancy_kind, bool last)
 {
     *present = r.u8("engine flag");
     if (!r.ok() || !*present) return r.ok();
@@ -127,7 +131,7 @@ bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particl
     const uint64_t n_dir = (uint64_t)img.particles * img.n_kinds() * img.dir_dim * img.dir_dim;
     // every count against the bytes that are left, before anything is allocated
     const uint64_t need = (uint64_t)img.used * 4 + n_dir * 4 + (uint64_t)img.used * img.slot_stride();
-    if (need != r.left()) { r.fail(need > r.left() ? "engine section exceeds the file" : "bytes after the engine section"); return false; }
+    if (need > r.left() || (last && need != r.left())) { r.fail(need > r.left() ? "engine section exceeds the file" : "bytes after the engine section"); return false; }
     r.array(img.refcount, img.used, "reference counts");
     r.array(img.dirs, n_dir, "directories");
     img.slot_bytes = r.take((size_t)img.used * img.slot_stride(), "slots");

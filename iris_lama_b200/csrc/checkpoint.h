@@ -1,9 +1,10 @@
-// checkpoint.h -- the file format of PFSlam2D / Slam2D checkpoints (host only, no CUDA).
+// checkpoint.h -- the file format of PFSlam2D / Slam2D / GraphSlam2D checkpoints (host only, no CUDA).
 //
 // Little endian.  A 32-byte header {u64 magic "LAMACKPT", u32 format version, u32 handle kind, u64 total file size, u64 FNV-1a-64 of every
 // byte after the header}, then the sections: options (field by field), front-end state, and the engine section -- u8 present, then
-// geometry, window, store counters, K, K reference counts, the directories of every particle and kind, and the K slot payloads last.
-// The byte-exact layout is in DESIGN.md §13; tests/test_checkpoint.py writes it independently.
+// geometry, window, store counters, K, K reference counts, the directories of every particle and kind, and the K slot payloads.  A
+// GraphSlam2D file holds two engine sections, each followed by its own slot payloads.
+// The byte-exact layout is in DESIGN.md §13; tests/test_checkpoint.py and tests/test_graph_checkpoint.py write it independently.
 #pragma once
 
 #include <cstdint>
@@ -18,7 +19,7 @@ namespace lama_b200 {
 constexpr uint64_t kCkptMagic      = 0x54504B43414D414Cull;   // "LAMACKPT"
 constexpr uint32_t kCkptVersion    = 1;
 constexpr size_t kCkptHeaderBytes  = 32;
-enum CkptKind : uint32_t { kCkptPFSlam2D = 1, kCkptSlam2D = 2, kCkptLidarOdometry2D = 3 };
+enum CkptKind : uint32_t { kCkptPFSlam2D = 1, kCkptSlam2D = 2, kCkptLidarOdometry2D = 3, kCkptGraphSlam2D = 4 };
 
 // what the last save / load took (ms) and moved
 struct CheckpointStats {
@@ -90,17 +91,22 @@ private:
 
 uint64_t fnv1a64(const uint8_t* p, size_t n, uint64_t h = 1469598103934665603ull);
 
-// Fills the header of w.buf and writes w.buf, then `tail` (the slot payloads), to `path`; the checksum covers both.
-int ckpt_write_file(const std::string& path, uint32_t kind, CkptWriter& w, const uint8_t* tail, size_t tail_bytes, std::string& err, CheckpointStats* st);
+// bytes written after the serialisation buffer without being copied into it (slot payloads, and the sections between them)
+struct CkptSegment {
+    const uint8_t* p;
+    size_t n;
+};
+// Fills the header of w.buf and writes w.buf, then the `tail` segments in order, to `path`; the checksum covers them all.
+int ckpt_write_file(const std::string& path, uint32_t kind, CkptWriter& w, const std::vector<CkptSegment>& tail, std::string& err, CheckpointStats* st);
 // Reads `path` into `file` and checks the header: magic, version, size, checksum.  *kind = the handle kind.
 int ckpt_read_file(const std::string& path, std::vector<uint8_t>& file, uint32_t* kind, std::string& err, CheckpointStats* st);
 
 // The engine section.  put writes everything but the slot payloads (the caller passes them as the file's tail); get reads and checks the
 // whole section -- geometry, window, counts against the file size, directory entries (slot < K, known flag bits only), every reference
 // count against its directory references -- and points img.slot_bytes into the reader's buffer.  `particles` / `occupancy_kind` are what
-// the front end expects (-1: any).
+// the front end expects (-1: any).  With `last`, the section must end the file; otherwise other sections may follow its slots.
 void ckpt_put_engine(CkptWriter& w, const EngineImage* img);
-bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particles, int occupancy_kind);
+bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particles, int occupancy_kind, bool last = true);
 
 // the text std::mt19937's operator<< writes: 624 state words and an index <= 624
 bool ckpt_check_rng(const std::string& text);

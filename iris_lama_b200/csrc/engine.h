@@ -180,6 +180,9 @@ public:
     // (checkpoint.h checks it).
     int snapshot(EngineImage* out, CheckpointTimes* t = nullptr);
     static Engine* restore(const EngineImage& img, int device, uint64_t stream, std::string& err, CheckpointTimes* t = nullptr);
+    // config().center_x / center_y: the world position the window was created around.  The image holds the window base, not the
+    // centre, so a restored engine reports (0, 0) until a front end that places other maps on that centre sets it back.
+    void set_center(double x, double y) { cfg_.center_x = x; cfg_.center_y = y; }
 
     // sticky device error bits (lama_core.h) -- reads the device word; 0 = ok
     uint32_t device_status();

@@ -1279,6 +1279,13 @@ OccupancyMapDev* OccupancyMapDev::create(double resolution, uint32_t patch_size,
     return m;
 }
 
+OccupancyMapDev* OccupancyMapDev::adopt(Engine* e)
+{
+    OccupancyMapDev* m = new OccupancyMapDev();
+    m->eng_.reset(e);
+    return m;
+}
+
 int OccupancyMapDev::insert_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states,
                                   bool full, uint64_t* cells)
 {
@@ -1575,6 +1582,19 @@ uint64_t sum_refs(const EngineImage& img)
     for (int32_t v : img.refcount) n += (uint64_t)v;
     return n;
 }
+// the refusal of a loader called on another handle kind's file
+std::string wrong_kind(uint32_t kind, const char* want)
+{
+    const char* held = kind == kCkptPFSlam2D ? "PFSlam2D"
+                       : kind == kCkptSlam2D || kind == kCkptLidarOdometry2D ? "Slam2D"
+                       : kind == kCkptGraphSlam2D ? "GraphSlam2D" : nullptr;
+    return held ? std::string("the checkpoint holds a ") + held + ", not a " + want : std::string("unknown checkpoint handle kind");
+}
+void add_times(CheckpointTimes& a, const CheckpointTimes& b)
+{
+    a.count_ms += b.count_ms; a.compact_ms += b.compact_ms; a.gather_ms += b.gather_ms;
+    a.copy_ms += b.copy_ms; a.create_ms += b.create_ms; a.tables_ms += b.tables_ms;
+}
 }  // namespace
 
 int PFSlam2D::save(const std::string& path, CheckpointStats* st)
@@ -1633,7 +1653,7 @@ int PFSlam2D::save(const std::string& path, CheckpointStats* st)
     ckpt_put_engine(w, eng_ ? &img : nullptr);
     s.encode_ms = ms_since(t1);
     std::string err;
-    const int rc = ckpt_write_file(path, kCkptPFSlam2D, w, img.slot_bytes, (size_t)img.used * img.slot_stride(), err, &s);
+    const int rc = ckpt_write_file(path, kCkptPFSlam2D, w, {{img.slot_bytes, (size_t)img.used * img.slot_stride()}}, err, &s);
     if (rc != LAMA_OK) return fail(err, rc);
     s.used_slots = img.used;
     s.references = sum_refs(img);
@@ -1653,7 +1673,7 @@ PFSlam2D* PFSlam2D::load(const std::string& path, const DeviceOptions& dev, std:
     if (*code != LAMA_OK) return nullptr;
     *code = LAMA_ERR_ARG;
     if (kind != kCkptPFSlam2D) {
-        err = kind == kCkptSlam2D || kind == kCkptLidarOdometry2D ? "the checkpoint holds a Slam2D, not a PFSlam2D" : "unknown checkpoint handle kind";
+        err = wrong_kind(kind, "PFSlam2D");
         return nullptr;
     }
     const auto t1 = clk::now();
@@ -1755,18 +1775,11 @@ int Slam2D::save(const std::string& path, CheckpointStats* st)
     }
     const auto t1 = clk::now();
     CkptWriter w;
-    for (double v : {opt_.trans_thresh, opt_.rot_thresh, opt_.l2_max, opt_.truncated_ray, opt_.truncated_range, opt_.resolution}) w.f64(v);
-    w.u32(opt_.patch_size); w.u32(opt_.max_iter); w.i32(opt_.strategy); w.i32(opt_.occupancy);
-    w.u8(opt_.transient_map); w.u8(opt_.lidar_odometry);
-    put_geometry(w, opt_.dev);
-    w.se2(pose_); w.se2(odom_); w.se2(map_update_pose_);
-    w.u8(has_first_); w.u8(engine_ready_);
-    w.u32(processed_); w.u64(removed_); w.u64(map_updates_);
-    put_counters(w, last_); put_counters(w, total_);
+    ckpt_put(w);
     ckpt_put_engine(w, eng_ ? &img : nullptr);
     s.encode_ms = ms_since(t1);
     std::string err;
-    const int rc = ckpt_write_file(path, opt_.lidar_odometry ? kCkptLidarOdometry2D : kCkptSlam2D, w, img.slot_bytes, (size_t)img.used * img.slot_stride(), err, &s);
+    const int rc = ckpt_write_file(path, opt_.lidar_odometry ? kCkptLidarOdometry2D : kCkptSlam2D, w, {{img.slot_bytes, (size_t)img.used * img.slot_stride()}}, err, &s);
     if (rc != LAMA_OK) { err_ = err; return rc; }
     s.used_slots = img.used;
     s.references = sum_refs(img);
@@ -1786,50 +1799,325 @@ Slam2D* Slam2D::load(const std::string& path, const DeviceOptions& dev, std::str
     if (*code != LAMA_OK) return nullptr;
     *code = LAMA_ERR_ARG;
     if (kind != kCkptSlam2D && kind != kCkptLidarOdometry2D) {
-        err = kind == kCkptPFSlam2D ? "the checkpoint holds a PFSlam2D, not a Slam2D" : "unknown checkpoint handle kind";
+        err = wrong_kind(kind, "Slam2D");
         return nullptr;
     }
     const auto t1 = clk::now();
     CkptReader r(file.data() + kCkptHeaderBytes, file.size() - kCkptHeaderBytes);
-    SlamOptions o;
+    SlamSaved sv;
+    ckpt_get(r, kind == kCkptLidarOdometry2D, sv);
+    EngineImage img;
+    bool present = false;
+    if (r.ok()) ckpt_get_engine(r, &present, img, 1, sv.opt.occupancy == 1 ? 1 : 0);
+    if (r.ok() && sv.has_first && !present) r.fail("a Slam2D past its first scan without device state");
+    if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
+    if (!r.ok()) { err = r.error(); return nullptr; }
+    if (!geometry_matches(dev, sv.opt.dev, present ? &img : nullptr, err)) return nullptr;
+    s.encode_ms += ms_since(t1);
+    if (cuda_device_count() < 1) { *code = LAMA_ERR_NO_DEVICE; err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
+    std::unique_ptr<Slam2D> p(ckpt_restore(sv, present ? &img : nullptr, dev, err, code, &s.dev));
+    if (!p) return nullptr;
+    s.used_slots = img.used;
+    s.references = sum_refs(img);
+    s.total_ms   = ms_since(t0);
+    *code = LAMA_OK;
+    return p.release();
+}
+
+void Slam2D::ckpt_put(CkptWriter& w) const
+{
+    for (double v : {opt_.trans_thresh, opt_.rot_thresh, opt_.l2_max, opt_.truncated_ray, opt_.truncated_range, opt_.resolution}) w.f64(v);
+    w.u32(opt_.patch_size); w.u32(opt_.max_iter); w.i32(opt_.strategy); w.i32(opt_.occupancy);
+    w.u8(opt_.transient_map); w.u8(opt_.lidar_odometry);
+    put_geometry(w, opt_.dev);
+    w.se2(pose_); w.se2(odom_); w.se2(map_update_pose_);
+    w.u8(has_first_); w.u8(engine_ready_);
+    w.u32(processed_); w.u64(removed_); w.u64(map_updates_);
+    put_counters(w, last_); put_counters(w, total_);
+}
+
+void Slam2D::ckpt_get(CkptReader& r, bool lidar_odometry, SlamSaved& s)
+{
+    SlamOptions& o = s.opt;
     for (double* v : {&o.trans_thresh, &o.rot_thresh, &o.l2_max, &o.truncated_ray, &o.truncated_range, &o.resolution}) *v = r.f64("options");
     o.patch_size = r.u32("options"); o.max_iter = r.u32("options"); o.strategy = r.i32("options"); o.occupancy = r.i32("options");
     o.transient_map = r.u8("options"); o.lidar_odometry = r.u8("options");
     get_geometry(r, o.dev);
     if (r.ok() && (o.patch_size != 32 || !(o.resolution > 0) || o.occupancy < 0 || o.occupancy > 1 || o.dev.dir_dim < 8 || o.dev.max_beams < 1 ||
-                   o.dev.pool_slots < 0 || o.lidar_odometry != (kind == kCkptLidarOdometry2D)))
+                   o.dev.pool_slots < 0 || o.lidar_odometry != lidar_odometry))
         r.fail("bad options");
-    const SE2 pose = r.se2("state"), odom = r.se2("state"), mu = r.se2("state");
-    const bool has_first = r.u8("state"), engine_ready = r.u8("state");
-    const uint32_t processed = r.u32("state");
-    const uint64_t removed = r.u64("state"), map_updates = r.u64("state");
-    const Counters last = get_counters(r), total = get_counters(r);
-    if (r.ok() && (!finite_se2(pose) || !finite_se2(odom) || !finite_se2(mu))) r.fail("non-finite pose");
-    EngineImage img;
-    bool present = false;
-    if (r.ok()) ckpt_get_engine(r, &present, img, 1, o.occupancy == 1 ? 1 : 0);
-    if (r.ok() && has_first && !present) r.fail("a Slam2D past its first scan without device state");
-    if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
-    if (!r.ok()) { err = r.error(); return nullptr; }
-    if (!geometry_matches(dev, o.dev, present ? &img : nullptr, err)) return nullptr;
-    s.encode_ms += ms_since(t1);
-    if (cuda_device_count() < 1) { *code = LAMA_ERR_NO_DEVICE; err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
+    s.pose = r.se2("state"); s.odom = r.se2("state"); s.map_update_pose = r.se2("state");
+    s.has_first = r.u8("state"); s.engine_ready = r.u8("state");
+    s.processed = r.u32("state");
+    s.removed = r.u64("state"); s.map_updates = r.u64("state");
+    s.last = get_counters(r); s.total = get_counters(r);
+    if (r.ok() && (!finite_se2(s.pose) || !finite_se2(s.odom) || !finite_se2(s.map_update_pose))) r.fail("non-finite pose");
+}
+
+Slam2D* Slam2D::ckpt_restore(const SlamSaved& s, const EngineImage* img, const DeviceOptions& dev, std::string& err, int* code, CheckpointTimes* t)
+{
+    SlamOptions o = s.opt;
     o.dev.device = dev.device; o.dev.stream = dev.stream; o.dev.timing = dev.timing;
     std::unique_ptr<Slam2D> p(create(o, err));
     if (!p) return nullptr;
-    p->pose_ = pose; p->odom_ = odom; p->map_update_pose_ = mu;
-    p->has_first_ = has_first; p->engine_ready_ = engine_ready;
-    p->processed_ = processed; p->removed_ = removed; p->map_updates_ = map_updates;
-    p->last_ = last; p->total_ = total;
-    if (present) {
-        Engine* e = Engine::restore(img, dev.device, dev.stream, err, &s.dev);
+    p->pose_ = s.pose; p->odom_ = s.odom; p->map_update_pose_ = s.map_update_pose;
+    p->has_first_ = s.has_first; p->engine_ready_ = s.engine_ready;
+    p->processed_ = s.processed; p->removed_ = s.removed; p->map_updates_ = s.map_updates;
+    p->last_ = s.last; p->total_ = s.total;
+    if (img) {
+        Engine* e = Engine::restore(*img, dev.device, dev.stream, err, t);
         if (!e) { *code = LAMA_ERR_CUDA; return nullptr; }
         p->eng_.reset(e);
         e->enable_timing(dev.timing != 0);
         e->set_lidar_odometry_rays(o.lidar_odometry);
     }
-    s.used_slots = img.used;
-    s.references = sum_refs(img);
+    return p.release();
+}
+
+// ---- GraphSlam2D (kind 4) ---------------------------------------------------------------------------------------------------------------
+namespace {
+void put_loss(CkptWriter& w, const PgoLoss& l)
+{
+    for (double v : l.sigma) w.f64(v);
+    w.f64(l.huber_k);
+}
+PgoLoss get_loss(CkptReader& r, const char* what)
+{
+    PgoLoss l;
+    for (double& v : l.sigma) v = r.f64(what);
+    l.huber_k = r.f64(what);
+    bool ok = l.huber_k >= 0 && std::isfinite(l.huber_k);
+    for (double v : l.sigma) ok = ok && v > 0 && std::isfinite(v);   // GraphSlam2D's sigmas are finite constants; inf would drop a factor
+    if (r.ok() && !ok) r.fail(std::string("bad loss (") + what + ")");
+    return l;
+}
+void put_betweens(CkptWriter& w, const std::vector<PgoBetween>& v)
+{
+    w.u32((uint32_t)v.size());
+    for (const PgoBetween& b : v) {
+        w.i32(b.from); w.i32(b.to); w.se2(b.measured);
+        put_loss(w, b.loss);
+    }
+}
+void get_betweens(CkptReader& r, std::vector<PgoBetween>& v, size_t n_keys, const char* what)
+{
+    v.resize(r.count(r.u32(what), 2 * 4 + 4 * 8 + 4 * 8, what));
+    for (PgoBetween& b : v) {
+        b.from = r.i32(what); b.to = r.i32(what); b.measured = r.se2(what);
+        b.loss = get_loss(r, what);
+        if (r.ok() && (b.from < 0 || (size_t)b.from >= n_keys || b.to < 0 || (size_t)b.to >= n_keys)) r.fail(std::string("a factor names no key (") + what + ")");
+        if (r.ok() && !finite_se2(b.measured)) r.fail(std::string("non-finite factor (") + what + ")");
+    }
+}
+bool finite3(const double* v, int n)
+{
+    for (int k = 0; k < n; ++k)
+        if (!std::isfinite(v[k])) return false;
+    return true;
+}
+}  // namespace
+
+int GraphSlam2D::save(const std::string& path, CheckpointStats* st)
+{
+    const auto t0 = clk::now();
+    CheckpointStats local;
+    CheckpointStats& s = st ? *st : local;
+    s = CheckpointStats();
+    Engine* ie = slam_->engine();
+    const bool global = mapping_keyid_ > 0 && occ_;   // only then does the next generate_occupancy_map draw on occ_
+    EngineImage inner, gimg;
+    if (ie) {
+        const int rc = ie->snapshot(&inner, &s.dev);
+        if (rc != LAMA_OK) { err_ = ie->last_error(); return rc; }
+    }
+    if (global) {
+        CheckpointTimes t;
+        const int rc = occ_->engine()->snapshot(&gimg, &t);
+        if (rc != LAMA_OK) { err_ = occ_->engine()->last_error(); return rc; }
+        add_times(s.dev, t);
+    }
+    const auto t1 = clk::now();
+    CkptWriter w;
+    // graph options
+    w.f64(opt_.key_pose_distance); w.f64(opt_.key_pose_angular_distance); w.i32(opt_.key_pose_head_delay);
+    w.f64(opt_.loop_search_max_distance); w.f64(opt_.loop_search_min_distance); w.i32(opt_.loop_max_candidates);
+    w.f64(opt_.loop_closure_scan_rmse); w.i32(opt_.loop_closure_max_candidates); w.i32(opt_.ignore_n_chain_poses);
+    // the inner Slam2D: the bytes of a kind-2 file's options and state
+    slam_->ckpt_put(w);
+    // graph state
+    w.se2(correction_); w.se2(prev_);
+    w.f64(accdist_); w.f64(factordist_);
+    w.u64(mapping_keyid_);
+    w.u64(stats_.loop_factors); w.u64(stats_.optimizations); w.u64(stats_.optimizations_ok);
+    const PgoReport& rep = stats_.last;
+    w.i32(rep.status); w.u32(rep.iterations); w.u32(rep.lambda_tries); w.u64(rep.cg_iterations);
+    w.f64(rep.initial_error); w.f64(rep.final_error); w.f64(rep.device_ms);
+    w.u32((uint32_t)last_candidates_.size());
+    for (int c : last_candidates_) w.i32(c);
+    double c[2];
+    slam_window_center(slam_.get(), c);   // a restored engine does not know its centre (Engine::set_center)
+    w.f64(c[0]); w.f64(c[1]);
+    // key poses
+    w.u32((uint32_t)keys_.size());
+    for (const KeyPose& k : keys_) {
+        w.i32(k.id); w.se2(k.pose); w.se2(k.original);
+        for (double v : k.origin) w.f64(v);
+        for (double v : k.quat) w.f64(v);
+        w.f64(k.stamp);
+        w.u32((uint32_t)(k.pts.size() / 3));
+        w.bytes(k.pts.data(), k.pts.size() * 8);
+    }
+    w.u32((uint32_t)links_.size());
+    for (const auto& l : links_) { w.i32(l.first); w.i32(l.second); }
+    // the pose graph
+    w.u32((uint32_t)priors_.size());
+    for (const PgoPrior& p : priors_) {
+        w.i32(p.node); w.se2(p.measured);
+        put_loss(w, p.loss);
+    }
+    put_betweens(w, factors_);
+    put_betweens(w, queue_);
+    // the inner engine, its slots, the global map's engine and its slots
+    ckpt_put_engine(w, ie ? &inner : nullptr);
+    CkptWriter g;
+    g.buf.clear();
+    ckpt_put_engine(g, global ? &gimg : nullptr);
+    s.encode_ms = ms_since(t1);
+    std::string err;
+    const int rc = ckpt_write_file(path, kCkptGraphSlam2D, w,
+                                   {{inner.slot_bytes, (size_t)inner.used * inner.slot_stride()}, {g.buf.data(), g.buf.size()},
+                                    {gimg.slot_bytes, (size_t)gimg.used * gimg.slot_stride()}},
+                                   err, &s);
+    if (rc != LAMA_OK) { err_ = err; return rc; }
+    s.used_slots = (uint64_t)inner.used + gimg.used;
+    s.references = sum_refs(inner) + sum_refs(gimg);
+    s.total_ms   = ms_since(t0);
+    return LAMA_OK;
+}
+
+GraphSlam2D* GraphSlam2D::load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st)
+{
+    const auto t0 = clk::now();
+    CheckpointStats local;
+    CheckpointStats& s = st ? *st : local;
+    s = CheckpointStats();
+    std::vector<uint8_t> file;
+    uint32_t kind = 0;
+    *code = ckpt_read_file(path, file, &kind, err, &s);
+    if (*code != LAMA_OK) return nullptr;
+    *code = LAMA_ERR_ARG;
+    if (kind != kCkptGraphSlam2D) {
+        err = wrong_kind(kind, "GraphSlam2D");
+        return nullptr;
+    }
+    const auto t1 = clk::now();
+    CkptReader r(file.data() + kCkptHeaderBytes, file.size() - kCkptHeaderBytes);
+    GraphOptions g;
+    g.key_pose_distance = r.f64("graph options"); g.key_pose_angular_distance = r.f64("graph options"); g.key_pose_head_delay = r.i32("graph options");
+    g.loop_search_max_distance = r.f64("graph options"); g.loop_search_min_distance = r.f64("graph options"); g.loop_max_candidates = r.i32("graph options");
+    g.loop_closure_scan_rmse = r.f64("graph options"); g.loop_closure_max_candidates = r.i32("graph options"); g.ignore_n_chain_poses = r.i32("graph options");
+    // an infinite threshold is a user's way to switch a test off (key_pose_angular_distance = inf: keys by distance only), so only NaN is refused
+    bool nan = false;
+    for (double v : {g.key_pose_distance, g.key_pose_angular_distance, g.loop_search_max_distance, g.loop_search_min_distance, g.loop_closure_scan_rmse})
+        nan = nan || std::isnan(v);
+    if (r.ok() && (nan || g.key_pose_head_delay < 0 || g.ignore_n_chain_poses < 0 || g.loop_max_candidates < 0)) r.fail("bad graph options");
+    SlamSaved sv;
+    Slam2D::ckpt_get(r, false, sv);
+    if (r.ok() && (!sv.opt.transient_map || sv.opt.truncated_ray != 1.0 || sv.opt.occupancy != 0))
+        r.fail("the inner Slam2D's options are not the ones GraphSlam2D forces (transient map, truncated_ray 1, frequency map, no lidar odometry)");
+    // graph state
+    const SE2 correction = r.se2("graph state"), prev = r.se2("graph state");
+    const double accdist = r.f64("graph state"), factordist = r.f64("graph state");
+    const uint64_t mapping_keyid = r.u64("graph state");
+    Stats stats;
+    stats.loop_factors = r.u64("graph stats"); stats.optimizations = r.u64("graph stats"); stats.optimizations_ok = r.u64("graph stats");
+    stats.last.status = r.i32("last report"); stats.last.iterations = r.u32("last report"); stats.last.lambda_tries = r.u32("last report");
+    stats.last.cg_iterations = r.u64("last report");
+    stats.last.initial_error = r.f64("last report"); stats.last.final_error = r.f64("last report"); stats.last.device_ms = r.f64("last report");
+    std::vector<int32_t> cands;
+    r.array(cands, r.u32("last candidates"), "last candidates");
+    double center[2];
+    center[0] = r.f64("window centre"); center[1] = r.f64("window centre");
+    if (r.ok() && (!finite_se2(correction) || !finite_se2(prev) || !std::isfinite(accdist) || !std::isfinite(factordist) || !finite3(center, 2)))
+        r.fail("non-finite graph state");
+    // key poses: every one at least 136 bytes before its points
+    std::vector<KeyPose> keys(r.count(r.u32("key poses"), 4 + 2 * 32 + 7 * 8 + 8 + 4, "key poses"));
+    for (size_t i = 0; i < keys.size() && r.ok(); ++i) {
+        KeyPose& k = keys[i];
+        k.id = r.i32("key pose"); k.pose = r.se2("key pose"); k.original = r.se2("key pose");
+        for (double& v : k.origin) v = r.f64("key pose");
+        for (double& v : k.quat) v = r.f64("key pose");
+        k.stamp = r.f64("key pose");
+        const size_t m = r.count(r.u32("key points"), 24, "key points");
+        r.array(k.pts, 3 * m, "key points");
+        if (r.ok() && k.id != (int)i) r.fail("a key pose id differs from its index");
+        if (r.ok() && (!finite_se2(k.pose) || !finite_se2(k.original) || !finite3(k.origin, 3) || !finite3(k.quat, 4))) r.fail("non-finite key pose");
+    }
+    const size_t n = keys.size();
+    auto is_key = [n](int32_t v) { return v >= 0 && (size_t)v < n; };
+    std::vector<int32_t> link_ids;
+    r.array(link_ids, 2 * (uint64_t)r.count(r.u32("links"), 8, "links"), "links");
+    std::vector<PgoPrior> priors(r.count(r.u32("priors"), 4 + 4 * 8 + 4 * 8, "priors"));
+    for (PgoPrior& p : priors) {
+        p.node = r.i32("priors"); p.measured = r.se2("priors");
+        p.loss = get_loss(r, "priors");
+        if (r.ok() && !is_key(p.node)) r.fail("a prior names no key");
+        if (r.ok() && !finite_se2(p.measured)) r.fail("non-finite prior");
+    }
+    std::vector<PgoBetween> factors, queue;
+    get_betweens(r, factors, n, "factors");
+    get_betweens(r, queue, n, "loop-factor queue");
+    if (r.ok()) {
+        for (int32_t v : link_ids)
+            if (!is_key(v)) r.fail("a link names no key");
+        for (int32_t v : cands)
+            if (!is_key(v)) r.fail("a loop candidate names no key");
+        if (mapping_keyid > n) r.fail("mapping key id past the key poses");
+    }
+    EngineImage inner, gimg;
+    bool inner_present = false, global_present = false;
+    if (r.ok()) ckpt_get_engine(r, &inner_present, inner, 1, 0, false);
+    if (r.ok() && inner_present && inner.known_plane) r.fail("the inner engine has a known plane");
+    if (r.ok() && (sv.has_first || n > 0) && !inner_present) r.fail("a GraphSlam2D past its first scan without device state");
+    if (r.ok()) ckpt_get_engine(r, &global_present, gimg, 1, 0, true);
+    if (r.ok() && global_present && !gimg.known_plane) r.fail("the global map's engine has no known plane");
+    if (r.ok() && global_present != (mapping_keyid > 0)) r.fail("a global map section must be present exactly when the mapping key id is above 0");
+    if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
+    if (!r.ok()) { err = r.error(); return nullptr; }
+    if (!geometry_matches(dev, sv.opt.dev, inner_present ? &inner : nullptr, err)) return nullptr;
+    s.encode_ms += ms_since(t1);
+    // the file is valid: from here on the device
+    if (cuda_device_count() < 1) { *code = LAMA_ERR_NO_DEVICE; err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
+    std::unique_ptr<Slam2D> slam(Slam2D::ckpt_restore(sv, inner_present ? &inner : nullptr, dev, err, code, &s.dev));
+    if (!slam) return nullptr;
+    if (slam->engine()) slam->engine()->set_center(center[0], center[1]);
+    std::unique_ptr<GraphSlam2D> p(new GraphSlam2D());
+    g.slam = sv.opt;
+    g.slam.dev.device = dev.device; g.slam.dev.stream = dev.stream; g.slam.dev.timing = dev.timing;   // pgo_optimize_graph runs there
+    p->opt_ = g;
+    p->slam_ = std::move(slam);
+    if (global_present) {
+        CheckpointTimes t;
+        Engine* e = Engine::restore(gimg, dev.device, dev.stream, err, &t);
+        if (!e) { *code = LAMA_ERR_CUDA; return nullptr; }
+        e->enable_timing(dev.timing != 0);
+        p->occ_.reset(OccupancyMapDev::adopt(e));
+        add_times(s.dev, t);
+    }
+    p->mapping_keyid_ = (size_t)mapping_keyid;
+    p->keys_ = std::move(keys);
+    for (size_t i = 0; i < link_ids.size(); i += 2) p->links_.push_back({link_ids[i], link_ids[i + 1]});
+    p->priors_ = std::move(priors);
+    p->factors_ = std::move(factors);
+    p->queue_ = std::move(queue);
+    p->last_candidates_.assign(cands.begin(), cands.end());
+    p->correction_ = correction;
+    p->accdist_ = accdist;
+    p->prev_ = prev;
+    p->factordist_ = factordist;
+    p->stats_ = stats;
+    s.used_slots = (uint64_t)inner.used + gimg.used;
+    s.references = sum_refs(inner) + sum_refs(gimg);
     s.total_ms   = ms_since(t0);
     *code = LAMA_OK;
     return p.release();

@@ -18,6 +18,8 @@ namespace lama_b200 {
 
 struct ShardComm;
 struct CheckpointStats;
+class CkptWriter;
+class CkptReader;
 
 struct DeviceOptions {
     int device = 0, dir_dim = 64, pool_slots = 0, max_beams = 2048, timing = 0;
@@ -174,6 +176,16 @@ struct SlamOptions {  // include/lama/slam2d.h:91-125
     DeviceOptions dev;
 };
 
+// the options and host state of a Slam2D checkpoint (every section of a kind-2 / kind-3 file but the engine), as read and checked
+struct SlamSaved {
+    SlamOptions opt;
+    SE2 pose{1, 0, 0, 0}, odom{1, 0, 0, 0}, map_update_pose{1, 0, 0, 0};
+    bool has_first = false, engine_ready = false;
+    uint32_t processed = 0;
+    uint64_t removed = 0, map_updates = 0;
+    Counters last, total;
+};
+
 class Slam2D {
 public:
     static Slam2D* create(const SlamOptions& o, std::string& err);
@@ -192,6 +204,12 @@ public:
     // checkpoints, as PFSlam2D::save / load; a handle saved before its first scan has no engine section
     int save(const std::string& path, CheckpointStats* st = nullptr);
     static Slam2D* load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st = nullptr);
+    // The options and state sections, shared by Slam2D files and the inner Slam2D of a GraphSlam2D file.  ckpt_get reads and checks them
+    // (lidar_odometry must match the file kind); ckpt_restore builds the handle on dev.device / dev.stream with dev.timing and, when
+    // `img` is given, restores its engine (*code = LAMA_ERR_CUDA when that fails).
+    void ckpt_put(CkptWriter& w) const;
+    static void ckpt_get(CkptReader& r, bool lidar_odometry, SlamSaved& s);
+    static Slam2D* ckpt_restore(const SlamSaved& s, const EngineImage* img, const DeviceOptions& dev, std::string& err, int* code, CheckpointTimes* t);
 
 private:
     SlamOptions opt_;
@@ -231,6 +249,7 @@ class OccupancyMapDev {
 public:
     // one-particle engine; dev.pool_slots 0 = dir_dim^2 slots, so a full window cannot run out of patches
     static OccupancyMapDev* create(double resolution, uint32_t patch_size, double cx, double cy, const DeviceOptions& dev, std::string& err);
+    static OccupancyMapDev* adopt(Engine* e);   // a map around a restored engine (one particle, frequency, known plane); takes ownership
     // GraphSlam2D::generateOccupancyMap's loop body (graph_slam2d.cpp:136-160) for any posed scans (Engine::render_scans)
     int insert_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states, bool full,
                      uint64_t* cells);
@@ -303,6 +322,11 @@ public:
     int generate_coarse_distance_map(DistanceMapDev** out, uint32_t* processed);
     OccupancyMapDev* occupancy_map() { return occ_.get(); }
     DistanceMapDev* coarse_distance_map() { return coarse_dm_.get(); }
+    // Checkpoints (format: checkpoint.h, kind 4), as PFSlam2D::save / load: the graph options, the inner Slam2D, the key poses with
+    // their clouds, the pose graph and loop bookkeeping, the inner engine and -- when the next generate_occupancy_map would reuse it --
+    // the global map.  The coarse distance map is rebuilt by every generate_coarse_distance_map and is not saved.
+    int save(const std::string& path, CheckpointStats* st = nullptr);
+    static GraphSlam2D* load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st = nullptr);
 
 private:
     GraphOptions opt_;
