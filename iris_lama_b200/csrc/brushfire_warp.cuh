@@ -26,11 +26,17 @@ constexpr unsigned kFullMask = 0xffffffffu;
 
 // Binary heap with libstdc++ push_heap / pop_heap move order (see ddm_core.h), stored with a one-slot offset so
 // that the two children of a node form an aligned 16-byte pair and are fetched with ONE shared-memory load.
+// Two levels: the heap starts in shared memory (`slot`); a push that finds either heap of a brushfire full moves both once
+// to the particle's regions in global memory (`spill`, same layout) and the brushfire carries on there with the same
+// indices (WarpBrushfire::push_spilled).  The two levels run separate instantiations of the brushfire, so that the shared
+// one keeps its shared-memory loads and stores.
 struct SmemHeap {
-    uint64_t* slot;  // element j lives in slot[j + 1]; slot is 16-byte aligned
-    uint32_t size, cap;
+    uint64_t* slot;      // shared memory: element j lives in slot[j + 1]; 16-byte aligned
+    uint32_t size, cap;  // cap: entries in shared memory (0 once the heap has moved: every shared-level push then fails)
+    uint64_t* spill;     // the global region
+    uint32_t spill_cap;  // its capacity in entries: the heap's total capacity
 
-    __device__ __forceinline__ bool push(uint64_t value)
+    __device__ __forceinline__ static bool push_at(uint64_t* slot, uint32_t& size, uint32_t cap, uint64_t value)
     {
         if (size >= cap) return false;
         int hole = (int)size++;
@@ -44,8 +50,7 @@ struct SmemHeap {
         slot[hole + 1] = value;
         return true;
     }
-    __device__ __forceinline__ uint64_t top() const { return slot[1]; }
-    __device__ __forceinline__ uint64_t pop()
+    __device__ __forceinline__ static uint64_t pop_at(uint64_t* slot, uint32_t& size)
     {
         const uint64_t t = slot[1];
         const uint32_t last = --size;
@@ -81,6 +86,7 @@ struct SmemHeap {
         slot[hole + 1] = value;
         return t;
     }
+    template <bool kGlobal> __device__ __forceinline__ uint64_t pop() { return kGlobal ? pop_at(spill, size) : pop_at(slot, size); }
 };
 
 struct WarpBrushfire {
@@ -95,6 +101,7 @@ struct WarpBrushfire {
     const uint32_t max_sqdist;
     uint32_t err;
     bool dead;           // the pool ran dry: stop touching the map
+    bool spilled;        // both heaps live in global memory
 #ifdef LAMA_PHASE_TIMING
     long long cyc[6] = {0, 0, 0, 0, 0, 0};   // pop, current + obstacle cell, neighbour fetch, obstacle-of-neighbour check, commit (pushes + stores), pushes alone
 #define BF_CLK(v) const long long v = clock64()
@@ -106,7 +113,7 @@ struct WarpBrushfire {
 
     __device__ WarpBrushfire(const StoreView& sv, int32_t* d, int32_t* g, uint32_t* sc, int l, SmemHeap lo, SmemHeap ra, uint32_t msq)
         : s(sv), dir(d), gdir(g), scratch(sc), side((uint32_t)sv.window.dim * kPatchLen), log2dim(ilog2(sv.window.dim)), lane(l), lower_q(lo),
-          raise_q(ra), max_sqdist(msq), err(0), dead(false) {}
+          raise_q(ra), max_sqdist(msq), err(0), dead(false), spilled(false) {}
 
     __host__ __device__ static int ilog2(int v)
     {
@@ -213,13 +220,26 @@ struct WarpBrushfire {
         return w;
     }
 
-    __device__ __forceinline__ void push_lower(uint32_t prio, uint32_t key)
+    // A push that found its heap's shared part full (all lanes, warp-uniform): the first one copies both heaps to global memory
+    // and sets their shared capacities to 0, so that every later push of the shared-level code lands here too.
+    __device__ __forceinline__ void push_spilled(SmemHeap& q, uint64_t value)
     {
-        if (!lower_q.push(heap_entry(prio, key))) err |= kErrHeapOverflow;
+        if (!spilled) {
+            for (uint32_t j = lane; j < lower_q.size; j += 32) lower_q.spill[j + 1] = lower_q.slot[j + 1];
+            for (uint32_t j = lane; j < raise_q.size; j += 32) raise_q.spill[j + 1] = raise_q.slot[j + 1];
+            __syncwarp();
+            lower_q.cap = raise_q.cap = 0;
+            spilled = true;
+        }
+        if (!SmemHeap::push_at(q.spill, q.size, q.spill_cap, value)) err |= kErrHeapOverflow;
     }
-    __device__ __forceinline__ void push_raise(uint32_t prio, uint32_t key)
+    template <bool kGlobal> __device__ __forceinline__ void push(SmemHeap& q, uint32_t prio, uint32_t key)
     {
-        if (!raise_q.push(heap_entry(prio, key))) err |= kErrHeapOverflow;
+        if (kGlobal) {
+            if (!SmemHeap::push_at(q.spill, q.size, q.spill_cap, heap_entry(prio, key))) err |= kErrHeapOverflow;
+        } else if (!SmemHeap::push_at(q.slot, q.size, q.cap, heap_entry(prio, key))) {
+            push_spilled(q, heap_entry(prio, key));
+        }
     }
 
     // dynamic_distance_map.cpp:212-226 / :228-242 (warp-uniform)
@@ -229,7 +249,7 @@ struct WarpBrushfire {
         const uint32_t w = touch(c);
         if ((w & kDmValid) && dm_sqdist(w) == 0) return;
         *c = dm_pack(0, 0, 0, true, true);
-        push_lower(0, key_of(x, y));
+        push<false>(lower_q, 0, key_of(x, y));
     }
     __device__ __forceinline__ void remove_obstacle(uint32_t x, uint32_t y)
     {
@@ -237,11 +257,11 @@ struct WarpBrushfire {
         const uint32_t w = touch(c);
         if (!((w & kDmValid) && dm_sqdist(w) == 0)) return;
         *c = dm_pack(0, 0, 0, false, true);
-        push_raise(0, key_of(x, y));
+        push<false>(raise_q, 0, key_of(x, y));
     }
 
     // :244-279
-    __device__ __forceinline__ void raise(uint32_t x, uint32_t y, uint32_t* cur)
+    template <bool G> __device__ __forceinline__ void raise(uint32_t x, uint32_t y, uint32_t* cur)
     {
         const int i = lane & 3;
         const bool act = lane < 4;
@@ -264,10 +284,10 @@ struct WarpBrushfire {
             const uint32_t k  = __shfl_sync(kFullMask, key, j);
             const uint32_t pr = __shfl_sync(kFullMask, dm_sqdist(n), j);
             if (clr) {
-                push_raise(pr, k);
+                push<G>(raise_q, pr, k);
                 if (lane == j) *p = dm_pack(0, 0, 0, false, true);
             } else {  // `else if (not neighbor->is_queued)` is always taken here
-                push_lower(pr, k);
+                push<G>(lower_q, pr, k);
                 if (lane == j) *p = n | kDmQueued;
             }
             __syncwarp();
@@ -277,7 +297,7 @@ struct WarpBrushfire {
     }
 
     // :281-330 ; `c` is the current cell word, known to be queued
-    __device__ __forceinline__ void lower(uint32_t x, uint32_t y, uint32_t* cur, uint32_t c)
+    template <bool G> __device__ __forceinline__ void lower(uint32_t x, uint32_t y, uint32_t* cur, uint32_t c)
     {
         const int cox = dm_ox(c), coy = dm_oy(c);
         const int i = lane & 3;
@@ -314,7 +334,7 @@ struct WarpBrushfire {
             const int l = __ffs(m) - 1;
             m &= m - 1;
             BF_CLK(c4);
-            push_lower(__shfl_sync(kFullMask, new_sq, l), __shfl_sync(kFullMask, key, l));
+            push<G>(lower_q, __shfl_sync(kFullMask, new_sq, l), __shfl_sync(kFullMask, key, l));
             BF_CLK(c5);
             BF_ACC(5, c4, c5);
             if (lane == l) *p = dm_pack(new_sq, rx, ry, true, true);
@@ -325,21 +345,22 @@ struct WarpBrushfire {
         BF_ACC(4, c2, c3);
     }
 
-    // :160-197
-    __device__ __forceinline__ uint32_t update()
+    // :160-197 at one heap level; returns true when the heaps moved to global memory (the caller continues with G = true)
+    template <bool G> __device__ __forceinline__ bool run(uint32_t& processed)
     {
-        uint32_t processed = 0;
         while (raise_q.size) {
-            const uint32_t key = heap_key(raise_q.pop());
+            if (!G && spilled) return true;
+            const uint32_t key = heap_key(raise_q.pop<G>());
             const uint32_t x = key & 0xFFFFu, y = key >> 16;
             uint32_t* cur = uptr(x, y);
             touch(cur);
             ++processed;
-            raise(x, y, cur);
+            raise<G>(x, y, cur);
         }
         while (lower_q.size) {
+            if (!G && spilled) return true;
             BF_CLK(a0);
-            const uint32_t key = heap_key(lower_q.pop());
+            const uint32_t key = heap_key(lower_q.pop<G>());
             BF_CLK(a1);
             BF_ACC(0, a0, a1);
             const uint32_t x = key & 0xFFFFu, y = key >> 16;
@@ -350,9 +371,15 @@ struct WarpBrushfire {
                 const uint32_t o = touch(rel_uptr(cur, x, y, dm_ox(c), dm_oy(c)));
                 BF_CLK(a2);
                 BF_ACC(1, a1, a2);
-                if (dm_sqdist(o) == 0 && (c & kDmQueued)) lower(x, y, cur, c);
+                if (dm_sqdist(o) == 0 && (c & kDmQueued)) lower<G>(x, y, cur, c);
             }
         }
+        return false;
+    }
+    __device__ __forceinline__ uint32_t update()
+    {
+        uint32_t processed = 0;
+        if (run<false>(processed)) run<true>(processed);
         return processed;
     }
 };

@@ -893,6 +893,19 @@ int lama_dm_import(lama_dm* dm, uint32_t x0, uint32_t y0, int w, int hgt, const 
                    const int16_t* ox, const int16_t* oy, const uint8_t* queued)
 try {
     if (!dm || !sqdist || !valid || !known) return set_err("null argument", LAMA_ERR_ARG);
+    // The packed cell holds 12 bits of sqdist and 7-bit offsets, and the scan matcher's distance table has max_sqdist + 1 entries:
+    // a cell outside those ranges would be stored truncated, or read past the table.  The reference keeps every valid cell below
+    // max_sqdist (an obstacle's wave stops there).
+    const uint32_t max_sqdist = dm->d->engine()->max_sqdist();
+    for (size_t i = 0; i < (size_t)w * hgt; ++i) {
+        if (!known[i]) continue;
+        if (sqdist[i] > kDmSqMask || (valid[i] && sqdist[i] >= max_sqdist))
+            return set_err("lama_dm_import: cell " + std::to_string(i) + " has sqdist " + std::to_string(sqdist[i]) + " (valid cells stay below max_sqdist " +
+                               std::to_string(max_sqdist) + ")",
+                           LAMA_ERR_ARG);
+        if ((ox && (ox[i] < -64 || ox[i] > 63)) || (oy && (oy[i] < -64 || oy[i] > 63)))
+            return set_err("lama_dm_import: cell " + std::to_string(i) + " has an obstacle offset outside [-64, 63]", LAMA_ERR_ARG);
+    }
     std::vector<uint32_t> words((size_t)w * hgt);
     for (size_t i = 0; i < words.size(); ++i) {
         if (!known[i]) { words[i] = 0; continue; }

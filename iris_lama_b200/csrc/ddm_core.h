@@ -29,6 +29,7 @@ struct Heap {
     uint64_t* data;
     uint32_t size;
     uint32_t cap;
+    uint32_t peak = 0;   // largest size reached (the host emulation reports it; the kernels use SmemHeap)
 };
 
 // std::push_heap after vector::push_back  (stl_heap.h __push_heap with topIndex = 0)
@@ -36,6 +37,7 @@ LAMA_HD bool heap_push(Heap& h, uint64_t value)
 {
     if (h.size >= h.cap) return false;
     int64_t hole = h.size++;
+    if (h.size > h.peak) h.peak = h.size;
     int64_t parent = (hole - 1) / 2;
     while (hole > 0 && heap_comp(h.data[parent], value)) {
         h.data[hole] = h.data[parent];

@@ -116,6 +116,17 @@ static int next_pow2_host(int v)
     return p;
 }
 
+bool Engine::reach_fits(double resolution, double l2_max, uint32_t* radius, std::string& err)
+{
+    const double r = std::ceil(l2_max * (1.0 / resolution));
+    if (!(resolution > 0) || !(r >= 0 && r <= kDmMaxRadius)) {
+        err = "l2_max / resolution exceeds 63 cells (packed distance cell limit)";
+        return false;
+    }
+    *radius = (uint32_t)r;
+    return true;
+}
+
 Engine* Engine::create(const EngineConfig& cfg, std::string& err)
 {
     int ndev = 0;
@@ -133,11 +144,8 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
         return nullptr;
     }
     const double scale = 1.0 / cfg.resolution;
-    uint32_t radius = (uint32_t)std::ceil(cfg.l2_max * scale);  // DynamicDistanceMap::setMaxDistance, dynamic_distance_map.cpp:149-153
-    if (radius > (uint32_t)kDmMaxRadius) {
-        err = "l2_max * scale exceeds 63 cells (packed distance cell limit)";
-        return nullptr;
-    }
+    uint32_t radius = 0;
+    if (!reach_fits(cfg.resolution, cfg.l2_max, &radius, err)) return nullptr;
     Engine* e = new Engine();
     e->cfg_ = cfg;
     e->max_sqdist_ = radius * radius;
@@ -223,8 +231,27 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     d->ray.event_cap = next_pow2_host(std::max(std::max(2048, cfg.max_beams), cfg.event_cap));
     d->ray.scan.n_beams = cfg.max_beams;  // shared-memory budget is registered for the largest scan
     d->brush.event_cap = d->ray.event_cap;
-    d->brush.lower_cap = 8192;
-    d->brush.raise_cap = 2048;
+    // The brushfire heaps start in shared memory (8 192 lower and 2 048 raise entries, sized with the L1 the kernel's prefetch
+    // needs) and move, when a push finds one full, to a per-particle region in global memory of 65 536 entries each: the
+    // capacities of the host emulation that the CPU tests run against the reference, seven times the largest lower heap
+    // measured on the synthetic datasets (9 344 at 0.015 m with a 61-cell reach).  1 MiB per particle.
+    d->brush.lower_cap   = 8192;
+    d->brush.raise_cap   = 2048;
+    d->brush.lower_total = 65536;
+    d->brush.raise_total = 65536;
+    if (const char* hc = std::getenv("LAMA_BRUSH_HEAP_CAP")) {   // test hook: total entries of each heap (overflow at a small size)
+        const int v = std::max(2, std::min(65536, std::atoi(hc))) & ~1;
+        d->brush.lower_total = d->brush.raise_total = v;
+    }
+    if (const char* sc = std::getenv("LAMA_BRUSH_SMEM_HEAP")) {  // test hook: shared entries of each heap (forces the spill to global memory)
+        const int v = std::max(2, std::atoi(sc)) & ~1;
+        d->brush.lower_cap = std::min(d->brush.lower_cap, v);
+        d->brush.raise_cap = std::min(d->brush.raise_cap, v);
+    }
+    d->brush.lower_cap = std::min(d->brush.lower_cap, d->brush.lower_total);
+    d->brush.raise_cap = std::min(d->brush.raise_cap, d->brush.raise_total);
+    CU_NEW(dalloc((void**)&d->brush.lower_spill, (size_t)cfg.particles * (d->brush.lower_total + 2 + d->brush.raise_total + 2) * 8));
+    d->brush.raise_spill = d->brush.lower_spill + (size_t)cfg.particles * (d->brush.lower_total + 2);
     d->brush.max_sqdist = e->max_sqdist_;
     CU_NEW(dalloc((void**)&d->d_events, (size_t)cfg.particles * d->ray.event_cap * 8));
     {   // scratch of the pull ray cast (k_ray_setup -> k_ray_pull)
@@ -395,7 +422,15 @@ int Engine::check_device_status()
     if (!st) return LAMA_OK;
     if (st & kErrWindow) return fail("map grew outside the directory window (raise dir_dim)", LAMA_ERR_WINDOW);
     if (st & kErrPoolEmpty) return fail("patch pool exhausted (raise pool_slots)", LAMA_ERR_POOL);
-    return fail("event log / heap overflow in the map update kernels", LAMA_ERR_OVERFLOW);
+    if (st & kErrHeapOverflow)
+        return fail("brushfire heap overflow: a distance-map update queued more than " + std::to_string(d_->brush.lower_total) + " (lower) or " +
+                        std::to_string(d_->brush.raise_total) + " (raise) cells at once",
+                    LAMA_ERR_OVERFLOW);
+    if (st & kErrPushOverflow)
+        return fail("obstacle event list overflow: more addObstacle / removeObstacle calls in one map update than the per-particle list holds (" +
+                        std::to_string(d_->brush.event_cap) + ")",
+                    LAMA_ERR_OVERFLOW);
+    return fail("ray-cast log overflow in the map update kernels", LAMA_ERR_OVERFLOW);
 }
 
 uint32_t Engine::device_status()
@@ -839,8 +874,7 @@ int Engine::dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_a
     std::vector<uint64_t> ev;
     int done = 0;
     do {  // One brushfire over the whole list reproduces the reference (all cells queued, then ONE update()).  Lists longer than the
-          // per-particle event buffer (2 048 cells: the waves they start already fill most of the 8 192-entry heap in shared
-          // memory) are applied in pieces with a brushfire after each, which gives a valid distance map but not necessarily the
+          // per-particle event buffer (2 048 cells) are applied in pieces with a brushfire after each, which gives a valid distance map but not necessarily the
           // reference's tie order -- big maps are loaded with lama_dm_read / lama_dm_import instead (DESIGN.md 10).
         int m = std::min(cap, n - done);
         ev.resize((size_t)std::max(m, 1));

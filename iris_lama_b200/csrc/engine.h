@@ -77,6 +77,10 @@ struct KernelTimes {  // accumulated CUDA-event durations (ms) and launch counts
 class Engine {
 public:
     static Engine* create(const EngineConfig& cfg, std::string& err);
+    // DynamicDistanceMap::setMaxDistance (dynamic_distance_map.cpp:149-153): the reach ceil(l2_max * scale) in cells.  False (and
+    // `err` set) when it exceeds kDmMaxRadius, the largest offset of the packed distance cell; front ends that create their engine
+    // on the first scan check it when they are created.
+    static bool reach_fits(double resolution, double l2_max, uint32_t* radius, std::string& err);
     ~Engine();
 
     const EngineConfig& config() const { return cfg_; }

@@ -57,6 +57,7 @@ PFSlam2D* PFSlam2D::create(const PFOptions& o, std::string& err)
 {
     if (o.particles < 1) { err = "PFSlam2D: Options::particles must be set (>= 1)"; return nullptr; }
     if (o.patch_size != 32) { err = "PFSlam2D: only patch_size 32 is supported on the device"; return nullptr; }
+    { uint32_t r; if (!Engine::reach_fits(o.resolution, o.l2_max, &r, err)) { err = "PFSlam2D: " + err; return nullptr; } }
     if (o.shard_count < 1 || o.shard_rank >= o.shard_count || o.particles % o.shard_count != 0) {
         err = "PFSlam2D: particles must divide evenly over shard_count";
         return nullptr;
@@ -1094,6 +1095,7 @@ int GraphSlam2D::generate_coarse_distance_map(DistanceMapDev** out, uint32_t* pr
 Slam2D* Slam2D::create(const SlamOptions& o, std::string& err)
 {
     if (o.patch_size != 32) { err = "Slam2D: only patch_size 32 is supported on the device"; return nullptr; }
+    { uint32_t r; if (!Engine::reach_fits(o.resolution, o.l2_max, &r, err)) { err = "Slam2D: " + err; return nullptr; } }
     if (cuda_device_count() < 1) { err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
     Slam2D* s = new Slam2D();
     s->opt_ = o;

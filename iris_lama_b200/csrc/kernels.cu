@@ -1413,7 +1413,9 @@ k_brushfire(StoreView s, BrushParams bp, const uint64_t* __restrict__ events, Ma
     bt[1] = clock64();
 #endif
 
-    WarpBrushfire bf(s, dir, gdir, scratch, lane, SmemHeap{lower_h, 0u, (uint32_t)bp.lower_cap}, SmemHeap{raise_h, 0u, (uint32_t)bp.raise_cap},
+    WarpBrushfire bf(s, dir, gdir, scratch, lane,
+                     SmemHeap{lower_h, 0u, (uint32_t)bp.lower_cap, bp.lower_spill + (size_t)blockIdx.x * (bp.lower_total + 2), (uint32_t)bp.lower_total},
+                     SmemHeap{raise_h, 0u, (uint32_t)bp.raise_cap, bp.raise_spill + (size_t)blockIdx.x * (bp.raise_total + 2), (uint32_t)bp.raise_total},
                      bp.max_sqdist);
     bf.err |= my_err;
     for (uint32_t i = 0; i < nev; ++i) {

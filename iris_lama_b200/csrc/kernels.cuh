@@ -71,7 +71,12 @@ struct BrushParams {
     int set;
     int particle_offset;
     int event_cap;         // stride of the per-particle event lists
-    int lower_cap, raise_cap;
+    int lower_cap, raise_cap;   // shared-memory part of the two brushfire heaps (entries)
+    // global part: per block of a launch, lower_spill + b * (lower_total + 2) and raise_spill + b * (raise_total + 2)
+    // (16-byte aligned, same layout as the shared heaps); a heap past lower_total / raise_total entries is an overflow
+    uint64_t* lower_spill;
+    uint64_t* raise_spill;
+    int lower_total, raise_total;
     uint32_t max_sqdist;
     int debug;             // LAMA_PHASE_TIMING builds only: print the per-particle phase cycles of this launch
 };

@@ -63,6 +63,7 @@ struct Emu {
     uint32_t max_iter = 100;
     int strategy = 0;
     uint32_t last_pops = 0, last_cells = 0, last_events = 0, last_log = 0, last_evals = 0, last_iters = 0;
+    uint32_t heap_peak[2] = {0, 0};   // largest lower / raise heap size of any brushfire since creation
     bool pull = false;   // map updates through the pull form of the ray cast (ray_pull.h) instead of the per-beam walk
     uint32_t pull_fallbacks = 0;
 };
@@ -169,6 +170,12 @@ void update_maps(Emu& e, const ScanParams& sp, const double* pts, const SE2& pos
     run_brushfire(e, events, cells, (uint32_t)log.size());
 }
 
+void note_heap_peak(Emu& e, const Brushfire<HostDm>& bf)
+{
+    e.heap_peak[0] = std::max(e.heap_peak[0], bf.lower_q.peak);
+    e.heap_peak[1] = std::max(e.heap_peak[1], bf.raise_q.peak);
+}
+
 void run_brushfire(Emu& e, std::vector<uint64_t>& events, uint32_t cells, uint32_t log_size)
 {
     const DirWindow win = e.occ.window;
@@ -183,6 +190,7 @@ void run_brushfire(Emu& e, std::vector<uint64_t>& events, uint32_t cells, uint32
         else bf.remove_obstacle(key_x(win, key), key_y(win, key));
     }
     e.last_pops   = bf.update();
+    note_heap_peak(e, bf);
     e.last_cells  = cells;
     e.last_events = (uint32_t)events.size();
     e.last_log    = log_size;
@@ -683,7 +691,17 @@ uint32_t emu_dm_apply(void* h, const uint32_t* cells_xy, const uint8_t* is_add, 
         if (is_add[i]) bf.add_obstacle(cells_xy[2 * i], cells_xy[2 * i + 1]);
         else bf.remove_obstacle(cells_xy[2 * i], cells_xy[2 * i + 1]);
     }
-    return bf.update();
+    const uint32_t pops = bf.update();
+    note_heap_peak(*e, bf);
+    return pops;
+}
+// largest lower [0] and raise [1] heap size of any brushfire of this emulation so far (k_brushfire keeps the first
+// BrushParams::lower_cap / raise_cap entries in shared memory)
+void emu_heap_peak(void* h, uint32_t* out)
+{
+    Emu* e = (Emu*)h;
+    out[0] = e->heap_peak[0];
+    out[1] = e->heap_peak[1];
 }
 // replay_cell (ray_core.h) on one frequency cell as k_raycast runs it: the touches kinds[i] (1 hit / 0 miss, beam order) are first
 // added to the packed word {visited, occupied} = word_in (packed adds carry from occupied into visited; they commute, so their

@@ -122,7 +122,8 @@ X0, Y0 = 0.0, 0.0   # the prior: cell (O, O)
 # the walk logs every touch of a candidate cell (hit in this scan or a distance-map obstacle); edge scans cross many of them, so the
 # engines get a 16 384-record log (3 * max_beams, rounded up to a power of two), which fits shared memory with a 32-patch window
 EDGE_DEV = dict(dir_dim=32, max_beams=4096)
-# every end cell of an edge scan is a separate new obstacle: with a one-cell distance-map reach their brushfire waves fit the device heaps
+# every end cell of an edge scan is a separate new obstacle: a one-cell distance-map reach keeps these tests about the ray cast
+# (test_gpu_reach.py covers reaches up to 63 cells and brushfire heaps that outgrow shared memory)
 EDGE_L2 = dict(l2_max=0.05)
 
 
