@@ -298,6 +298,11 @@ int lama_dm_match_error(lama_dm* dm, const double* pts_xyz, int n, const double 
  * nodes (measured = node[i]^-1 node[i+1]) and on the edges, sigmas (0.5, 0.5, 0.1), miniSAM Levenberg-Marquardt with diagonal damping
  * (vendor/minisam/minisam/nonlinear/LevenbergMarquardtOptimizer.cpp:56-332).  *status = miniSAM's NonlinearOptimizationStatus (0 SUCCESS,
  * 1 MAX_ITERATION, 2 ERROR_INCREASE, 3 RANK_DEFICIENCY, 4 INVALID); like the reference, nodes_xyr is only updated on SUCCESS.
+ * A lambda try whose damped system cannot be solved is rejected and lambda raised, as the reference does when its sparse LDL^T reports
+ * RANK_DEFICIENCY: a damped diagonal block with a zero diagonal entry (a node that no factor references) or a conjugate-gradient solve
+ * that stops at its cap of 4 n_nodes + 200 iterations above its 1e-10 relative residual.  If every try up to lambda 1e10 fails the status
+ * is 2 (ERROR_INCREASE, after 10 tries from the first linearisation).  4 (INVALID) means non-finite numbers in an otherwise regular system.
+ * An edge with from == to is refused with LAMA_ERR_ARG before any device call.
  * report = {LM iterations, lambda tries, CG iterations, initial error, final error, device ms}. */
 int lama_pgo_optimize(int device, double* nodes_xyr, int n_nodes, const int* edges_from_to, const double* edges_xyr, int n_edges, const int* fixed_nodes,
                       const double* fixed_xyr, int n_fixed, int* status, double report[6]);
@@ -327,7 +332,8 @@ int lama_dm_coarse_correlate_candidate_scan(lama_dm* dm, const double* ref_pts_x
  * priors: PriorFactor<SE2> on prior_nodes[i] measured prior_xyr[i]; betweens: BetweenFactor<SE2> between_from_to[2i] -> [2i+1] measured between_xyr[i].
  * Each factor's loss is loss[4] = {sigma_x, sigma_y, sigma_theta, huber_k}: huber_k <= 0 gives DiagonalLoss::Sigmas (core/LossFunction.cpp:95-114),
  * huber_k > 0 gives HuberLoss::Huber(huber_k) on the raw error (:190-203; the sigmas are ignored).  Factors enter the graph priors first, then
- * betweens, in the given order.  *status, report and the SUCCESS-only update of nodes_xyr are those of lama_pgo_optimize.  accepted (may be NULL)
+ * betweens, in the given order; a between factor with from == to is refused with LAMA_ERR_ARG (miniSAM's Hessian assembly assumes two distinct
+ * keys).  *status, report, the rejected tries and the SUCCESS-only update of nodes_xyr are those of lama_pgo_optimize.  accepted (may be NULL)
  * receives one byte per tried lambda, 1 accepted / 0 rejected, at most accepted_cap of them; *n_tries (may be NULL) = the number of tries. */
 int lama_pgo_optimize_graph(int device, double* nodes_xyr, int n_nodes, const int* prior_nodes, const double* prior_xyr, const double* prior_loss, int n_priors,
                             const int* between_from_to, const double* between_xyr, const double* between_loss, int n_betweens, int* status, double report[6],

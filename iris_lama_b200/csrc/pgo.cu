@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstdlib>
 
 #include "engine.h"   // status codes
 
@@ -126,7 +127,7 @@ struct PcgBuffers {
     double* x;  double* r;  double* z;  double* p;  double* Ap;   // n_nodes x 3 each
     double* Minv;      // n_nodes x 9: inverse of the damped diagonal block
     double* partial;   // gridDim x 4 scratch of the reductions
-    double* out;       // {r.r at exit, b.b, 0.5 dx.(lambda diag dx + b), iterations}
+    double* out;       // {r.r at exit, b.b, 0.5 dx.(lambda diag dx + b), iterations, damped diagonal blocks with a zero diagonal entry}
 };
 
 __device__ __forceinline__ double block_sum(double v, double* sh)
@@ -159,11 +160,13 @@ k_pgo_pcg(PgoView g, PcgBuffers w, double lambda, double rel_tol, int max_iter)
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
     const int n = g.n_nodes;
     // damped diagonal blocks and their inverses (block-Jacobi preconditioner); x = 0, r = b, z = M^-1 r, p = z
-    double loc_rz = 0.0, loc_bb = 0.0;
+    double loc_rz = 0.0, loc_bb = 0.0, loc_zero = 0.0;
     for (int i = tid; i < n; i += nthreads) {
         double m[9];
         for (int k = 0; k < 9; ++k) m[k] = g.D[9 * (size_t)i + k];
         m[0] += lambda * m[0]; m[4] += lambda * m[4]; m[8] += lambda * m[8];   // updateDumpingHessianDiag (LevenbergMarquardtOptimizer.cpp:369-374)
+        // a zero diagonal entry: a node no factor references (lambda * 0 = 0), where the reference's LDL^T meets a zero pivot
+        if (m[0] == 0.0 || m[4] == 0.0 || m[8] == 0.0) loc_zero += 1.0;
         const double c0 = m[4] * m[8] - m[5] * m[7], c1 = m[5] * m[6] - m[3] * m[8], c2 = m[3] * m[7] - m[4] * m[6];
         const double det = m[0] * c0 + m[1] * c1 + m[2] * c2, id = 1.0 / det;
         double* mi = w.Minv + 9 * (size_t)i;
@@ -185,9 +188,10 @@ k_pgo_pcg(PgoView g, PcgBuffers w, double lambda, double rel_tol, int max_iter)
     }
     double rz = grid_sum(grid, loc_rz, sh, w.partial, 0);
     const double bb = grid_sum(grid, loc_bb, sh, w.partial, 1);
+    const double zero_blocks = grid_sum(grid, loc_zero, sh, w.partial, 3);   // the factorisation failed: no solve, x stays 0
     double rr = bb;
     int it = 0;
-    while (it < max_iter && rr > rel_tol * rel_tol * bb && bb > 0.0) {
+    while (zero_blocks == 0.0 && it < max_iter && rr > rel_tol * rel_tol * bb && bb > 0.0) {
         // Ap = (D + lambda diag D) p + off-diagonal blocks, gathered per node in adjacency order
         double loc_pap = 0.0;
         for (int i = tid; i < n; i += nthreads) {
@@ -262,6 +266,7 @@ k_pgo_pcg(PgoView g, PcgBuffers w, double lambda, double rel_tol, int max_iter)
         w.out[1] = bb;
         w.out[2] = 0.5 * lin;
         w.out[3] = (double)it;
+        w.out[4] = zero_blocks;
     }
 }
 
@@ -335,6 +340,7 @@ int pgo_optimize_graph(int device, std::vector<SE2>& nodes, const std::vector<Pg
     }
     for (const PgoBetween& e : betweens) {
         if (e.from < 0 || e.from >= n || e.to < 0 || e.to >= n) { err = "pose graph: between factor index out of range"; return LAMA_ERR_ARG; }
+        if (e.from == e.to) { err = "pose graph: a between factor needs two distinct nodes (from == to)"; return LAMA_ERR_ARG; }
         if (bad_loss(e.loss)) { err = "pose graph: a between factor's loss needs sigmas > 0 or a finite Huber k > 0"; return LAMA_ERR_ARG; }
     }
     int ndev = 0;
@@ -423,6 +429,12 @@ int pgo_optimize_graph(int device, std::vector<SE2>& nodes, const std::vector<Pg
     const uint32_t max_iterations = 100;                                                             // NonlinearOptimizer.h:54-58
     const double min_rel = 1e-5, min_abs = 1e-5;
     double lambda = 1e-5, inc = 2.0;
+    const double cg_tol = 1e-10;    // relative residual of the damped normal equations
+    int cg_max = 4 * n + 200;       // iteration cap of a solve; one that stops there above cg_tol gave a truncated step
+    if (const char* cm = std::getenv("LAMA_PGO_CG_MAX")) {   // test hook: overrides the cap (a low one forces truncated solves)
+        const int v = std::atoi(cm);
+        if (v > 0) cg_max = v;
+    }
     cudaEventRecord(e0, st);
     double last_err = 0;
     ce = graph_error(X, &last_err);                                                                  // NonlinearOptimizer.cpp:175
@@ -436,22 +448,26 @@ int pgo_optimize_graph(int device, std::vector<SE2>& nodes, const std::vector<Pg
         double new_err = 0;
         while (lambda < lambda_max) {                                                                // LevenbergMarquardtOptimizer.cpp:121-151
             ++rep.lambda_tries;
-            double lam = lambda, tol = 1e-10;   // relative residual of the damped normal equations
-            int cg_max = 4 * n + 200;
-            void* args[] = {&g, &w, &lam, &tol, &cg_max};
+            double lam = lambda, tol = cg_tol;
+            int cap = cg_max;
+            void* args[] = {&g, &w, &lam, &tol, &cap};
             ce = cudaLaunchCooperativeKernel((void*)k_pgo_pcg, dim3(grid), dim3(256), args, 0, st);
             if (ce != cudaSuccess) return done(LAMA_ERR_CUDA, std::string("pose graph: cooperative launch: ") + cudaGetErrorString(ce));
             k_pgo_retract<<<nbk, 128, 0, st>>>(n, X, w.x, Xn);
-            double out[4];
+            double out[5];
             ce = cudaMemcpyAsync(out, w.out, sizeof(out), cudaMemcpyDeviceToHost, st);
             if (ce == cudaSuccess) ce = graph_error(Xn, &new_err);
             if (ce != cudaSuccess) return done(LAMA_ERR_CUDA, std::string("pose graph: ") + cudaGetErrorString(ce));
             rep.cg_iterations += (uint64_t)out[3];
             rep.accepted.push_back(0);
-            if (!std::isfinite(out[0]) || !std::isfinite(out[2])) { rep.status = 4; return done(LAMA_OK, ""); }   // INVALID: the linear solver broke down
+            // RANK_DEFICIENCY (SparseCholesky.cpp:26-31): a zero diagonal entry in a damped block, or a solve truncated at its cap above
+            // the tolerance.  No step; lambda is raised and the next try goes on (LevenbergMarquardtOptimizer.cpp:139-144)
+            const bool truncated = (int)out[3] >= cap && out[0] > tol * tol * out[1];
+            const bool rank_deficient = out[4] != 0.0 || truncated;
+            if (!rank_deficient && (!std::isfinite(out[0]) || !std::isfinite(out[2]))) { rep.status = 4; return done(LAMA_OK, ""); }   // INVALID
             const double nonlinear = last_err - new_err, linear = out[2];
             const double gain = nonlinear / linear;
-            if (gain > gain_thresh) {                                                                // :256-265
+            if (!rank_deficient && gain > gain_thresh) {                                             // :256-265
                 rep.accepted.back() = 1;
                 std::swap(X, Xn);
                 lambda *= std::max(dec_min, 1.0 - std::pow(2.0 * gain - 1.0, 3.0));                  // decreaseLambda_ :342-348
@@ -492,8 +508,10 @@ int pgo_optimize(int device, std::vector<SE2>& nodes, const std::vector<PgoEdge>
     rep = PgoReport();
     const int n = (int)nodes.size();
     if (n < 1) { err = "SimplePGO: no nodes"; return LAMA_ERR_ARG; }
-    for (const PgoEdge& e : edges)
+    for (const PgoEdge& e : edges) {
         if (e.from < 0 || e.from >= n || e.to < 0 || e.to >= n) { err = "SimplePGO: edge index out of range"; return LAMA_ERR_ARG; }
+        if (e.from == e.to) { err = "SimplePGO: an edge needs two distinct nodes (from == to)"; return LAMA_ERR_ARG; }
+    }
     for (const PgoFixed& f : fixed)
         if (f.node < 0 || f.node >= n) { err = "SimplePGO: fixed node out of range"; return LAMA_ERR_ARG; }
 

@@ -13,7 +13,9 @@
 // preconditioned conjugate gradient running in ONE cooperative kernel (grid-wide barriers between the phases of an iteration, all
 // reductions in a fixed order) instead of Eigen's SimplicialLDLT: the system is symmetric positive definite, so the solution is the
 // same up to the CG tolerance (relative residual 1e-10), and the LM decisions (gain ratio, lambda schedule, stop rule) follow the
-// reference line by line on the host in fp64.
+// reference line by line on the host in fp64.  Where the reference's LDL^T would report RANK_DEFICIENCY the device rejects the lambda try
+// the same way (no step, lambda raised): a damped diagonal block with a zero diagonal entry (a node no factor references), and a PCG solve
+// truncated at its iteration cap above the tolerance.
 #pragma once
 
 #include <cstdint>

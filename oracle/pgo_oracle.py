@@ -85,6 +85,8 @@ class SimplePGO:
     def __init__(self, nodes_xyr, edges=(), fixed=()):
         self.nodes = from_xyr(nodes_xyr)
         self.edges = list(edges)
+        if any(e[0] == e[1] for e in self.edges):
+            raise ValueError("an edge needs two distinct nodes (from == to)")   # miniSAM's Hessian assembly assumes distinct keys
         self.fixed = list(fixed)
         self.iterations = 0
         self.lambda_tries = 0
@@ -167,6 +169,10 @@ class SimplePGO:
             ok = False
             while lam < self.LAMBDA_MAX:                                     # :121-151
                 self.lambda_tries += 1
+                if (diag + lam * diag == 0).any():                           # zero pivot: RANK_DEFICIENCY (SparseCholesky.cpp:26-31), no step (:139-144)
+                    lam *= inc
+                    inc *= self.INC_UPDATE
+                    continue
                 Ad = (A + sp.diags(lam * diag)).tocsc()                      # dumpLinearSystem_, diagonal damping (:275-283, :369-374)
                 dx = spla.spsolve(Ad, b)
                 Xn = mul(X, exp(dx.reshape(-1, 3)))                          # Variables::retract -> origin * exp(v) (Sophus.h:64-68)

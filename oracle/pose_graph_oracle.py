@@ -33,6 +33,41 @@ def huber(k):
     return np.ones(3), float(k)
 
 
+def pcg(A, b, lam, tol=1e-10, cap=None):
+    """k_pgo_pcg restated: block-Jacobi preconditioned conjugate gradient on (A + lam diag(A)) x = b from x = 0, stopping when
+    |r|^2 <= tol^2 |b|^2 or after `cap` iterations (default 4 n + 200).  Returns (x, iterations, |r| / |b|, truncated), truncated meaning
+    the cap was reached above the tolerance; (None, 0, nan, False) when a damped diagonal entry is zero (the device solves nothing then)."""
+    n = A.shape[0] // 3
+    cap = 4 * n + 200 if cap is None else cap
+    d = A.diagonal()
+    if (d + lam * d == 0).any():
+        return None, 0, float("nan"), False
+    Ad = (A + sp.diags(lam * d)).tocsr()
+    C = Ad.tocoo()
+    on = C.row // 3 == C.col // 3
+    blk = np.zeros((n, 3, 3))
+    np.add.at(blk, (C.row[on] // 3, C.row[on] % 3, C.col[on] % 3), C.data[on])
+    Minv = np.linalg.inv(blk)
+    x = np.zeros_like(b)
+    r = b.copy()
+    z = np.einsum("nij,nj->ni", Minv, r.reshape(-1, 3)).ravel()
+    p = z.copy()
+    rz, bb = float(z @ r), float(b @ b)
+    rr, it = bb, 0
+    while it < cap and rr > tol * tol * bb and bb > 0.0:
+        Ap = Ad @ p
+        alpha = rz / float(p @ Ap)
+        x += alpha * p
+        r -= alpha * Ap
+        rr = float(r @ r)
+        z = np.einsum("nij,nj->ni", Minv, r.reshape(-1, 3)).ravel()
+        rz2 = float(z @ r)
+        p = z + (rz2 / rz) * p
+        rz = rz2
+        it += 1
+    return x, it, (np.sqrt(rr / bb) if bb > 0 else 0.0), bool(it >= cap and rr > tol * tol * bb)
+
+
 def _states(meas):
     """measured poses given as xyr triples or as SE2 states (cos, sin, tx, ty), which are taken as they are"""
     if not meas:
@@ -44,16 +79,26 @@ class PoseGraph:
     """miniSAM FactorGraph of PriorFactor<SE2> / BetweenFactor<SE2>, each with a DiagonalLoss or a HuberLoss, optimised by
     LevenbergMarquardtOptimizer::optimize.  nodes: n x 3 xyr; priors [(node, meas, (w, k))]; betweens [(from, to, meas, (w, k))], in graph.add order
     (priors first).  After optimize(): status (0 SUCCESS, 1 MAX_ITERATION, 2 ERROR_INCREASE), iterations, lambda_tries, errors (0.5 errorSquaredNorm
-    per accepted step), accepted (1 / 0 per lambda try), and nodes (updated only on SUCCESS)."""
+    per accepted step), accepted (1 / 0 per lambda try), lambdas (lambda per try), try_iterations (the LM iteration of each try), decreases
+    ((last error - trial error, last error) per try, None where no step was solved), and nodes (updated only on SUCCESS).
+
+    A try whose damped system has a zero diagonal entry (a node no factor references) is rejected and lambda raised, as the reference does
+    when its LDL^T reports RANK_DEFICIENCY.  With cg_cap set, every try also runs pcg() with that cap, cg_iterations records its iterations,
+    and a solve truncated at the cap is rejected the same way (the device's rule); the step itself is the direct solve either way."""
 
     # LevenbergMarquardtOptimizerParams / NonlinearOptimizerParams defaults
     LAMBDA_INIT, INC_INIT, INC_UPDATE, DEC_MIN, LAMBDA_MIN, LAMBDA_MAX, GAIN_THRESH = 1e-5, 2.0, 2.0, 1.0 / 3.0, 1e-20, 1e10, 1e-3
     MAX_ITER, MIN_REL, MIN_ABS = 100, 1e-5, 1e-5
 
-    def __init__(self, nodes_xyr, priors=(), betweens=()):
+    def __init__(self, nodes_xyr, priors=(), betweens=(), cg_cap=None):
         self.nodes = from_xyr(nodes_xyr)
         pr = list(priors)
         bt = list(betweens)
+        if any(b[0] == b[1] for b in bt):
+            raise ValueError("a between factor needs two distinct nodes (from == to)")   # miniSAM's Hessian assembly assumes distinct keys
+        self.cg_cap = cg_cap
+        self.cg_iterations = []
+        self.lambdas = []
         self.pri = (np.array([p[0] for p in pr], int), _states([p[1] for p in pr]),
                     np.array([p[2][0] for p in pr], float).reshape(-1, 3), np.array([p[2][1] for p in pr], float))
         self.btw = (np.array([b[0] for b in bt], int), np.array([b[1] for b in bt], int), _states([b[2] for b in bt]),
@@ -108,14 +153,19 @@ class PoseGraph:
         A = sp.coo_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(3 * n, 3 * n)).tocsc()
         return A, b.ravel()
 
-    def optimize(self):
-        """True on NonlinearOptimizationStatus::SUCCESS; node states updated in place then"""
+    def optimize(self, on_solve=None):
+        """True on NonlinearOptimizationStatus::SUCCESS; node states updated in place then.  on_solve(A, b, lam), if given, sees the
+        undamped system of every lambda try."""
         pri, btw = self.pri, self.btw
         X = self.nodes.copy()
         lam, inc = self.LAMBDA_INIT, self.INC_INIT
         last_err = self._err2(X, pri, btw)                                   # NonlinearOptimizer.cpp:175
         self.errors = [last_err]
         self.accepted = []
+        self.lambdas = []
+        self.cg_iterations = []
+        self.decreases = []
+        self.try_iterations = []
         self.iterations = 0
         self.status = 1                                                      # MAX_ITERATION unless decided otherwise
         while self.iterations < self.MAX_ITER:
@@ -124,11 +174,26 @@ class PoseGraph:
             ok = False
             while lam < self.LAMBDA_MAX:                                     # :121-151
                 self.lambda_tries += 1
+                self.lambdas.append(lam)
+                self.try_iterations.append(self.iterations)
+                self.decreases.append(None)
+                if on_solve is not None:
+                    on_solve(A, b, lam)
+                truncated = False
+                if self.cg_cap is not None:
+                    _, it, _, truncated = pcg(A, b, lam, cap=self.cg_cap)
+                    self.cg_iterations.append(it)
+                if (diag + lam * diag == 0).any() or truncated:              # RANK_DEFICIENCY (SparseCholesky.cpp:26-31): no step (:139-144, :198-204)
+                    self.accepted.append(0)
+                    lam *= inc
+                    inc *= self.INC_UPDATE
+                    continue
                 Ad = (A + sp.diags(lam * diag)).tocsc()                      # dumpLinearSystem_, diagonal damping (:275-283, :369-374)
                 dx = spla.spsolve(Ad, b)
                 Xn = mul(X, exp(dx.reshape(-1, 3)))                          # Variables::retract -> origin * exp(v) (Sophus.h:64-68)
                 new_err = self._err2(Xn, pri, btw)
                 nonlin = last_err - new_err                                  # values_curr_err = last_err_squared_norm_ (:115-116)
+                self.decreases[-1] = (nonlin, last_err)
                 lin = 0.5 * float(dx @ (lam * diag * dx + b))                # :241-247
                 gain = nonlin / lin
                 self.accepted.append(int(gain > self.GAIN_THRESH))

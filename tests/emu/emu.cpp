@@ -738,14 +738,16 @@ float emu_prob_replay(const uint8_t* kinds, int n, const double* constants, int 
     *obstacle_out = obstacle;
     return p;
 }
-// SE2 helpers of lama_core.h for comparison with the oracle's
+// SE2 helpers of lama_core.h for comparison with the oracle's.  a is a state (c, s, tx, ty) for ops 0, 1 and 4 and a 3-vector for 2 and 3.
 void emu_se2(int op, const double* a, const double* b, double* out)
 {
-    SE2 A{a[0], a[1], a[2], a[3]}, r{1, 0, 0, 0};
+    SE2 A{1, 0, 0, 0}, r{1, 0, 0, 0};
+    if (op == 0 || op == 1 || op == 4) A = SE2{a[0], a[1], a[2], a[3]};
     if (op == 0) r = se2_mul(A, SE2{b[0], b[1], b[2], b[3]});
     else if (op == 1) r = se2_inv(A);
     else if (op == 2) r = se2_exp(a);
     else if (op == 3) r = se2_from_xyr(a[0], a[1], a[2]);
+    else if (op == 4) { se2_log(A, out); out[3] = 0.0; return; }   // (upsilon, theta)
     out[0] = r.c; out[1] = r.s; out[2] = r.tx; out[3] = r.ty;
 }
 }
