@@ -495,6 +495,58 @@ int lama_om3_read(lama_om3* h, const char* path);
 int lama_om3_export_image(lama_om3* h, double zed, uint8_t* pixels, size_t cap, int dims[2]);
 /* with dev->timing: ms = device time of [0] insert_point_clouds, [1] apply, [2] query; launches likewise */
 int lama_om3_kernel_times(lama_om3* h, double ms[3], uint64_t launches[3]);
+/* ------------------------------------------------------------------------------------------------
+ * 3-D DynamicDistanceMap -- DynamicDistanceMap(resolution, patch_size, is3d = true) (include/lama/sdm/dynamic_distance_map.h,
+ * src/sdm/dynamic_distance_map.cpp): the six-neighbour dynamic brushfire, cells {obstacle offset, sqdist, valid, queued} and a known
+ * bit, in a dense window of window[0] x window[1] x window[2] patches of 32 x 32 x 32 cells.  Cells are absolute map coordinates
+ * (x, y, z) as Map::w2m gives them (lama_w2m3).  update() is one sequential device thread, so the result is the reference's bit for bit.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct lama_dm3 lama_dm3;
+/* the map with setMaxDistance(l2_max) (:149-153), which is fixed at creation; ceil(l2_max / resolution) = R must be at most 63 cells and
+ * patch_size 32.  The window is centred on center_xyz (NULL: origin); window_patches NULL = (8, 8, 4), at most 2048 per axis and 65 536
+ * entries in all.  dev->pool_slots 0 = one patch per window entry (a patch is 256 KiB, so the default takes 64 MiB).  Test hooks read
+ * here: LAMA_DM3_HEAP_CAP (initial entries of each brushfire heap, default 65 536) and LAMA_DM3_POP_BUDGET (pops per brushfire launch,
+ * default 2^20). */
+int lama_dm3_create(double resolution, uint32_t patch_size, double l2_max, const double center_xyz[3], const int32_t window_patches[3],
+                    const lama_device_options* dev, lama_dm3** out);
+int lama_dm3_destroy(lama_dm3* h);
+int lama_dm3_max_sqdist(lama_dm3* h, uint32_t* v);
+int lama_dm3_max_distance(lama_dm3* h, double* v);   /* maxDistance (:155-158) */
+/* addObstacle / removeObstacle (:212-242) of n cells (n x 3) in list order.  They are queued: update() applies them first, and every
+ * reader below applies them before it reads.  A batch is refused before anything changes with LAMA_ERR_WINDOW when a cell lies less
+ * than R + 1 cells inside the window on some axis, and with LAMA_ERR_POOL when the patches it could make the brushfire allocate (those
+ * within R cells of any cell ever added or removed) could exceed the free pool slots; the default pool never refuses. */
+int lama_dm3_add_obstacles(lama_dm3* h, const uint32_t* cells_xyz, int n);
+int lama_dm3_remove_obstacles(lama_dm3* h, const uint32_t* cells_xyz, int n);
+/* update() (:160-197); *processed (may be NULL) = its return value.  A failed device allocation (a brushfire heap grows by doubling)
+ * gives LAMA_ERR_CUDA with the remaining work still queued: a later call continues it. */
+int lama_dm3_update(lama_dm3* h, uint32_t* processed);
+/* distance(Vector3d, gradient) (:93-133) of n world points, trilinear; gradient (n x 3) may be NULL */
+int lama_dm3_distance(lama_dm3* h, const double* pts_xyz, int n, double* distance, double* gradient);
+/* distance(Vector3ui) (:140-147) of n cells: sqrt(max_sqdist) * resolution where the cell is absent, unknown or not valid */
+int lama_dm3_cell_distance(lama_dm3* h, const uint32_t* cells_xyz, int n, double* distance);
+/* Map::bounds (map.cpp:139-157) in cells, all three axes; *patches (may be NULL) = allocated patches */
+int lama_dm3_bounds(lama_dm3* h, uint32_t mn[3], uint32_t mx[3], int* patches);
+/* the box lo + [0, size) (x fastest, then y, then z): 64-bit cells, the little-endian image of {int8 ox, oy, oz; uint8 flags (1 valid,
+ * 2 queued, 4 known); uint16 sqdist; uint16 0}, 0 where there is no patch, and known bits; either output may be NULL */
+int lama_dm3_export(lama_dm3* h, const uint32_t lo[3], const int32_t size[3], uint64_t* cells, uint8_t* known);
+/* Map::write (map.cpp:490-529) with is_3d = 1 and max_sqdist (:200-203): 10-byte distance_t cells, patches in ascending window entry,
+ * where the reference iterates an unordered_map */
+int lama_dm3_write(lama_dm3* h, const char* path);
+/* Map::read (map.cpp:531-575) + readParameters (:205-208) into an empty map, which takes the file's resolution and max_sqdist.  The
+ * file is checked before anything changes: LAMA_ERR_WINDOW for a patch outside the window or a valid cell whose obstacle lies less
+ * than R + 1 cells inside it, LAMA_ERR_ARG for R above 63 or a cell that breaks the map's invariants (a valid cell has sqdist =
+ * |offset|^2 < max_sqdist; an invalid or unknown cell has sqdist 0 and offset 0), LAMA_ERR_POOL when the pool cannot hold the file's
+ * patches and those its obstacles can reach. */
+int lama_dm3_read(lama_dm3* h, const char* path);
+/* the z-slice image of sdm::export_to_png(dm, file, zed) (export.cpp:74-96): dims = {width, height} from the x / y bounds, slice
+ * z = w2m((0, 0, zed)).z, 127 where no cell is known; pixels (row-major, width per row) written when cap >= width * height */
+int lama_dm3_export_image(lama_dm3* h, double zed, uint8_t* pixels, size_t cap, int dims[2]);
+/* with dev->timing: ms = device time of [0] update (and the queue flushes of the readers), [1] distance, [2] cell_distance and export;
+ * launches likewise */
+int lama_dm3_kernel_times(lama_dm3* h, double ms[3], uint64_t launches[3]);
+/* {brushfire launches, heap growths, raise heap capacity, lower heap capacity} since creation */
+int lama_dm3_run_stats(lama_dm3* h, uint64_t stats[4]);
 /* Map::w2m (map.h:125-126) on all three axes: world points (n x 3) -> cells (n x 3) */
 int lama_w2m3(double resolution, const double* pts_xyz, int n, uint32_t* cells_xyz);
 

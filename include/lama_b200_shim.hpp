@@ -329,4 +329,28 @@ private:
     lama_om3* h_ = nullptr;
 };
 
+// lama::DynamicDistanceMap with is3d = true on the device.  Cells are map coordinates {x, y, z}; setMaxDistance is fixed at creation
+// (l2_max).  addObstacle / removeObstacle are queued and applied by update() or the next read of the map.
+class DynamicDistanceMap3D {
+public:
+    explicit DynamicDistanceMap3D(double resolution, double l2_max = 0.5, uint32_t patch_size = 32)
+    {
+        check(lama_dm3_create(resolution, patch_size, l2_max, nullptr, nullptr, nullptr, &h_));
+    }
+    ~DynamicDistanceMap3D() { lama_dm3_destroy(h_); }
+    DynamicDistanceMap3D(const DynamicDistanceMap3D&) = delete;
+    DynamicDistanceMap3D& operator=(const DynamicDistanceMap3D&) = delete;
+    void addObstacle(const uint32_t xyz[3]) { check(lama_dm3_add_obstacles(h_, xyz, 1)); }         // dynamic_distance_map.cpp:212-226
+    void removeObstacle(const uint32_t xyz[3]) { check(lama_dm3_remove_obstacles(h_, xyz, 1)); }   // :228-242
+    uint32_t update() { uint32_t n = 0; check(lama_dm3_update(h_, &n)); return n; }                // :160-197
+    double distance(const double xyz[3], double gradient[3] = nullptr) const { double d = 0; check(lama_dm3_distance(h_, xyz, 1, &d, gradient)); return d; }
+    double distance(const uint32_t xyz[3]) const { double d = 0; check(lama_dm3_cell_distance(h_, xyz, 1, &d)); return d; }
+    double maxDistance() const { double d = 0; check(lama_dm3_max_distance(h_, &d)); return d; }
+    bool write(const std::string& path) const { check(lama_dm3_write(h_, path.c_str())); return true; }
+    bool read(const std::string& path) { check(lama_dm3_read(h_, path.c_str())); return true; }
+
+private:
+    lama_dm3* h_ = nullptr;
+};
+
 }  // namespace lama_b200_shim

@@ -92,6 +92,9 @@ EXPORTED_SYMBOLS = [
     "lama_tsdm_distance", "lama_tsdm_bounds", "lama_tsdm_export", "lama_tsdm_to_mesh", "lama_tsdm_write_ply", "lama_tsdm_kernel_times",
     "lama_om3_create", "lama_om3_destroy", "lama_om3_insert_point_clouds", "lama_om3_apply", "lama_om3_query", "lama_om3_prune",
     "lama_om3_bounds", "lama_om3_export", "lama_om3_write", "lama_om3_read", "lama_om3_export_image", "lama_om3_kernel_times", "lama_w2m3",
+    "lama_dm3_create", "lama_dm3_destroy", "lama_dm3_max_sqdist", "lama_dm3_max_distance", "lama_dm3_add_obstacles", "lama_dm3_remove_obstacles",
+    "lama_dm3_update", "lama_dm3_distance", "lama_dm3_cell_distance", "lama_dm3_bounds", "lama_dm3_export", "lama_dm3_write", "lama_dm3_read",
+    "lama_dm3_export_image", "lama_dm3_kernel_times", "lama_dm3_run_stats",
     "lama_pf_save_state", "lama_pf_load_state", "lama_slam_save_state", "lama_slam_load_state", "lama_checkpoint_last_stats",
     "lama_graph_save_state", "lama_graph_load_state", "lama_pf_save_shard_state", "lama_pf_load_state_sharded",
 ]
@@ -1177,6 +1180,134 @@ class OccupancyMap3D:
         _chk(lib().lama_om3_kernel_times(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
         keys = ("insert", "apply", "query")
         return dict(zip(keys, ms.tolist())), dict(zip(keys, ln.tolist()))
+
+
+class DynamicDistanceMap3D:
+    """Device-resident lama::DynamicDistanceMap with is3d = true (include/lama/sdm/dynamic_distance_map.h): the six-neighbour dynamic
+    brushfire.  setMaxDistance is fixed at creation (`l2_max`); `window` = patches per axis (None: 8 x 8 x 4), centred on `center`.
+
+    Cells are (n, 3) integer map coordinates; floating-point arrays passed as cells are world points and go through Map::w2m
+    (w2m3), as the reference's Vector3d overloads do.  addObstacle / removeObstacle are queued and applied, in order, by update()
+    or by the next read of the map."""
+
+    def __init__(self, resolution, l2_max=0.5, patch_size=32, center=(0.0, 0.0, 0.0), window=None, **dev):
+        d = DeviceOptions(device=0, dir_dim=64, pool_slots=0, max_beams=2048, timing=0, stream=0)
+        for k, v in dev.items():
+            setattr(d, k, v)
+        c, cp = _d(center)
+        win = None if window is None else (C.c_int32 * 3)(*[int(x) for x in window])
+        self.resolution = float(resolution)
+        self.h = C.c_void_p()
+        _chk(lib().lama_dm3_create(C.c_double(resolution), C.c_uint32(patch_size), C.c_double(l2_max), cp, win, C.byref(d), C.byref(self.h)))
+
+    def __del__(self):
+        if getattr(self, "h", None) and _lib is not None:
+            _lib.lama_dm3_destroy(self.h)
+            self.h = None
+
+    def _cells(self, cells):
+        a = np.asarray(cells)
+        if np.issubdtype(a.dtype, np.floating):
+            return np.ascontiguousarray(w2m3(self.resolution, a.reshape(-1, 3)))
+        return np.ascontiguousarray(a, np.uint32).reshape(-1, 3)
+
+    @property
+    def max_sqdist(self):
+        v = C.c_uint32(0)
+        _chk(lib().lama_dm3_max_sqdist(self.h, C.byref(v)))
+        return v.value
+
+    def maxDistance(self):
+        """maxDistance (dynamic_distance_map.cpp:155-158)"""
+        v = C.c_double(0)
+        _chk(lib().lama_dm3_max_distance(self.h, C.byref(v)))
+        return v.value
+
+    def addObstacle(self, cells):
+        """addObstacle (:212-226) of every cell, in order"""
+        c = self._cells(cells)
+        _chk(lib().lama_dm3_add_obstacles(self.h, _vp(c), C.c_int(len(c))))
+
+    def removeObstacle(self, cells):
+        """removeObstacle (:228-242) of every cell, in order"""
+        c = self._cells(cells)
+        _chk(lib().lama_dm3_remove_obstacles(self.h, _vp(c), C.c_int(len(c))))
+
+    def update(self) -> int:
+        """update() (:160-197): the number of processed cells"""
+        n = C.c_uint32(0)
+        _chk(lib().lama_dm3_update(self.h, C.byref(n)))
+        return n.value
+
+    def distance(self, pts, grad=True):
+        """distance(Vector3d, gradient) (:93-133) of world points (n, 3): distances (n,) and, with grad, gradients (n, 3)"""
+        p, pp = _d(pts)
+        n = p.size // 3
+        d = np.zeros(n)
+        g = np.zeros((n, 3)) if grad else None
+        _chk(lib().lama_dm3_distance(self.h, pp, C.c_int(n), d.ctypes.data_as(c_dp), g.ctypes.data_as(c_dp) if grad else None))
+        return (d, g) if grad else d
+
+    def cellDistance(self, cells):
+        """distance(Vector3ui) (:140-147) of integer cells (n, 3)"""
+        c = np.ascontiguousarray(cells, np.uint32).reshape(-1, 3)
+        d = np.zeros(len(c))
+        _chk(lib().lama_dm3_cell_distance(self.h, _vp(c), C.c_int(len(c)), d.ctypes.data_as(c_dp)))
+        return d
+
+    def bounds(self):
+        """(allocated patches, min cell (3,), max cell (3,)) as Map::bounds"""
+        mn, mx, n = np.zeros(3, np.uint32), np.zeros(3, np.uint32), C.c_int(0)
+        _chk(lib().lama_dm3_bounds(self.h, mn.ctypes.data_as(c_u32p), mx.ctypes.data_as(c_u32p), C.byref(n)))
+        return n.value, mn, mx
+
+    def export(self, lo, size):
+        """cells of the box lo + [0, size), shaped (size z, size y, size x): dict(word (raw uint64), sqdist, ox, oy, oz, valid, queued,
+        known)"""
+        lo = np.ascontiguousarray(lo, np.uint32)
+        sz = np.ascontiguousarray(size, np.int32)
+        shape = (int(sz[2]), int(sz[1]), int(sz[0]))
+        w, k = np.zeros(shape, np.uint64), np.zeros(shape, np.uint8)
+        _chk(lib().lama_dm3_export(self.h, _vp(lo), _vp(sz), _vp(w), _vp(k)))
+        return dm3_fields(w, k)
+
+    def write(self, path):
+        """Map::write (map.cpp:490-529) + writeParameters: a 3-D .sdm file"""
+        _chk(lib().lama_dm3_write(self.h, str(path).encode()))
+
+    def read(self, path):
+        """Map::read (map.cpp:531-575) + readParameters into this (empty) map, which takes the file's resolution and max_sqdist"""
+        _chk(lib().lama_dm3_read(self.h, str(path).encode()))
+        with open(path, "rb") as f:   # IOHeader.resolution (map.h:95-103), a float at byte 24
+            self.resolution = float(np.frombuffer(f.read(28)[24:28], np.float32)[0])
+
+    def exportImage(self, zed=0.0):
+        """the z-slice image of sdm::export_to_png(dm, file, zed) (export.cpp:74-96), (height, width) uint8"""
+        return _image(lib().lama_dm3_export_image, (self.h, C.c_double(zed)))
+
+    def saveImage(self, path, zed=0.0):
+        write_png(path, self.exportImage(zed))
+
+    def kernelTimes(self):
+        ms, ln = np.zeros(3), np.zeros(3, np.uint64)
+        _chk(lib().lama_dm3_kernel_times(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
+        keys = ("update", "distance", "cells")
+        return dict(zip(keys, ms.tolist())), dict(zip(keys, ln.tolist()))
+
+    def runStats(self):
+        """{launches, grows, raise_cap, lower_cap} of the brushfire since creation"""
+        s = np.zeros(4, np.uint64)
+        _chk(lib().lama_dm3_run_stats(self.h, _vp(s)))
+        return dict(zip(("launches", "grows", "raise_cap", "lower_cap"), s.tolist()))
+
+
+def dm3_fields(words, known):
+    """the fields of 64-bit 3-D distance cells (lama_dm3_export's layout)"""
+    w = np.asarray(words, np.uint64)
+    b = w.view(np.uint8).reshape(w.shape + (8,))
+    return dict(word=w, ox=b[..., 0].view(np.int8).astype(np.int16), oy=b[..., 1].view(np.int8).astype(np.int16),
+                oz=b[..., 2].view(np.int8).astype(np.int16), valid=(b[..., 3] & 1), queued=(b[..., 3] >> 1) & 1,
+                sqdist=(w >> np.uint64(32)).astype(np.uint16), known=np.asarray(known, np.uint8))
 
 
 class DynamicDistanceMap:

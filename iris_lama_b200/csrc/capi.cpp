@@ -17,6 +17,7 @@
 #include "pgo.h"
 #include "tsdm.h"
 #include "om3d.h"
+#include "ddm3d.h"
 
 #include "../../include/lama_b200.h"
 
@@ -1719,6 +1720,145 @@ try {
     return LAMA_OK;
 }
 LAMA_CATCH
+// ---- 3-D DynamicDistanceMap (include/lama/sdm/dynamic_distance_map.h with is3d) ---------------------------------------------------
+struct lama_dm3 { DistMap3Dev* m; };
+// DynamicDistanceMap(resolution, patch_size, true) + setMaxDistance(l2_max) (dynamic_distance_map.cpp:36-46,149-153) on the device
+int lama_dm3_create(double resolution, uint32_t patch_size, double l2_max, const double center_xyz[3], const int32_t window_patches[3],
+                    const lama_device_options* dev, lama_dm3** out)
+try {
+    if (!out) return set_err("null argument", LAMA_ERR_ARG);
+    *out = nullptr;
+    lama_device_options d;
+    if (dev) d = *dev; else dev_default(&d);
+    std::string err;
+    const bool bad_arg = !(resolution > 0) || patch_size != 32 || !(std::ceil(l2_max / resolution) >= 0 && std::ceil(l2_max / resolution) <= 63);
+    if (bad_arg) return set_err("resolution must be positive, patch_size 32 and ceil(l2_max / resolution) 0..63", LAMA_ERR_ARG);
+    DistMap3Dev* m = DistMap3Dev::create(resolution, patch_size, l2_max, center_xyz, window_patches, dev_from(d), err);
+    if (!m) {
+        const bool win = err.find("window") != std::string::npos;
+        return set_err(err, win ? LAMA_ERR_ARG : (lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_CUDA));
+    }
+    *out = new lama_dm3{m};
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_dm3_destroy(lama_dm3* h)
+try {
+    if (!h) return LAMA_OK;
+    delete h->m;
+    delete h;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_dm3_max_sqdist(lama_dm3* h, uint32_t* v)
+try {
+    if (!h || !v) return set_err("null argument", LAMA_ERR_ARG);
+    *v = h->m->max_sqdist();
+    return LAMA_OK;
+}
+LAMA_CATCH
+// maxDistance (dynamic_distance_map.cpp:155-158)
+int lama_dm3_max_distance(lama_dm3* h, double* v)
+try {
+    if (!h || !v) return set_err("null argument", LAMA_ERR_ARG);
+    *v = h->m->max_distance();
+    return LAMA_OK;
+}
+LAMA_CATCH
+// addObstacle (:212-226) of n cells in list order
+int lama_dm3_add_obstacles(lama_dm3* h, const uint32_t* cells_xyz, int n)
+try {
+    if (!h || (n > 0 && !cells_xyz)) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->add_remove(cells_xyz, n, false);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// removeObstacle (:228-242) of n cells in list order
+int lama_dm3_remove_obstacles(lama_dm3* h, const uint32_t* cells_xyz, int n)
+try {
+    if (!h || (n > 0 && !cells_xyz)) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->add_remove(cells_xyz, n, true);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// update (:160-197)
+int lama_dm3_update(lama_dm3* h, uint32_t* processed)
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    int rc = h->m->update(processed);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// distance(Vector3d, gradient) (:93-133)
+int lama_dm3_distance(lama_dm3* h, const double* pts_xyz, int n, double* distance, double* gradient)
+try {
+    if (!h || (n > 0 && (!pts_xyz || !distance))) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->distance(pts_xyz, n, distance, gradient);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// distance(Vector3ui) (:140-147)
+int lama_dm3_cell_distance(lama_dm3* h, const uint32_t* cells_xyz, int n, double* distance)
+try {
+    if (!h || (n > 0 && (!cells_xyz || !distance))) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->cell_distance(cells_xyz, n, distance);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// Map::bounds (map.cpp:139-157)
+int lama_dm3_bounds(lama_dm3* h, uint32_t mn[3], uint32_t mx[3], int* patches)
+try {
+    if (!h || !mn || !mx) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->bounds(mn, mx, patches);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+int lama_dm3_export(lama_dm3* h, const uint32_t lo[3], const int32_t size[3], uint64_t* cells, uint8_t* known)
+try {
+    if (!h || !lo || !size) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->export_box(lo, size, cells, known);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// Map::write (map.cpp:490-529) + writeParameters (:200-203)
+int lama_dm3_write(lama_dm3* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->write(path);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// Map::read (map.cpp:531-575) + readParameters (:205-208)
+int lama_dm3_read(lama_dm3* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->read(path);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+// sdm::export_to_png(dm, file, zed) (export.cpp:74-96,105-110): the grey image
+int lama_dm3_export_image(lama_dm3* h, double zed, uint8_t* pixels, size_t cap, int dims[2])
+try {
+    if (!h || !dims) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = h->m->export_image(zed, pixels, cap, dims);
+    return rc == LAMA_OK ? rc : set_err(h->m->error(), rc);
+}
+LAMA_CATCH
+int lama_dm3_kernel_times(lama_dm3* h, double ms[3], uint64_t launches[3])
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    h->m->kernel_times(ms, launches);
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_dm3_run_stats(lama_dm3* h, uint64_t stats[4])
+try {
+    if (!h || !stats) return set_err("null argument", LAMA_ERR_ARG);
+    h->m->run_stats(stats);
+    return LAMA_OK;
+}
+LAMA_CATCH
+
 // Map::w2m (map.h:125-126), all three axes
 int lama_w2m3(double resolution, const double* pts_xyz, int n, uint32_t* cells_xyz)
 try {

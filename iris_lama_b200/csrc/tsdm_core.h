@@ -13,6 +13,7 @@
 #include "ray_core.h"
 #include "match_core.h"
 #include "patch_window.h"
+#include "trilinear.h"
 
 namespace lama_b200 {
 
@@ -107,43 +108,14 @@ LAMA_HD void tsdm_fold(float& cd, float& cw, float d, float w, float max_weight)
 template <class Value>
 LAMA_HD double tsdm_distance(const double pt[3], const TsdmParams& p, Value&& value, double grad[3])
 {
+    if (p.is3d) return trilinear_distance(pt, p.scale, value, grad);   // trilinear.h, shared with the 3-D DynamicDistanceMap
     double mu[3], nu[3];
     uint32_t c[3];
-    for (int k = 0; k < 3; ++k) {
-        const double m = w2m_nocast(pt[k], p.scale);
-        c[k] = (uint32_t)m;
-        mu[k] = add_rn(m, -(double)c[k]);
-        nu[k] = add_rn(1.0, -mu[k]);
-    }
-    if (!p.is3d) {
-        const double v[4] = {value(c[0], c[1], c[2]), value(c[0] + 1, c[1], c[2]), value(c[0], c[1] + 1, c[2]), value(c[0] + 1, c[1] + 1, c[2])};
-        const BeamEval e = bilinear(v, mu[0], mu[1], p.scale, 0.0, 0.0);
-        grad[0] = e.gx; grad[1] = e.gy; grad[2] = 0.0;
-        return e.dist;
-    }
-    double v[8];
-    for (int i = 0; i < 8; ++i) v[i] = value(c[0] + (i & 1), c[1] + ((i >> 1) & 1), c[2] + (i >> 2));   // V000 V100 V010 V110 V001 ...
-    const double dist =
-        add_rn(add_rn(add_rn(add_rn(add_rn(add_rn(add_rn(
-            mul_rn(v[0], mul_rn(mul_rn(nu[0], nu[1]), nu[2])),
-            mul_rn(mul_rn(mul_rn(v[1], mu[0]), nu[1]), nu[2])),
-            mul_rn(mul_rn(mul_rn(v[2], nu[0]), mu[1]), nu[2])),
-            mul_rn(mul_rn(mul_rn(v[3], mu[0]), mu[1]), nu[2])),
-            mul_rn(mul_rn(mul_rn(v[4], nu[0]), nu[1]), mu[2])),
-            mul_rn(mul_rn(mul_rn(v[5], mu[0]), nu[1]), mu[2])),
-            mul_rn(mul_rn(mul_rn(v[6], nu[0]), mu[1]), mu[2])),
-            mul_rn(v[7], mul_rn(mul_rn(mu[0], mu[1]), mu[2])));
-    double a, b;
-    a = add_rn(mul_rn(add_rn(v[0], -v[1]), nu[1]), mul_rn(add_rn(v[2], -v[3]), mu[1]));
-    b = add_rn(mul_rn(add_rn(v[4], -v[5]), nu[1]), mul_rn(add_rn(v[6], -v[7]), mu[1]));
-    grad[0] = mul_rn(-add_rn(mul_rn(a, nu[2]), mul_rn(b, mu[2])), p.scale);
-    a = add_rn(mul_rn(add_rn(v[0], -v[2]), nu[0]), mul_rn(add_rn(v[1], -v[3]), mu[0]));
-    b = add_rn(mul_rn(add_rn(v[4], -v[6]), nu[0]), mul_rn(add_rn(v[5], -v[7]), mu[0]));
-    grad[1] = mul_rn(-add_rn(mul_rn(a, nu[2]), mul_rn(b, mu[2])), p.scale);
-    a = add_rn(mul_rn(add_rn(v[0], -v[4]), nu[0]), mul_rn(add_rn(v[1], -v[5]), mu[0]));
-    b = add_rn(mul_rn(add_rn(v[2], -v[6]), nu[0]), mul_rn(add_rn(v[3], -v[7]), mu[0]));
-    grad[2] = mul_rn(-add_rn(mul_rn(a, nu[1]), mul_rn(b, mu[1])), p.scale);
-    return dist;
+    cell_fraction(pt, p.scale, c, mu, nu);
+    const double v[4] = {value(c[0], c[1], c[2]), value(c[0] + 1, c[1], c[2]), value(c[0], c[1] + 1, c[2]), value(c[0] + 1, c[1] + 1, c[2])};
+    const BeamEval e = bilinear(v, mu[0], mu[1], p.scale, 0.0, 0.0);
+    grad[0] = e.gx; grad[1] = e.gy; grad[2] = 0.0;
+    return e.dist;
 }
 
 // ---- marching cubes (toMesh :220-272) --------------------------------------------------------------------------------------
