@@ -547,6 +547,17 @@ int lama_dm3_export_image(lama_dm3* h, double zed, uint8_t* pixels, size_t cap, 
 int lama_dm3_kernel_times(lama_dm3* h, double ms[3], uint64_t launches[3]);
 /* {brushfire launches, heap growths, raise heap capacity, lower heap capacity} since creation */
 int lama_dm3_run_stats(lama_dm3* h, uint64_t stats[4]);
+/* The map update of the reference's SLAM (slam2d.cpp:271-316, pf_slam2d.cpp:439-509) for every point of n_clouds clouds in order,
+ * the insertion of lama_om3_insert_point_clouds with the distance map kept in step: `if (om.setOccupied(hit)) dm.addObstacle(hit)`,
+ * then along the ray `if (om.setFree(c)) dm.removeObstacle(c)`, and dm.update() after every cloud.  Both maps end cell for cell as that
+ * sequence leaves them.  processed (n_clouds entries, may be NULL) = every cloud's update(); counts (may be NULL) = {events, pushes}:
+ * the setter calls that returned true, and those of them whose addObstacle / removeObstacle pushed a heap entry.  Ops queued on dm
+ * are applied first.  LAMA_ERR_ARG when the maps differ in device, resolution or window, or a cloud makes 2^30 cell updates or more;
+ * LAMA_ERR_WINDOW when a hit or ray cell lies less than R + 1 cells inside the window (R = dm's reach); LAMA_ERR_POOL when either
+ * pool could run out.  After a refusal both maps are unchanged.  Timing: the occupancy side in om's kernel_times[0], the brushfire
+ * in dm's kernel_times[0]. */
+int lama_om3_insert_point_clouds_dm3(lama_om3* om, lama_dm3* dm, const double* pts_xyz, const int64_t* offsets, int n_clouds, const double* origins,
+                                     const double* quats_xyzw, int full, uint64_t* cells, uint32_t* processed, uint64_t counts[2]);
 /* Map::w2m (map.h:125-126) on all three axes: world points (n x 3) -> cells (n x 3) */
 int lama_w2m3(double resolution, const double* pts_xyz, int n, uint32_t* cells_xyz);
 

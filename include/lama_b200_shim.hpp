@@ -292,6 +292,8 @@ private:
     lama_tsdm* h_ = nullptr;
 };
 
+class DynamicDistanceMap3D;
+
 // lama::FrequencyOccupancyMap (kind 0) / lama::ProbabilisticOccupancyMap (kind 1) with is3d = true on the device.  Cells are map
 // coordinates {x, y, z}; insertPointCloud is the loop body of GraphSlam2D::generateOccupancyMap for every point of the cloud.
 class OccupancyMap3D {
@@ -312,6 +314,9 @@ public:
         check(lama_om3_insert_point_clouds(h_, f.pts.data(), offsets, 1, f.origin, f.quat, full ? 1 : 0, &n));
         return n;
     }
+    // the map update of Slam2D::updateMaps (slam2d.cpp:271-316) for the cloud with dm kept in step; returns dm.update()'s count
+    template <typename CloudPtr>
+    uint32_t updateMaps(DynamicDistanceMap3D& dm, const CloudPtr& cloud, bool full = true);
     bool setFree(const uint32_t xyz[3]) { return set(xyz, LAMA_OM3_SET_FREE); }
     bool setOccupied(const uint32_t xyz[3]) { return set(xyz, LAMA_OM3_SET_OCCUPIED); }
     bool setUnknown(const uint32_t xyz[3]) { return set(xyz, LAMA_OM3_SET_UNKNOWN); }
@@ -350,7 +355,18 @@ public:
     bool read(const std::string& path) { check(lama_dm3_read(h_, path.c_str())); return true; }
 
 private:
+    friend class OccupancyMap3D;
     lama_dm3* h_ = nullptr;
 };
+
+template <typename CloudPtr>
+uint32_t OccupancyMap3D::updateMaps(DynamicDistanceMap3D& dm, const CloudPtr& cloud, bool full)
+{
+    FlatCloud<typename std::remove_reference<decltype(*cloud)>::type> f(*cloud);
+    const int64_t offsets[2] = {0, (int64_t)(f.pts.size() / 3)};
+    uint32_t processed = 0;
+    check(lama_om3_insert_point_clouds_dm3(h_, dm.h_, f.pts.data(), offsets, 1, f.origin, f.quat, full ? 1 : 0, nullptr, &processed, nullptr));
+    return processed;
+}
 
 }  // namespace lama_b200_shim

@@ -94,7 +94,7 @@ EXPORTED_SYMBOLS = [
     "lama_om3_bounds", "lama_om3_export", "lama_om3_write", "lama_om3_read", "lama_om3_export_image", "lama_om3_kernel_times", "lama_w2m3",
     "lama_dm3_create", "lama_dm3_destroy", "lama_dm3_max_sqdist", "lama_dm3_max_distance", "lama_dm3_add_obstacles", "lama_dm3_remove_obstacles",
     "lama_dm3_update", "lama_dm3_distance", "lama_dm3_cell_distance", "lama_dm3_bounds", "lama_dm3_export", "lama_dm3_write", "lama_dm3_read",
-    "lama_dm3_export_image", "lama_dm3_kernel_times", "lama_dm3_run_stats",
+    "lama_dm3_export_image", "lama_dm3_kernel_times", "lama_dm3_run_stats", "lama_om3_insert_point_clouds_dm3",
     "lama_pf_save_state", "lama_pf_load_state", "lama_slam_save_state", "lama_slam_load_state", "lama_checkpoint_last_stats",
     "lama_graph_save_state", "lama_graph_load_state", "lama_pf_save_shard_state", "lama_pf_load_state_sharded",
 ]
@@ -1101,6 +1101,24 @@ class OccupancyMap3D:
         _chk(lib().lama_om3_insert_point_clouds(self.h, _vp(p), offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int(len(offsets) - 1), _vp(o), _vp(q),
                                                 C.c_int(1 if full else 0), C.byref(n)))
         return n.value
+
+    def updateMaps(self, distance_map, clouds, origins=None, quats=None, full=True, counts=False):
+        """insertPointClouds with the DynamicDistanceMap3D `distance_map` kept in step, as the reference's map update (slam2d.cpp:271-316):
+        a setOccupied that returns true is an addObstacle, a setFree that returns true a removeObstacle, and distance_map.update() runs
+        after every cloud.  Both maps must share device, resolution and window.  Returns (cell updates, processed (S,) uint32, every
+        cloud's update()), and with counts also {"events", "pushes"}: the setter calls that returned true, and those whose distance-map
+        op pushed a heap entry."""
+        p, offsets = _clouds(clouds)
+        o = None if origins is None else np.ascontiguousarray(origins, np.float64).reshape(-1, 3)
+        q = None if quats is None else np.ascontiguousarray(quats, np.float64).reshape(-1, 4)
+        n = C.c_uint64(0)
+        processed = np.zeros(len(offsets) - 1, np.uint32)
+        cnt = np.zeros(2, np.uint64)
+        _chk(lib().lama_om3_insert_point_clouds_dm3(self.h, distance_map.h, _vp(p), offsets.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int(len(offsets) - 1),
+                                                    _vp(o), _vp(q), C.c_int(1 if full else 0), C.byref(n), _vp(processed), _vp(cnt)))
+        if counts:
+            return n.value, processed, dict(events=int(cnt[0]), pushes=int(cnt[1]))
+        return n.value, processed
 
     def apply(self, cells, ops):
         """the setters in list order: ops (n,) of SET_FREE / SET_OCCUPIED / SET_UNKNOWN.  Returns what each call returns, (n,) bool."""

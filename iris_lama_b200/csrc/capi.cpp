@@ -1858,6 +1858,15 @@ try {
     return LAMA_OK;
 }
 LAMA_CATCH
+// the map update of Slam2D::updateMaps (slam2d.cpp:271-316) for every point of every cloud, update() after each cloud
+int lama_om3_insert_point_clouds_dm3(lama_om3* om, lama_dm3* dm, const double* pts_xyz, const int64_t* offsets, int n_clouds, const double* origins,
+                                     const double* quats_xyzw, int full, uint64_t* cells, uint32_t* processed, uint64_t counts[2])
+try {
+    if (!om || !dm || (n_clouds > 0 && !offsets)) return set_err("null argument", LAMA_ERR_ARG);
+    int rc = om->m->insert_point_clouds_dm3(*dm->m, pts_xyz, offsets, n_clouds, origins, quats_xyzw, full != 0, cells, processed, counts);
+    return rc == LAMA_OK ? rc : set_err(om->m->error(), rc);
+}
+LAMA_CATCH
 
 // Map::w2m (map.h:125-126), all three axes
 int lama_w2m3(double resolution, const double* pts_xyz, int n, uint32_t* cells_xyz)

@@ -80,7 +80,7 @@ struct Dm3State {
     uint32_t used;                     // pool slots taken
     uint32_t err;                      // kErr* bits (lama_core.h); never set when the host admission holds
     uint32_t stop;                     // how the last run ended: kDm3Done, kDm3NeedRoom (a heap lacks room), kDm3Budget (pop budget spent)
-    uint32_t pad;
+    uint32_t seg;                      // run_segments: segments finished so far
 };
 // a pending op: x, y, z, kind (0 addObstacle, 1 removeObstacle)
 constexpr int kDm3OpWords = 4;
@@ -204,7 +204,36 @@ struct Brushfire3 {
             }
         }
     }
+
+    // The ops cut into n_seg segments, segment k ending at op seg_end[k]: from segment s.seg on, applies the segment's ops and runs
+    // update() to the end, and writes its count to processed[k] (the reference's per-cloud update(), slam2d.cpp:271-316).  Stops and
+    // resumes as run() does; `budget` bounds the pops of the whole call.
+    LAMA_HD void run_segments(Dm3State& s, const uint32_t* ops, const uint32_t* seg_end, uint32_t n_seg, uint64_t budget, uint32_t* processed)
+    {
+        s.stop = kDm3Done;
+        while (s.seg < n_seg) {
+            const uint32_t p0 = s.processed;
+            run(s, ops, seg_end[s.seg], true, budget);
+            budget -= s.processed - p0;   // run() pops at most `budget`
+            if (s.stop != kDm3Done) return;
+            processed[s.seg] = s.processed;
+            s.processed = 0;
+            ++s.seg;
+        }
+    }
 };
+
+// at least `margin` cells inside the window on every axis
+LAMA_HD bool dm3_inside(const PatchWindow& w, uint32_t x, uint32_t y, uint32_t z, int margin)
+{
+    const uint32_t c[3] = {x, y, z};
+    for (int k = 0; k < 3; ++k) {
+        const int64_t lo = ((int64_t)w.base[k] << kPatchLog2) + margin;
+        const int64_t hi = (((int64_t)w.base[k] + w.dim[k]) << kPatchLog2) - 1 - margin;
+        if ((int64_t)c[k] < lo || (int64_t)c[k] > hi) return false;
+    }
+    return true;
+}
 
 // ---- host admission --------------------------------------------------------------------------------------------------------------
 // Decides, before anything is written, whether a batch of add / remove cells may enter the map.  `reachable` marks the directory
@@ -222,16 +251,7 @@ struct Dm3Guard {
         reachable.assign((size_t)w.dim[0] * w.dim[1] * w.dim[2], 0);
     }
     // at least R + 1 cells inside the window on every axis: then every cell within R of it is inside too
-    bool inside(uint32_t x, uint32_t y, uint32_t z) const
-    {
-        const uint32_t c[3] = {x, y, z};
-        for (int k = 0; k < 3; ++k) {
-            const int64_t lo = ((int64_t)win.base[k] << kPatchLog2) + reach + 1;
-            const int64_t hi = (((int64_t)win.base[k] + win.dim[k]) << kPatchLog2) - 1 - (reach + 1);
-            if ((int64_t)c[k] < lo || (int64_t)c[k] > hi) return false;
-        }
-        return true;
-    }
+    bool inside(uint32_t x, uint32_t y, uint32_t z) const { return dm3_inside(win, x, y, z, reach + 1); }
     // marks in r the entries of the cells within R of (x, y, z), which must be inside()
     void mark(std::vector<uint8_t>& r, uint32_t x, uint32_t y, uint32_t z) const
     {
@@ -240,6 +260,34 @@ struct Dm3Guard {
             for (uint32_t py = (y - R) >> kPatchLog2; py <= (y + R) >> kPatchLog2; ++py)
                 for (uint32_t px = (x - R) >> kPatchLog2; px <= (x + R) >> kPatchLog2; ++px)
                     r[(size_t)window_dir_index(win, px << kPatchLog2, py << kPatchLog2, pz << kPatchLog2)] = 1;
+    }
+    // marks in r the entries within R of any cell of entry di (those outside the window aside)
+    void mark_entry(std::vector<uint8_t>& r, int di) const
+    {
+        uint32_t a[3];
+        window_anchor(win, di, a);
+        const uint32_t R = (uint32_t)reach;
+        for (uint32_t pz = (a[2] - R) >> kPatchLog2; pz <= (a[2] + kPatchLen - 1 + R) >> kPatchLog2; ++pz)
+            for (uint32_t py = (a[1] - R) >> kPatchLog2; py <= (a[1] + kPatchLen - 1 + R) >> kPatchLog2; ++py)
+                for (uint32_t px = (a[0] - R) >> kPatchLog2; px <= (a[0] + kPatchLen - 1 + R) >> kPatchLog2; ++px) {
+                    const int e = window_dir_index(win, px << kPatchLog2, py << kPatchLog2, pz << kPatchLog2);
+                    if (e >= 0) r[(size_t)e] = 1;
+                }
+    }
+    // The pool check of a batch that may add or remove obstacles anywhere in the marked entries (marks[i] != 0): -5 (pool) when the
+    // reachable entries, with those within R of the marked ones, that have no patch could exceed free_slots; else 0 and next = them.
+    // Nothing changes here: the caller commits next to `reachable` once the batch is admitted.
+    int admit_entries(const std::vector<uint32_t>& marks, const std::vector<int32_t>& dir, int64_t free_slots, std::vector<uint8_t>& next,
+                      std::string& err) const
+    {
+        next = reachable;
+        for (size_t i = 0; i < marks.size(); ++i)
+            if (marks[i]) mark_entry(next, (int)i);
+        if (missing(next, dir) > free_slots) {
+            err = "the distance-map patches this batch can reach could exceed the free pool slots (raise pool_slots)";
+            return -5;
+        }
+        return 0;
     }
     // reachable entries of r without a patch in dir (-1 = none)
     static int64_t missing(const std::vector<uint8_t>& r, const std::vector<int32_t>& dir)

@@ -62,13 +62,16 @@ struct DevMap3 {
     }
 };
 
+// run(), or with seg_end run_segments() over n_seg segments
 __global__ void __launch_bounds__(1) k_dm3_brushfire(View v, uint64_t* rq, uint32_t rcap, uint64_t* lq, uint32_t lcap, const uint32_t* ops,
-                                                     uint32_t n_ops, int do_update, uint64_t budget, uint32_t max_sqdist, Dm3State* st)
+                                                     uint32_t n_ops, int do_update, uint64_t budget, uint32_t max_sqdist, Dm3State* st,
+                                                     const uint32_t* seg_end, uint32_t n_seg, uint32_t* seg_processed)
 {
     Dm3State s = *st;
     DevMap3 m{v.win, v.dir, v.cells, v.pool, s.used, 0u, 0ull};
     Brushfire3<DevMap3> b(m, Heap{rq, s.raise_size, rcap}, Heap{lq, s.lower_size, lcap}, max_sqdist);
-    b.run(s, ops, n_ops, do_update != 0, budget);
+    if (seg_end) b.run_segments(s, ops, seg_end, n_seg, budget, seg_processed);
+    else b.run(s, ops, n_ops, do_update != 0, budget);
     s.raise_size = b.raise_q.size;
     s.lower_size = b.lower_q.size;
     s.used = m.used;
@@ -153,7 +156,7 @@ struct DistMap3Dev::Impl : PatchStore {
     uint64_t runs = 0, grows = 0;
     std::vector<uint32_t> pending;            // queued ops, kDm3OpWords words each
     uint32_t pending_kind[2] = {0, 0};        // queued adds, removes
-    Buf ops, qin, qout, qgrad, qflag;
+    Buf ops, qin, qout, qgrad, qflag, seg;
 
     ~Impl()
     {
@@ -276,11 +279,24 @@ int DistMap3Dev::run(bool do_update, uint32_t* processed)
         PS_TRY(cudaMemcpyAsync(d.ops.p, d.pending.data(), d.pending.size() * 4, cudaMemcpyHostToDevice, d.stream));
     }
     if (do_update) d.h_st.processed = 0;
+    const int rc = drive((const uint32_t*)d.ops.p, n_ops, do_update, nullptr, 0, nullptr);
+    if (rc != LAMA_OK) return rc;
+    d.pending.clear();
+    d.pending_kind[0] = d.pending_kind[1] = 0;
+    if (processed) *processed = d.h_st.processed;
+    return LAMA_OK;
+}
+
+// the launch loop of run() and run_segments() from h_st; on success h_st is back at op 0 and segment 0, and the host directory is
+// read back
+int DistMap3Dev::drive(const uint32_t* ops, uint32_t n_ops, bool do_update, const uint32_t* seg_end, uint32_t n_seg, uint32_t* seg_processed)
+{
+    Impl& d = *d_;
     PS_TRY(cudaMemcpyAsync(d.st, &d.h_st, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream));
     PS_TRY(d.record(0));
     for (;;) {
-        k_dm3_brushfire<<<1, 1, 0, d.stream>>>(d.view(), d.heap[0], d.cap[0], d.heap[1], d.cap[1], (const uint32_t*)d.ops.p, n_ops, do_update ? 1 : 0,
-                                               d.budget, d.max_sqdist, d.st);
+        k_dm3_brushfire<<<1, 1, 0, d.stream>>>(d.view(), d.heap[0], d.cap[0], d.heap[1], d.cap[1], ops, n_ops, do_update ? 1 : 0, d.budget, d.max_sqdist,
+                                               d.st, seg_end, n_seg, seg_processed);
         d.launches[0] += 1;
         ++d.runs;
         PS_TRY(cudaGetLastError());
@@ -298,17 +314,69 @@ int DistMap3Dev::run(bool do_update, uint32_t* processed)
     }
     PS_TRY(d.record(1));
     PS_TRY(d.finish(0));
-    d.pending.clear();
-    d.pending_kind[0] = d.pending_kind[1] = 0;
     d.h_st.next_op = 0;
+    d.h_st.seg = 0;
     PS_TRY(cudaMemcpyAsync(d.h_dir.data(), d.dir, (size_t)d.ndir * 4, cudaMemcpyDeviceToHost, d.stream));
     PS_TRY(cudaStreamSynchronize(d.stream));
     d.used = (int)d.h_st.used;
-    if (processed) *processed = d.h_st.processed;
     return LAMA_OK;
 }
 
 int DistMap3Dev::flush() { return d_->pending.empty() ? LAMA_OK : run(false, nullptr); }
+
+DistMap3Dev::Coupling DistMap3Dev::coupling() const
+{
+    const Impl& d = *d_;
+    return Coupling{d.device, (void*)d.stream, d.resolution, d.win, d.guard.reach, d.dir, (uint64_t*)d.cells};
+}
+
+int DistMap3Dev::admit_entries(const std::vector<uint32_t>& marks, std::vector<uint8_t>& next)
+{
+    Impl& d = *d_;
+    return d.guard.admit_entries(marks, d.h_dir, (int64_t)d.pool - (int64_t)d.h_st.used, next, err_) == 0 ? LAMA_OK : LAMA_ERR_POOL;
+}
+
+void DistMap3Dev::commit_reachable(std::vector<uint8_t>& next) { d_->guard.reachable.swap(next); }
+
+int DistMap3Dev::alloc_entries(const std::vector<uint32_t>& marks, void* done)
+{
+    Impl& d = *d_;
+    PS_TRY(cudaSetDevice(d.device));
+    bool fresh = false;
+    for (int i = 0; i < d.ndir; ++i)
+        if (marks[(size_t)i] && d.h_dir[(size_t)i] < 0) {
+            if (d.h_st.used >= (uint32_t)d.pool) { err_ = "internal: an admitted batch found the pool full"; return LAMA_ERR_STATE; }
+            d.h_dir[(size_t)i] = (int32_t)d.h_st.used++;   // the pool was zeroed at creation and slots are never freed
+            fresh = true;
+        }
+    if (fresh) {
+        d.used = (int)d.h_st.used;
+        PS_TRY(cudaMemcpyAsync(d.dir, d.h_dir.data(), (size_t)d.ndir * 4, cudaMemcpyHostToDevice, d.stream));
+        PS_TRY(cudaMemcpyAsync(d.st, &d.h_st, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream));
+    }
+    PS_TRY(cudaEventRecord((cudaEvent_t)done, d.stream));
+    return LAMA_OK;
+}
+
+int DistMap3Dev::run_segments(const uint32_t* ops, const std::vector<uint32_t>& seg_end, uint32_t* processed, void* wait)
+{
+    Impl& d = *d_;
+    const uint32_t n_seg = (uint32_t)seg_end.size();
+    if (n_seg == 0) return LAMA_OK;
+    PS_TRY(cudaSetDevice(d.device));
+    if (wait) PS_TRY(cudaStreamWaitEvent(d.stream, (cudaEvent_t)wait, 0));
+    PS_TRY(d.ensure(d.seg, (size_t)n_seg * 8));
+    uint32_t* dseg = (uint32_t*)d.seg.p;
+    PS_TRY(cudaMemcpyAsync(dseg, seg_end.data(), (size_t)n_seg * 4, cudaMemcpyHostToDevice, d.stream));
+    d.h_st.processed = 0;
+    d.h_st.seg = 0;
+    const int rc = drive(ops, seg_end.back(), true, dseg, n_seg, dseg + n_seg);
+    if (rc != LAMA_OK) return rc;
+    PS_TRY(cudaMemcpyAsync(processed, dseg + n_seg, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, d.stream));
+    PS_TRY(cudaStreamSynchronize(d.stream));
+    d.h_st.processed = 0;
+    return LAMA_OK;
+}
 
 int DistMap3Dev::update(uint32_t* processed)
 {

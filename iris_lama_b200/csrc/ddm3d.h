@@ -4,8 +4,10 @@
 #include <cstddef>
 #include <cstdint>
 #include <string>
+#include <vector>
 
 #include "frontend.h"
+#include "patch_window.h"
 
 namespace lama_b200 {
 
@@ -47,10 +49,34 @@ public:
     void run_stats(uint64_t out[4]) const;
     const std::string& error() const { return err_; }
 
+    // ---- for OccMap3Dev::insert_point_clouds_dm3 (om3d.cu), which drives the map through these ----------------------------------------
+    struct Coupling {
+        int device;
+        void* stream;          // cudaStream_t
+        double resolution;
+        PatchWindow win;
+        int reach;             // R = ceil(l2_max * scale)
+        const int32_t* dir;    // device directory and pool (ddm3_core.h cells)
+        uint64_t* cells;
+    };
+    Coupling coupling() const;
+    // the pool check of a batch whose distance-map ops may fall anywhere in the marked directory entries (Dm3Guard::admit_entries):
+    // LAMA_ERR_POOL, or LAMA_OK with *next the reachable entries to commit once the batch is admitted
+    int admit_entries(const std::vector<uint32_t>& marks, std::vector<uint8_t>& next);
+    void commit_reachable(std::vector<uint8_t>& next);
+    // applies the queued ops without update() (every reader does this first)
+    int flush();
+    // allocates the marked entries that have no patch, ascending directory index, and records `done` (a cudaEvent_t) on the map's
+    // stream; the caller admitted them (admit_entries), so the pool holds them
+    int alloc_entries(const std::vector<uint32_t>& marks, void* done);
+    // After `wait` (a cudaEvent_t, may be null): the device op list ops (kDm3OpWords words per op) cut into segments ending at seg_end,
+    // applied and updated segment by segment (Brushfire3::run_segments); processed[k] = update()'s count of segment k.
+    int run_segments(const uint32_t* ops, const std::vector<uint32_t>& seg_end, uint32_t* processed, void* wait);
+
 private:
     DistMap3Dev() = default;
-    int flush();
     int run(bool do_update, uint32_t* processed);
+    int drive(const uint32_t* ops, uint32_t n_ops, bool do_update, const uint32_t* seg_end, uint32_t n_seg, uint32_t* seg_processed);
     struct Impl;
     Impl* d_ = nullptr;
     std::string err_;

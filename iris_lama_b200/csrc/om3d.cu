@@ -20,6 +20,7 @@
 // apply() uses the same record -> sort -> fold path for both kinds, with the op's list index in the value.
 // The store, the patch allocation, the scan, the chunks and the sort and fold are patch_store.cuh, shared with the TSDM.
 #include "om3d.h"
+#include "occ_dist3_core.h"
 #include "om3d_core.h"
 #include "patch_store.cuh"
 #include "sdm_io.h"
@@ -52,9 +53,10 @@ struct InsertParams {
     const uint64_t* offs;     // exclusive scan of counts
     uint64_t rec_base;
     uint32_t* rkeys;          // record: directory index << 15 | cell index
-    uint32_t* rvals;          // record: op
+    uint32_t* rvals;          // record: its index within the chunk << 2 | op (the index is read by the coupled fold only)
     uint32_t* marks;          // per directory entry: touched by this batch
     uint32_t* status;
+    int margin;               // mark pass: the cells a touched cell must lie inside the window (0: inside it)
 };
 
 // kPass 0 (mark): window check, directory marks, record counts.  1 (count, frequency maps): counter reductions.  2 (emit, log-odds
@@ -73,7 +75,7 @@ __global__ void __launch_bounds__(kThreads) k_om3_points(InsertParams f, View v)
     auto touch = [&](uint32_t x, uint32_t y, uint32_t z, uint32_t op) {
         const int di = window_dir_index(v.w, x, y, z);
         if (kPass == 0) {
-            if (di < 0) { bad = true; return; }
+            if (di < 0 || (f.margin && !dm3_inside(v.w, x, y, z, f.margin))) { bad = true; return; }
             if (di != last_di) {
                 last_di = di;
                 if (!f.marks[di]) f.marks[di] = 1;
@@ -86,7 +88,7 @@ __global__ void __launch_bounds__(kThreads) k_om3_points(InsertParams f, View v)
             const size_t g = pool_index(v, slot, ci);
             atomicOr(&v.mask[g >> 5], 1u << (g & 31));
             f.rkeys[out] = ((uint32_t)di << kOm3Log2Cells) | ci;
-            f.rvals[out] = op;
+            f.rvals[out] = (uint32_t)(out << 2) | op;   // plain insertion folds the op bits only, whatever the chunk's length
             ++out;
             return;
         }
@@ -161,6 +163,80 @@ struct OpFold {
     }
 };
 
+// ---- the coupled insertion (insert_point_clouds_dm3) ----------------------------------------------------------------------------
+// the distance map's directory and pool; its window is the occupancy map's, so a record key addresses the same cell in both
+struct DmView {
+    const int32_t* dir;
+    uint64_t* cells;
+};
+
+// one thread per run of equal cell keys, as k_fold_runs: folds the run's records into the occupancy word in record order and runs the
+// filter (od3_record) from the distance-map cell's obstacle state; flags[index] = its result
+__global__ void __launch_bounds__(kThreads) k_od3_fold(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals, uint64_t n, View v,
+                                                       int kind, ProbParams pp, DmView dm, uint8_t* flags)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t k = keys[i];
+    if (i > 0 && keys[i - 1] == k) return;
+    const uint32_t di = k >> kOm3Log2Cells, ci = k & (kOm3Cells - 1);
+    const size_t g = pool_index(v, v.dir[di], ci);
+    uint32_t word = v.cells[g];
+    const int32_t ds = dm.dir[di];
+    bool obstacle = ds >= 0 && dm3_obstacle(dm.cells[((size_t)ds << kDm3Log2Cells) | ci]);
+    for (uint64_t j = i; j < n && keys[j] == k; ++j) {
+        const uint32_t r = vals[j];
+        flags[r >> 2] = (uint8_t)od3_record(kind, pp, word, r, obstacle);
+    }
+    v.cells[g] = word;
+}
+
+// per record (record order) with an event: marks the distance map's directory entry
+__global__ void __launch_bounds__(kThreads) k_od3_mark(const uint32_t* __restrict__ keys, const uint8_t* __restrict__ flags, uint64_t n, uint32_t* marks)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !(flags[i] & kOd3Event)) return;
+    const uint32_t di = keys[i] >> kOm3Log2Cells;
+    if (!marks[di]) marks[di] = 1;
+}
+
+// per record: push[i] = 1 when it pushes; an event sets the distance-map cell's known bit (the mutable get() of add / removeObstacle)
+// and is counted in *events
+__global__ void __launch_bounds__(kThreads) k_od3_known(const uint32_t* __restrict__ keys, const uint8_t* __restrict__ flags, uint64_t n, DmView dm,
+                                                        uint32_t* push, unsigned long long* events)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t f = i < n ? flags[i] : 0u;
+    const unsigned ev = __ballot_sync(0xffffffffu, (f & kOd3Event) != 0);
+    if ((threadIdx.x & 31) == 0 && ev) atomicAdd(events, (unsigned long long)__popc(ev));
+    if (i >= n) return;
+    push[i] = (f & kOd3Push) ? 1u : 0u;
+    if (!(f & kOd3Event)) return;
+    const uint32_t k = keys[i];
+    unsigned long long* c = (unsigned long long*)dm.cells + (((size_t)dm.dir[k >> kOm3Log2Cells] << kDm3Log2Cells) | (k & (kOm3Cells - 1)));
+    if (!(*c & kDm3KnownBit)) atomicOr(c, (unsigned long long)kDm3KnownBit);
+}
+
+// the pushing records, in record order, into the brushfire's op list (x, y, z, kind) at their exclusive-scan position
+__global__ void __launch_bounds__(kThreads) k_od3_ops(const uint32_t* __restrict__ keys, const uint8_t* __restrict__ flags,
+                                                      const uint32_t* __restrict__ pos, uint64_t n, PatchWindow w, uint32_t* ops)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t f = flags[i];
+    if (!(f & kOd3Push)) return;
+    uint32_t* o = ops + (size_t)kDm3OpWords * pos[i];
+    dm3_key_cell(w, keys[i], o[0], o[1], o[2]);
+    o[3] = (f & kOd3Remove) ? 1u : 0u;
+}
+
+// the op list's segment ends: seg_end[j] = the ops of clouds c0 .. c0 + j (bound: every cloud's first record, rec_base that of c0)
+__global__ void k_od3_segments(const uint32_t* __restrict__ pos, const uint64_t* __restrict__ bound, int c0, int n, uint64_t rec_base, uint32_t* seg_end)
+{
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < n) seg_end[j] = pos[bound[c0 + 1 + j] - rec_base];
+}
+
 // the cells the const get() returns (map.cpp:414-455, container.h:119-123): word and present (patch allocated, known bit set)
 __global__ void __launch_bounds__(kThreads) k_om3_gather(const uint32_t* __restrict__ xyz, int n, View v, uint32_t* words, uint8_t* present)
 {
@@ -218,7 +294,7 @@ struct OccMap3Dev::Impl : PatchStore {
     int kind = kOm3Frequency;
     double resolution = 0, scale = 0;
     ProbParams pp{};
-    Buf qin, qout, qflag, ops, changed;
+    Buf qin, qout, qflag, ops, changed, dops, dseg;
 
     View view() const { return View{dir, (uint32_t*)cells, mask, win}; }
 };
@@ -330,6 +406,160 @@ int OccMap3Dev::insert_point_clouds(const double* pts, const int64_t* offsets, i
     PS_TRY(d.record(1));
     PS_TRY(d.finish(0));
     if (cells) *cells = bound[n_clouds];
+    return LAMA_OK;
+}
+
+// The coupled insertion.  Both maps are admitted before either changes: the mark pass checks every hit and ray cell against a margin
+// of R + 1 (R = the distance map's reach), then the distance map's pool check (the marked entries dilated by R), then the occupancy
+// map's allocation, which refuses a full pool before it writes.  The distance map's queue is then flushed, and per chunk of whole
+// clouds:
+//   1. k_om3_points<2> emits the records (value = index << 2 | op) and sets the occupancy known bits; a stable sort groups them by cell.
+//   2. k_od3_fold folds each cell's run in record order and writes every record's filter flags.
+//   3. k_od3_mark marks the distance map's entries of the events; the distance map allocates them (ascending directory index).
+//   4. k_od3_known sets their known bits and counts events, a scan places the pushes, k_od3_ops writes the op list in record order and
+//      k_od3_segments its per-cloud ends.
+//   5. The distance map applies and updates the list cloud by cloud (k_dm3_brushfire, Brushfire3::run_segments).
+// The next chunk's fold reads the obstacle state this chunk's ops left.  Each map works on its own stream; the hand-overs are events.
+int OccMap3Dev::insert_point_clouds_dm3(DistMap3Dev& dm, const double* pts, const int64_t* offsets, int n_clouds, const double* origins,
+                                        const double* quats, bool full, uint64_t* cells, uint32_t* processed, uint64_t counts[2])
+{
+    Impl& d = *d_;
+    if (cells) *cells = 0;
+    if (counts) counts[0] = counts[1] = 0;
+    if (processed)
+        for (int c = 0; c < n_clouds; ++c) processed[c] = 0;
+    int64_t n_pts = 0;
+    int rc = PatchStore::check_clouds(pts, offsets, n_clouds, n_pts, err_);
+    if (rc != LAMA_OK) return rc;
+    const DistMap3Dev::Coupling cp = dm.coupling();
+    bool same = cp.device == d.device && cp.resolution == d.resolution;
+    for (int k = 0; k < 3; ++k) same = same && cp.win.base[k] == d.win.base[k] && cp.win.dim[k] == d.win.dim[k];
+    if (!same) { err_ = "the occupancy and distance maps must share device, resolution and window"; return LAMA_ERR_ARG; }
+    if (n_clouds == 0) return LAMA_OK;
+    std::vector<uint32_t> proc((size_t)n_clouds, 0);
+    uint64_t events = 0, pushes = 0;
+    PS_TRY(cudaSetDevice(d.device));
+
+    std::vector<uint64_t> bound((size_t)n_clouds + 1, 0);
+    const View v = d.view();
+    InsertParams f{};
+    if (n_pts > 0) {
+        PS_TRY(d.record(0));
+        PS_TRY(d.upload_clouds(pts, offsets, n_clouds, n_pts, origins, quats));
+        f.pts = (const double*)d.pts.p;
+        f.offsets = (const int64_t*)d.off.p;
+        f.tf = (const Affine*)d.tf.p;
+        f.n_clouds = n_clouds;
+        f.p0 = 0;
+        f.p1 = n_pts;
+        f.scale = d.scale;
+        f.full = full ? 1 : 0;
+        f.counts = (uint64_t*)d.counts.p;
+        f.offs = (const uint64_t*)d.offs.p;
+        f.marks = d.marks;
+        f.status = d.status;
+        f.margin = cp.reach + 1;
+
+        // admission: window margin, record counts, both pools; nothing is written before all three pass
+        k_om3_points<0><<<blocks_for(n_pts), kThreads, 0, d.stream>>>(f, v);
+        d.launches[0] += 1;
+        PS_TRY(cudaGetLastError());
+        uint32_t status = 0;
+        std::vector<uint32_t> marks;
+        PS_TRY(d.read_marks(status, marks));
+        if (status & kErrWindow) {
+            err_ = "a hit or ray cell lies less than " + std::to_string(cp.reach + 1) + " cells (the distance map's reach + 1) inside the directory window";
+            return LAMA_ERR_WINDOW;
+        }
+        PS_TRY(d.scan_records(n_pts, n_clouds, bound));
+        d.launches[0] += 2;
+        for (int c = 0; c < n_clouds; ++c)
+            if (bound[(size_t)c + 1] - bound[(size_t)c] >= (uint64_t(1) << 30)) { err_ = "a cloud has 2^30 cell updates or more"; return LAMA_ERR_ARG; }
+        std::vector<uint8_t> next;
+        rc = dm.admit_entries(marks, next);
+        if (rc != LAMA_OK) { err_ = dm.error(); return rc; }
+        rc = d.alloc_marked(marks, v, err_, d.launches[0]);
+        if (rc != LAMA_OK) return rc;
+        dm.commit_reachable(next);
+        PS_TRY(cudaGetLastError());
+        PS_TRY(d.record(1));
+        PS_TRY(d.finish(0));
+    }
+    rc = dm.flush();   // queued ops first: they already sit in the reference's heaps
+    if (rc != LAMA_OK) { err_ = dm.error(); return rc; }
+
+    cudaEvent_t ev[2] = {nullptr, nullptr};   // [0] distance map -> occupancy map, [1] the reverse
+    struct Events {
+        cudaEvent_t* e;
+        ~Events() { for (int k = 0; k < 2; ++k) if (e[k]) cudaEventDestroy(e[k]); }
+    } guard{ev};
+    for (int k = 0; k < 2; ++k) PS_TRY(cudaEventCreateWithFlags(&ev[k], cudaEventDisableTiming));
+    const DmView dv{cp.dir, cp.cells};
+    rc = PatchStore::for_each_chunk(bound, n_clouds, [&](int c0, int c1, uint64_t nrec) -> int {
+        std::vector<uint32_t> seg_end((size_t)(c1 - c0), 0);
+        if (nrec > 0) {
+            PS_TRY(d.record(0));
+            PS_TRY(d.ensure_records<uint32_t>(nrec + 1));
+            PS_TRY(d.ensure(d.changed, (size_t)nrec));
+            f.p0 = offsets[c0];
+            f.p1 = offsets[c1];
+            f.rec_base = bound[(size_t)c0];
+            f.rkeys = (uint32_t*)d.rk[0].p;
+            f.rvals = (uint32_t*)d.rv[0].p;
+            const uint32_t* keys = (const uint32_t*)d.rk[0].p;   // record order
+            uint8_t* flags = (uint8_t*)d.changed.p;
+            const unsigned nb = blocks_for(nrec);
+            k_om3_points<2><<<blocks_for((uint64_t)(f.p1 - f.p0)), kThreads, 0, d.stream>>>(f, v);
+            PS_TRY(d.sort_records<uint32_t>((int64_t)nrec));
+            k_od3_fold<<<nb, kThreads, 0, d.stream>>>((const uint32_t*)d.rk[1].p, (const uint32_t*)d.rv[1].p, nrec, v, d.kind, d.pp, dv, flags);
+            PS_TRY(d.clear_marks());
+            k_od3_mark<<<nb, kThreads, 0, d.stream>>>(keys, flags, nrec, d.marks);
+            d.launches[0] += 4;
+            PS_TRY(cudaGetLastError());
+            uint32_t status = 0;
+            std::vector<uint32_t> marks;
+            PS_TRY(d.read_marks(status, marks));
+            rc = dm.alloc_entries(marks, ev[0]);
+            if (rc != LAMA_OK) { err_ = dm.error(); return rc; }
+            PS_TRY(cudaStreamWaitEvent(d.stream, ev[0], 0));
+            // the sorted values are spent: rv[0] takes the push flags, rv[1] their exclusive scan (nrec + 1 entries)
+            uint32_t* push = (uint32_t*)d.rv[0].p;
+            uint32_t* pos = (uint32_t*)d.rv[1].p;
+            PS_TRY(d.ensure(d.dseg, (size_t)(c1 - c0) * 4 + 8));
+            unsigned long long* ev_count = (unsigned long long*)d.dseg.p;
+            uint32_t* dseg_end = (uint32_t*)((char*)d.dseg.p + 8);
+            PS_TRY(cudaMemsetAsync(ev_count, 0, 8, d.stream));
+            PS_TRY(cudaMemsetAsync(push + nrec, 0, 4, d.stream));
+            k_od3_known<<<nb, kThreads, 0, d.stream>>>(keys, flags, nrec, dv, push, ev_count);
+            size_t bytes = 0;
+            PS_TRY(cub::DeviceScan::ExclusiveSum(nullptr, bytes, push, pos, (int64_t)nrec + 1, d.stream));
+            PS_TRY(d.ensure(d.temp, bytes));
+            PS_TRY(cub::DeviceScan::ExclusiveSum(d.temp.p, bytes, push, pos, (int64_t)nrec + 1, d.stream));
+            k_od3_segments<<<blocks_for((uint64_t)(c1 - c0)), kThreads, 0, d.stream>>>(pos, (const uint64_t*)d.bound.p, c0, c1 - c0, bound[(size_t)c0], dseg_end);
+            d.launches[0] += 3;
+            unsigned long long h_events = 0;
+            PS_TRY(cudaMemcpyAsync(&h_events, ev_count, 8, cudaMemcpyDeviceToHost, d.stream));
+            PS_TRY(cudaMemcpyAsync(seg_end.data(), dseg_end, seg_end.size() * 4, cudaMemcpyDeviceToHost, d.stream));
+            PS_TRY(cudaStreamSynchronize(d.stream));
+            const uint32_t n_push = seg_end.back();
+            PS_TRY(d.ensure(d.dops, (size_t)std::max<uint32_t>(n_push, 1) * kDm3OpWords * 4));
+            k_od3_ops<<<nb, kThreads, 0, d.stream>>>(keys, flags, pos, nrec, d.win, (uint32_t*)d.dops.p);
+            d.launches[0] += 1;
+            PS_TRY(cudaGetLastError());
+            PS_TRY(d.record(1));
+            PS_TRY(cudaEventRecord(ev[1], d.stream));
+            PS_TRY(d.finish(0));
+            events += h_events;
+            pushes += n_push;
+        }
+        rc = dm.run_segments((const uint32_t*)d.dops.p, seg_end, proc.data() + c0, nrec > 0 ? ev[1] : nullptr);
+        if (rc != LAMA_OK) { err_ = dm.error(); return rc; }
+        return LAMA_OK;
+    });
+    if (rc != LAMA_OK) return rc;
+    if (cells) *cells = bound[(size_t)n_clouds];
+    if (counts) { counts[0] = events; counts[1] = pushes; }
+    if (processed) std::copy(proc.begin(), proc.end(), processed);
     return LAMA_OK;
 }
 

@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <string>
 
+#include "ddm3d.h"
 #include "frontend.h"
 
 namespace lama_b200 {
@@ -26,6 +27,15 @@ public:
     // A cell outside the window fails with LAMA_ERR_WINDOW, a full pool with LAMA_ERR_POOL, before anything is written.
     int insert_point_clouds(const double* pts, const int64_t* offsets, int n_clouds, const double* origins, const double* quats, bool full,
                             uint64_t* cells);
+    // The same loop with the distance map dm kept in step, as the reference's map update does (slam2d.cpp:271-316): a setOccupied
+    // that returns true is an addObstacle, a setFree that returns true a removeObstacle, and dm.update() follows every cloud.
+    // processed[c] (may be NULL) = cloud c's update(); counts (may be NULL) = {events, pushes} (the setter calls that returned true,
+    // and those of them whose add / remove pushed a heap entry).  dm's queued ops are applied first.  Both maps must share device,
+    // resolution and window (LAMA_ERR_ARG); LAMA_ERR_WINDOW when a hit or ray cell lies less than dm's reach + 1 cells inside the
+    // window, LAMA_ERR_POOL when either pool could run out, and one cloud of 2^30 records or more is LAMA_ERR_ARG: all before either
+    // map changes.
+    int insert_point_clouds_dm3(DistMap3Dev& dm, const double* pts, const int64_t* offsets, int n_clouds, const double* origins,
+                                const double* quats, bool full, uint64_t* cells, uint32_t* processed, uint64_t counts[2]);
     // setFree / setOccupied / setUnknown (kOm3Set*) of n cells in list order; changed[i] (may be NULL) = the return value of op i
     int apply(const uint32_t* cells_xyz, const uint8_t* ops, int n, uint8_t* changed);
     // getProbability and the isFree / isOccupied / isUnknown flags (bits 0 / 1 / 2) of n cells
@@ -40,7 +50,8 @@ public:
     int export_image(double zed, uint8_t* pixels, size_t cap, int dims[2]);
     int kind() const;
     double resolution() const;
-    // ms / launches: [0] insert_point_clouds, [1] apply, [2] query (times only with dev.timing)
+    // ms / launches: [0] insert_point_clouds (and the occupancy side of insert_point_clouds_dm3), [1] apply, [2] query (times only
+    // with dev.timing)
     void kernel_times(double ms[3], uint64_t launches[3]) const;
     const std::string& error() const { return err_; }
 

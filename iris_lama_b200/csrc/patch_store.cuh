@@ -342,10 +342,10 @@ struct PatchStore {
         return e;
     }
 
-    // Stable radix sort of the n records in rk[0] / rv[0] by key (bits 0 .. end_bit) into rk[1] / rv[1], then k_fold_runs over them.
-    // N is CUB's item count type.
-    template <class Word, class Fold, class N, class V, class... Args>
-    cudaError_t sort_fold(N n, const V& v, Args... args)
+    // Stable radix sort of the n records in rk[0] / rv[0] by key (bits 0 .. end_bit) into rk[1] / rv[1]; rk[0] / rv[0] keep the
+    // records in record order.  N is CUB's item count type.
+    template <class Word, class N>
+    cudaError_t sort_records(N n)
     {
         size_t bytes = 0;
         cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const Word*)rk[0].p, (Word*)rk[1].p, (const Word*)rv[0].p, (Word*)rv[1].p, n, 0,
@@ -354,6 +354,14 @@ struct PatchStore {
         if (e == cudaSuccess)
             e = cub::DeviceRadixSort::SortPairs(temp.p, bytes, (const Word*)rk[0].p, (Word*)rk[1].p, (const Word*)rv[0].p, (Word*)rv[1].p, n, 0, end_bit,
                                                 stream);
+        return e;
+    }
+
+    // sort_records, then k_fold_runs over the sorted records
+    template <class Word, class Fold, class N, class V, class... Args>
+    cudaError_t sort_fold(N n, const V& v, Args... args)
+    {
+        const cudaError_t e = sort_records<Word>(n);
         if (e != cudaSuccess) return e;
         k_fold_runs<Word, Fold><<<blocks_for((uint64_t)n), kThreads, 0, stream>>>((const Word*)rk[1].p, (const Word*)rv[1].p, (uint64_t)n, v, args...);
         return cudaSuccess;
