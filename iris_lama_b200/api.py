@@ -977,24 +977,88 @@ def _clouds(clouds):
     return np.ascontiguousarray(np.concatenate(clouds) if clouds else np.zeros((0, 3))), offsets
 
 
-class TruncatedSignedDistanceMap:
-    """Device-resident lama::TruncatedSignedDistanceMap (include/lama/sdm/truncated_signed_distance_map.h).  `window` = patches per
-    axis (None: dir_dim x dir_dim x 1 in 2-D, 8 x 8 x 4 in 3-D), centred on `center`."""
+class _Map3D:
+    """What the device-resident 3-D maps share: device options and the handle's lifetime, cells from world points, bounds, box
+    shapes and kernel times.  The C-ABI functions are lama_<_PREFIX>_*; _TIMES are the keys of kernelTimes."""
 
-    def __init__(self, resolution, patch_size=32, is3d=False, center=(0.0, 0.0, 0.0), window=None, **dev):
+    _PREFIX = None
+    _TIMES = ()
+
+    def __init__(self, resolution, patch_size, arg, center, window, dev):
+        """lama_<_PREFIX>_create(resolution, patch_size, arg, center, window, dev): arg is the map's own ctypes argument"""
         d = DeviceOptions(device=0, dir_dim=64, pool_slots=0, max_beams=2048, timing=0, stream=0)
         for k, v in dev.items():
             setattr(d, k, v)
         c, cp = _d(center)
         win = None if window is None else (C.c_int32 * 3)(*[int(x) for x in window])
-        self.is3d = bool(is3d)
+        self.resolution = float(resolution)
         self.h = C.c_void_p()
-        _chk(lib().lama_tsdm_create(C.c_double(resolution), C.c_uint32(patch_size), C.c_int(1 if is3d else 0), cp, win, C.byref(d), C.byref(self.h)))
+        _chk(self._fn("create")(C.c_double(resolution), C.c_uint32(patch_size), arg, cp, win, C.byref(d), C.byref(self.h)))
 
     def __del__(self):
         if getattr(self, "h", None) and _lib is not None:
-            _lib.lama_tsdm_destroy(self.h)
+            getattr(_lib, "lama_%s_destroy" % self._PREFIX)(self.h)
             self.h = None
+
+    def _fn(self, name):
+        return getattr(lib(), "lama_%s_%s" % (self._PREFIX, name))
+
+    def _cells(self, cells):
+        a = np.asarray(cells)
+        if np.issubdtype(a.dtype, np.floating):
+            return np.ascontiguousarray(w2m3(self.resolution, a.reshape(-1, 3)))
+        return np.ascontiguousarray(a, np.uint32).reshape(-1, 3)
+
+    @staticmethod
+    def _box(lo, size):
+        """the C arguments of the box lo + [0, size) and the shape of its planes, (size z, size y, size x)"""
+        lo = np.ascontiguousarray(lo, np.uint32)
+        sz = np.ascontiguousarray(size, np.int32)
+        return lo, sz, (int(sz[2]), int(sz[1]), int(sz[0]))
+
+    def bounds(self):
+        """(allocated patches, min cell (3,), max cell (3,)) as Map::bounds"""
+        mn, mx, n = np.zeros(3, np.uint32), np.zeros(3, np.uint32), C.c_int(0)
+        _chk(self._fn("bounds")(self.h, mn.ctypes.data_as(c_u32p), mx.ctypes.data_as(c_u32p), C.byref(n)))
+        return n.value, mn, mx
+
+    def kernelTimes(self):
+        ms, ln = np.zeros(3), np.zeros(3, np.uint64)
+        _chk(self._fn("kernel_times")(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
+        return dict(zip(self._TIMES, ms.tolist())), dict(zip(self._TIMES, ln.tolist()))
+
+
+class _SdmMap3D(_Map3D):
+    """a 3-D map with .sdm files and z-slice images (the TSDM has neither)"""
+
+    def write(self, path):
+        """Map::write (map.cpp:490-529): a 3-D .sdm file"""
+        _chk(self._fn("write")(self.h, str(path).encode()))
+
+    def read(self, path):
+        """Map::read (map.cpp:531-575) into this (empty) map, which takes the file's resolution (map.cpp:548)"""
+        _chk(self._fn("read")(self.h, str(path).encode()))
+        with open(path, "rb") as f:   # IOHeader.resolution (map.h:95-103), a float at byte 24
+            self.resolution = float(np.frombuffer(f.read(28)[24:28], np.float32)[0])
+
+    def exportImage(self, zed=0.0):
+        """the z-slice image of sdm::export_to_png(map, file, zed) (export.cpp:46-96), (height, width) uint8"""
+        return _image(self._fn("export_image"), (self.h, C.c_double(zed)))
+
+    def saveImage(self, path, zed=0.0):
+        write_png(path, self.exportImage(zed))
+
+
+class TruncatedSignedDistanceMap(_Map3D):
+    """Device-resident lama::TruncatedSignedDistanceMap (include/lama/sdm/truncated_signed_distance_map.h).  `window` = patches per
+    axis (None: dir_dim x dir_dim x 1 in 2-D, 8 x 8 x 4 in 3-D), centred on `center`."""
+
+    _PREFIX = "tsdm"
+    _TIMES = ("insert", "distance", "mesh")
+
+    def __init__(self, resolution, patch_size=32, is3d=False, center=(0.0, 0.0, 0.0), window=None, **dev):
+        self.is3d = bool(is3d)
+        super().__init__(resolution, patch_size, C.c_int(1 if is3d else 0), center, window, dev)
 
     def setMaxDistance(self, distance):
         _chk(lib().lama_tsdm_set_max_distance(self.h, C.c_double(distance)))
@@ -1027,17 +1091,9 @@ class TruncatedSignedDistanceMap:
         _chk(lib().lama_tsdm_distance(self.h, pp, C.c_int(n), dist.ctypes.data_as(c_dp), grad.ctypes.data_as(c_dp) if gradient else None))
         return (dist, grad) if gradient else dist
 
-    def bounds(self):
-        """(allocated patches, min cell (3,), max cell (3,)) as Map::bounds"""
-        mn, mx, n = np.zeros(3, np.uint32), np.zeros(3, np.uint32), C.c_int(0)
-        _chk(lib().lama_tsdm_bounds(self.h, mn.ctypes.data_as(c_u32p), mx.ctypes.data_as(c_u32p), C.byref(n)))
-        return n.value, mn, mx
-
     def export(self, lo, size):
         """cells of the box lo + [0, size): dict(distance, weight, on) shaped (size z, size y, size x)"""
-        lo = np.ascontiguousarray(lo, np.uint32)
-        sz = np.ascontiguousarray(size, np.int32)
-        shape = (int(sz[2]), int(sz[1]), int(sz[0]))
+        lo, sz, shape = self._box(lo, size)
         o = dict(distance=np.zeros(shape, np.float32), weight=np.zeros(shape, np.float32), on=np.zeros(shape, np.uint8))
         _chk(lib().lama_tsdm_export(self.h, _vp(lo), _vp(sz), _vp(o["distance"]), _vp(o["weight"]), _vp(o["on"])))
         return o
@@ -1051,14 +1107,8 @@ class TruncatedSignedDistanceMap:
             _chk(lib().lama_tsdm_to_mesh(self.h, _vp(v), C.c_size_t(n.value), C.byref(n)))
         return v, np.arange(n.value, dtype=np.uint32)
 
-    def kernelTimes(self):
-        ms, ln = np.zeros(3), np.zeros(3, np.uint64)
-        _chk(lib().lama_tsdm_kernel_times(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
-        keys = ("insert", "distance", "mesh")
-        return dict(zip(keys, ms.tolist())), dict(zip(keys, ln.tolist()))
 
-
-class OccupancyMap3D:
+class OccupancyMap3D(_SdmMap3D):
     """Device-resident lama::FrequencyOccupancyMap (kind="frequency") or lama::ProbabilisticOccupancyMap (kind="logodds") with
     is3d = true (include/lama/sdm/*_occupancy_map.h).  `window` = patches per axis (None: 8 x 8 x 4), centred on `center`.
 
@@ -1067,28 +1117,12 @@ class OccupancyMap3D:
 
     KINDS = {"frequency": 0, "logodds": 1}
     SET_FREE, SET_OCCUPIED, SET_UNKNOWN = 0, 1, 2
+    _PREFIX = "om3"
+    _TIMES = ("insert", "apply", "query")
 
     def __init__(self, resolution, kind="frequency", patch_size=32, center=(0.0, 0.0, 0.0), window=None, **dev):
-        d = DeviceOptions(device=0, dir_dim=64, pool_slots=0, max_beams=2048, timing=0, stream=0)
-        for k, v in dev.items():
-            setattr(d, k, v)
-        c, cp = _d(center)
-        win = None if window is None else (C.c_int32 * 3)(*[int(x) for x in window])
         self.kind = kind
-        self.resolution = float(resolution)
-        self.h = C.c_void_p()
-        _chk(lib().lama_om3_create(C.c_double(resolution), C.c_uint32(patch_size), C.c_int(self.KINDS[kind]), cp, win, C.byref(d), C.byref(self.h)))
-
-    def __del__(self):
-        if getattr(self, "h", None) and _lib is not None:
-            _lib.lama_om3_destroy(self.h)
-            self.h = None
-
-    def _cells(self, cells):
-        a = np.asarray(cells)
-        if np.issubdtype(a.dtype, np.floating):
-            return np.ascontiguousarray(w2m3(self.resolution, a.reshape(-1, 3)))
-        return np.ascontiguousarray(a, np.uint32).reshape(-1, 3)
+        super().__init__(resolution, patch_size, C.c_int(self.KINDS[kind]), center, window, dev)
 
     def insertPointClouds(self, clouds, origins=None, quats=None, full=True) -> int:
         """generateOccupancyMap's loop body (graph_slam2d.cpp:146-158) for every point of every (n_k, 3) cloud in order: setOccupied
@@ -1160,74 +1194,30 @@ class OccupancyMap3D:
         """FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158)"""
         _chk(lib().lama_om3_prune(self.h))
 
-    def bounds(self):
-        """(allocated patches, min cell (3,), max cell (3,)) as Map::bounds"""
-        mn, mx, n = np.zeros(3, np.uint32), np.zeros(3, np.uint32), C.c_int(0)
-        _chk(lib().lama_om3_bounds(self.h, mn.ctypes.data_as(c_u32p), mx.ctypes.data_as(c_u32p), C.byref(n)))
-        return n.value, mn, mx
-
     def export(self, lo, size):
         """cells of the box lo + [0, size), shaped (size z, size y, size x): dict(occupied, visited, known) for a frequency map,
         dict(prob (float32 log-odds), known) for a log-odds map, and `word`, the raw 32-bit cells"""
-        lo = np.ascontiguousarray(lo, np.uint32)
-        sz = np.ascontiguousarray(size, np.int32)
-        shape = (int(sz[2]), int(sz[1]), int(sz[0]))
+        lo, sz, shape = self._box(lo, size)
         w, k = np.zeros(shape, np.uint32), np.zeros(shape, np.uint8)
         _chk(lib().lama_om3_export(self.h, _vp(lo), _vp(sz), _vp(w), _vp(k)))
         if self.kind == "frequency":
             return dict(word=w, occupied=(w & 0xFFFF).astype(np.uint16), visited=(w >> 16).astype(np.uint16), known=k)
         return dict(word=w, prob=w.view(np.float32), known=k)
 
-    def write(self, path):
-        """Map::write (map.cpp:490-529): a 3-D .sdm file"""
-        _chk(lib().lama_om3_write(self.h, str(path).encode()))
 
-    def read(self, path):
-        """Map::read (map.cpp:531-575) into this (empty) map"""
-        _chk(lib().lama_om3_read(self.h, str(path).encode()))
-
-    def exportImage(self, zed=0.0):
-        """the z-slice image of sdm::export_to_png(occ, file, zed) (export.cpp:46-72), (height, width) uint8"""
-        return _image(lib().lama_om3_export_image, (self.h, C.c_double(zed)))
-
-    def saveImage(self, path, zed=0.0):
-        write_png(path, self.exportImage(zed))
-
-    def kernelTimes(self):
-        ms, ln = np.zeros(3), np.zeros(3, np.uint64)
-        _chk(lib().lama_om3_kernel_times(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
-        keys = ("insert", "apply", "query")
-        return dict(zip(keys, ms.tolist())), dict(zip(keys, ln.tolist()))
-
-
-class DynamicDistanceMap3D:
+class DynamicDistanceMap3D(_SdmMap3D):
     """Device-resident lama::DynamicDistanceMap with is3d = true (include/lama/sdm/dynamic_distance_map.h): the six-neighbour dynamic
     brushfire.  setMaxDistance is fixed at creation (`l2_max`); `window` = patches per axis (None: 8 x 8 x 4), centred on `center`.
 
     Cells are (n, 3) integer map coordinates; floating-point arrays passed as cells are world points and go through Map::w2m
     (w2m3), as the reference's Vector3d overloads do.  addObstacle / removeObstacle are queued and applied, in order, by update()
-    or by the next read of the map."""
+    or by the next read of the map, which also takes the file's max_sqdist (readParameters)."""
+
+    _PREFIX = "dm3"
+    _TIMES = ("update", "distance", "cells")
 
     def __init__(self, resolution, l2_max=0.5, patch_size=32, center=(0.0, 0.0, 0.0), window=None, **dev):
-        d = DeviceOptions(device=0, dir_dim=64, pool_slots=0, max_beams=2048, timing=0, stream=0)
-        for k, v in dev.items():
-            setattr(d, k, v)
-        c, cp = _d(center)
-        win = None if window is None else (C.c_int32 * 3)(*[int(x) for x in window])
-        self.resolution = float(resolution)
-        self.h = C.c_void_p()
-        _chk(lib().lama_dm3_create(C.c_double(resolution), C.c_uint32(patch_size), C.c_double(l2_max), cp, win, C.byref(d), C.byref(self.h)))
-
-    def __del__(self):
-        if getattr(self, "h", None) and _lib is not None:
-            _lib.lama_dm3_destroy(self.h)
-            self.h = None
-
-    def _cells(self, cells):
-        a = np.asarray(cells)
-        if np.issubdtype(a.dtype, np.floating):
-            return np.ascontiguousarray(w2m3(self.resolution, a.reshape(-1, 3)))
-        return np.ascontiguousarray(a, np.uint32).reshape(-1, 3)
+        super().__init__(resolution, patch_size, C.c_double(l2_max), center, window, dev)
 
     @property
     def max_sqdist(self):
@@ -1273,44 +1263,13 @@ class DynamicDistanceMap3D:
         _chk(lib().lama_dm3_cell_distance(self.h, _vp(c), C.c_int(len(c)), d.ctypes.data_as(c_dp)))
         return d
 
-    def bounds(self):
-        """(allocated patches, min cell (3,), max cell (3,)) as Map::bounds"""
-        mn, mx, n = np.zeros(3, np.uint32), np.zeros(3, np.uint32), C.c_int(0)
-        _chk(lib().lama_dm3_bounds(self.h, mn.ctypes.data_as(c_u32p), mx.ctypes.data_as(c_u32p), C.byref(n)))
-        return n.value, mn, mx
-
     def export(self, lo, size):
         """cells of the box lo + [0, size), shaped (size z, size y, size x): dict(word (raw uint64), sqdist, ox, oy, oz, valid, queued,
         known)"""
-        lo = np.ascontiguousarray(lo, np.uint32)
-        sz = np.ascontiguousarray(size, np.int32)
-        shape = (int(sz[2]), int(sz[1]), int(sz[0]))
+        lo, sz, shape = self._box(lo, size)
         w, k = np.zeros(shape, np.uint64), np.zeros(shape, np.uint8)
         _chk(lib().lama_dm3_export(self.h, _vp(lo), _vp(sz), _vp(w), _vp(k)))
         return dm3_fields(w, k)
-
-    def write(self, path):
-        """Map::write (map.cpp:490-529) + writeParameters: a 3-D .sdm file"""
-        _chk(lib().lama_dm3_write(self.h, str(path).encode()))
-
-    def read(self, path):
-        """Map::read (map.cpp:531-575) + readParameters into this (empty) map, which takes the file's resolution and max_sqdist"""
-        _chk(lib().lama_dm3_read(self.h, str(path).encode()))
-        with open(path, "rb") as f:   # IOHeader.resolution (map.h:95-103), a float at byte 24
-            self.resolution = float(np.frombuffer(f.read(28)[24:28], np.float32)[0])
-
-    def exportImage(self, zed=0.0):
-        """the z-slice image of sdm::export_to_png(dm, file, zed) (export.cpp:74-96), (height, width) uint8"""
-        return _image(lib().lama_dm3_export_image, (self.h, C.c_double(zed)))
-
-    def saveImage(self, path, zed=0.0):
-        write_png(path, self.exportImage(zed))
-
-    def kernelTimes(self):
-        ms, ln = np.zeros(3), np.zeros(3, np.uint64)
-        _chk(lib().lama_dm3_kernel_times(self.h, ms.ctypes.data_as(c_dp), _vp(ln)))
-        keys = ("update", "distance", "cells")
-        return dict(zip(keys, ms.tolist())), dict(zip(keys, ln.tolist()))
 
     def runStats(self):
         """{launches, grows, raise_cap, lower_cap} of the brushfire since creation"""

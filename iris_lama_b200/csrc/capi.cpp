@@ -1213,7 +1213,8 @@ try {
     // Map::read adopts the file's resolution (map.cpp:549-558); this map's scale is fixed at Init, so a different one is refused
     if (f.header.resolution != (float)h->l->occupancy_map()->resolution()) return set_err("the file's resolution differs from this map's", LAMA_ERR_ARG);
     for (size_t i = 0; i < f.ids.size(); ++i) {
-        const uint32_t ax = (uint32_t)(f.ids[i] / 2642244ull) << kPatchLog2, ay = (uint32_t)(f.ids[i] % 2642244ull) << kPatchLog2;
+        uint32_t ax, ay;
+        p2m(f.ids[i], ax, ay);
         const int8_t* c = reinterpret_cast<const int8_t*>(f.cells.data() + i * (size_t)kPatchCells);
         const uint64_t* mask = f.masks.data() + i * (kPatchCells / 64);
         for (uint32_t ci = 0; ci < (uint32_t)kPatchCells; ++ci)
@@ -1514,11 +1515,9 @@ try {
     lama_device_options d;
     if (dev) d = *dev; else dev_default(&d);
     std::string err;
-    TsdmDev* t = TsdmDev::create(resolution, patch_size, is3d != 0, center_xyz, window_patches, dev_from(d), err);
-    if (!t) {
-        const bool bad_arg = !(resolution > 0) || patch_size != 32 || err.find("window") != std::string::npos;
-        return set_err(err, !bad_arg && lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : (bad_arg ? LAMA_ERR_ARG : LAMA_ERR_CUDA));
-    }
+    int code = LAMA_OK;
+    TsdmDev* t = TsdmDev::create(resolution, patch_size, is3d != 0, center_xyz, window_patches, dev_from(d), err, &code);
+    if (!t) return set_err(err, code);
     *out = new lama_tsdm{t};
     return LAMA_OK;
 }
@@ -1624,11 +1623,9 @@ try {
     lama_device_options d;
     if (dev) d = *dev; else dev_default(&d);
     std::string err;
-    OccMap3Dev* m = OccMap3Dev::create(resolution, patch_size, kind, center_xyz, window_patches, dev_from(d), err);
-    if (!m) {
-        const bool bad_arg = !(resolution > 0) || patch_size != 32 || (kind != 0 && kind != 1) || err.find("window") != std::string::npos;
-        return set_err(err, !bad_arg && lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : (bad_arg ? LAMA_ERR_ARG : LAMA_ERR_CUDA));
-    }
+    int code = LAMA_OK;
+    OccMap3Dev* m = OccMap3Dev::create(resolution, patch_size, kind, center_xyz, window_patches, dev_from(d), err, &code);
+    if (!m) return set_err(err, code);
     *out = new lama_om3{m};
     return LAMA_OK;
 }
@@ -1731,13 +1728,9 @@ try {
     lama_device_options d;
     if (dev) d = *dev; else dev_default(&d);
     std::string err;
-    const bool bad_arg = !(resolution > 0) || patch_size != 32 || !(std::ceil(l2_max / resolution) >= 0 && std::ceil(l2_max / resolution) <= 63);
-    if (bad_arg) return set_err("resolution must be positive, patch_size 32 and ceil(l2_max / resolution) 0..63", LAMA_ERR_ARG);
-    DistMap3Dev* m = DistMap3Dev::create(resolution, patch_size, l2_max, center_xyz, window_patches, dev_from(d), err);
-    if (!m) {
-        const bool win = err.find("window") != std::string::npos;
-        return set_err(err, win ? LAMA_ERR_ARG : (lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_CUDA));
-    }
+    int code = LAMA_OK;
+    DistMap3Dev* m = DistMap3Dev::create(resolution, patch_size, l2_max, center_xyz, window_patches, dev_from(d), err, &code);
+    if (!m) return set_err(err, code);
     *out = new lama_dm3{m};
     return LAMA_OK;
 }

@@ -27,7 +27,6 @@ namespace lama_b200 {
 
 namespace {
 
-constexpr uint64_t kUniversalConstant = 2642244ull;   // map.h:68
 constexpr uint64_t kPopBudget = uint64_t(1) << 20;     // pops per brushfire launch
 constexpr uint32_t kHeapCap0 = 1u << 16;               // initial entries of each heap
 
@@ -83,11 +82,10 @@ __global__ void __launch_bounds__(1) k_dm3_brushfire(View v, uint64_t* rq, uint3
 // obstacle, reads sqrt(max_sqdist) * resolution
 __device__ __forceinline__ double dm3_distance_at(const View& v, uint32_t x, uint32_t y, uint32_t z, uint32_t max_sqdist, double resolution)
 {
-    const int di = window_dir_index(v.win, x, y, z);
-    const int32_t slot = di < 0 ? -1 : v.dir[di];
+    const int64_t g = cell_pool_index(v.win, v.dir, kDm3Log2Cells, x, y, z);
     uint32_t sq = max_sqdist;
-    if (slot >= 0) {
-        const uint64_t c = v.cells[((size_t)slot << kDm3Log2Cells) | dm3_cell_index(x, y, z)];
+    if (g >= 0) {
+        const uint64_t c = v.cells[g];
         if (dm3_known(c) && dm3_valid(c)) sq = dm3_sqdist(c);
     }
     return mul_rn(sqrt((double)sq), resolution);
@@ -112,18 +110,17 @@ __global__ void __launch_bounds__(kThreads) k_dm3_cell_distance(View v, const ui
     if (i < n) dist[i] = dm3_distance_at(v, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], max_sqdist, resolution);
 }
 
-__global__ void k_dm3_export(View v, uint32_t x0, uint32_t y0, uint32_t z0, int w, int h, int dd, uint64_t* words, uint8_t* known)
-{
-    const size_t n = (size_t)w * h * dd;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t x = x0 + (uint32_t)(i % w), y = y0 + (uint32_t)((i / w) % h), z = z0 + (uint32_t)(i / ((size_t)w * h));
-        const int di = window_dir_index(v.win, x, y, z);
-        const int32_t slot = di < 0 ? -1 : v.dir[di];
-        const uint64_t c = slot < 0 ? 0ull : v.cells[((size_t)slot << kDm3Log2Cells) | dm3_cell_index(x, y, z)];
-        words[i] = c;
-        known[i] = dm3_known(c);
+// k_export_box's cell: the word (0 where there is no patch) and its known bit
+struct BoxCell {
+    static constexpr int kPlanes = 2;
+    static constexpr size_t kBytes[kPlanes] = {8, 1};
+    static __device__ __forceinline__ void put(const View& v, int64_t g, size_t i, const Planes& out)
+    {
+        const uint64_t c = g < 0 ? 0ull : v.cells[g];
+        ((uint64_t*)out.p[0])[i] = c;
+        ((uint8_t*)out.p[1])[i] = dm3_known(c);
     }
-}
+};
 
 uint64_t env_u64(const char* name, uint64_t dflt)
 {
@@ -156,7 +153,7 @@ struct DistMap3Dev::Impl : PatchStore {
     uint64_t runs = 0, grows = 0;
     std::vector<uint32_t> pending;            // queued ops, kDm3OpWords words each
     uint32_t pending_kind[2] = {0, 0};        // queued adds, removes
-    Buf ops, qin, qout, qgrad, qflag, seg;
+    Buf ops, qin, qout, qgrad, seg;
 
     ~Impl()
     {
@@ -189,17 +186,15 @@ struct DistMap3Dev::Impl : PatchStore {
 };
 
 DistMap3Dev* DistMap3Dev::create(double resolution, uint32_t patch_size, double l2_max, const double center[3], const int32_t window[3],
-                                 const DeviceOptions& dev, std::string& err)
+                                 const DeviceOptions& dev, std::string& err, int* code)
 {
-    if (!(resolution > 0)) { err = "resolution must be positive"; return nullptr; }
-    if (patch_size != (uint32_t)kPatchLen) { err = "patch_size must be 32 (the device patch layout)"; return nullptr; }
-    const double r = std::ceil(l2_max * (1.0 / resolution));
-    if (!(r >= 0 && r <= kDmMaxRadius)) { err = "l2_max / resolution exceeds 63 cells (8-bit cell offsets)"; return nullptr; }
-    int32_t dim[3] = {8, 8, 4};
-    if (window) for (int k = 0; k < 3; ++k) dim[k] = window[k];
     PatchWindow win;
-    if (!PatchStore::make_window(dim, center, 1.0 / resolution, true, win, err)) return nullptr;
-    if ((int64_t)dim[0] * dim[1] * dim[2] > kDm3MaxEntries) { err = "window has more than 65536 patches"; return nullptr; }
+    *code = PatchStore::make_window(resolution, patch_size, window, kWindow3D, center, true, kDm3MaxEntries, win, err);
+    if (*code != LAMA_OK) return nullptr;
+    const double r = std::ceil(l2_max * (1.0 / resolution));
+    *code = LAMA_ERR_ARG;
+    if (!(r >= 0 && r <= kDmMaxRadius)) { err = "l2_max / resolution exceeds 63 cells (8-bit cell offsets)"; return nullptr; }
+    if (dev.pool_slots >= (1 << 24)) { err = "pool_slots must be below 2^24"; return nullptr; }
 
     DistMap3Dev* t = new DistMap3Dev();
     t->d_ = new Impl();
@@ -210,8 +205,8 @@ DistMap3Dev* DistMap3Dev::create(double resolution, uint32_t patch_size, double 
     d.guard.init(win, (int)r);
     d.budget = env_u64("LAMA_DM3_POP_BUDGET", kPopBudget);                       // test hook: a small pop budget per launch
     const uint64_t cap0 = std::min<uint64_t>(env_u64("LAMA_DM3_HEAP_CAP", kHeapCap0), 1u << 30);   // test hook: a small initial heap
-    if (!d.init(dev, win, kDm3Log2Cells, 8, err)) { delete t; return nullptr; }
-    if (d.pool >= (1 << 24)) { err = "pool_slots must be below 2^24"; delete t; return nullptr; }
+    *code = d.init(dev, win, kDm3Log2Cells, 8, err);
+    if (*code != LAMA_OK) { delete t; return nullptr; }
     cudaError_t e = cudaMemsetAsync(d.cells, 0, (size_t)d.pool << kDm3Log2Cells << 3, d.stream);
     if (e == cudaSuccess) e = cudaMalloc((void**)&d.st, sizeof(Dm3State));
     for (int k = 0; k < 2 && e == cudaSuccess; ++k) {
@@ -222,6 +217,7 @@ DistMap3Dev* DistMap3Dev::create(double resolution, uint32_t patch_size, double 
     if (e == cudaSuccess) e = cudaStreamSynchronize(d.stream);
     if (e != cudaSuccess) {
         err = std::string("DistMap3Dev::create: ") + cudaGetErrorString(e);
+        *code = PatchStore::cuda_failure();
         delete t;
         return nullptr;
     }
@@ -439,22 +435,12 @@ int DistMap3Dev::bounds(uint32_t mn[3], uint32_t mx[3], int* patches)
 
 int DistMap3Dev::export_box(const uint32_t lo[3], const int32_t size[3], uint64_t* words, uint8_t* known)
 {
-    Impl& d = *d_;
-    if (size[0] < 1 || size[1] < 1 || size[2] < 1) { err_ = "empty box"; return LAMA_ERR_ARG; }
     int rc = flush();
     if (rc != LAMA_OK) return rc;
-    const size_t n = (size_t)size[0] * size[1] * size[2];
-    PS_TRY(cudaSetDevice(d.device));
-    PS_TRY(d.ensure(d.qout, n * 8));
-    PS_TRY(d.ensure(d.qflag, n));
-    k_dm3_export<<<std::min<uint64_t>(8192, blocks_for(n)), kThreads, 0, d.stream>>>(d.view(), lo[0], lo[1], lo[2], size[0], size[1], size[2],
-                                                                                     (uint64_t*)d.qout.p, (uint8_t*)d.qflag.p);
-    d.launches[2] += 1;
-    PS_TRY(cudaGetLastError());
-    if (words) PS_TRY(cudaMemcpyAsync(words, d.qout.p, n * 8, cudaMemcpyDeviceToHost, d.stream));
-    if (known) PS_TRY(cudaMemcpyAsync(known, d.qflag.p, n, cudaMemcpyDeviceToHost, d.stream));
-    PS_TRY(cudaStreamSynchronize(d.stream));
-    return LAMA_OK;
+    void* const host[] = {words, known};
+    rc = d_->export_box<BoxCell>(d_->view(), lo, size, host, err_);
+    if (rc == LAMA_OK) d_->launches[2] += 1;
+    return rc;
 }
 
 // Map::write (map.cpp:490-529) with is_3d and writeParameters (:200-203): 10-byte distance_t cells, patches in ascending directory
@@ -466,23 +452,14 @@ int DistMap3Dev::write(const std::string& path)
     if (rc != LAMA_OK) return rc;
     PS_TRY(cudaSetDevice(d.device));
     SdmFile f;
-    f.header.magic = kSdmMagic;
-    f.header.version = kSdmVersion;
-    f.header.cell_size = sizeof(SdmDistanceCell);
-    f.header.patch_length = kPatchLen;
-    f.header.resolution = (float)d.resolution;
-    f.header.is_3d = 1;
+    const std::vector<int32_t> list = d.sdm_begin(f, sizeof(SdmDistanceCell), d.resolution);
     f.params.resize(4);
     std::memcpy(f.params.data(), &d.max_sqdist, 4);
-    const std::vector<int32_t> list = d.allocated();
     f.cells.assign(list.size() * (size_t)kDm3Cells * sizeof(SdmDistanceCell), 0);
     f.masks.assign(list.size() * (size_t)kDm3Cells / 64, 0);
     std::vector<uint64_t> words((size_t)kDm3Cells);
     const View v = d.view();
     for (size_t j = 0; j < list.size(); ++j) {
-        uint32_t a[3];
-        window_anchor(d.win, list[j], a);
-        f.ids.push_back(((uint64_t)(a[0] >> kPatchLog2) * kUniversalConstant + (a[1] >> kPatchLog2)) * kUniversalConstant + (a[2] >> kPatchLog2));   // map.h:153-161
         PS_TRY(cudaMemcpyAsync(words.data(), v.cells + ((size_t)d.h_dir[list[j]] << kDm3Log2Cells), (size_t)kDm3Cells * 8, cudaMemcpyDeviceToHost, d.stream));
         PS_TRY(cudaStreamSynchronize(d.stream));
         SdmDistanceCell* c = reinterpret_cast<SdmDistanceCell*>(f.cells.data()) + j * (size_t)kDm3Cells;
@@ -497,7 +474,6 @@ int DistMap3Dev::write(const std::string& path)
             c[i].is_queued = dm3_queued(w);
         }
     }
-    f.header.num_patches = f.ids.size();
     std::string err;
     if (!sdm_write(path, f, err)) { err_ = err; return LAMA_ERR_ARG; }
     return LAMA_OK;
@@ -520,18 +496,13 @@ int DistMap3Dev::read(const std::string& path)
     const uint32_t R = reach_of(msq);
     if (R > (uint32_t)kDmMaxRadius) { err_ = "the file's max_sqdist " + std::to_string(msq) + " is a reach above 63 cells"; return LAMA_ERR_ARG; }
     if (!(f.header.resolution > 0)) { err_ = "the file's resolution is not positive"; return LAMA_ERR_ARG; }
-    std::vector<int> entry(f.ids.size());
+    std::vector<int> entry;
+    const int rc = d.sdm_entries(f, path, entry, err_);
+    if (rc != LAMA_OK) return rc;
     std::vector<int32_t> file_dir((size_t)d.ndir, -1);
-    const uint64_t uc2 = kUniversalConstant * kUniversalConstant;
-    for (size_t j = 0; j < f.ids.size(); ++j) {   // Map::p2m (map.h:166-177) with is_3d
-        const uint64_t id = f.ids[j];
-        const uint64_t px = id / uc2, py = (id % uc2) / kUniversalConstant, pz = id % kUniversalConstant;
-        const int di = px > 0x7FFFFFF || py > 0x7FFFFFF ? -1
-                                                         : window_dir_index(d.win, (uint32_t)(px << kPatchLog2), (uint32_t)(py << kPatchLog2), (uint32_t)(pz << kPatchLog2));
-        if (di < 0) { err_ = "a patch of " + path + " lies outside the directory window"; return LAMA_ERR_WINDOW; }
-        if (file_dir[(size_t)di] >= 0) { err_ = path + " holds a patch twice"; return LAMA_ERR_ARG; }
-        file_dir[(size_t)di] = (int32_t)j;
-        entry[j] = di;
+    for (size_t j = 0; j < f.ids.size(); ++j) {
+        if (file_dir[(size_t)entry[j]] >= 0) { err_ = path + " holds a patch twice"; return LAMA_ERR_ARG; }
+        file_dir[(size_t)entry[j]] = (int32_t)j;
     }
     if ((int64_t)f.ids.size() > d.pool) { err_ = "the file has more patches than the pool has slots (raise pool_slots)"; return LAMA_ERR_POOL; }
     Dm3Guard guard;
@@ -591,35 +562,27 @@ int DistMap3Dev::read(const std::string& path)
     return LAMA_OK;
 }
 
-// build_image (export.cpp:74-96): bounds in x / y, the slice z = w2m((0, 0, zed)).z; 127 where no cell is known, else
-// distance(coords) * 255 / maxDistance()
+// build_image (export.cpp:74-96) of the z-slice at w2m((0, 0, zed)).z, through the 2-D pixel rule of sdm_io.h
 int DistMap3Dev::export_image(double zed, uint8_t* pixels, size_t cap, int dims[2])
 {
     Impl& d = *d_;
-    uint32_t mn[3], mx[3];
-    int np = 0;
-    int rc = bounds(mn, mx, &np);
+    int rc = flush();
     if (rc != LAMA_OK) return rc;
-    if (np == 0) {
-        dims[0] = dims[1] = 0;
-        return LAMA_OK;
-    }
-    const int w = (int)(mx[0] - mn[0]), h = (int)(mx[1] - mn[1]);
-    dims[0] = w;
-    dims[1] = h;
-    if (!pixels || cap < (size_t)w * h) return LAMA_OK;
-    const uint32_t lo[3] = {mn[0], mn[1], w2m(zed, d.scale)};
-    const int32_t size[3] = {w, h, 1};
-    std::vector<uint64_t> words((size_t)w * h);
-    std::vector<uint8_t> known((size_t)w * h);
+    uint32_t lo[3];
+    int32_t size[3];
+    if (!d.image_box(zed, d.scale, pixels, cap, dims, lo, size)) return LAMA_OK;
+    const size_t n = (size_t)size[0] * size[1];
+    std::vector<uint64_t> words(n);
+    std::vector<uint8_t> known(n);
     rc = export_box(lo, size, words.data(), known.data());
     if (rc != LAMA_OK) return rc;
-    const double max_distance = std::sqrt((double)d.max_sqdist) * d.resolution;   // :155-158
-    for (size_t i = 0; i < words.size(); ++i) {
-        if (!known[i]) { pixels[i] = 127; continue; }
-        const double dist = std::sqrt((double)(dm3_valid(words[i]) ? dm3_sqdist(words[i]) : d.max_sqdist)) * d.resolution;   // :140-147
-        pixels[i] = (uint8_t)(dist * 255 / max_distance);
+    std::vector<uint16_t> sqdist(n);
+    std::vector<uint8_t> valid(n);
+    for (size_t i = 0; i < n; ++i) {
+        sqdist[i] = (uint16_t)dm3_sqdist(words[i]);
+        valid[i] = dm3_valid(words[i]);
     }
+    sdm_distance_image(SdmWindow{lo[0], lo[1], size[0], size[1]}, sqdist.data(), valid.data(), known.data(), d.max_sqdist, d.resolution, pixels);
     return LAMA_OK;
 }
 

@@ -17,9 +17,10 @@ namespace lama_b200 {
 // list order and runs the brushfire, one sequential thread (k_dm3_brushfire).  Every reader applies the queue first.
 class DistMap3Dev {
 public:
-    // setMaxDistance(l2_max) at creation (dynamic_distance_map.cpp:149-153); ceil(l2_max / resolution) must be at most 63 cells
+    // setMaxDistance(l2_max) at creation (dynamic_distance_map.cpp:149-153); ceil(l2_max / resolution) must be at most 63 cells and
+    // dev.pool_slots below 2^24.  Null on failure, with err and its status in *code.
     static DistMap3Dev* create(double resolution, uint32_t patch_size, double l2_max, const double center[3], const int32_t window[3],
-                               const DeviceOptions& dev, std::string& err);
+                               const DeviceOptions& dev, std::string& err, int* code);
     ~DistMap3Dev();
     DistMap3Dev(const DistMap3Dev&) = delete;
     DistMap3Dev& operator=(const DistMap3Dev&) = delete;

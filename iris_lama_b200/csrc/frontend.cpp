@@ -2,6 +2,7 @@
 #include "frontend.h"
 #include "checkpoint.h"
 #include "rng_skip.h"
+#include "sdm_io.h"
 
 #include <cuda_runtime.h>
 
@@ -1306,7 +1307,7 @@ int OccupancyMapDev::prune()
 // ---- SimpleOccupancyHost ---------------------------------------------------------------------------------------
 void SimpleOccupancyHost::set(uint32_t x, uint32_t y, int state)
 {
-    const uint64_t key = (uint64_t)(x >> kPatchLog2) * 2642244ull + (uint64_t)(y >> kPatchLog2);  // Map::m2p, map.h:153-161
+    const uint64_t key = m2p(x, y);
     auto it = patches_.find(key);
     if (it == patches_.end()) it = patches_.emplace(key, std::vector<int8_t>(kPatchCells, 0)).first;
     it->second[cell_index(x, y)] = (int8_t)(state < 0 ? -1 : (state > 0 ? 1 : 0));
@@ -1314,7 +1315,7 @@ void SimpleOccupancyHost::set(uint32_t x, uint32_t y, int state)
 bool SimpleOccupancyHost::is_free_world(double wx, double wy) const
 {
     const uint32_t x = w2m(wx, scale_), y = w2m(wy, scale_);
-    auto it = patches_.find((uint64_t)(x >> kPatchLog2) * 2642244ull + (uint64_t)(y >> kPatchLog2));
+    auto it = patches_.find(m2p(x, y));
     return it != patches_.end() && it->second[cell_index(x, y)] == -1;
 }
 bool SimpleOccupancyHost::bounds_world(double mn[2], double mx[2]) const
@@ -1322,7 +1323,8 @@ bool SimpleOccupancyHost::bounds_world(double mn[2], double mx[2]) const
     if (patches_.empty()) return false;
     uint32_t lo[2] = {0xffffffffu, 0xffffffffu}, hi[2] = {0, 0};
     for (auto& kv : patches_) {
-        const uint32_t ax = (uint32_t)(kv.first / 2642244ull) << kPatchLog2, ay = (uint32_t)(kv.first % 2642244ull) << kPatchLog2;  // Map::p2m
+        uint32_t ax, ay;
+        p2m(kv.first, ax, ay);
         lo[0] = std::min(lo[0], ax); lo[1] = std::min(lo[1], ay);
         hi[0] = std::max(hi[0], ax); hi[1] = std::max(hi[1], ay);
     }

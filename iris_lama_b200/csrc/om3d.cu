@@ -29,8 +29,6 @@ namespace lama_b200 {
 
 namespace {
 
-constexpr uint64_t kUniversalConstant = 2642244ull;   // map.h:68
-
 struct View {
     static constexpr int log2v = kOm3Log2Cells;
     const int32_t* dir;   // slot of each directory entry, -1 = absent
@@ -242,38 +240,22 @@ __global__ void __launch_bounds__(kThreads) k_om3_gather(const uint32_t* __restr
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t x = xyz[3 * i], y = xyz[3 * i + 1], z = xyz[3 * i + 2];
-    const int di = window_dir_index(v.w, x, y, z);
-    const int slot = di < 0 ? -1 : v.dir[di];
-    uint32_t w = 0;
-    bool k = false;
-    if (slot >= 0) {
-        const size_t g = pool_index(v, slot, cell_index(x, y, z));
-        k = (v.mask[g >> 5] >> (g & 31)) & 1u;
-        w = k ? v.cells[g] : 0u;
-    }
-    words[i] = w;
+    const int64_t g = cell_pool_index(v.w, v.dir, kOm3Log2Cells, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2]);
+    const bool k = g >= 0 && ((v.mask[g >> 5] >> (g & 31)) & 1u);
+    words[i] = k ? v.cells[g] : 0u;
     present[i] = k;
 }
 
-__global__ void k_om3_export(View v, uint32_t x0, uint32_t y0, uint32_t z0, int w, int h, int dd, uint32_t* words, uint8_t* known)
-{
-    const size_t n = (size_t)w * h * dd;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t x = x0 + (uint32_t)(i % w), y = y0 + (uint32_t)((i / w) % h), z = z0 + (uint32_t)(i / ((size_t)w * h));
-        const int di = window_dir_index(v.w, x, y, z);
-        const int slot = di < 0 ? -1 : v.dir[di];
-        uint32_t c = 0;
-        uint8_t k = 0;
-        if (slot >= 0) {
-            const size_t g = pool_index(v, slot, cell_index(x, y, z));
-            c = v.cells[g];
-            k = (v.mask[g >> 5] >> (g & 31)) & 1u;
-        }
-        words[i] = c;
-        known[i] = k;
+// k_export_box's cell: the word and the known bit, 0 where there is no patch
+struct BoxCell {
+    static constexpr int kPlanes = 2;
+    static constexpr size_t kBytes[kPlanes] = {4, 1};
+    static __device__ __forceinline__ void put(const View& v, int64_t g, size_t i, const Planes& out)
+    {
+        ((uint32_t*)out.p[0])[i] = g < 0 ? 0u : v.cells[g];
+        ((uint8_t*)out.p[1])[i] = g < 0 ? 0 : (v.mask[g >> 5] >> (g & 31)) & 1u;
     }
-}
+};
 
 // FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158) over the known cells of the first n_slots pool slots
 __global__ void k_om3_prune(View v, int n_slots)
@@ -300,16 +282,16 @@ struct OccMap3Dev::Impl : PatchStore {
 };
 
 OccMap3Dev* OccMap3Dev::create(double resolution, uint32_t patch_size, int kind, const double center[3], const int32_t window[3],
-                               const DeviceOptions& dev, std::string& err)
+                               const DeviceOptions& dev, std::string& err, int* code)
 {
-    if (!(resolution > 0)) { err = "resolution must be positive"; return nullptr; }
-    if (patch_size != (uint32_t)kPatchLen) { err = "patch_size must be 32 (the device patch layout)"; return nullptr; }
-    if (kind != kOm3Frequency && kind != kOm3LogOdds) { err = "kind must be 0 (frequency) or 1 (log-odds)"; return nullptr; }
-    int32_t dim[3] = {8, 8, 4};
-    if (window) for (int k = 0; k < 3; ++k) dim[k] = window[k];
     PatchWindow win;
-    if (!PatchStore::make_window(dim, center, 1.0 / resolution, true, win, err)) return nullptr;
-    if ((int64_t)dim[0] * dim[1] * dim[2] > kOm3MaxEntries) { err = "window has more than 65536 patches"; return nullptr; }
+    *code = PatchStore::make_window(resolution, patch_size, window, kWindow3D, center, true, kOm3MaxEntries, win, err);
+    if (*code != LAMA_OK) return nullptr;
+    if (kind != kOm3Frequency && kind != kOm3LogOdds) {
+        err = "kind must be 0 (frequency) or 1 (log-odds)";
+        *code = LAMA_ERR_ARG;
+        return nullptr;
+    }
 
     OccMap3Dev* t = new OccMap3Dev();
     t->d_ = new Impl();
@@ -325,7 +307,8 @@ OccMap3Dev* OccMap3Dev::create(double resolution, uint32_t patch_size, int kind,
         d.pp.clamp_max = logods(0.97f);
         d.pp.thresh    = 0.0 * logods(0.5f);
     }
-    if (!d.init(dev, win, kOm3Log2Cells, 4, err)) { delete t; return nullptr; }
+    *code = d.init(dev, win, kOm3Log2Cells, 4, err);
+    if (*code != LAMA_OK) { delete t; return nullptr; }
     return t;
 }
 
@@ -657,19 +640,8 @@ int OccMap3Dev::bounds(uint32_t mn[3], uint32_t mx[3], int* patches) const
 
 int OccMap3Dev::export_box(const uint32_t lo[3], const int32_t size[3], uint32_t* words, uint8_t* known)
 {
-    Impl& d = *d_;
-    if (size[0] < 1 || size[1] < 1 || size[2] < 1) { err_ = "empty box"; return LAMA_ERR_ARG; }
-    const size_t n = (size_t)size[0] * size[1] * size[2];
-    PS_TRY(cudaSetDevice(d.device));
-    PS_TRY(d.ensure(d.qout, n * 4));
-    PS_TRY(d.ensure(d.qflag, n));
-    k_om3_export<<<std::min<uint64_t>(8192, blocks_for(n)), kThreads, 0, d.stream>>>(d.view(), lo[0], lo[1], lo[2], size[0], size[1], size[2],
-                                                                                     (uint32_t*)d.qout.p, (uint8_t*)d.qflag.p);
-    PS_TRY(cudaGetLastError());
-    if (words) PS_TRY(cudaMemcpyAsync(words, d.qout.p, n * 4, cudaMemcpyDeviceToHost, d.stream));
-    if (known) PS_TRY(cudaMemcpyAsync(known, d.qflag.p, n, cudaMemcpyDeviceToHost, d.stream));
-    PS_TRY(cudaStreamSynchronize(d.stream));
-    return LAMA_OK;
+    void* const host[] = {words, known};
+    return d_->export_box<BoxCell>(d_->view(), lo, size, host, err_);
 }
 
 // Map::write (map.cpp:490-529) with is_3d: patches in ascending directory index (the reference iterates an unordered_map)
@@ -678,20 +650,11 @@ int OccMap3Dev::write(const std::string& path)
     Impl& d = *d_;
     PS_TRY(cudaSetDevice(d.device));
     SdmFile f;
-    f.header.magic = kSdmMagic;
-    f.header.version = kSdmVersion;
-    f.header.cell_size = 4;
-    f.header.patch_length = kPatchLen;
-    f.header.resolution = (float)d.resolution;
-    f.header.is_3d = 1;
+    const std::vector<int32_t> list = d.sdm_begin(f, 4, d.resolution);
     const View v = d.view();
-    const std::vector<int32_t> list = d.allocated();
     f.cells.resize(list.size() * (size_t)kOm3Cells * 4);
     f.masks.resize(list.size() * (size_t)kOm3Cells / 64);
     for (size_t j = 0; j < list.size(); ++j) {
-        uint32_t a[3];
-        window_anchor(d.win, list[j], a);
-        f.ids.push_back(((uint64_t)(a[0] >> kPatchLog2) * kUniversalConstant + (a[1] >> kPatchLog2)) * kUniversalConstant + (a[2] >> kPatchLog2));   // map.h:153-161
         const int slot = d.h_dir[list[j]];
         PS_TRY(cudaMemcpyAsync(f.cells.data() + j * (size_t)kOm3Cells * 4, v.cells + ((size_t)slot << kOm3Log2Cells), (size_t)kOm3Cells * 4,
                                cudaMemcpyDeviceToHost, d.stream));
@@ -700,13 +663,13 @@ int OccMap3Dev::write(const std::string& path)
                                cudaMemcpyDeviceToHost, d.stream));
     }
     PS_TRY(cudaStreamSynchronize(d.stream));
-    f.header.num_patches = f.ids.size();
     std::string err;
     if (!sdm_write(path, f, err)) { err_ = err; return LAMA_ERR_ARG; }
     return LAMA_OK;
 }
 
-// Map::read (map.cpp:531-575) into an empty map: the cell size and is_3d must match; the file's resolution is taken
+// Map::read (map.cpp:531-575) into an empty map: the cell size and is_3d must match; the file's resolution is taken.  A patch the
+// file holds twice is read twice: the last copy wins, as the reference's insert + read does.
 int OccMap3Dev::read(const std::string& path)
 {
     Impl& d = *d_;
@@ -714,20 +677,14 @@ int OccMap3Dev::read(const std::string& path)
     SdmFile f;
     std::string err;
     if (!sdm_read(path, 4, 0, f, err, true)) { err_ = err; return LAMA_ERR_ARG; }
+    std::vector<int> entry;
+    int rc = d.sdm_entries(f, path, entry, err_);
+    if (rc != LAMA_OK) return rc;
     std::vector<uint32_t> marks((size_t)d.ndir, 0);
-    std::vector<int> entry(f.ids.size());
-    const uint64_t uc2 = kUniversalConstant * kUniversalConstant;
-    for (size_t j = 0; j < f.ids.size(); ++j) {   // Map::p2m (map.h:166-177) with is_3d
-        const uint64_t id = f.ids[j];
-        const uint64_t px = id / uc2, py = (id % uc2) / kUniversalConstant, pz = id % kUniversalConstant;
-        const int di = window_dir_index(d.win, (uint32_t)(px << kPatchLog2), (uint32_t)(py << kPatchLog2), (uint32_t)(pz << kPatchLog2));
-        if (di < 0) { err_ = "a patch of " + path + " lies outside the directory window"; return LAMA_ERR_WINDOW; }
-        marks[di] = 1;
-        entry[j] = di;
-    }
+    for (int di : entry) marks[di] = 1;
     PS_TRY(cudaSetDevice(d.device));
     const View v = d.view();
-    const int rc = d.alloc_marked(marks, v, err_, d.launches[1]);
+    rc = d.alloc_marked(marks, v, err_, d.launches[1]);
     if (rc != LAMA_OK) return rc;
     d.resolution = (double)f.header.resolution;   // map.cpp:548
     d.scale = 1.0 / d.resolution;
@@ -742,31 +699,30 @@ int OccMap3Dev::read(const std::string& path)
     return LAMA_OK;
 }
 
-// build_image (export.cpp:46-72): bounds in x / y, the slice z = w2m((0, 0, zed)).z; 90 = no known cell, 255 free, 0 occupied, 127 else
+// build_image (export.cpp:46-72) of the z-slice at w2m((0, 0, zed)).z, through the 2-D pixel rules of sdm_io.h
 int OccMap3Dev::export_image(double zed, uint8_t* pixels, size_t cap, int dims[2])
 {
     Impl& d = *d_;
-    uint32_t mn[3], mx[3];
-    int np = 0;
-    bounds(mn, mx, &np);
-    if (np == 0) {
-        dims[0] = dims[1] = 0;
-        return LAMA_OK;
-    }
-    const int w = (int)(mx[0] - mn[0]), h = (int)(mx[1] - mn[1]);
-    dims[0] = w;
-    dims[1] = h;
-    if (!pixels || cap < (size_t)w * h) return LAMA_OK;
-    const uint32_t lo[3] = {mn[0], mn[1], w2m(zed, d.scale)};
-    const int32_t size[3] = {w, h, 1};
-    std::vector<uint32_t> words((size_t)w * h);
-    std::vector<uint8_t> known((size_t)w * h);
-    int rc = export_box(lo, size, words.data(), known.data());
+    uint32_t lo[3];
+    int32_t size[3];
+    if (!d.image_box(zed, d.scale, pixels, cap, dims, lo, size)) return LAMA_OK;
+    const size_t n = (size_t)size[0] * size[1];
+    std::vector<uint32_t> words(n);
+    std::vector<uint8_t> known(n);
+    const int rc = export_box(lo, size, words.data(), known.data());
     if (rc != LAMA_OK) return rc;
-    for (size_t i = 0; i < words.size(); ++i) {
-        if (!known[i]) { pixels[i] = 90; continue; }
-        const uint32_t fl = om3_flags(d.kind, true, words[i], d.pp);
-        pixels[i] = (fl & 1u) ? 255 : ((fl & 2u) ? 0 : 127);
+    const SdmWindow win{lo[0], lo[1], size[0], size[1]};
+    if (d.kind == kOm3Frequency) {
+        std::vector<uint16_t> occupied(n), visited(n);
+        for (size_t i = 0; i < n; ++i) {
+            occupied[i] = (uint16_t)occ_occupied(words[i]);
+            visited[i] = (uint16_t)occ_visited(words[i]);
+        }
+        sdm_occupancy_image_frequency(win, occupied.data(), visited.data(), known.data(), pixels);
+    } else {
+        std::vector<float> prob(n);
+        for (size_t i = 0; i < n; ++i) prob[i] = om3_bits_float(words[i]);
+        sdm_occupancy_image_logodds(win, prob.data(), known.data(), d.pp.thresh, pixels);
     }
     return LAMA_OK;
 }

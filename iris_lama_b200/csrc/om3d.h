@@ -16,9 +16,9 @@ namespace lama_b200 {
 // mask), 132 KiB in all.  Patches come from a pool of pool_slots (0: one per directory entry).
 class OccMap3Dev {
 public:
-    // kind: kOm3Frequency or kOm3LogOdds (om3d_core.h)
+    // kind: kOm3Frequency or kOm3LogOdds (om3d_core.h).  Null on failure, with err and its status in *code.
     static OccMap3Dev* create(double resolution, uint32_t patch_size, int kind, const double center[3], const int32_t window[3],
-                              const DeviceOptions& dev, std::string& err);
+                              const DeviceOptions& dev, std::string& err, int* code);
     ~OccMap3Dev();
     OccMap3Dev(const OccMap3Dev&) = delete;
     OccMap3Dev& operator=(const OccMap3Dev&) = delete;

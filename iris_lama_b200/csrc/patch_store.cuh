@@ -1,5 +1,7 @@
-// patch_store.cuh -- the device patch store of TsdmDev (tsdm.cu) and OccMap3Dev (om3d.cu): one map in a dense directory window of
-// patches (patch_window.h) taken from a pool, and the pipeline that fills it from a batch of point clouds in the reference's order.
+// patch_store.cuh -- the device patch store of TsdmDev (tsdm.cu), OccMap3Dev (om3d.cu) and DistMap3Dev (ddm3d.cu): one map in a dense
+// directory window of patches (patch_window.h) taken from a pool, the map-level plumbing the three share (window setup, cell lookup,
+// box exports, z-slice image boxes and the patch placement of .sdm files), and the pipeline that fills a map from a batch of point
+// clouds in the reference's order (TsdmDev and OccMap3Dev).
 //   1. The map's mark pass checks the window, marks the directory entries it touches and counts every point's records; read_marks
 //      reads the status and the marks back.  Nothing in the map is written yet, so a window error leaves it unchanged.
 //   2. alloc_marked allocates the marked entries that have no patch, in ascending directory index (a full pool is refused before any
@@ -8,7 +10,7 @@
 //   4. for_each_chunk cuts the batch at cloud boundaries into chunks of at most kRecordCap records.
 //   5. Per chunk the map emits its records; sort_fold stable-sorts them by cell and k_fold_runs folds each cell's run in record order,
 //      loading and storing the cell once.
-// Included by tsdm.cu and om3d.cu only: everything here has internal linkage in each.
+// Included by tsdm.cu, om3d.cu and ddm3d.cu only: everything here has internal linkage in each.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -23,6 +25,7 @@
 
 #include "frontend.h"
 #include "patch_window.h"
+#include "sdm_io.h"
 
 // evaluates a CUDA call; on failure sets err_ to "<call>: <error>" and returns LAMA_ERR_CUDA
 #define PS_TRY(...)                                                                                         \
@@ -33,11 +36,14 @@
 
 namespace lama_b200 {
 
+int cuda_device_count();   // engine.cu
+
 namespace {
 
 constexpr uint64_t kRecordCap = uint64_t(1) << 24;   // records of one sort chunk (a longer single cloud gets a chunk of its own)
 constexpr int kMaxDim = 2048;                         // patches per window axis: window-relative cells fit 16 bits
 constexpr int kThreads = 256;
+constexpr int32_t kWindow3D[3] = {8, 8, 4};           // the default window of a 3-D map, in patches
 
 inline unsigned blocks_for(uint64_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
@@ -45,6 +51,32 @@ inline unsigned blocks_for(uint64_t n) { return (unsigned)((n + kThreads - 1) / 
 // log2v, the log2 of the cells of a patch: a member, or a static constexpr where it is fixed at compile time.
 template <class V>
 __device__ __forceinline__ size_t pool_index(const V& v, int slot, uint32_t ci) { return ((size_t)slot << v.log2v) | ci; }
+
+// the pool index of cell (x, y, z) in a store of patches of 1 << log2v cells, or -1 when the cell lies outside the window or its
+// patch is absent (the patch lookup of the const get, map.cpp:414-455)
+__device__ __forceinline__ int64_t cell_pool_index(const PatchWindow& w, const int32_t* dir, int log2v, uint32_t x, uint32_t y, uint32_t z)
+{
+    const int di = window_dir_index(w, x, y, z);
+    if (di < 0) return -1;
+    const int slot = dir[di];
+    if (slot < 0) return -1;
+    return (int64_t)(((size_t)slot << log2v) | window_cell_index(x, y, z, w.is3d));
+}
+
+// the device output planes of a box export
+struct Planes { void* p[3]; };
+
+// the box lo + [0, size), x fastest, then y, then z, one grid-stride thread per cell: Cell::put(v, g, i, out) writes entry i of the
+// output planes from the cell at pool index g (-1: no cell there)
+template <class Cell, class V>
+__global__ void k_export_box(V v, PatchWindow w, const int32_t* dir, int log2v, uint32_t x0, uint32_t y0, uint32_t z0, int sx, int sy, int sz, Planes out)
+{
+    const size_t n = (size_t)sx * sy * sz;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t x = x0 + (uint32_t)(i % sx), y = y0 + (uint32_t)((i / sx) % sy), z = z0 + (uint32_t)(i / ((size_t)sx * sy));
+        Cell::put(v, cell_pool_index(w, dir, log2v, x, y, z), i, out);
+    }
+}
 
 __device__ __forceinline__ int cloud_of(const int64_t* off, int n, int64_t p)
 {
@@ -107,7 +139,7 @@ struct PatchStore {
     uint32_t* marks = nullptr;      // per directory entry: touched by this batch
     double ms[3] = {0, 0, 0};
     uint64_t launches[3] = {0, 0, 0};
-    Buf pts, off, tf, counts, offs, bound, slots, rk[2], rv[2], temp;
+    Buf pts, off, tf, counts, offs, bound, slots, rk[2], rv[2], temp, box[3];
 
     PatchStore() = default;
     PatchStore(const PatchStore&) = delete;
@@ -124,24 +156,35 @@ struct PatchStore {
         if (own_stream && stream) cudaStreamDestroy(stream);
     }
 
-    // the window of dim patches centred on center (the origin when null; z = 0 in 2-D); false when an axis is not 1..2048 patches
-    static bool make_window(const int32_t dim[3], const double center[3], double scale, bool is3d, PatchWindow& w, std::string& err)
+    // The window of a map's create(): resolution > 0 and patch_size 32; `window` patches per axis (dflt when null; one on z in 2-D),
+    // 1..2048 on every axis and at most max_entries in all, centred on center (the origin when null).  LAMA_ERR_ARG when refused.
+    static int make_window(double resolution, uint32_t patch_size, const int32_t window[3], const int32_t dflt[3], const double center[3], bool is3d,
+                           int64_t max_entries, PatchWindow& w, std::string& err)
     {
+        if (!(resolution > 0)) { err = "resolution must be positive"; return LAMA_ERR_ARG; }
+        if (patch_size != (uint32_t)kPatchLen) { err = "patch_size must be 32 (the device patch layout)"; return LAMA_ERR_ARG; }
+        int32_t dim[3];
+        for (int k = 0; k < 3; ++k) dim[k] = window ? window[k] : dflt[k];
+        if (!is3d) dim[2] = 1;
         for (int k = 0; k < 3; ++k)
-            if (dim[k] < 1 || dim[k] > kMaxDim) { err = "window must be 1..2048 patches per axis"; return false; }
+            if (dim[k] < 1 || dim[k] > kMaxDim) { err = "window must be 1..2048 patches per axis"; return LAMA_ERR_ARG; }
+        if ((int64_t)dim[0] * dim[1] * dim[2] > max_entries) { err = "window has more than " + std::to_string(max_entries) + " patches"; return LAMA_ERR_ARG; }
         w.is3d = is3d;
         for (int k = 0; k < 3; ++k) {
             w.dim[k] = dim[k];
             const double c = center ? center[k] : 0.0;
-            w.base[k] = (k < 2 || is3d) ? (int32_t)(w2m(c, scale) >> kPatchLog2) - dim[k] / 2 : 0;
+            w.base[k] = (k < 2 || is3d) ? (int32_t)(w2m(c, 1.0 / resolution) >> kPatchLog2) - dim[k] / 2 : 0;
         }
-        return true;
+        return LAMA_OK;
     }
+
+    // the status of a create() whose CUDA call failed
+    static int cuda_failure() { return cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_CUDA; }
 
     // Takes the device and stream of dev (a new non-blocking stream when it names none) and allocates the directory of w, all entries
     // absent, and a pool of dev.pool_slots patches (0: one per entry) of 1 << log2 cells of cell_bytes and one mask bit each.
-    // err = "<call>: <error>" of the CUDA call that failed.
-    bool init(const DeviceOptions& dev, const PatchWindow& w, int log2, size_t cell_bytes, std::string& err)
+    // On failure err = "<call>: <error>" of the CUDA call that failed, and the status is cuda_failure().
+    int init(const DeviceOptions& dev, const PatchWindow& w, int log2, size_t cell_bytes, std::string& err)
     {
         device = dev.device;
         timing = dev.timing != 0;
@@ -156,7 +199,7 @@ struct PatchStore {
 #define PS_INIT(expr)                                                                                        \
         do {                                                                                                 \
             cudaError_t _e = (expr);                                                                         \
-            if (_e != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(_e); return false; } \
+            if (_e != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(_e); return cuda_failure(); } \
         } while (0)
         PS_INIT(cudaSetDevice(dev.device));
         if (dev.stream) {
@@ -175,7 +218,7 @@ struct PatchStore {
         PS_INIT(cudaMemcpyAsync(dir, h_dir.data(), (size_t)ndir * 4, cudaMemcpyHostToDevice, stream));
         PS_INIT(cudaStreamSynchronize(stream));
 #undef PS_INIT
-        return true;
+        return LAMA_OK;
     }
 
     cudaError_t ensure(Buf& b, size_t bytes)
@@ -394,6 +437,83 @@ struct PatchStore {
         for (int i = 0; i < ndir; ++i)
             if (h_dir[i] >= 0) list.push_back(i);
         return list;
+    }
+
+    // ---- exports -----------------------------------------------------------------------------------------------------------------------
+    // The box lo + [0, size) through k_export_box<Cell> into Cell::kPlanes planes of Cell::kBytes[k] bytes per cell; each plane k with
+    // a non-null host[k] is copied there.  Waits for the stream.
+    template <class Cell, class V>
+    int export_box(const V& v, const uint32_t lo[3], const int32_t size[3], void* const host[], std::string& err)
+    {
+        if (size[0] < 1 || size[1] < 1 || size[2] < 1) { err = "empty box"; return LAMA_ERR_ARG; }
+        const size_t n = (size_t)size[0] * size[1] * size[2];
+        Planes out{};
+        cudaError_t e = cudaSetDevice(device);
+        for (int k = 0; k < Cell::kPlanes && e == cudaSuccess; ++k) {
+            e = ensure(box[k], n * Cell::kBytes[k]);
+            out.p[k] = box[k].p;
+        }
+        if (e == cudaSuccess) {
+            k_export_box<Cell><<<std::min<uint64_t>(8192, blocks_for(n)), kThreads, 0, stream>>>(v, win, dir, log2v, lo[0], lo[1], lo[2], size[0], size[1],
+                                                                                               size[2], out);
+            e = cudaGetLastError();
+        }
+        for (int k = 0; k < Cell::kPlanes && e == cudaSuccess; ++k)
+            if (host[k]) e = cudaMemcpyAsync(host[k], out.p[k], n * Cell::kBytes[k], cudaMemcpyDeviceToHost, stream);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+        if (e != cudaSuccess) { err = std::string("box export: ") + cudaGetErrorString(e); return LAMA_ERR_CUDA; }
+        return LAMA_OK;
+    }
+
+    // The slice of build_image (export.cpp:46-96) at z = w2m(zed): the x / y bounds of the allocated patches, one cell deep, as lo and
+    // size; dims = {width, height}, 0 x 0 without patches.  False when there is no image to export: no patch, or pixels is null or
+    // smaller than the image.
+    bool image_box(double zed, double scale, const uint8_t* pixels, size_t cap, int dims[2], uint32_t lo[3], int32_t size[3]) const
+    {
+        uint32_t mn[3], mx[3];
+        int np = 0;
+        bounds(mn, mx, &np);
+        dims[0] = np ? (int)(mx[0] - mn[0]) : 0;
+        dims[1] = np ? (int)(mx[1] - mn[1]) : 0;
+        lo[0] = mn[0];
+        lo[1] = mn[1];
+        lo[2] = w2m(zed, scale);
+        size[0] = dims[0];
+        size[1] = dims[1];
+        size[2] = 1;
+        return np > 0 && pixels && cap >= (size_t)dims[0] * dims[1];
+    }
+
+    // ---- .sdm files ----------------------------------------------------------------------------------------------------------------------
+    // Map::write (map.cpp:490-529): the header of a file of cell_size-byte cells and the ids of the allocated patches, in ascending
+    // directory index (the reference iterates an unordered_map).  Returns their directory entries, in the same order.
+    std::vector<int32_t> sdm_begin(SdmFile& f, uint32_t cell_size, double resolution) const
+    {
+        sdm_begin_file(f, cell_size, (float)resolution);
+        f.header.is_3d = win.is3d ? 1 : 0;
+        const std::vector<int32_t> list = allocated();
+        for (int32_t i : list) {
+            uint32_t a[3];
+            window_anchor(win, i, a);
+            f.ids.push_back(win.is3d ? m2p(a[0], a[1], a[2]) : m2p(a[0], a[1]));
+        }
+        f.header.num_patches = list.size();
+        return list;
+    }
+
+    // Map::read (map.cpp:531-575): entry[j] = the directory entry of the file's patch j (Map::p2m); LAMA_ERR_WINDOW when one lies
+    // outside the window
+    int sdm_entries(const SdmFile& f, const std::string& path, std::vector<int>& entry, std::string& err) const
+    {
+        entry.resize(f.ids.size());
+        for (size_t j = 0; j < f.ids.size(); ++j) {
+            uint32_t a[3] = {0, 0, 0};
+            if (win.is3d) p2m(f.ids[j], a[0], a[1], a[2]);
+            else p2m(f.ids[j], a[0], a[1]);
+            entry[j] = window_dir_index(win, a[0], a[1], a[2]);
+            if (entry[j] < 0) { err = "a patch of " + path + " lies outside the directory window"; return LAMA_ERR_WINDOW; }
+        }
+        return LAMA_OK;
     }
 
 private:

@@ -1,5 +1,5 @@
-// patch_window.h -- the dense directory window of the device patch stores (TsdmDev, OccMap3Dev): a directory index per patch and a
-// cell index per cell.  Plain C++ usable from host and device.
+// patch_window.h -- the dense directory window of the device patch stores (TsdmDev, OccMap3Dev, DistMap3Dev): a directory index per
+// patch and a cell index per cell.  Plain C++ usable from host and device.
 #pragma once
 
 #include "lama_core.h"

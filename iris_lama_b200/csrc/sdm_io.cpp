@@ -5,12 +5,9 @@
 #include <cstdio>
 #include <cstring>
 
-#include "lama_core.h"
-
 namespace lama_b200 {
 
 namespace {
-constexpr uint64_t kUniversalConstant = 2642244ull;  // map.h:68
 constexpr int kMaskWords = kPatchCells / 64;
 
 struct File {
@@ -35,13 +32,14 @@ void for_each_patch(const SdmWindow& win, const uint8_t* known, Emit&& emit)
                         any = true;
                     }
             if (!any) continue;
-            const uint64_t id = (uint64_t)((win.x0 >> kPatchLog2) + (uint32_t)bx) * kUniversalConstant + (uint64_t)((win.y0 >> kPatchLog2) + (uint32_t)by);
-            emit(id, bx, by, mask);
+            emit(m2p(win.x0 + (uint32_t)(bx * kPatchLen), win.y0 + (uint32_t)(by * kPatchLen)), bx, by, mask);
         }
 }
 // cells of one patch: 32 x 32, or 32 x 32 x 32 when the header says is_3d (Map::read, map.cpp:550)
 size_t patch_volume(const SdmHeader& h) { return (size_t)kPatchCells * (h.is_3d ? kPatchLen : 1); }
-void begin_file(SdmFile& out, uint32_t cell_size, float resolution)
+}  // namespace
+
+void sdm_begin_file(SdmFile& out, uint32_t cell_size, float resolution)
 {
     out = SdmFile();
     out.header.magic        = kSdmMagic;
@@ -51,7 +49,6 @@ void begin_file(SdmFile& out, uint32_t cell_size, float resolution)
     out.header.resolution   = resolution;
     out.header.is_3d        = 0;
 }
-}  // namespace
 
 bool sdm_write(const std::string& path, const SdmFile& f, std::string& err)
 {
@@ -104,7 +101,7 @@ bool sdm_read(const std::string& path, uint32_t expect_cell_size, size_t n_param
 void sdm_from_distance(const SdmWindow& win, float resolution, uint32_t max_sqdist, const uint16_t* sqdist, const uint8_t* valid, const uint8_t* known,
                        const int16_t* ox, const int16_t* oy, const uint8_t* queued, SdmFile& out)
 {
-    begin_file(out, sizeof(SdmDistanceCell), resolution);
+    sdm_begin_file(out, sizeof(SdmDistanceCell), resolution);
     out.params.resize(4);
     std::memcpy(out.params.data(), &max_sqdist, 4);  // dynamic_distance_map.cpp:200-203
     for_each_patch(win, known, [&](uint64_t id, int bx, int by, const uint64_t* mask) {
@@ -127,7 +124,7 @@ void sdm_from_distance(const SdmWindow& win, float resolution, uint32_t max_sqdi
 
 void sdm_from_frequency(const SdmWindow& win, float resolution, const uint16_t* occupied, const uint16_t* visited, const uint8_t* known, SdmFile& out)
 {
-    begin_file(out, sizeof(SdmFrequencyCell), resolution);
+    sdm_begin_file(out, sizeof(SdmFrequencyCell), resolution);
     for_each_patch(win, known, [&](uint64_t id, int bx, int by, const uint64_t* mask) {
         out.ids.push_back(id);
         out.masks.insert(out.masks.end(), mask, mask + kMaskWords);
@@ -145,7 +142,7 @@ void sdm_from_frequency(const SdmWindow& win, float resolution, const uint16_t* 
 
 void sdm_from_logodds(const SdmWindow& win, float resolution, const float* prob, const uint8_t* known, SdmFile& out)
 {
-    begin_file(out, sizeof(float), resolution);
+    sdm_begin_file(out, sizeof(float), resolution);
     for_each_patch(win, known, [&](uint64_t id, int bx, int by, const uint64_t* mask) {
         out.ids.push_back(id);
         out.masks.insert(out.masks.end(), mask, mask + kMaskWords);

@@ -12,10 +12,28 @@
 #include <string>
 #include <vector>
 
+#include "lama_core.h"
+
 namespace lama_b200 {
 
 constexpr uint32_t kSdmMagic   = 0x6d64732e;  // map.h:72
 constexpr uint16_t kSdmVersion = 0x0103;      // map.h:75
+constexpr uint64_t kUniversalConstant = 2642244;   // map.h:68
+
+// Map::m2p (map.h:153-161): the id of the patch holding cell (x, y), or (x, y, z) in a 3-D map
+inline uint64_t m2p(uint32_t x, uint32_t y) { return (uint64_t)(x >> kPatchLog2) * kUniversalConstant + (y >> kPatchLog2); }
+inline uint64_t m2p(uint32_t x, uint32_t y, uint32_t z) { return m2p(x, y) * kUniversalConstant + (z >> kPatchLog2); }
+// Map::p2m (map.h:166-177): the anchor cell of patch id
+inline void p2m(uint64_t id, uint32_t& x, uint32_t& y)
+{
+    x = (uint32_t)(id / kUniversalConstant) << kPatchLog2;
+    y = (uint32_t)(id % kUniversalConstant) << kPatchLog2;
+}
+inline void p2m(uint64_t id, uint32_t& x, uint32_t& y, uint32_t& z)
+{
+    p2m(id / kUniversalConstant, x, y);
+    z = (uint32_t)(id % kUniversalConstant) << kPatchLog2;
+}
 
 struct SdmHeader {   // the reference's IOHeader with its natural padding made explicit
     uint32_t magic;
@@ -61,6 +79,8 @@ struct SdmWindow {
     int w = 0, h = 0;
 };
 
+// an empty 2-D file of cell_size-byte cells (is_3d = 0)
+void sdm_begin_file(SdmFile& out, uint32_t cell_size, float resolution);
 bool sdm_write(const std::string& path, const SdmFile& f, std::string& err);
 // expect_3d: the file must hold a 3-D map (is_3d = 1, 32 x 32 x 32 patches); otherwise a 2-D one
 bool sdm_read(const std::string& path, uint32_t expect_cell_size, size_t n_params, SdmFile& f, std::string& err, bool expect_3d = false);

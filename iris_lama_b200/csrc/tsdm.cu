@@ -40,12 +40,8 @@ struct View {
 // the const get() (map.cpp:414-455): false when the patch is absent or the cell is off
 __device__ __forceinline__ bool cell_get(const View& v, uint32_t x, uint32_t y, uint32_t z, float2& out)
 {
-    const int di = window_dir_index(v.w, x, y, z);
-    if (di < 0) return false;
-    const int slot = v.dir[di];
-    if (slot < 0) return false;
-    const size_t g = pool_index(v, slot, window_cell_index(x, y, z, v.w.is3d));
-    if (!((v.mask[g >> 5] >> (g & 31)) & 1u)) return false;
+    const int64_t g = cell_pool_index(v.w, v.dir, v.log2v, x, y, z);
+    if (g < 0 || !((v.mask[g >> 5] >> (g & 31)) & 1u)) return false;
     out = v.cells[g];
     return true;
 }
@@ -187,18 +183,19 @@ __global__ void __launch_bounds__(kThreads) k_tsdm_distance(const double* __rest
     for (int k = 0; k < 3; ++k) grad[3 * i + k] = g[k];
 }
 
-__global__ void k_tsdm_export(View v, uint32_t x0, uint32_t y0, uint32_t z0, int w, int h, int dd, float* dist, float* weight, uint8_t* on)
-{
-    const size_t n = (size_t)w * h * dd;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const uint32_t x = x0 + (uint32_t)(i % w), y = y0 + (uint32_t)((i / w) % h), z = z0 + (uint32_t)(i / ((size_t)w * h));
-        float2 c = make_float2(0.f, 0.f);
-        const bool b = cell_get(v, x, y, z, c);
-        dist[i] = c.x;
-        weight[i] = c.y;
-        on[i] = b;
+// k_export_box's cell: distance, weight and the "on" bit, zeros where the const get() returns nothing
+struct BoxCell {
+    static constexpr int kPlanes = 3;
+    static constexpr size_t kBytes[kPlanes] = {4, 4, 1};
+    static __device__ __forceinline__ void put(const View& v, int64_t g, size_t i, const Planes& out)
+    {
+        const bool on = g >= 0 && ((v.mask[g >> 5] >> (g & 31)) & 1u);
+        const float2 c = on ? v.cells[g] : make_float2(0.f, 0.f);
+        ((float*)out.p[0])[i] = c.x;
+        ((float*)out.p[1])[i] = c.y;
+        ((uint8_t*)out.p[2])[i] = on;
     }
-}
+};
 
 // toMesh (:220-272): one thread per cell of the listed patches (ascending directory index, then cell index).  kEmit = false: the
 // vertex count of the cell; true: its vertices from offs.
@@ -241,23 +238,18 @@ __global__ void __launch_bounds__(kThreads) k_tsdm_mesh(const int32_t* __restric
 struct TsdmDev::Impl : PatchStore {
     double resolution = 0;
     TsdmParams prm{};
-    Buf hkeys, hval, hslot, surv, inserted, qout, list, mesh, box[3];
+    Buf hkeys, hval, hslot, surv, inserted, qout, list, mesh;
 
     View view() const { return View{dir, (float2*)cells, mask, win, log2v}; }
 };
 
 TsdmDev* TsdmDev::create(double resolution, uint32_t patch_size, bool is3d, const double center[3], const int32_t window[3], const DeviceOptions& dev,
-                         std::string& err)
+                         std::string& err, int* code)
 {
-    if (!(resolution > 0)) { err = "resolution must be positive"; return nullptr; }
-    if (patch_size != (uint32_t)kPatchLen) { err = "patch_size must be 32 (the device patch layout)"; return nullptr; }
-    int32_t dim[3] = {dev.dir_dim, dev.dir_dim, 1};
-    if (is3d) { dim[0] = 8; dim[1] = 8; dim[2] = 4; }
-    if (window) for (int k = 0; k < 3; ++k) dim[k] = window[k];
-    if (!is3d) dim[2] = 1;
+    const int32_t dim2d[3] = {dev.dir_dim, dev.dir_dim, 1};
     PatchWindow win;
-    if (!PatchStore::make_window(dim, center, 1.0 / resolution, is3d, win, err)) return nullptr;
-    if ((int64_t)dim[0] * dim[1] * dim[2] > (1 << 22)) { err = "window has more than 2^22 patches"; return nullptr; }
+    *code = PatchStore::make_window(resolution, patch_size, window, is3d ? kWindow3D : dim2d, center, is3d, 1 << 22, win, err);
+    if (*code != LAMA_OK) return nullptr;
 
     TsdmDev* t = new TsdmDev();
     t->d_ = new Impl();
@@ -269,12 +261,18 @@ TsdmDev* TsdmDev::create(double resolution, uint32_t patch_size, bool is3d, cons
     d.prm.epsilon = (float)resolution;
     d.prm.max_weight = 10000.0f;
     d.prm.is3d = is3d;
-    if (!d.init(dev, win, is3d ? 3 * kPatchLog2 : 2 * kPatchLog2, sizeof(float2), err)) { delete t; return nullptr; }
+    *code = d.init(dev, win, is3d ? 3 * kPatchLog2 : 2 * kPatchLog2, sizeof(float2), err);
+    if (*code != LAMA_OK) { delete t; return nullptr; }
     const McTable mc = mc_build_table();
     cudaError_t e = cudaMemcpyToSymbolAsync(c_mc_tri, mc.tri, sizeof(mc.tri), 0, cudaMemcpyHostToDevice, d.stream);
     if (e == cudaSuccess) e = cudaMemcpyToSymbolAsync(c_mc_ntri, mc.ntri, sizeof(mc.ntri), 0, cudaMemcpyHostToDevice, d.stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(d.stream);
-    if (e != cudaSuccess) { err = std::string("marching-cubes table: ") + cudaGetErrorString(e); delete t; return nullptr; }
+    if (e != cudaSuccess) {
+        err = std::string("marching-cubes table: ") + cudaGetErrorString(e);
+        *code = PatchStore::cuda_failure();
+        delete t;
+        return nullptr;
+    }
     return t;
 }
 
@@ -409,21 +407,8 @@ int TsdmDev::bounds(uint32_t mn[3], uint32_t mx[3], int* patches) const
 
 int TsdmDev::export_box(const uint32_t lo[3], const int32_t size[3], float* dist, float* weight, uint8_t* on)
 {
-    Impl& d = *d_;
-    if (size[0] < 1 || size[1] < 1 || size[2] < 1) { err_ = "empty box"; return LAMA_ERR_ARG; }
-    const size_t n = (size_t)size[0] * size[1] * size[2];
-    PS_TRY(cudaSetDevice(d.device));
-    PS_TRY(d.ensure(d.box[0], n * 4));
-    PS_TRY(d.ensure(d.box[1], n * 4));
-    PS_TRY(d.ensure(d.box[2], n));
-    k_tsdm_export<<<std::min<uint64_t>(8192, blocks_for(n)), kThreads, 0, d.stream>>>(d.view(), lo[0], lo[1], lo[2], size[0], size[1], size[2],
-                                                                                      (float*)d.box[0].p, (float*)d.box[1].p, (uint8_t*)d.box[2].p);
-    PS_TRY(cudaGetLastError());
-    if (dist) PS_TRY(cudaMemcpyAsync(dist, d.box[0].p, n * 4, cudaMemcpyDeviceToHost, d.stream));
-    if (weight) PS_TRY(cudaMemcpyAsync(weight, d.box[1].p, n * 4, cudaMemcpyDeviceToHost, d.stream));
-    if (on) PS_TRY(cudaMemcpyAsync(on, d.box[2].p, n, cudaMemcpyDeviceToHost, d.stream));
-    PS_TRY(cudaStreamSynchronize(d.stream));
-    return LAMA_OK;
+    void* const host[] = {dist, weight, on};
+    return d_->export_box<BoxCell>(d_->view(), lo, size, host, err_);
 }
 
 int TsdmDev::to_mesh(float* vertices, size_t cap, size_t* n_vertices)

@@ -14,8 +14,9 @@ namespace lama_b200 {
 // pool_slots (0: one per directory entry, so a full window cannot run out).
 class TsdmDev {
 public:
+    // null on failure, with err and its status in *code
     static TsdmDev* create(double resolution, uint32_t patch_size, bool is3d, const double center[3], const int32_t window[3],
-                           const DeviceOptions& dev, std::string& err);
+                           const DeviceOptions& dev, std::string& err, int* code);
     ~TsdmDev();
     TsdmDev(const TsdmDev&) = delete;
     TsdmDev& operator=(const TsdmDev&) = delete;
