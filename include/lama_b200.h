@@ -27,7 +27,8 @@ extern "C" {
 #define LAMA_ERR_ARG (-1)
 #define LAMA_ERR_CUDA (-2)
 #define LAMA_ERR_NO_DEVICE (-3)
-#define LAMA_ERR_WINDOW (-4)   /* the map grew outside the device directory window (raise dir_dim) */
+#define LAMA_ERR_WINDOW (-4)   /* an update touched a cell outside the directory window that no window of dir_dim patches could hold
+                                  (PFSlam2D / Slam2D move their window with the robot; other maps: raise dir_dim) */
 #define LAMA_ERR_POOL (-5)     /* device patch pool exhausted (raise pool_slots) */
 #define LAMA_ERR_OVERFLOW (-6) /* per-scan event log / brushfire heap overflow */
 #define LAMA_ERR_STATE (-7)
@@ -42,7 +43,9 @@ int lama_device_count(void);
 /* device-side knobs shared by all front ends (no counterpart in the reference) */
 typedef struct lama_device_options {
     int32_t device;      /* CUDA device ordinal */
-    int32_t dir_dim;     /* map window = dir_dim x dir_dim patches of 32 x 32 cells, power of two, default 64 */
+    int32_t dir_dim;     /* working window = dir_dim x dir_dim patches of 32 x 32 cells, power of two, default 64.  PFSlam2D and Slam2D
+                            (and LidarOdometry2D) move it with the robot and park the patches it leaves, so pool_slots, not dir_dim,
+                            bounds the size of their maps; the other maps keep a fixed window of this size */
     int32_t pool_slots;  /* 4 KiB patches in the device pool, 0 = auto */
     int32_t max_beams;   /* largest scan accepted, default 2048 */
     int32_t timing;      /* 1: record CUDA-event times per kernel (lama_*_kernel_times) */
@@ -124,6 +127,10 @@ int lama_pf_get_counters(lama_pf* h, uint64_t last[6], uint64_t total[6]);
 int lama_pf_kernel_times(lama_pf* h, double ms[4], uint64_t launches[5]);
 /* Map::bounds of a particle's map (kind 0 occupancy, 1 distance): min/max cell, *patches = numOfPatches */
 int lama_pf_map_bounds(lama_pf* h, int particle, int kind, uint32_t mn[2], uint32_t mx[2], int* patches);
+/* The working window of the maps: base[2] = patch coordinates (cell >> 5) of its first patch, *dim = dir_dim, and
+ * counts = {window shifts so far, directory entries parked outside the window now (every particle and map), entries restored so far}.
+ * LAMA_ERR_STATE before the first update. */
+int lama_pf_get_window(lama_pf* h, int32_t base[2], int32_t* dim, uint64_t counts[3]);
 /* Map::write (src/sdm/map.cpp:490-529) of getOccupancyMap(particle) (kind 0) / getDistanceMap(particle) (kind 1): the reference's
  * ".sdm" file -- IOHeader (map.h:95-103), DynamicDistanceMap's max_sqdist_ (dynamic_distance_map.cpp:200-203), then per patch
  * its id, its 1024 cells in the reference cell layout and the 128-byte known mask (container.cpp:143-163). */
@@ -209,6 +216,7 @@ int lama_slam_get_map_stats(lama_slam* h, uint64_t stats[2]);                /* 
 int lama_slam_get_counters(lama_slam* h, uint64_t last[6], uint64_t total[6]);
 int lama_slam_kernel_times(lama_slam* h, double ms[4], uint64_t launches[5]);
 int lama_slam_map_bounds(lama_slam* h, int kind, uint32_t mn[2], uint32_t mx[2], int* patches);
+int lama_slam_get_window(lama_slam* h, int32_t base[2], int32_t* dim, uint64_t counts[3]);   /* as lama_pf_get_window */
 int lama_slam_export_occupancy(lama_slam* h, uint32_t x0, uint32_t y0, int w, int hgt, uint16_t* occupied, uint16_t* visited, uint8_t* known);
 /* occupancy == 1 only: dense window of ProbabilisticOccupancyMap cells (float log-odds, prob_tag) + Container known bit */
 int lama_slam_occupancy_query(lama_slam* h, const uint32_t* cells_xy, int n, double* prob, uint8_t* flags);   /* as lama_pf_occupancy_query */

@@ -37,6 +37,22 @@ struct FlatCloud {
 };
 
 // lama::PFSlam2D (include/lama/pf_slam2d.h:187-232)
+// the maps' working window (lama_pf_get_window / lama_slam_get_window): base in patch coordinates, dir_dim, shifts so far, entries
+// parked outside the window now, entries restored so far
+struct MapWindow {
+    int32_t base[2] = {0, 0};
+    int32_t dim = 0;
+    uint64_t shifts = 0, parked = 0, restored = 0;
+};
+inline MapWindow map_window(int rc, const int32_t base[2], int32_t dim, const uint64_t c[3])
+{
+    check(rc);
+    MapWindow w;
+    w.base[0] = base[0]; w.base[1] = base[1]; w.dim = dim;
+    w.shifts = c[0]; w.parked = c[1]; w.restored = c[2];
+    return w;
+}
+
 class PFSlam2D {
 public:
     using Options = lama_pf_options;
@@ -106,6 +122,13 @@ public:
         return std::unique_ptr<PFSlam2D>(new PFSlam2D(h));
     }
 
+    MapWindow window() const
+    {
+        int32_t b[2], d = 0;
+        uint64_t c[3];
+        return map_window(lama_pf_get_window(h_, b, &d, c), b, d, c);
+    }
+
 private:
     explicit PFSlam2D(lama_pf* h) : h_(h) {}
     lama_pf* h_ = nullptr;
@@ -135,6 +158,12 @@ public:
     uint32_t getNumberOfProcessedCells() const { uint32_t n = 0; check(lama_slam_get_processed_cells(h_, &n)); return n; }
     void writeMap(int kind, const std::string& path) const { check(lama_slam_write_map(h_, kind, path.c_str())); }
     lama_slam* handle() const { return h_; }
+    MapWindow window() const
+    {
+        int32_t b[2], d = 0;
+        uint64_t c[3];
+        return map_window(lama_slam_get_window(h_, b, &d, c), b, d, c);
+    }
     // checkpoints (no counterpart in the reference), as PFSlam2D::saveState / loadState
     void saveState(const std::string& path) const { check(lama_slam_save_state(h_, path.c_str())); }
     static std::unique_ptr<Slam2D> loadState(const std::string& path, int device = 0)
@@ -220,6 +249,12 @@ public:
         return did != 0;
     }
     void getOdom(double xyr[3]) const { check(lama_slam_get_pose(h_, xyr)); }   // the public member `odom`
+    MapWindow window() const
+    {
+        int32_t b[2], d = 0;
+        uint64_t c[3];
+        return map_window(lama_slam_get_window(h_, b, &d, c), b, d, c);
+    }
 
 private:
     lama_slam* h_ = nullptr;

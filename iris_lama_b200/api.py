@@ -70,11 +70,11 @@ EXPORTED_SYMBOLS = [
     "lama_pf_options_default", "lama_pf_create", "lama_pf_destroy", "lama_pf_set_prior", "lama_pf_update", "lama_pf_get_pose",
     "lama_pf_stage_scans", "lama_pf_update_staged", "lama_pf_get_traffic",
     "lama_pf_get_best_particle", "lama_pf_get_neff", "lama_pf_get_particles", "lama_pf_get_trajectory", "lama_pf_get_last_resample", "lama_pf_get_resample_digest", "lama_pf_get_summary", "lama_pf_get_memory_usage", "lama_pf_get_timestamps", "lama_shard_unique_id", "lama_pf_shard_connect", "lama_pf_shard_stats", "lama_pgo_optimize", "lama_loop_closure_candidates", "lama_slam_correlate_candidate_scan", "lama_dm_correlate_candidate_scan", "lama_slam_coarse_correlate_candidate_scan", "lama_dm_coarse_correlate_candidate_scan", "lama_dm_match_error",
-    "lama_pf_get_counters", "lama_pf_kernel_times", "lama_pf_map_bounds", "lama_pf_export_occupancy", "lama_pf_export_distance",
+    "lama_pf_get_counters", "lama_pf_kernel_times", "lama_pf_map_bounds", "lama_pf_get_window", "lama_pf_export_occupancy", "lama_pf_export_distance",
     "lama_pf_shard_begin", "lama_pf_shard_finish", "lama_pf_shard_apply", "lama_pf_shard_apply_local", "lama_pf_shard_map_update",
     "lama_pf_particle_pack_size", "lama_pf_particle_pack", "lama_pf_particle_unpack",
     "lama_slam_options_default", "lama_slam_create", "lama_slam_destroy", "lama_slam_set_pose", "lama_slam_update", "lama_slam_get_pose",
-    "lama_slam_get_state", "lama_slam_get_processed_cells", "lama_slam_get_counters", "lama_slam_kernel_times", "lama_slam_map_bounds",
+    "lama_slam_get_state", "lama_slam_get_processed_cells", "lama_slam_get_counters", "lama_slam_kernel_times", "lama_slam_map_bounds", "lama_slam_get_window",
     "lama_slam_export_occupancy", "lama_slam_export_distance", "lama_slam_export_logodds",
     "lama_loc_options_default", "lama_loc_create", "lama_loc_destroy", "lama_loc_distance_map", "lama_loc_set_pose", "lama_loc_update",
     "lama_loc_get_pose", "lama_loc_get_state", "lama_loc_get_covar", "lama_loc_get_rmse", "lama_loc_get_solve_stats",
@@ -214,6 +214,14 @@ def _times(fn, h):
         zip(("match", "raycast", "brushfire", "resample", "misc"), ln.tolist()))
 
 
+def _window(fn, h):
+    base = np.zeros(2, np.int32)
+    dim = C.c_int32(0)
+    counts = np.zeros(3, np.uint64)
+    _chk(fn(h, base.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(dim), counts.ctypes.data_as(C.POINTER(C.c_uint64))))
+    return dict(base=(int(base[0]), int(base[1])), dim=dim.value, shifts=int(counts[0]), parked=int(counts[1]), restored=int(counts[2]))
+
+
 def _bounds(fn, args):
     mn = np.zeros(2, np.uint32)
     mx = np.zeros(2, np.uint32)
@@ -321,13 +329,14 @@ def checkpoint_kind(path) -> tuple:
     """(handle kind, first options word) of a checkpoint file's header -- the particle count of a PFSlam2D checkpoint.  Only the header is
     read here; loading checks the whole file."""
     with open(path, "rb") as f:
-        head = f.read(52)
+        head = f.read(60)
     if len(head) < 36 or head[:8] != b"LAMACKPT":
         raise LamaError(-1, f"{path} is not a checkpoint")
     kind = int.from_bytes(head[12:16], "little")
+    body = 40 if int.from_bytes(head[8:12], "little") == 2 else 32   # version 2: the 8-byte parked-entry marker opens the body
     if kind == CKPT_PFSLAM2D_SHARD:   # the particle count follows the 16-byte shard record
-        return kind, int.from_bytes(head[48:52], "little")
-    return kind, int.from_bytes(head[32:36], "little")
+        return kind, int.from_bytes(head[body + 16:body + 20], "little")
+    return kind, int.from_bytes(head[body:body + 4], "little")
 
 
 def _load_state(fn, path, device, stream, timing):
@@ -471,6 +480,10 @@ class PFSlam2D:
 
     def mapBounds(self, particle, kind):
         return _bounds(lib().lama_pf_map_bounds, (self.h, C.c_int(particle), C.c_int(kind)))
+
+    def window(self):
+        """The maps' working window: base (patch coordinates), dim (dir_dim), shifts so far, entries parked now, entries restored so far."""
+        return _window(lib().lama_pf_get_window, self.h)
 
     def exportOccupancy(self, particle, x0, y0, w, h):
         o = _occ_arrays(w, h)
@@ -670,6 +683,10 @@ class Slam2D:
 
     def mapBounds(self, kind):
         return _bounds(lib().lama_slam_map_bounds, (self.h, C.c_int(kind)))
+
+    def window(self):
+        """The maps' working window: base (patch coordinates), dim (dir_dim), shifts so far, entries parked now, entries restored so far."""
+        return _window(lib().lama_slam_get_window, self.h)
 
     def exportOccupancy(self, x0, y0, w, h):
         o = _occ_arrays(w, h)

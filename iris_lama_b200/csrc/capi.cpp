@@ -479,6 +479,22 @@ try {
     return bounds_out(h->p->engine(), pf_local(h, particle), kind, mn, mx, patches);
 }
 LAMA_CATCH
+int window_out(Engine* e, int32_t base[2], int32_t* dim, uint64_t counts[3])
+{
+    if (!e) return set_err("no map yet (update() has not been called)", LAMA_ERR_STATE);
+    if (!base || !dim || !counts) return set_err("null output", LAMA_ERR_ARG);
+    const Engine::WindowInfo wi = e->window_info();
+    base[0] = wi.window.base_px; base[1] = wi.window.base_py;
+    *dim = wi.window.dim;
+    counts[0] = wi.shifts; counts[1] = wi.parked; counts[2] = wi.restored;
+    return LAMA_OK;
+}
+int lama_pf_get_window(lama_pf* h, int32_t base[2], int32_t* dim, uint64_t counts[3])
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    return window_out(h->p->engine(), base, dim, counts);
+}
+LAMA_CATCH
 int lama_pf_export_occupancy(lama_pf* h, int particle, uint32_t x0, uint32_t y0, int w, int hgt, uint16_t* occupied, uint16_t* visited, uint8_t* known)
 try {
     if (!h || pf_local(h, particle) < 0) return set_err("particle not resident on this shard", LAMA_ERR_ARG);
@@ -710,6 +726,12 @@ try {
     if (!h) return set_err("null handle", LAMA_ERR_ARG);
     if (kind == 1) return bounds_dm_union(h->s->engine(), 0, mn, mx, patches);
     return bounds_out(h->s->engine(), 0, kind, mn, mx, patches);
+}
+LAMA_CATCH
+int lama_slam_get_window(lama_slam* h, int32_t base[2], int32_t* dim, uint64_t counts[3])
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    return window_out(h->s->engine(), base, dim, counts);
 }
 LAMA_CATCH
 int lama_slam_export_occupancy(lama_slam* h, uint32_t x0, uint32_t y0, int w, int hgt, uint16_t* occupied, uint16_t* visited, uint8_t* known)

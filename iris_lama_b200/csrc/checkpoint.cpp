@@ -27,6 +27,10 @@ uint64_t fnv1a64(const uint8_t* p, size_t n, uint64_t h)
 int ckpt_write_file(const std::string& path, uint32_t kind, CkptWriter& w, const std::vector<CkptSegment>& tail, std::string& err, CheckpointStats* st)
 {
     const auto t0 = std::chrono::steady_clock::now();
+    if (w.version == kCkptVersionParked) {   // the marker opens the body, so that a reader of version 1 bodies cannot take it for one
+        const uint8_t* m = reinterpret_cast<const uint8_t*>(&kCkptParkMarker);
+        w.buf.insert(w.buf.begin() + kCkptHeaderBytes, m, m + 8);
+    }
     uint8_t* h = w.buf.data();
     uint64_t total = (uint64_t)w.buf.size();
     uint64_t sum = fnv1a64(h + kCkptHeaderBytes, w.buf.size() - kCkptHeaderBytes);
@@ -35,7 +39,7 @@ int ckpt_write_file(const std::string& path, uint32_t kind, CkptWriter& w, const
         sum = fnv1a64(s.p, s.n, sum);
     }
     std::memcpy(h, &kCkptMagic, 8);
-    std::memcpy(h + 8, &kCkptVersion, 4);
+    std::memcpy(h + 8, &w.version, 4);
     std::memcpy(h + 12, &kind, 4);
     std::memcpy(h + 16, &total, 8);
     std::memcpy(h + 24, &sum, 8);
@@ -78,7 +82,12 @@ int ckpt_read_file(const std::string& path, std::vector<uint8_t>& file, uint32_t
     std::memcpy(&total, file.data() + 16, 8);
     std::memcpy(&sum, file.data() + 24, 8);
     if (magic != kCkptMagic) { err = "not a checkpoint (bad magic)"; return LAMA_ERR_ARG; }
-    if (version != kCkptVersion) { err = "unsupported checkpoint format version " + std::to_string(version); return LAMA_ERR_ARG; }
+    uint64_t marker = 0;
+    if (file.size() >= kCkptHeaderBytes + 8) std::memcpy(&marker, file.data() + kCkptHeaderBytes, 8);
+    if (version != kCkptVersion && !(version == kCkptVersionParked && marker == kCkptParkMarker)) {
+        err = "unsupported checkpoint format version " + std::to_string(version) + (version == kCkptVersionParked ? " (no parked-entry marker)" : "");
+        return LAMA_ERR_ARG;
+    }
     if (total != (uint64_t)file.size()) { err = "checkpoint size field differs from the file size (truncated or extended file)"; return LAMA_ERR_ARG; }
     if (fnv1a64(file.data() + kCkptHeaderBytes, file.size() - kCkptHeaderBytes) != sum) { err = "checkpoint checksum mismatch"; return LAMA_ERR_ARG; }
     if (st) {
@@ -89,8 +98,17 @@ int ckpt_read_file(const std::string& path, std::vector<uint8_t>& file, uint32_t
     return LAMA_OK;
 }
 
+CkptReader ckpt_body(const std::vector<uint8_t>& file)
+{
+    uint32_t version = kCkptVersion;
+    std::memcpy(&version, file.data() + 8, 4);
+    const size_t skip = kCkptHeaderBytes + (version == kCkptVersionParked ? 8 : 0);
+    return CkptReader(file.data() + skip, file.size() - skip, version);
+}
+
 void ckpt_put_engine(CkptWriter& w, const EngineImage* img)
 {
+    if (img && !img->parked.empty()) w.version = kCkptVersionParked;
     w.u8(img != nullptr);
     if (!img) return;
     w.i32(img->particles); w.i32(img->dir_dim); w.i32(img->pool_slots); w.i32(img->max_beams); w.i32(img->occupancy_kind);
@@ -101,6 +119,11 @@ void ckpt_put_engine(CkptWriter& w, const EngineImage* img)
     w.u32(img->used);
     w.bytes(img->refcount.data(), img->refcount.size() * 4);
     w.bytes(img->dirs.data(), img->dirs.size() * 4);
+    if (w.version == kCkptVersionParked) {
+        const size_t n_lists = (size_t)img->particles * img->n_kinds();
+        for (size_t li = 0; li < n_lists; ++li) w.u32(li < img->park_len.size() ? (uint32_t)img->park_len[li] : 0u);
+        for (const ParkEntry& e : img->parked) { w.i32(e.px); w.i32(e.py); w.i32(e.entry); }
+    }
 }
 
 bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particles, int occupancy_kind, bool last)
@@ -130,10 +153,41 @@ bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particl
     if (img.used > (uint32_t)img.pool_slots) { r.fail("more used slots than pool slots"); return false; }
     const uint64_t n_dir = (uint64_t)img.particles * img.n_kinds() * img.dir_dim * img.dir_dim;
     // every count against the bytes that are left, before anything is allocated
-    const uint64_t need = (uint64_t)img.used * 4 + n_dir * 4 + (uint64_t)img.used * img.slot_stride();
-    if (need > r.left() || (last && need != r.left())) { r.fail(need > r.left() ? "engine section exceeds the file" : "bytes after the engine section"); return false; }
+    uint64_t need = (uint64_t)img.used * 4 + n_dir * 4 + (uint64_t)img.used * img.slot_stride();
+    if (need > r.left()) { r.fail("engine section exceeds the file"); return false; }
     r.array(img.refcount, img.used, "reference counts");
     r.array(img.dirs, n_dir, "directories");
+    img.park_len.clear();
+    img.parked.clear();
+    if (r.version == kCkptVersionParked) {   // the parked lists
+        const size_t n_lists = (size_t)img.particles * img.n_kinds();
+        r.array(img.park_len, n_lists, "parked list lengths");
+        uint64_t total = 0;
+        for (int32_t n : img.park_len) {
+            if (n < 0) { r.fail("negative parked list length"); return false; }
+            total += (uint64_t)n;
+        }
+        r.count(total, 12, "parked entries");
+        std::vector<int32_t> raw;
+        r.array(raw, (size_t)total * 3, "parked entries");
+        if (!r.ok()) return false;
+        img.parked.resize((size_t)total);
+        for (size_t i = 0; i < img.parked.size(); ++i) img.parked[i] = ParkEntry{raw[3 * i], raw[3 * i + 1], raw[3 * i + 2]};
+        size_t at = 0;
+        for (int32_t n : img.park_len) {
+            for (int32_t k = 0; k < n; ++k, ++at) {
+                const ParkEntry& e = img.parked[at];
+                if (k > 0 && !park_before(img.parked[at - 1].px, img.parked[at - 1].py, e.px, e.py)) { r.fail("parked list not strictly sorted"); return false; }
+                if (e.px < 0 || e.py < 0 || e.px >= max_patch || e.py >= max_patch || patch_in_window(img.window, e.px, e.py)) {
+                    r.fail("parked entry inside the saved window or outside the map");
+                    return false;
+                }
+            }
+        }
+        if (total == 0) img.park_len.clear();
+    }
+    need = (uint64_t)img.used * img.slot_stride();
+    if (need > r.left() || (last && need != r.left())) { r.fail(need > r.left() ? "engine section exceeds the file" : "bytes after the engine section"); return false; }
     img.slot_bytes = r.take((size_t)img.used * img.slot_stride(), "slots");
     if (!r.ok()) return false;
     std::vector<int32_t> refs(img.used, 0);
@@ -143,6 +197,13 @@ bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particl
         if (e < 0 || (e & ~(kDirSlotMask | flags)) != 0) { r.fail("directory entry with unknown flag bits"); return false; }
         const uint32_t slot = (uint32_t)(e & kDirSlotMask);
         if (slot >= img.used) { r.fail("directory entry points past the saved slots"); return false; }
+        ++refs[slot];
+    }
+    for (const ParkEntry& p : img.parked) {
+        const int32_t e = p.entry;
+        if (e < 0 || (e & ~(kDirSlotMask | flags)) != 0) { r.fail("parked entry with unknown flag bits"); return false; }
+        const uint32_t slot = (uint32_t)(e & kDirSlotMask);
+        if (slot >= img.used) { r.fail("parked entry points past the saved slots"); return false; }
         ++refs[slot];
     }
     for (uint32_t s = 0; s < img.used; ++s)

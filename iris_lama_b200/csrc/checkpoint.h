@@ -4,6 +4,9 @@
 // byte after the header}, then the sections: options (field by field), front-end state, and the engine section -- u8 present, then
 // geometry, window, store counters, K, K reference counts, the directories of every particle and kind, and the K slot payloads.  A
 // GraphSlam2D file holds two engine sections, each followed by its own slot payloads.
+// Version 2 (written only when a map has parked entries, window_shift_core.h; everything else is still written as version 1): the body
+// starts with the 8-byte marker "LAMAPARK", and every engine section carries, between its directories and its slots, the parked lists:
+// particles x kinds u32 lengths, then the entries {i32 patch x, i32 patch y, i32 directory entry} list after list.
 // The byte-exact layout is in DESIGN.md §13; tests/test_checkpoint.py, tests/test_graph_checkpoint.py and tests/test_shard_checkpoint.py
 // write it independently.
 #pragma once
@@ -19,6 +22,8 @@ namespace lama_b200 {
 
 constexpr uint64_t kCkptMagic      = 0x54504B43414D414Cull;   // "LAMACKPT"
 constexpr uint32_t kCkptVersion    = 1;
+constexpr uint32_t kCkptVersionParked = 2;
+constexpr uint64_t kCkptParkMarker = 0x4B524150414D414Cull;   // "LAMAPARK"
 constexpr size_t kCkptHeaderBytes  = 32;
 // kind 5 is one rank's shard of a sharded PFSlam2D: {u32 shard_rank, u32 shard_count, u64 session id}, then the options and state
 // sections of kind 1, then the engine section of the rank's own particles (DESIGN.md §13)
@@ -34,6 +39,7 @@ struct CheckpointStats {
 class CkptWriter {
 public:
     std::vector<uint8_t> buf = std::vector<uint8_t>(kCkptHeaderBytes, 0);
+    uint32_t version = kCkptVersion;   // ckpt_put_engine raises it to kCkptVersionParked for an image with parked entries
     void bytes(const void* p, size_t n) { const uint8_t* b = (const uint8_t*)p; buf.insert(buf.end(), b, b + n); }
     template <typename T> void put(T v) { bytes(&v, sizeof(T)); }   // the hosts this builds for are little endian
     void u8(bool v) { put<uint8_t>(v ? 1 : 0); }
@@ -48,7 +54,8 @@ public:
 // Bounds-checked reads: a read past the end sets the error and returns zeros, so a parser can check once per section.
 class CkptReader {
 public:
-    CkptReader(const uint8_t* p, size_t n) : p_(p), n_(n) {}
+    CkptReader(const uint8_t* p, size_t n, uint32_t version = kCkptVersion) : version(version), p_(p), n_(n) {}
+    uint32_t version;
     bool ok() const { return err_.empty(); }
     const std::string& error() const { return err_; }
     void fail(const std::string& m) { if (err_.empty()) err_ = m; }
@@ -102,12 +109,17 @@ struct CkptSegment {
 };
 // Fills the header of w.buf and writes w.buf, then the `tail` segments in order, to `path`; the checksum covers them all.
 int ckpt_write_file(const std::string& path, uint32_t kind, CkptWriter& w, const std::vector<CkptSegment>& tail, std::string& err, CheckpointStats* st);
-// Reads `path` into `file` and checks the header: magic, version, size, checksum.  *kind = the handle kind.
+// Reads `path` into `file` and checks the header: magic, version (and a version-2 body's marker), size, checksum.  *kind = the handle kind.
 int ckpt_read_file(const std::string& path, std::vector<uint8_t>& file, uint32_t* kind, std::string& err, CheckpointStats* st);
+// a reader of the body of a file ckpt_read_file accepted: after the header (and the marker), with the file's version
+CkptReader ckpt_body(const std::vector<uint8_t>& file);
 
 // The engine section.  put writes everything but the slot payloads (the caller passes them as the file's tail); get reads and checks the
-// whole section -- geometry, window, counts against the file size, directory entries (slot < K, known flag bits only), every reference
-// count against its directory references -- and points img.slot_bytes into the reader's buffer.  `particles` / `occupancy_kind` are what
+// whole section -- geometry, window, counts against the file size, directory entries (slot < K, known flag bits only), in a version-2
+// file the parked lists (each strictly sorted, every entry outside the saved window, slot < K, known flag bits only), every reference
+// count against its directory and parked references -- and points img.slot_bytes into the reader's buffer.  An image with parked
+// entries raises w.version; the sections of a file must all be written with its final version (a file's first engine section is the
+// only one that can hold parked entries).  `particles` / `occupancy_kind` are what
 // the front end expects (-1: any).  With `last`, the section must end the file; otherwise other sections may follow its slots.
 void ckpt_put_engine(CkptWriter& w, const EngineImage* img);
 bool ckpt_get_engine(CkptReader& r, bool* present, EngineImage& img, int particles, int occupancy_kind, bool last = true);

@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 
 #include "lama_core.h"
+#include "window_shift_core.h"
 
 namespace lama_b200 {
 
@@ -31,6 +32,13 @@ struct StoreView {
     DirWindow window;
 };
 
+// The parked lists of one directory set (window_shift_core.h), passed apart from StoreView to the kernels that read them: the map-update
+// kernels never do.  ol[particle * n_kinds + kind] = {offset in park, length}; park is null while nothing is parked.
+struct ParkView {
+    ParkEntry* park;
+    int2* ol;
+};
+
 enum MapKind : int { kMapOcc = 0, kMapDm = 1, kMapScratch = 2 };
 
 // A directory entry is -1 (patch absent) or slot | flags:
@@ -44,6 +52,15 @@ enum MapKind : int { kMapOcc = 0, kMapDm = 1, kMapScratch = 2 };
 __device__ __forceinline__ int32_t* dir_of(const StoreView& s, int set, int particle, int kind)
 {
     return s.dirs + (((size_t)set * s.n_particles + particle) * s.n_kinds + kind) * (size_t)(s.window.dim * s.window.dim);
+}
+// the directory entry of the patch holding cell (x, y) of one map: through the window, else from the parked list (-1 = absent)
+__device__ __forceinline__ int32_t map_entry(const StoreView& s, const ParkView& pv, int particle, int kind, const int32_t* dir, uint32_t x, uint32_t y)
+{
+    const int di = dir_index(s.window, x, y);
+    if (di >= 0) return dir[di];
+    if (!pv.park) return -1;
+    const int2 ol = pv.ol[particle * s.n_kinds + kind];
+    return park_find(pv.park + ol.x, ol.y, (int32_t)(x >> kPatchLog2), (int32_t)(y >> kPatchLog2));
 }
 __device__ __forceinline__ uint32_t* patch_ptr(const StoreView& s, int slot) { return s.pool + (size_t)slot * kPatchCells; }
 __device__ __forceinline__ uint32_t* fbits_ptr(const StoreView& s, int slot) { return s.fbits + (size_t)slot * 32; }

@@ -62,6 +62,35 @@ struct Engine::Impl {
     std::vector<std::pair<char*, size_t>> mig_chunks;
     size_t mig_chunk = 0, mig_off = 0;
     std::vector<void*> allocs;
+    // parked entries (window_shift_core.h): per set one device arena (park[set]) and the {offset, length} of every list, on the device
+    // (d_park_ol[set]) and here; they change only in shift_window, resample and prune_outside
+    ParkEntry* park[2] = {nullptr, nullptr};
+    int2* d_park_ol[2] = {nullptr, nullptr};
+    std::vector<int2> park_ol[2];
+    uint64_t shifts = 0, restored = 0;
+    ParkView pv(int set) const { return ParkView{park[set], d_park_ol[set]}; }
+    int n_lists() const { return (int)park_ol[0].size(); }
+    size_t parked(int set) const
+    {
+        size_t n = 0;
+        for (const int2& o : park_ol[set]) n += (size_t)o.y;
+        return n;
+    }
+    cudaError_t fetch(int set, size_t list, std::vector<ParkEntry>& out)   // one parked list, synchronously
+    {
+        const int2 ol = park_ol[set][list];
+        out.resize((size_t)ol.y);
+        if (!ol.y) return cudaSuccess;
+        cudaError_t e = cudaMemcpyAsync(out.data(), park[set] + ol.x, out.size() * sizeof(ParkEntry), cudaMemcpyDeviceToHost, stream);
+        return e == cudaSuccess ? cudaStreamSynchronize(stream) : e;
+    }
+    void drop_arena(int set)   // the stream must have passed every use of the arena
+    {
+        if (park[set]) cudaFree(park[set]);
+        park[set] = nullptr;
+        std::fill(park_ol[set].begin(), park_ol[set].end(), make_int2(0, 0));
+        cudaMemsetAsync(d_park_ol[set], 0, park_ol[set].size() * sizeof(int2), stream);
+    }
 };
 
 
@@ -210,6 +239,11 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     v.status      = reinterpret_cast<uint32_t*>(v.free_count + 2);
     v.counters    = reinterpret_cast<uint64_t*>(v.free_count + 4);
     CU_NEW(dalloc((void**)&v.dirs, 2 * (size_t)cfg.particles * v.n_kinds * dim2 * 4));
+    for (int set = 0; set < 2; ++set) {
+        d->park_ol[set].assign((size_t)cfg.particles * v.n_kinds, make_int2(0, 0));
+        CU_NEW(dalloc((void**)&d->d_park_ol[set], d->park_ol[set].size() * sizeof(int2)));
+        CU_NEW(cudaMemset(d->d_park_ol[set], 0, d->park_ol[set].size() * sizeof(int2)));
+    }
     CU_NEW(dalloc((void**)&d->d_scan_buf, (size_t)cfg.max_beams * 3 * 8));
     d->d_points = d->d_scan_buf;
 
@@ -304,6 +338,8 @@ Engine::~Engine()
     cudaSetDevice(cfg_.device);
     if (d_->stream) cudaStreamSynchronize(d_->stream);
     for (void* p : d_->allocs) cudaFree(p);
+    for (int set = 0; set < 2; ++set)
+        if (d_->park[set]) cudaFree(d_->park[set]);
     if (d_->d_states) cudaFree(d_->d_states);
     if (d_->d_results) cudaFree(d_->d_results);
     if (d_->h_states) cudaFreeHost(d_->h_states);
@@ -476,6 +512,7 @@ int Engine::match(const SE2* states, int count, int first_particle, bool shared_
     mp.particle_offset = first_particle;
     mp.shared_map = shared_map ? 1 : 0;
     mp.mode = mode;
+    mp.parked_any = d_->parked(cur_set_) != 0;
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
     launch_match(d_->view, mp, d_->d_states, d_->d_results, count, d_->stream);
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
@@ -506,7 +543,7 @@ int Engine::match_error(const SE2* states, int count, int first_particle, bool s
     std::memcpy(d_->h_states, states, (size_t)count * sizeof(SE2));
     CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d_->stream));
     double* d_out = reinterpret_cast<double*>(d_->d_results);   // count doubles fit in count MatchResults
-    launch_match_error(d_->view, cur_set_, first_particle, shared_map, d_->d_points, d_->scan, d_->d_states, count, cfg_.resolution, max_sqdist_, d_out, d_->stream);
+    launch_match_error(d_->view, d_->pv(cur_set_), cur_set_, first_particle, shared_map, d_->d_points, d_->scan, d_->d_states, count, cfg_.resolution, max_sqdist_, d_out, d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(out, d_out, (size_t)count * 8, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
@@ -620,6 +657,7 @@ int Engine::step_enqueue(const double* pts, int n, const double origin[3], const
     mp.particle_offset = 0;
     mp.shared_map = 0;
     mp.mode = 0;
+    mp.parked_any = d_->parked(cur_set_) != 0;
     const int tbuf = 1 - pending_buf_;   // the report buffer enqueue_report() will hand to this step
     if (timing_) CU_TRY(cudaEventRecord(d_->evp[tbuf][0], d_->stream));
     launch_match(d_->view, mp, d_->d_states, d_->d_results, count, d_->stream);
@@ -745,6 +783,7 @@ int Engine::share_from(int src_particle, int dst_first, int count)
     if (src_particle < 0 || src_particle >= cfg_.particles || dst_first < 0 || dst_first + count > cfg_.particles ||
         (src_particle >= dst_first && src_particle < dst_first + count))
         return fail("share_from: bad particle range", LAMA_ERR_ARG);
+    if (has_parked()) return fail("share_from: the maps have parked entries (the window has moved); share_from builds a filter's first maps", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
     for (int i = 0; i < count; ++i) d_->h_idx[i] = src_particle;
     CU_TRY(cudaMemcpyAsync(d_->d_idx, d_->h_idx, (size_t)count * 4, cudaMemcpyHostToDevice, d_->stream));
@@ -769,8 +808,26 @@ int Engine::resample(const int32_t* idx)
     CU_TRY(cudaMemcpyAsync(d_->d_idx, d_->h_idx, (size_t)P * 4, cudaMemcpyHostToDevice, d_->stream));
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
     const int other = 1 - cur_set_;
+    // the offspring's parked lists: copies of their ancestors' (kinds 0 and 1, like the directories), in a new arena of the other set
+    const bool parked = d_->parked(cur_set_) != 0;
+    if (parked) {
+        const int nk = d_->view.n_kinds;
+        std::vector<int2>& ol = d_->park_ol[other];
+        int32_t off = 0;
+        for (int p = 0; p < P; ++p)
+            for (int k = 0; k < nk; ++k) {
+                const int32_t len = idx[p] >= 0 && k < 2 ? d_->park_ol[cur_set_][(size_t)idx[p] * nk + k].y : 0;
+                ol[(size_t)p * nk + k] = make_int2(off, len);
+                off += len;
+            }
+        if (off) CU_TRY(cudaMalloc((void**)&d_->park[other], (size_t)off * sizeof(ParkEntry)));
+        CU_TRY(cudaMemcpyAsync(d_->d_park_ol[other], ol.data(), ol.size() * sizeof(int2), cudaMemcpyHostToDevice, d_->stream));
+    }
     launch_copy_dirs(d_->view, cur_set_, other, d_->d_idx, 0, P, d_->stream);  // share first ...
+    if (parked && d_->park[other])
+        launch_copy_parked(d_->view, d_->park[cur_set_], d_->d_park_ol[cur_set_], d_->park[other], d_->d_park_ol[other], d_->d_idx, P, d_->stream);
     launch_release(d_->view, cur_set_, 0, P, d_->stream);                       // ... then drop the old set
+    launch_release_parked(d_->view, d_->pv(cur_set_), 0, P, d_->stream);
     launch_merge_free(d_->view, d_->stream);
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
     CU_TRY(cudaGetLastError());
@@ -781,6 +838,10 @@ int Engine::resample(const int32_t* idx)
         times_.resample_ms += ms;
     }
     times_.resample_launches += 3;
+    if (parked) {
+        d_->drop_arena(cur_set_);
+        times_.resample_launches += 2;
+    }
     cur_set_ = other;
     return LAMA_OK;
 }
@@ -793,6 +854,77 @@ static int ensure_scratch(Engine::Impl* d, size_t bytes)
     if (cudaMalloc(&d->d_scratch, bytes) != cudaSuccess) return -1;
     d->scratch_bytes = bytes;
     return 0;
+}
+
+bool Engine::has_parked(int particle) const
+{
+    if (particle < 0) return d_->parked(cur_set_) != 0;
+    if (particle >= cfg_.particles) return false;
+    for (int k = 0; k < d_->view.n_kinds; ++k)
+        if (d_->park_ol[cur_set_][(size_t)particle * d_->view.n_kinds + k].y) return true;
+    return false;
+}
+
+Engine::WindowInfo Engine::window_info() const
+{
+    return WindowInfo{window_, d_->shifts, (uint64_t)d_->parked(cur_set_), d_->restored};
+}
+
+int Engine::shift_window(int32_t base_px, int32_t base_py)
+{
+    { int rc = settle(nullptr); if (rc != LAMA_OK) return rc; }   // ordered after the pending map update
+    if (base_px == window_.base_px && base_py == window_.base_py) return LAMA_OK;
+    const int32_t dim = window_.dim, max_patch = (int32_t)(0xFFFFFFFFu >> kPatchLog2) + 1 - dim;
+    if (base_px < 0 || base_py < 0 || base_px > max_patch || base_py > max_patch) return fail("shift_window: window base outside the map's cell range", LAMA_ERR_ARG);
+    CU_TRY(cudaSetDevice(cfg_.device));
+    const int set = cur_set_, n_lists = d_->n_lists();
+    const DirWindow nw{base_px, base_py, dim};
+    // scratch: counts | new {offset, length} | enter prefixes (window_shift_core.h: the arena may have gaps after a prune)
+    const size_t b_cnt = (size_t)n_lists * sizeof(int2);
+    const size_t b_enter = shift_scratch_ints(reinterpret_cast<const int32_t*>(d_->park_ol[set].data()), n_lists) * 4;
+    if (ensure_scratch(d_, 2 * b_cnt + b_enter)) return fail("shift_window: out of device memory", LAMA_ERR_CUDA);
+    int2* d_cnt = (int2*)d_->d_scratch;
+    int2* d_new_ol = d_cnt + n_lists;
+    int32_t* d_enter = (int32_t*)(d_new_ol + n_lists);
+    if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
+    launch_shift_count(d_->view, d_->pv(set), set, nw, d_cnt, n_lists, d_->stream);
+    CU_TRY(cudaGetLastError());
+    std::vector<int2> cnt((size_t)n_lists), nol((size_t)n_lists);
+    CU_TRY(cudaMemcpyAsync(cnt.data(), d_cnt, b_cnt, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaStreamSynchronize(d_->stream));
+    int64_t total = 0, entered = 0;
+    for (int i = 0; i < n_lists; ++i) {
+        nol[i] = make_int2((int32_t)total, cnt[i].x);
+        total += cnt[i].x;
+        entered += cnt[i].y;
+    }
+    if (total > INT32_MAX) return fail("shift_window: too many parked entries", LAMA_ERR_POOL);
+    ParkEntry* arena = nullptr;
+    if (total) CU_TRY(cudaMalloc((void**)&arena, (size_t)total * sizeof(ParkEntry)));
+    auto give_up = [&](cudaError_t e) {
+        if (arena) cudaFree(arena);
+        return fail(std::string("shift_window: ") + cudaGetErrorString(e), LAMA_ERR_CUDA);
+    };
+    cudaError_t e = cudaMemcpyAsync(d_new_ol, nol.data(), b_cnt, cudaMemcpyHostToDevice, d_->stream);
+    if (e == cudaSuccess) e = launch_shift_apply(d_->view, d_->pv(set), set, nw, arena, d_new_ol, d_enter, n_lists, d_->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_->d_park_ol[set], d_new_ol, b_cnt, cudaMemcpyDeviceToDevice, d_->stream);
+    if (timing_ && e == cudaSuccess) e = cudaEventRecord(d_->ev[1], d_->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(d_->stream);
+    if (e != cudaSuccess) return give_up(e);
+    if (timing_) {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, d_->ev[0], d_->ev[1]);
+        times_.shift_ms += ms;
+    }
+    if (d_->park[set]) cudaFree(d_->park[set]);
+    d_->park[set] = arena;
+    d_->park_ol[set] = nol;
+    window_ = nw;
+    d_->view.window = nw;
+    d_->shifts += 1;
+    d_->restored += (uint64_t)entered;
+    times_.misc_launches += 2;
+    return LAMA_OK;
 }
 
 int Engine::render_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states, bool full,
@@ -919,7 +1051,7 @@ int Engine::sampling_likelihood(int particle, const SE2& pose, const double* off
     double* d_off = (double*)d_->d_scratch;
     double* d_out = d_off + 2 * (size_t)n;
     CU_TRY(cudaMemcpyAsync(d_off, offsets_xy, (size_t)n * 16, cudaMemcpyHostToDevice, d_->stream));
-    launch_sampling(d_->view, cur_set_, particle, d_->d_points, d_->scan, pose, d_off, n, stride, cfg_.resolution, max_sqdist_, d_out, d_->stream);
+    launch_sampling(d_->view, d_->pv(cur_set_), cur_set_, particle, d_->d_points, d_->scan, pose, d_off, n, stride, cfg_.resolution, max_sqdist_, d_out, d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(out, d_out, (size_t)n * 8, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
@@ -936,7 +1068,7 @@ int Engine::dm_distance(int particle, const double* pts, int n, double* dist, do
     if (ensure_scratch(d_, bp + bd + bg)) return fail("dm_distance: out of device memory", LAMA_ERR_CUDA);
     char* base = (char*)d_->d_scratch;
     CU_TRY(cudaMemcpyAsync(base, pts, bp, cudaMemcpyHostToDevice, d_->stream));
-    launch_distance(d_->view, cur_set_, particle, (const double*)base, n, cfg_.resolution, max_sqdist_, (double*)(base + bp),
+    launch_distance(d_->view, d_->pv(cur_set_), cur_set_, particle, (const double*)base, n, cfg_.resolution, max_sqdist_, (double*)(base + bp),
                     grad ? (double*)(base + bp + bd) : nullptr, d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(dist, base + bp, bd, cudaMemcpyDeviceToHost, d_->stream));
@@ -954,7 +1086,7 @@ int Engine::export_window(int particle, int kind, uint32_t x0, uint32_t y0, int 
     const size_t bw = (size_t)w * h * 4, bpz = (size_t)w * h;
     if (ensure_scratch(d_, bw + bpz)) return fail("export_window: out of device memory", LAMA_ERR_CUDA);
     char* base = (char*)d_->d_scratch;
-    launch_export(d_->view, cur_set_, particle, kind, x0, y0, w, h, (uint32_t*)base, (uint8_t*)(base + bw), d_->stream);
+    launch_export(d_->view, d_->pv(cur_set_), cur_set_, particle, kind, x0, y0, w, h, (uint32_t*)base, (uint8_t*)(base + bw), d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(words, base, bw, cudaMemcpyDeviceToHost, d_->stream));
     if (present) CU_TRY(cudaMemcpyAsync(present, base + bw, bpz, cudaMemcpyDeviceToHost, d_->stream));
@@ -974,7 +1106,7 @@ int Engine::gather_cells(int particle, int kind, const uint32_t* cells_xy, int n
     if (ensure_scratch(d_, bc + bw + bf)) return fail("gather_cells: out of device memory", LAMA_ERR_CUDA);
     char* base = (char*)d_->d_scratch;
     CU_TRY(cudaMemcpyAsync(base, cells_xy, bc, cudaMemcpyHostToDevice, d_->stream));
-    launch_gather_cells(d_->view, cur_set_, particle, kind, (const uint32_t*)base, n, (uint32_t*)(base + bc), (uint8_t*)(base + bc + bw), d_->stream);
+    launch_gather_cells(d_->view, d_->pv(cur_set_), cur_set_, particle, kind, (const uint32_t*)base, n, (uint32_t*)(base + bc), (uint8_t*)(base + bc + bw), d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(words, base + bc, bw, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaMemcpyAsync(flags, base + bc + bw, bf, cudaMemcpyDeviceToHost, d_->stream));
@@ -989,7 +1121,7 @@ int Engine::export_bits(int particle, int plane, uint32_t x0, uint32_t y0, int w
     if (particle < 0 || particle >= cfg_.particles || plane < 0 || plane > 1 || w < 1 || h < 1) return fail("export_bits: bad arguments", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
     if (ensure_scratch(d_, (size_t)w * h)) return fail("export_bits: out of device memory", LAMA_ERR_CUDA);
-    launch_export_bits(d_->view, plane, cur_set_, particle, x0, y0, w, h, (uint8_t*)d_->d_scratch, d_->stream);
+    launch_export_bits(d_->view, d_->pv(cur_set_), plane, cur_set_, particle, x0, y0, w, h, (uint8_t*)d_->d_scratch, d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(out, d_->d_scratch, (size_t)w * h, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
@@ -1021,6 +1153,7 @@ int Engine::pack_size(int particle, size_t* bytes)
 {
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
     if (particle < 0 || particle >= cfg_.particles) return fail("pack_size: bad particle", LAMA_ERR_ARG);
+    if (has_parked(particle)) return fail("pack: the particle's maps have parked entries (the window has moved), which a blob does not carry", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
     const size_t dim2 = (size_t)cfg_.dir_dim * cfg_.dir_dim;
     std::vector<int32_t> dir(2 * dim2);
@@ -1068,6 +1201,7 @@ int Engine::pack_device(int particle, DeviceBlob* out)
 {
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
     if (particle < 0 || particle >= cfg_.particles) return fail("pack: bad particle", LAMA_ERR_ARG);
+    if (has_parked(particle)) return fail("pack: the particle's maps have parked entries (the window has moved), which a blob does not carry", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
     const size_t dim2 = (size_t)cfg_.dir_dim * cfg_.dir_dim;
     std::vector<int32_t> dir(2 * dim2);
@@ -1107,6 +1241,7 @@ int Engine::unpack_device(int particle, const DeviceBlob& blob, bool check)
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
     const size_t n = (size_t)blob.n_occ + blob.n_dm, ne = blob_entry_bytes(n);
     if (particle < 0 || particle >= cfg_.particles || blob.bytes < ne + n * (size_t)(kPatchBytes + 128)) return fail("unpack: bad arguments", LAMA_ERR_ARG);
+    if (has_parked(particle)) return fail("unpack: the slot's maps have parked entries (the window has moved)", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
     launch_release(d_->view, cur_set_, particle, 1, d_->stream);
     launch_merge_free(d_->view, d_->stream);
@@ -1196,14 +1331,57 @@ int Engine::prune_outside(int particle, const double center[2], const double hwi
             }
             if (!meets) list.push_back((int32_t)di);
         }
-    if (removed) *removed = (int)list.size();
-    if (list.empty()) return LAMA_OK;
-    std::memcpy(d_->h_idx, list.data(), list.size() * 4);
-    CU_TRY(cudaMemcpyAsync(d_->d_idx, d_->h_idx, list.size() * 4, cudaMemcpyHostToDevice, d_->stream));
-    launch_delete_patches(d_->view, cur_set_, particle, d_->d_idx, (int)list.size(), d_->stream);
+    // parked patches: the same test; each list keeps its offset and shrinks to the entries that stay
+    const int nk = d_->view.n_kinds;
+    std::vector<int32_t> dropped;                       // their directory entries, one reference each
+    std::vector<std::pair<int32_t, int32_t>> gone;      // patch coordinates removed from kinds 0 / 1 (counted once per patch)
+    for (int k = 0; k < nk; ++k) {
+        const size_t li = (size_t)particle * nk + k;
+        const int2 ol = d_->park_ol[cur_set_][li];
+        if (ol.y == 0) continue;
+        std::vector<ParkEntry> l((size_t)ol.y), keep;
+        CU_TRY(cudaMemcpyAsync(l.data(), d_->park[cur_set_] + ol.x, l.size() * sizeof(ParkEntry), cudaMemcpyDeviceToHost, d_->stream));
+        CU_TRY(cudaStreamSynchronize(d_->stream));
+        for (const ParkEntry& e : l) {
+            const uint32_t c0[2] = {(uint32_t)e.px << kPatchLog2, (uint32_t)e.py << kPatchLog2};
+            bool meets = true;
+            for (int a = 0; a < 2; ++a) {
+                const double ws = ((double)c0[a] - off) / scale, we = ((double)(c0[a] + kPatchLen) - off) / scale;
+                const double bh = (we - ws) * 0.5, bc = ws + bh;
+                meets = meets && (std::abs(center[a] - bc) <= (hwidth[a] + bh));
+            }
+            if (meets) {
+                keep.push_back(e);
+            } else {
+                dropped.push_back(e.entry);
+                if (k < 2) gone.push_back({e.py, e.px});
+            }
+        }
+        if (keep.size() == l.size()) continue;
+        if (!keep.empty())
+            CU_TRY(cudaMemcpyAsync(d_->park[cur_set_] + ol.x, keep.data(), keep.size() * sizeof(ParkEntry), cudaMemcpyHostToDevice, d_->stream));
+        d_->park_ol[cur_set_][li].y = (int32_t)keep.size();
+        CU_TRY(cudaMemcpyAsync(d_->d_park_ol[cur_set_] + li, &d_->park_ol[cur_set_][li], sizeof(int2), cudaMemcpyHostToDevice, d_->stream));
+        CU_TRY(cudaStreamSynchronize(d_->stream));   // `keep` and the host list entry are read by the copies
+    }
+    std::sort(gone.begin(), gone.end());
+    const size_t n_gone = (size_t)(std::unique(gone.begin(), gone.end()) - gone.begin());
+    if (removed) *removed = (int)(list.size() + n_gone);
+    if (list.empty() && dropped.empty()) return LAMA_OK;
+    if (!list.empty()) {
+        std::memcpy(d_->h_idx, list.data(), list.size() * 4);
+        CU_TRY(cudaMemcpyAsync(d_->d_idx, d_->h_idx, list.size() * 4, cudaMemcpyHostToDevice, d_->stream));
+        launch_delete_patches(d_->view, cur_set_, particle, d_->d_idx, (int)list.size(), d_->stream);
+    }
+    if (!dropped.empty()) {
+        if (ensure_scratch(d_, dropped.size() * 4)) return fail("prune_outside: out of device memory", LAMA_ERR_CUDA);
+        CU_TRY(cudaMemcpyAsync(d_->d_scratch, dropped.data(), dropped.size() * 4, cudaMemcpyHostToDevice, d_->stream));
+        launch_release_entries(d_->view, (const int32_t*)d_->d_scratch, (int)dropped.size(), d_->stream);
+    }
     launch_merge_free(d_->view, d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaStreamSynchronize(d_->stream));
+    if (d_->parked(cur_set_) == 0 && d_->park[cur_set_]) d_->drop_arena(cur_set_);
     times_.misc_launches += 2;
     return LAMA_OK;
 }
@@ -1229,6 +1407,14 @@ int Engine::bounds(int particle, int kind, uint32_t mn[2], uint32_t mx[2])
                 mx[0] = std::max(mx[0], x + kPatchLen); mx[1] = std::max(mx[1], y + kPatchLen);
                 ++n;
             }
+    std::vector<ParkEntry> l;
+    if (d_->fetch(cur_set_, (size_t)particle * d_->view.n_kinds + kind, l) != cudaSuccess) return -1;
+    for (const ParkEntry& e : l) {
+        const uint32_t x = (uint32_t)e.px << kPatchLog2, y = (uint32_t)e.py << kPatchLog2;
+        mn[0] = std::min(mn[0], x); mn[1] = std::min(mn[1], y);
+        mx[0] = std::max(mx[0], x + kPatchLen); mx[1] = std::max(mx[1], y + kPatchLen);
+        ++n;
+    }
     return n;
 }
 
@@ -1262,6 +1448,24 @@ int Engine::memory_usage(int kind, uint32_t cell_bytes, uint64_t* out)
                 if (dir[e] < 0) continue;
                 uses = ref[(size_t)(dir[e] & kDirSlotMask)];
             }
+            total += 72.0;
+            total += container / (double)(uses > 0 ? uses : 1);
+        }
+        // parked patches, by the same rule: the two lists are sorted by patch, so walk them side by side
+        std::vector<ParkEntry> lk, lo;
+        if (d_->fetch(cur_set_, (size_t)p * d_->view.n_kinds + kind, lk) != cudaSuccess) return -1;
+        if (kind == 1 && d_->fetch(cur_set_, (size_t)p * d_->view.n_kinds, lo) != cudaSuccess) return -1;
+        size_t i = 0, j = 0;
+        while (i < lk.size() || j < lo.size()) {
+            const ParkEntry* a = i < lk.size() ? &lk[i] : nullptr;
+            const ParkEntry* b = j < lo.size() ? &lo[j] : nullptr;
+            const bool take_a = a && (!b || !park_before(b->px, b->py, a->px, a->py));
+            const bool take_b = b && (!a || !park_before(a->px, a->py, b->px, b->py));
+            const int ud = take_a ? ref[(size_t)(a->entry & kDirSlotMask)] : 0, uo = take_b ? ref[(size_t)(b->entry & kDirSlotMask)] : 0;
+            i += take_a;
+            j += take_b;
+            const int uses = kind == 0 ? ud : (ud > 0 && uo > 0 ? std::min(ud, uo) : std::max(ud, uo));
+            if (uses <= 0 && kind == 1) continue;
             total += 72.0;
             total += container / (double)(uses > 0 ? uses : 1);
         }
@@ -1326,6 +1530,27 @@ int Engine::snapshot(EngineImage* out, CheckpointTimes* t, int particles)
     CU_TRY(mem.alloc((void**)&c.dirs, n_dir * 4));
     CU_TRY(mem.alloc((void**)&c.bad, 16));
     CU_TRY(mem.alloc(&c.temp, c.temp_bytes));
+    // the parked entries of the saved particles, gathered list by list in (particle, kind) order; counted and remapped with the directories
+    std::vector<int32_t> park_len((size_t)particles * v.n_kinds, 0);
+    std::vector<ParkEntry> parked;
+    for (size_t li = 0; li < park_len.size(); ++li) {
+        std::vector<ParkEntry> l;
+        CU_TRY(d_->fetch(cur_set_, li, l));
+        park_len[li] = (int32_t)l.size();
+        parked.insert(parked.end(), l.begin(), l.end());
+    }
+    std::vector<int32_t> park_entries(parked.size());
+    for (size_t i = 0; i < parked.size(); ++i) park_entries[i] = parked[i].entry;
+    c.n_parked = parked.size();
+    c.parked = nullptr;
+    c.parked_out = nullptr;
+    if (c.n_parked) {
+        int32_t* pin = nullptr;
+        CU_TRY(mem.alloc((void**)&pin, c.n_parked * 4));
+        CU_TRY(mem.alloc((void**)&c.parked_out, c.n_parked * 4));
+        CU_TRY(cudaMemcpyAsync(pin, park_entries.data(), c.n_parked * 4, cudaMemcpyHostToDevice, d_->stream));
+        c.parked = pin;
+    }
     cudaEvent_t ev[4] = {};
     struct Events { cudaEvent_t* e; ~Events() { for (int k = 0; k < 4; ++k) if (e[k]) cudaEventDestroy(e[k]); } } ev_guard{ev};
     for (int k = 0; k < 4; ++k) CU_TRY(cudaEventCreate(&ev[k]));
@@ -1351,6 +1576,15 @@ int Engine::snapshot(EngineImage* out, CheckpointTimes* t, int particles)
     img.occupancy_kind = cfg_.occupancy_kind; img.known_plane = cfg_.known_plane; img.resolution = cfg_.resolution; img.l2_max = cfg_.l2_max;
     img.window = window_;
     img.used = K;
+    img.park_len.clear();
+    img.parked.clear();
+    if (c.n_parked) {
+        CU_TRY(cudaMemcpyAsync(park_entries.data(), c.parked_out, c.n_parked * 4, cudaMemcpyDeviceToHost, d_->stream));
+        CU_TRY(cudaStreamSynchronize(d_->stream));
+        for (size_t i = 0; i < parked.size(); ++i) parked[i].entry = park_entries[i];
+        img.park_len = park_len;
+        img.parked = parked;
+    }
     const size_t stride = img.slot_stride(), bytes = (size_t)K * stride;
     char* stage = nullptr;
     CU_TRY(mem.alloc((void**)&stage, bytes));
@@ -1484,6 +1718,19 @@ Engine* Engine::restore(const EngineImage& img, int device, uint64_t stream, std
                 fill = 0;
             }
         }
+    }
+    // the parked lists into set 0's arena, in the image's order
+    if (!img.parked.empty()) {
+        std::vector<int2>& ol = d->park_ol[0];
+        int32_t off = 0;
+        for (size_t li = 0; li < img.park_len.size(); ++li) {
+            ol[li] = make_int2(off, img.park_len[li]);
+            off += img.park_len[li];
+        }
+        if (!cu(cudaMalloc((void**)&d->park[0], img.parked.size() * sizeof(ParkEntry)), "parked entries") ||
+            !cu(cudaMemcpyAsync(d->park[0], img.parked.data(), img.parked.size() * sizeof(ParkEntry), cudaMemcpyHostToDevice, d->stream), "parked entries") ||
+            !cu(cudaMemcpyAsync(d->d_park_ol[0], ol.data(), ol.size() * sizeof(int2), cudaMemcpyHostToDevice, d->stream), "parked lists"))
+            return nullptr;
     }
     if (!cu(cudaStreamSynchronize(d->stream), "synchronize")) return nullptr;
     e->h2d_bytes_ = 0;

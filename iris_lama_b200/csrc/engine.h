@@ -9,6 +9,7 @@
 #include "lama_core.h"
 #include "match_core.h"
 #include "ray_core.h"
+#include "window_shift_core.h"
 
 namespace lama_b200 {
 
@@ -17,7 +18,7 @@ struct EngineConfig {
     int particles     = 1;      // particles resident on THIS device
     double resolution = 0.05;
     double l2_max     = 0.5;
-    int dir_dim       = 64;     // directory window: dir_dim x dir_dim patches of 32 x 32 cells
+    int dir_dim       = 64;     // working window: dir_dim x dir_dim patches of 32 x 32 cells (shift_window moves it; the pool bounds the map)
     int pool_slots    = 0;      // 0 = auto (particles * 768 + 1024)
     int max_beams     = 2048;
     double center_x   = 0.0;    // world position the directory window is centred on
@@ -50,6 +51,10 @@ struct EngineImage {
     uint32_t used = 0;                     // K
     std::vector<int32_t> refcount;         // [K]
     std::vector<int32_t> dirs;             // [particles][n_kinds][dir_dim^2] of the current set
+    // parked entries (window_shift_core.h) of the current set: park_len[particle * n_kinds + kind] entries each, in that order in
+    // `parked`, entries renumbered like `dirs`; both empty when nothing is parked
+    std::vector<int32_t> park_len;
+    std::vector<ParkEntry> parked;
     // K x 4 KiB of cells, then K x 128 B of obstacle-mirror bits, then (known plane) K x 128 B of known bits
     const uint8_t* slot_bytes = nullptr;
     std::vector<uint8_t> slot_store;       // owns slot_bytes after a snapshot
@@ -70,7 +75,7 @@ struct CheckpointTimes {
 };
 
 struct KernelTimes {  // accumulated CUDA-event durations (ms) and launch counts since reset
-    double match_ms = 0, raycast_ms = 0, brushfire_ms = 0, resample_ms = 0;
+    double match_ms = 0, raycast_ms = 0, brushfire_ms = 0, resample_ms = 0, shift_ms = 0;
     uint64_t match_launches = 0, raycast_launches = 0, brushfire_launches = 0, resample_launches = 0, misc_launches = 0;
 };
 
@@ -214,6 +219,17 @@ public:
     void reset_traffic() { h2d_bytes_ = d2h_bytes_ = 0; }
 
     DirWindow window() const { return window_; }
+
+    // Moves the directory window of the current set to base (base_px, base_py) (patch coordinates) for every particle and kind.
+    // Entries the window leaves are parked (window_shift_core.h), parked entries it covers again return to the directory; slots,
+    // flags and reference counts do not change.  Waits for a pending map update, then synchronises once.
+    int shift_window(int32_t base_px, int32_t base_py);
+    struct WindowInfo {
+        DirWindow window;
+        uint64_t shifts, parked, restored;   // shifts so far, parked entries now (current set, every particle and kind), entries restored so far
+    };
+    WindowInfo window_info() const;
+    bool has_parked(int particle = -1) const;   // particle -1: any particle
 
     struct Impl;
 

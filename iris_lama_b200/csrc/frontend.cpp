@@ -3,6 +3,7 @@
 #include "checkpoint.h"
 #include "rng_skip.h"
 #include "sdm_io.h"
+#include "window_guard.h"
 
 #include <cuda_runtime.h>
 
@@ -50,6 +51,20 @@ static EngineConfig engine_config(const DeviceOptions& dev, int particles, doubl
 }
 
 static double xy_norm(const SE2& s) { return std::sqrt(s.tx * s.tx + s.ty * s.ty); }
+
+// Before an update of `count` particles at predicted poses `poses`: moves the engine's window so that every cell the update can touch
+// lies inside it (window_guard.h), or leaves it where it is when no window holds that box
+static int follow_window(Engine* e, const SE2* poses, int count, const double* origin, const double* quat, const double* pts, int n)
+{
+    const EngineConfig& c = e->config();
+    const uint32_t reach = (uint32_t)std::lround(std::sqrt((double)e->max_sqdist()));
+    double mn[2], mx[2];
+    guard_box(poses, count, moving_tf(origin, quat), pts, n, c.resolution, reach, mn, mx);
+    const double robot[2] = {poses[0].tx, poses[0].ty};
+    int32_t base[2];
+    if (window_guard(e->window(), mn, mx, robot, 1.0 / c.resolution, base) != kGuardShift) return LAMA_OK;
+    return e->shift_window(base[0], base[1]);
+}
 
 // =====================================================================================================
 // PFSlam2D
@@ -361,6 +376,12 @@ int PFSlam2D::update_pipelined(const double* pts, int n, const double* origin, c
     const auto t1 = clk::now();
     t_sample_ += ms(t0, t1);
     std::vector<double> all((size_t)P_ * 5);
+    if (moved) {
+        const bool staged = staged_index_ >= 0;
+        int rcw = follow_window(eng_.get(), &pose_[lo_], hi_ - lo_, origin, quat, staged ? staged_host_.data() + (size_t)staged_index_ * staged_beams_ * 3 : pts,
+                                staged ? staged_beams_ : n);
+        if (rcw != LAMA_OK) return engine_fail(rcw);
+    }
     int rc = pipelined_begin(pts, n, origin, quat, moved, did_update, all.data());
     const auto t2 = clk::now();
     t_solve_ += ms(t1, t2);
@@ -655,6 +676,8 @@ int PFSlam2D::shard_begin(const double* pts, int n, const double* origin, const 
     last_idx_.clear();
     int rc = ensure_engine(staged_index_ >= 0 ? staged_beams_ : n);
     if (rc != LAMA_OK) return rc;
+    const double* scan_pts = staged_index_ >= 0 ? staged_host_.data() + (size_t)staged_index_ * staged_beams_ * 3 : pts;
+    const int scan_n = staged_index_ >= 0 ? staged_beams_ : n;
     if (staged_index_ >= 0) rc = eng_->select_staged(staged_index_, origin, quat, opt_.truncated_ray, opt_.truncated_range);
     else rc = eng_->set_scan(pts, n, origin, quat, opt_.truncated_ray, opt_.truncated_range);
     staged_index_ = -1;
@@ -669,6 +692,10 @@ int PFSlam2D::shard_begin(const double* pts, int n, const double* origin, const 
     if (!moved) return LAMA_OK;
     *did_update = true;
     maps_enqueued_ = false;
+    if (opt_.shard_count == 1) {   // sharded ranks keep a fixed window
+        rc = follow_window(eng_.get(), &pose_[lo_], hi_ - lo_, origin, quat, scan_pts, scan_n);
+        if (rc != LAMA_OK) return engine_fail(rc);
+    }
     rc = match_local(local_out);
     if (rc != LAMA_OK) return rc;
     pending_maps_ = true;
@@ -689,8 +716,6 @@ int PFSlam2D::ensure_engine(int n)
     eng_->enable_timing(opt_.dev.timing != 0);
     if (!staged_host_.empty()) {
         int rc = eng_->stage_scans(staged_host_.data(), staged_scans_, staged_beams_);
-        staged_host_.clear();
-        staged_host_.shrink_to_fit();
         if (rc != LAMA_OK) return engine_fail(rc);
     }
     return LAMA_OK;
@@ -701,11 +726,11 @@ int PFSlam2D::stage_scans(const double* pts, int n_scans, int n)
     if (!pts || n_scans < 1 || n < 1) return fail("stage_scans: bad arguments", LAMA_ERR_ARG);
     staged_scans_ = n_scans;
     staged_beams_ = n;
+    staged_host_.assign(pts, pts + (size_t)n_scans * n * 3);   // the window guard reads the points of every update on the host
     if (eng_) {
         int rc = eng_->stage_scans(pts, n_scans, n);
         return rc == LAMA_OK ? rc : engine_fail(rc);
     }
-    staged_host_.assign(pts, pts + (size_t)n_scans * n * 3);
     return LAMA_OK;
 }
 
@@ -1038,6 +1063,14 @@ int GraphSlam2D::generate_coarse_distance_map(DistanceMapDev** out, uint32_t* pr
     if (!e) { err_ = "no map yet (update() has not been called)"; return LAMA_ERR_STATE; }
     double c[2];
     slam_window_center(slam_.get(), c);
+    {   // centred where the inner map's window now is: the creation centre moved by the patches between the window the engine was
+        // created with around it and the window it has now
+        const EngineConfig& ec = e->config();
+        const double scale = 1.0 / ec.resolution, patch = (double)kPatchLen * ec.resolution;
+        const DirWindow w = e->window();
+        c[0] += (double)(w.base_px - ((int32_t)(w2m(c[0], scale) >> kPatchLog2) - w.dim / 2)) * patch;
+        c[1] += (double)(w.base_py - ((int32_t)(w2m(c[1], scale) >> kPatchLog2) - w.dim / 2)) * patch;
+    }
     // visit_all_cells of the inner distance map (:171): its known cells are those of its own patches and, for a frequency map, every
     // touched occupancy cell (see unpack_distance_words); both maps are read over the union of their patches
     uint32_t a0[2], a1[2], b0[2], b1[2];
@@ -1146,6 +1179,7 @@ int Slam2D::update_maps(const double* pts, int n)
 int Slam2D::update_lidar_odometry(const double* pts, int n, const double* origin, const double* quat, bool* did_update)
 {
     int rc = eng_->set_scan(pts, n, origin, quat, 0.0, 0.0);
+    if (rc == LAMA_OK) rc = follow_window(eng_.get(), &pose_, 1, origin, quat, pts, n);
     if (rc != LAMA_OK) { err_ = eng_->last_error(); return rc; }
     *did_update = true;
     if (!has_first_) {
@@ -1193,6 +1227,7 @@ int Slam2D::update(const double* pts, int n, const double* origin, const double*
     const SE2 odometry = se2_from_xyr(odom_xyr[0], odom_xyr[1], odom_xyr[2]);
     if (!has_first_) {  // slam2d.cpp:147-161
         int rc = eng_->set_scan(pts, n, origin, quat, opt_.truncated_ray, opt_.truncated_range);
+        if (rc == LAMA_OK) rc = follow_window(eng_.get(), &pose_, 1, origin, quat, pts, n);
         if (rc != LAMA_OK) { err_ = eng_->last_error(); return rc; }
         odom_ = odometry;
         rc = update_maps(pts, n);
@@ -1207,6 +1242,7 @@ int Slam2D::update(const double* pts, int n, const double* origin, const double*
     pose_ = ppose;
     odom_ = odometry;
     int rc = eng_->set_scan(pts, n, origin, quat, opt_.truncated_ray, opt_.truncated_range);
+    if (rc == LAMA_OK) rc = follow_window(eng_.get(), &pose_, 1, origin, quat, pts, n);
     if (rc != LAMA_OK) { err_ = eng_->last_error(); return rc; }
     HostMatchResult res;
     rc = eng_->match(&pose_, 1, 0, false, make_solver(opt_.strategy, opt_.max_iter), 0.05, 0, &res);
@@ -1707,6 +1743,8 @@ struct ShardSource {
     std::vector<uint8_t> slots;              // otherwise the kept slots only, laid out as a payload of kept.size() slots
     const uint8_t* payload = nullptr;
     uint32_t payload_count = 0;
+    std::vector<int32_t> park_len;           // the parked lists of a whole-session file (never of a set of shards)
+    std::vector<ParkEntry> parked;
 };
 bool same_engine_geometry(const EngineImage& a, const EngineImage& b)
 {
@@ -1746,7 +1784,7 @@ PFSlam2D* PFSlam2D::load_sharded(const std::vector<std::string>& paths, uint32_t
         if (kind != kCkptPFSlam2D && kind != kCkptPFSlam2DShard) { err = wrong_kind(kind, "PFSlam2D"); return nullptr; }
         if (kind == kCkptPFSlam2D && paths.size() > 1) { err = "a whole-filter checkpoint (kind 1) cannot be mixed with other files: load it alone"; return nullptr; }
         const auto t1 = clk::now();
-        CkptReader r(file.data() + kCkptHeaderBytes, file.size() - kCkptHeaderBytes);
+        CkptReader r = ckpt_body(file);
         uint32_t rank = 0, count = 1;
         uint64_t id = 0;
         if (kind == kCkptPFSlam2DShard) {
@@ -1768,6 +1806,8 @@ PFSlam2D* PFSlam2D::load_sharded(const std::vector<std::string>& paths, uint32_t
         EngineImage img;
         bool has_engine = false;
         if (r.ok()) ckpt_get_engine(r, &has_engine, img, (int)(P / count), 0);
+        if (r.ok() && !img.parked.empty() && !whole_only)
+            r.fail("the session's maps have parked entries (its window moved with the robot); sharded sessions keep a fixed window, load it with lama_pf_load_state");
         if (r.ok() && fs.has_first && !has_engine) r.fail("a filter past its first scan without device state");
         if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
         if (!r.ok()) { err = r.error(); return nullptr; }
@@ -1775,7 +1815,7 @@ PFSlam2D* PFSlam2D::load_sharded(const std::vector<std::string>& paths, uint32_t
         if (f == 0) {
             G = count; per_src = P / count;
             options0.assign(opts, opts + (marks[0] - shared));
-            geo = img; geo.dirs.clear(); geo.refcount.clear(); geo.slot_bytes = nullptr;
+            geo = img; geo.dirs.clear(); geo.refcount.clear(); geo.slot_bytes = nullptr; geo.park_len.clear(); geo.parked.clear();
             present = has_engine;
             session = id;
             sv = fs;
@@ -1807,6 +1847,9 @@ PFSlam2D* PFSlam2D::load_sharded(const std::vector<std::string>& paths, uint32_t
             so.remap.assign(img.used, -1);
             for (int32_t e : so.dirs)
                 if (e != -1) so.remap[(size_t)(e & kDirSlotMask)] = 0;
+            for (const ParkEntry& pe : img.parked) so.remap[(size_t)(pe.entry & kDirSlotMask)] = 0;   // whole-session files only
+            so.park_len = img.park_len;
+            so.parked = img.parked;
             for (uint32_t k = 0; k < img.used; ++k)
                 if (so.remap[k] == 0) { so.remap[k] = (int32_t)so.kept.size(); so.kept.push_back(k); }
             const size_t stride = img.slot_stride(), n = so.kept.size();
@@ -1866,6 +1909,12 @@ PFSlam2D* PFSlam2D::load_sharded(const std::vector<std::string>& paths, uint32_t
                 const uint32_t id = base[k] + (uint32_t)so.remap[(size_t)(e & kDirSlotMask)];
                 ++img.refcount[id];
                 img.dirs.push_back((int32_t)id | (e & ~kDirSlotMask));
+            }
+            if (!so.parked.empty()) img.park_len = so.park_len;
+            for (const ParkEntry& pe : so.parked) {
+                const uint32_t id = base[k] + (uint32_t)so.remap[(size_t)(pe.entry & kDirSlotMask)];
+                ++img.refcount[id];
+                img.parked.push_back(ParkEntry{pe.px, pe.py, (int32_t)id | (pe.entry & ~kDirSlotMask)});
             }
             for (size_t j = 0; j < so.kept.size(); ++j)
                 img.slot_src[base[k] + j] = EngineImage::SlotRef{so.payload, so.payload_count, so.payload == so.slots.data() ? (uint32_t)j : so.kept[j]};
@@ -1954,7 +2003,7 @@ Slam2D* Slam2D::load(const std::string& path, const DeviceOptions& dev, std::str
         return nullptr;
     }
     const auto t1 = clk::now();
-    CkptReader r(file.data() + kCkptHeaderBytes, file.size() - kCkptHeaderBytes);
+    CkptReader r = ckpt_body(file);
     SlamSaved sv;
     ckpt_get(r, kind == kCkptLidarOdometry2D, sv);
     EngineImage img;
@@ -2132,6 +2181,7 @@ int GraphSlam2D::save(const std::string& path, CheckpointStats* st)
     ckpt_put_engine(w, ie ? &inner : nullptr);
     CkptWriter g;
     g.buf.clear();
+    g.version = w.version;   // the global map's section is framed like the inner one
     ckpt_put_engine(g, global ? &gimg : nullptr);
     s.encode_ms = ms_since(t1);
     std::string err;
@@ -2162,7 +2212,7 @@ GraphSlam2D* GraphSlam2D::load(const std::string& path, const DeviceOptions& dev
         return nullptr;
     }
     const auto t1 = clk::now();
-    CkptReader r(file.data() + kCkptHeaderBytes, file.size() - kCkptHeaderBytes);
+    CkptReader r = ckpt_body(file);
     GraphOptions g;
     g.key_pose_distance = r.f64("graph options"); g.key_pose_angular_distance = r.f64("graph options"); g.key_pose_head_delay = r.i32("graph options");
     g.loop_search_max_distance = r.f64("graph options"); g.loop_search_min_distance = r.f64("graph options"); g.loop_max_candidates = r.i32("graph options");

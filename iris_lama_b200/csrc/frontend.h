@@ -177,7 +177,7 @@ private:
     int update_sharded(const double* pts, int n, const double* origin, const double* quat, const double odom_xyr[3], bool* did_update);
     int write_checkpoint(const std::string& path, bool shard, CheckpointStats& s);
     int migrate_and_apply(const std::vector<int32_t>& idx);
-    std::vector<double> staged_host_;  // kept until the engine exists
+    std::vector<double> staged_host_;  // the staged scans on the host too: the window guard reads them
     int staged_scans_ = 0, staged_beams_ = 0, staged_index_ = -1;
     int ensure_engine(int n);
 

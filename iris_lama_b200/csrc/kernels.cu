@@ -46,12 +46,16 @@ struct MatchShared {
     uint32_t evals_done;
 };
 
-// metric distance of one cell: DynamicDistanceMap::distance(Vector3ui) (dynamic_distance_map.cpp:140-147)
+// metric distance of one cell: DynamicDistanceMap::distance(Vector3ui) (dynamic_distance_map.cpp:140-147).  A cell outside the window is
+// absent while nothing is parked (`parked` 0); otherwise it may exist in a parked patch, and the read sets kErrWindow in `status`.
 __device__ __forceinline__ double cell_distance(const uint32_t* __restrict__ pool, const int32_t* dir, const DirWindow& win, uint32_t x, uint32_t y,
-                                                const double* dtab, uint32_t max_sqdist)
+                                                const double* dtab, uint32_t max_sqdist, int parked, uint32_t* status)
 {
     int di = dir_index(win, x, y);
-    if (di < 0) return dtab[max_sqdist];
+    if (di < 0) {
+        if (parked) atomicOr(status, kErrWindow);
+        return dtab[max_sqdist];
+    }
     int slot = dir[di];
     if (slot < 0) return dtab[max_sqdist];
     uint32_t w = __ldg(pool + (size_t)(slot & kDirSlotMask) * kPatchCells + cell_index(x, y));
@@ -60,7 +64,7 @@ __device__ __forceinline__ double cell_distance(const uint32_t* __restrict__ poo
 
 __device__ __forceinline__ void eval_beam(double s[kNumSums], const Affine& tf, const double* __restrict__ pt, double scale,
                                           const uint32_t* __restrict__ pool, const int32_t* dir, const DirWindow& win, const double* dtab,
-                                          uint32_t max_sqdist, const SolverOptions& so, double meas_sigma)
+                                          uint32_t max_sqdist, const SolverOptions& so, double meas_sigma, int parked, uint32_t* status)
 {
     double hit[3];
     apply_tf(tf, __ldg(pt), __ldg(pt + 1), __ldg(pt + 2), hit);
@@ -73,6 +77,7 @@ __device__ __forceinline__ void eval_beam(double s[kNumSums], const Affine& tf, 
         // all four stencil cells live in one patch: one directory lookup
         const double dmax = dtab[max_sqdist];
         int di = dir_index(win, dx, dy);
+        if (di < 0 && parked) atomicOr(status, kErrWindow);
         int slot = di < 0 ? -1 : dir[di];
         if (slot < 0) {
             v[0] = v[1] = v[2] = v[3] = dmax;
@@ -85,10 +90,10 @@ __device__ __forceinline__ void eval_beam(double s[kNumSums], const Affine& tf, 
             v[3] = (w3 & kDmValid) ? dtab[dm_sqdist(w3)] : dmax;
         }
     } else {
-        v[0] = cell_distance(pool, dir, win, dx, dy, dtab, max_sqdist);
-        v[1] = cell_distance(pool, dir, win, dx + 1, dy, dtab, max_sqdist);
-        v[2] = cell_distance(pool, dir, win, dx, dy + 1, dtab, max_sqdist);
-        v[3] = cell_distance(pool, dir, win, dx + 1, dy + 1, dtab, max_sqdist);
+        v[0] = cell_distance(pool, dir, win, dx, dy, dtab, max_sqdist, parked, status);
+        v[1] = cell_distance(pool, dir, win, dx + 1, dy, dtab, max_sqdist, parked, status);
+        v[2] = cell_distance(pool, dir, win, dx, dy + 1, dtab, max_sqdist, parked, status);
+        v[3] = cell_distance(pool, dir, win, dx + 1, dy + 1, dtab, max_sqdist, parked, status);
     }
     BeamEval e = bilinear(v, mu0, mu1, scale, hit[0], hit[1]);
     accumulate(s, e, so.robust_kind, so.robust_param, meas_sigma);
@@ -130,7 +135,8 @@ k_match(StoreView s, MatchParams mp, const SE2* __restrict__ states_in, MatchRes
         for (int k = 0; k < kNumSums; ++k) acc[k] = 0.0;
         const Affine tf = sh.tf;
         for (int b = tid; b < n; b += blockDim.x)
-            eval_beam(acc, tf, mp.points + 3 * (size_t)b, mp.scan.scale, s.pool, dir, s.window, dtab, mp.max_sqdist, mp.solver, mp.meas_sigma);
+            eval_beam(acc, tf, mp.points + 3 * (size_t)b, mp.scan.scale, s.pool, dir, s.window, dtab, mp.max_sqdist, mp.solver, mp.meas_sigma,
+                      mp.parked_any, s.status);
         // Block reduction through shared memory, fixed order (deterministic): every thread parks its 12 partial sums, then warp k adds
         // up sum k over all threads (a strided pass + one warp shuffle tree) -- 12 stores per thread instead of 60 shuffles per value.
 #pragma unroll
@@ -1490,6 +1496,122 @@ __global__ void k_delete_patches(StoreView s, int set, int particle, const int32
     }
 }
 
+// ---- parked entries and the window shift (window_shift_core.h) ---------------------------------------------------------------------
+constexpr int kShiftThreads = 256;
+
+// exclusive prefix sums of flag(i), i in [0, n), into out[0 .. n] (out[n] = total) by one CTA of kShiftThreads threads: every thread
+// sums a contiguous chunk, thread 0 scans the chunk sums.  Ends with the block synchronised.
+template <typename F>
+__device__ void block_exclusive_scan(int n, F flag, int32_t* out, int32_t* part)
+{
+    const int t = threadIdx.x, chunk = (n + kShiftThreads - 1) / kShiftThreads;
+    const int lo = min(n, t * chunk), hi = min(n, lo + chunk);
+    int32_t sum = 0;
+    for (int i = lo; i < hi; ++i) sum += flag(i) ? 1 : 0;
+    part[t] = sum;
+    __syncthreads();
+    if (t == 0) {
+        int32_t run = 0;
+        for (int k = 0; k < kShiftThreads; ++k) { const int32_t v = part[k]; part[k] = run; run += v; }
+        out[n] = run;
+    }
+    __syncthreads();
+    int32_t run = part[t];
+    for (int i = lo; i < hi; ++i) { out[i] = run; run += flag(i) ? 1 : 0; }
+    __syncthreads();
+}
+
+__device__ __forceinline__ int block_sum(int v, int* part)
+{
+    v = __reduce_add_sync(0xffffffffu, v);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+    __syncthreads();
+    int total = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) total += part[w];
+    return total;
+}
+
+// one CTA per list (particle * n_kinds + kind) of `set`: counts[list] = {length of its parked list after a shift to nw, entries that
+// return to the directory}
+__global__ void __launch_bounds__(kShiftThreads) k_shift_count(StoreView s, ParkView pv, int set, DirWindow nw, int2* __restrict__ counts)
+{
+    __shared__ int part[2][kShiftThreads / 32];
+    const int list = blockIdx.x, p = list / s.n_kinds, kind = list % s.n_kinds;
+    const int dim2 = s.window.dim * s.window.dim;
+    const int32_t* dir = dir_of(s, set, p, kind);
+    const int2 ol = pv.ol[list];
+    int leave = 0, enter = 0;
+    for (int i = threadIdx.x; i < dim2; i += blockDim.x) leave += shift_leaves(s.window, nw, i, dir[i]) ? 1 : 0;
+    for (int i = threadIdx.x; i < ol.y; i += blockDim.x) enter += shift_enters(nw, pv.park[ol.x + i]) ? 1 : 0;
+    leave = block_sum(leave, part[0]);
+    enter = block_sum(enter, part[1]);
+    if (threadIdx.x == 0) counts[list] = make_int2(ol.y - enter + leave, enter);
+}
+
+// one CTA per list of `set`: the directory re-based to nw in place (the old one staged in shared memory), and the new parked list
+// (entries that stay parked merged with those that leave, in key order) written at out + out_ol[list].x.  enter_scratch holds
+// old length + 1 values per list at offset old offset + list.
+__global__ void __launch_bounds__(kShiftThreads) k_shift_apply(StoreView s, ParkView pv, int set, DirWindow nw, ParkEntry* __restrict__ out, const int2* __restrict__ out_ol,
+                                                           int32_t* __restrict__ enter_scratch)
+{
+    extern __shared__ __align__(16) int32_t shift_smem[];
+    __shared__ int32_t part[kShiftThreads];
+    const int list = blockIdx.x, p = list / s.n_kinds, kind = list % s.n_kinds;
+    const DirWindow w = s.window;
+    const int dim2 = w.dim * w.dim;
+    int32_t* od = shift_smem;                 // the old directory
+    int32_t* leave_before = shift_smem + dim2;   // dim2 + 1
+    int32_t* dir = dir_of(s, set, p, kind);
+    const int2 ol = pv.ol[list];
+    const ParkEntry* A = pv.park ? pv.park + ol.x : nullptr;
+    const int na = ol.y;
+    int32_t* enter_before = enter_scratch + shift_enter_base(ol.x, list);
+    for (int i = threadIdx.x; i < dim2; i += blockDim.x) od[i] = dir[i];
+    __syncthreads();
+    block_exclusive_scan(dim2, [&](int i) { return shift_leaves(w, nw, i, od[i]); }, leave_before, part);
+    block_exclusive_scan(na, [&](int i) { return shift_enters(nw, A[i]); }, enter_before, part);
+    for (int j = threadIdx.x; j < dim2; j += blockDim.x) dir[j] = shift_new_entry(w, nw, j, od, A, na);
+    ParkEntry* C = out + out_ol[list].x;
+    for (int i = threadIdx.x; i < na; i += blockDim.x)
+        if (!shift_enters(nw, A[i])) C[shift_pos_parked(w, A, i, enter_before, leave_before)] = A[i];
+    for (int i = threadIdx.x; i < dim2; i += blockDim.x)
+        if (shift_leaves(w, nw, i, od[i])) {
+            ParkEntry e;
+            e.px = w.base_px + i % w.dim;
+            e.py = w.base_py + i / w.dim;
+            e.entry = od[i];
+            C[shift_pos_leaving(w, i, A, na, enter_before, leave_before)] = e;
+        }
+}
+
+// resampling: the parked lists of kinds 0 and 1 of dst particle k become shared copies of those of src particle from[k] (-1: empty),
+// like k_copy_dirs does for the directories (+1 reference, kDirOwn cleared, kDirHot kept)
+__global__ void k_copy_parked(StoreView s, const ParkEntry* __restrict__ src, const int2* __restrict__ src_ol, ParkEntry* __restrict__ dst,
+                              const int2* __restrict__ dst_ol, const int32_t* __restrict__ from)
+{
+    const int p = blockIdx.x, kind = blockIdx.y, a = from[p];
+    if (a < 0) return;
+    const int2 so = src_ol[a * s.n_kinds + kind], d = dst_ol[p * s.n_kinds + kind];
+    for (int i = threadIdx.x; i < so.y; i += blockDim.x) {
+        ParkEntry e = src[so.x + i];
+        atomicAdd(&s.refcount[e.entry & kDirSlotMask], 1);
+        e.entry &= ~kDirOwn;
+        dst[d.x + i] = e;
+    }
+}
+// drops the references of the parked lists of particles [first, first + gridDim.x) of one set (every kind)
+__global__ void k_release_parked(StoreView s, ParkView pv, int first)
+{
+    const int2 ol = pv.ol[(first + blockIdx.x) * s.n_kinds + blockIdx.y];
+    for (int i = threadIdx.x; i < ol.y; i += blockDim.x) release_slot(s, pv.park[ol.x + i].entry & kDirSlotMask);
+}
+// drops one reference per listed directory entry (parked patches deleted by a prune)
+__global__ void k_release_entries(StoreView s, const int32_t* __restrict__ entries, int n)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) release_slot(s, entries[i] & kDirSlotMask);
+}
+
 // the per-particle payload of the sharded exchange: {state (4), likelihood, reference evaluations, iterations}, then one digest word
 __global__ void k_pack_results(const MatchResult* __restrict__ res, int n, double digest, double* __restrict__ out)
 {
@@ -1537,28 +1659,26 @@ __global__ void k_init_store(StoreView s, int n_sets)
     }
 }
 
-__global__ void k_export(StoreView s, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, uint32_t* __restrict__ out,
+__global__ void k_export(StoreView s, ParkView pv, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, uint32_t* __restrict__ out,
                          uint8_t* __restrict__ present)
 {
     const int32_t* d = dir_of(s, set, particle, kind);
     for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < w * h; k += gridDim.x * blockDim.x) {
         uint32_t x = x0 + (uint32_t)(k % w), y = y0 + (uint32_t)(k / w);
-        int di   = dir_index(s.window, x, y);
-        int slot = di < 0 ? -1 : d[di];
+        int slot = map_entry(s, pv, particle, kind, d, x, y);
         out[k]   = slot < 0 ? 0u : __ldcg(patch_ptr(s, slot & kDirSlotMask) + cell_index(x, y));
         if (present) present[k] = slot >= 0;
     }
 }
 
 // the words of n scattered cells of one map; flags bit 0: the patch exists, bit 1: the cell's bit in the `known` plane (log-odds maps)
-__global__ void k_gather_cells(StoreView s, int set, int particle, int kind, const uint32_t* __restrict__ cells, int n, uint32_t* __restrict__ words,
+__global__ void k_gather_cells(StoreView s, ParkView pv, int set, int particle, int kind, const uint32_t* __restrict__ cells, int n, uint32_t* __restrict__ words,
                                uint8_t* __restrict__ flags)
 {
     const int32_t* d = dir_of(s, set, particle, kind);
     for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
         const uint32_t x = cells[2 * k], y = cells[2 * k + 1];
-        const int di   = dir_index(s.window, x, y);
-        const int slot = di < 0 ? -1 : d[di];
+        const int slot = map_entry(s, pv, particle, kind, d, x, y);
         uint32_t w = 0;
         uint8_t f = 0;
         if (slot >= 0) {
@@ -1572,13 +1692,12 @@ __global__ void k_gather_cells(StoreView s, int set, int particle, int kind, con
     }
 }
 
-__global__ void k_export_bits(StoreView s, int plane, int set, int particle, uint32_t x0, uint32_t y0, int w, int h, uint8_t* __restrict__ out)
+__global__ void k_export_bits(StoreView s, ParkView pv, int plane, int set, int particle, uint32_t x0, uint32_t y0, int w, int h, uint8_t* __restrict__ out)
 {
     const int32_t* d = dir_of(s, set, particle, kMapOcc);
     for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < w * h; k += gridDim.x * blockDim.x) {
         uint32_t x = x0 + (uint32_t)(k % w), y = y0 + (uint32_t)(k / w);
-        int di   = dir_index(s.window, x, y);
-        int slot = di < 0 ? -1 : d[di];
+        int slot = map_entry(s, pv, particle, kMapOcc, d, x, y);
         uint8_t v = 0;
         const uint32_t* base = plane == 0 ? s.fbits : s.kbits;
         if (slot >= 0 && base) {
@@ -1649,6 +1768,20 @@ __global__ void k_ckpt_count(StoreView s, int set, size_t n, int32_t* __restrict
         atomicAdd(&cnt[slot], 1);
     }
 }
+// the same for a plain list of n directory entries (the parked entries of the saved particles, gathered by the host)
+__global__ void k_ckpt_count_list(StoreView s, const int32_t* __restrict__ e, size_t n, int32_t* __restrict__ cnt, uint32_t* __restrict__ bad)
+{
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const int32_t slot = e[i] & kDirSlotMask;
+        if (e[i] < 0 || slot >= s.n_slots) { atomicOr(bad, 1u); continue; }
+        atomicAdd(&cnt[slot], 1);
+    }
+}
+__global__ void k_ckpt_remap_list(const int32_t* __restrict__ e, size_t n, const int32_t* __restrict__ new_id, int32_t* __restrict__ out)
+{
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        out[i] = e[i] < 0 ? -1 : (new_id[e[i] & kDirSlotMask] | (e[i] & ~kDirSlotMask));
+}
 // one thread per slot: used[slot] = 1 when a directory references it.  bad bit 1: the count differs from the slot's reference count
 // (a store that is not self-consistent is never written; neither is one where a particle that is not saved still references a slot)
 __global__ void k_ckpt_mark(StoreView s, const int32_t* __restrict__ cnt, int32_t* __restrict__ used, uint32_t* __restrict__ bad)
@@ -1698,7 +1831,7 @@ __global__ void k_scatter_patches(StoreView s, int set, int particle, int kind, 
 // Loc2D::addSamplingCovariance (src/loc2d.cpp:199-236): for every sampling offset the likelihood
 //   l = sum over every `stride`-th beam of exp(-d^2 / 0.01)^3,  d = nearest-cell distance at the offset pose.
 // One block per offset; the host accumulates K, u, s in the reference's order.
-__global__ void k_sampling(StoreView s, int set, int particle, const double* __restrict__ points, ScanParams scan, SE2 pose, const double* __restrict__ offsets,
+__global__ void k_sampling(StoreView s, ParkView pv, int set, int particle, const double* __restrict__ points, ScanParams scan, SE2 pose, const double* __restrict__ offsets,
                            int stride, double resolution, uint32_t max_sqdist, double* __restrict__ out)
 {
     __shared__ Affine tf;
@@ -1717,8 +1850,7 @@ __global__ void k_sampling(StoreView s, int set, int particle, const double* __r
         double hit[3];
         apply_tf(tf, points[3 * k], points[3 * k + 1], points[3 * k + 2], hit);
         const uint32_t x = w2m(hit[0], scan.scale), y = w2m(hit[1], scan.scale);
-        const int di = dir_index(s.window, x, y);
-        const int slot = di < 0 ? -1 : d[di];
+        const int slot = map_entry(s, pv, particle, kMapDm, d, x, y);
         const uint32_t w = slot < 0 ? 0u : __ldcg(patch_ptr(s, slot & kDirSlotMask) + cell_index(x, y));
         const double dist = (w & kDmValid) ? mul_rn(sqrt((double)dm_sqdist(w)), resolution) : dmax;
         const double e = exp(-mul_rn(dist, dist) / 0.01);
@@ -1736,7 +1868,7 @@ __global__ void k_sampling(StoreView s, int set, int particle, const double* __r
 
 // MatchSurface2D::error() (src/match_surface_2d.cpp:92-116): sqrt(sum d^2 / N) with d the NEAREST-cell distance (w2m rounding +
 // DynamicDistanceMap::distance(Vector3ui), dynamic_distance_map.cpp:140-147) of every point at the given state.  One block per state.
-__global__ void k_match_error(StoreView s, int set, int particle0, int shared_map, const double* __restrict__ points, ScanParams scan, const SE2* __restrict__ states,
+__global__ void k_match_error(StoreView s, ParkView pv, int set, int particle0, int shared_map, const double* __restrict__ points, ScanParams scan, const SE2* __restrict__ states,
                               double resolution, uint32_t max_sqdist, double* __restrict__ out)
 {
     __shared__ Affine tf;
@@ -1750,8 +1882,7 @@ __global__ void k_match_error(StoreView s, int set, int particle0, int shared_ma
         double hit[3];
         apply_tf(tf, points[3 * k], points[3 * k + 1], points[3 * k + 2], hit);
         const uint32_t x = w2m(hit[0], scan.scale), y = w2m(hit[1], scan.scale);
-        const int di = dir_index(s.window, x, y);
-        const int slot = di < 0 ? -1 : d[di];
+        const int slot = map_entry(s, pv, (shared_map ? particle0 : particle0 + (int)blockIdx.x), kMapDm, d, x, y);
         const uint32_t w = slot < 0 ? 0u : __ldcg(patch_ptr(s, slot & kDirSlotMask) + cell_index(x, y));
         const double dist = (w & kDmValid) ? mul_rn(sqrt((double)dm_sqdist(w)), resolution) : dmax;
         acc += mul_rn(dist, dist);
@@ -1766,7 +1897,7 @@ __global__ void k_match_error(StoreView s, int set, int particle0, int shared_ma
     }
 }
 
-__global__ void k_distance(StoreView s, int set, int particle, const double* __restrict__ pts, int n, double resolution, uint32_t max_sqdist,
+__global__ void k_distance(StoreView s, ParkView pv, int set, int particle, const double* __restrict__ pts, int n, double resolution, uint32_t max_sqdist,
                            double* __restrict__ dist, double* __restrict__ grad)
 {
     const int32_t* d = dir_of(s, set, particle, kMapDm);
@@ -1778,8 +1909,7 @@ __global__ void k_distance(StoreView s, int set, int particle, const double* __r
         double v[4];
         for (int k = 0; k < 4; ++k) {
             uint32_t x = dx + (k & 1), y = dy + (k >> 1);
-            int di = dir_index(s.window, x, y);
-            int slot = di < 0 ? -1 : d[di];
+            int slot = map_entry(s, pv, particle, kMapDm, d, x, y);
             uint32_t w = slot < 0 ? 0u : __ldcg(patch_ptr(s, slot & kDirSlotMask) + cell_index(x, y));
             v[k] = (w & kDmValid) ? mul_rn(sqrt((double)dm_sqdist(w)), resolution) : dmax;
         }
@@ -2032,6 +2162,36 @@ void launch_release(const StoreView& s, int set, int first, int count, cudaStrea
     k_release<<<dim3(count, s.n_kinds), 256, 0, st>>>(s, set, first);
 }
 void launch_merge_free(const StoreView& s, cudaStream_t st) { k_merge_free<<<1, 256, 0, st>>>(s); }
+void launch_shift_count(const StoreView& s, const ParkView& pv, int set, const DirWindow& nw, int2* d_counts, int n_lists, cudaStream_t st)
+{
+    k_shift_count<<<n_lists, kShiftThreads, 0, st>>>(s, pv, set, nw, d_counts);
+}
+size_t shift_smem_bytes(int dir_dim) { return (2 * (size_t)dir_dim * dir_dim + 1) * 4; }
+cudaError_t launch_shift_apply(const StoreView& s, const ParkView& pv, int set, const DirWindow& nw, ParkEntry* d_out, const int2* d_out_ol, int32_t* d_scratch, int n_lists,
+                               cudaStream_t st)
+{
+    const size_t smem = shift_smem_bytes(s.window.dim);
+    cudaError_t e = cudaFuncSetAttribute(k_shift_apply, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    k_shift_apply<<<n_lists, kShiftThreads, smem, st>>>(s, pv, set, nw, d_out, d_out_ol, d_scratch);
+    return cudaGetLastError();
+}
+void launch_copy_parked(const StoreView& s, const ParkEntry* d_src, const int2* d_src_ol, ParkEntry* d_dst, const int2* d_dst_ol, const int32_t* d_from,
+                        int count, cudaStream_t st)
+{
+    if (count <= 0) return;
+    k_copy_parked<<<dim3(count, 2), 256, 0, st>>>(s, d_src, d_src_ol, d_dst, d_dst_ol, d_from);
+}
+void launch_release_parked(const StoreView& s, const ParkView& pv, int first, int count, cudaStream_t st)
+{
+    if (count <= 0 || !pv.park) return;
+    k_release_parked<<<dim3(count, s.n_kinds), 256, 0, st>>>(s, pv, first);
+}
+void launch_release_entries(const StoreView& s, const int32_t* d_entries, int n, cudaStream_t st)
+{
+    if (n <= 0) return;
+    k_release_entries<<<(n + 255) / 256, 256, 0, st>>>(s, d_entries, n);
+}
 void launch_pack_results(const MatchResult* d_results, int n, double digest, double* d_out, cudaStream_t st)
 {
     k_pack_results<<<(n + 127) / 128, 128, 0, st>>>(d_results, n, digest, d_out);
@@ -2042,26 +2202,26 @@ void launch_delete_patches(const StoreView& s, int set, int particle, const int3
     k_delete_patches<<<count, 32, 0, st>>>(s, set, particle, d_list);
 }
 void launch_init_store(const StoreView& s, int n_sets, cudaStream_t st) { k_init_store<<<296, 256, 0, st>>>(s, n_sets); }
-void launch_export(const StoreView& s, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, uint32_t* d_out, uint8_t* d_present,
+void launch_export(const StoreView& s, const ParkView& pv, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, uint32_t* d_out, uint8_t* d_present,
                    cudaStream_t st)
 {
     int blocks = (w * h + 255) / 256;
     if (blocks > 1184) blocks = 1184;
     if (blocks < 1) blocks = 1;
-    k_export<<<blocks, 256, 0, st>>>(s, set, particle, kind, x0, y0, w, h, d_out, d_present);
+    k_export<<<blocks, 256, 0, st>>>(s, pv, set, particle, kind, x0, y0, w, h, d_out, d_present);
 }
-void launch_gather_cells(const StoreView& s, int set, int particle, int kind, const uint32_t* d_cells, int n, uint32_t* d_words, uint8_t* d_flags,
+void launch_gather_cells(const StoreView& s, const ParkView& pv, int set, int particle, int kind, const uint32_t* d_cells, int n, uint32_t* d_words, uint8_t* d_flags,
                          cudaStream_t st)
 {
     if (n <= 0) return;
-    k_gather_cells<<<(n + 255) / 256 < 592 ? (n + 255) / 256 : 592, 256, 0, st>>>(s, set, particle, kind, d_cells, n, d_words, d_flags);
+    k_gather_cells<<<(n + 255) / 256 < 592 ? (n + 255) / 256 : 592, 256, 0, st>>>(s, pv, set, particle, kind, d_cells, n, d_words, d_flags);
 }
-void launch_export_bits(const StoreView& s, int plane, int set, int particle, uint32_t x0, uint32_t y0, int w, int h, uint8_t* d_out, cudaStream_t st)
+void launch_export_bits(const StoreView& s, const ParkView& pv, int plane, int set, int particle, uint32_t x0, uint32_t y0, int w, int h, uint8_t* d_out, cudaStream_t st)
 {
     int blocks = (w * h + 255) / 256;
     if (blocks > 1184) blocks = 1184;
     if (blocks < 1) blocks = 1;
-    k_export_bits<<<blocks, 256, 0, st>>>(s, plane, set, particle, x0, y0, w, h, d_out);
+    k_export_bits<<<blocks, 256, 0, st>>>(s, pv, plane, set, particle, x0, y0, w, h, d_out);
 }
 void launch_import(const StoreView& s, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, const uint32_t* d_in, cudaStream_t st)
 {
@@ -2086,12 +2246,15 @@ void launch_ckpt_compact(const StoreView& s, int set, int particles, const CkptS
     const size_t n_dir = (size_t)particles * s.n_kinds * s.window.dim * s.window.dim;
     const int dir_blocks = (int)std::min<size_t>((n_dir + 255) / 256, 4736), slot_blocks = std::min((s.n_slots + 255) / 256, 4736);
     k_ckpt_count<<<dir_blocks, 256, 0, st>>>(s, set, n_dir, c.cnt, c.bad);
+    const int park_blocks = (int)std::min<size_t>((c.n_parked + 255) / 256, 4736);
+    if (c.n_parked) k_ckpt_count_list<<<park_blocks, 256, 0, st>>>(s, c.parked, c.n_parked, c.cnt, c.bad);
     if (after_count) cudaEventRecord(after_count, st);
     k_ckpt_mark<<<slot_blocks, 256, 0, st>>>(s, c.cnt, c.used, c.bad);
     size_t temp = c.temp_bytes;
     cub::DeviceScan::ExclusiveSum(c.temp, temp, c.used, c.new_id, s.n_slots, st);
     k_ckpt_list<<<slot_blocks, 256, 0, st>>>(s, c.used, c.new_id, c.list, c.ref);
     k_ckpt_remap<<<dir_blocks, 256, 0, st>>>(s, set, n_dir, c.new_id, c.dirs);
+    if (c.n_parked) k_ckpt_remap_list<<<park_blocks, 256, 0, st>>>(c.parked, c.n_parked, c.new_id, c.parked_out);
 }
 void launch_scatter_patches(const StoreView& s, int set, int particle, int kind, const int32_t* d_entries, int n, const uint32_t* d_in,
                             const uint32_t* d_in_fbits, cudaStream_t st)
@@ -2099,25 +2262,25 @@ void launch_scatter_patches(const StoreView& s, int set, int particle, int kind,
     if (n <= 0) return;
     k_scatter_patches<<<(n + 3) / 4, 128, 0, st>>>(s, set, particle, kind, d_entries, n, d_in, d_in_fbits);
 }
-void launch_sampling(const StoreView& s, int set, int particle, const double* d_points, const ScanParams& scan, const SE2& pose, const double* d_offsets,
+void launch_sampling(const StoreView& s, const ParkView& pv, int set, int particle, const double* d_points, const ScanParams& scan, const SE2& pose, const double* d_offsets,
                      int n_offsets, int stride, double resolution, uint32_t max_sqdist, double* d_out, cudaStream_t st)
 {
     if (n_offsets <= 0) return;
-    k_sampling<<<n_offsets, 128, 0, st>>>(s, set, particle, d_points, scan, pose, d_offsets, stride, resolution, max_sqdist, d_out);
+    k_sampling<<<n_offsets, 128, 0, st>>>(s, pv, set, particle, d_points, scan, pose, d_offsets, stride, resolution, max_sqdist, d_out);
 }
-void launch_match_error(const StoreView& s, int set, int particle0, bool shared_map, const double* d_points, const ScanParams& scan, const SE2* d_states, int count,
+void launch_match_error(const StoreView& s, const ParkView& pv, int set, int particle0, bool shared_map, const double* d_points, const ScanParams& scan, const SE2* d_states, int count,
                         double resolution, uint32_t max_sqdist, double* d_out, cudaStream_t st)
 {
     if (count <= 0) return;
-    k_match_error<<<count, 256, 0, st>>>(s, set, particle0, shared_map ? 1 : 0, d_points, scan, d_states, resolution, max_sqdist, d_out);
+    k_match_error<<<count, 256, 0, st>>>(s, pv, set, particle0, shared_map ? 1 : 0, d_points, scan, d_states, resolution, max_sqdist, d_out);
 }
-void launch_distance(const StoreView& s, int set, int particle, const double* d_pts, int n, double resolution, uint32_t max_sqdist, double* d_dist,
+void launch_distance(const StoreView& s, const ParkView& pv, int set, int particle, const double* d_pts, int n, double resolution, uint32_t max_sqdist, double* d_dist,
                      double* d_grad, cudaStream_t st)
 {
     if (n <= 0) return;
     int blocks = (n + 255) / 256;
     if (blocks > 1184) blocks = 1184;
-    k_distance<<<blocks, 256, 0, st>>>(s, set, particle, d_pts, n, resolution, max_sqdist, d_dist, d_grad);
+    k_distance<<<blocks, 256, 0, st>>>(s, pv, set, particle, d_pts, n, resolution, max_sqdist, d_dist, d_grad);
 }
 void launch_render_scans(const StoreView& s, int set, const RenderParams& p, int n_scans, cudaStream_t st)
 {

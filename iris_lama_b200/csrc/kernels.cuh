@@ -30,6 +30,7 @@ struct MatchParams {
     int particle_offset;   // particle handled by block 0
     int shared_map;        // 1: every block reads particle `particle_offset`'s map (pose batches on one map)
     int mode;              // 0 = solve + final evaluation, 1 = single evaluation at the input state
+    int parked_any;        // 1: the maps have parked entries, so a cell outside the window may exist: a read there sets kErrWindow
 };
 
 // per-particle output of k_ray_setup, input of k_ray_pull (the pull form of the ray cast, ray_pull.h)
@@ -109,17 +110,31 @@ void launch_copy_dirs(const StoreView& s, int src_set, int dst_set, const int32_
 // releases every patch referenced by particles [first, first+count) of `set` and clears their directories
 void launch_release(const StoreView& s, int set, int first, int count, cudaStream_t st);
 void launch_merge_free(const StoreView& s, cudaStream_t st);
+// Window shift of every list (particle * n_kinds + kind) of `set` to window nw (window_shift_core.h).  k_shift_count: d_counts[list] =
+// {new parked length, entries that return}.  k_shift_apply: directories re-based in place, new lists written to d_out at d_out_ol[list].x;
+// d_scratch holds (old arena length + n_lists) ints.  The view still carries the old window.
+void launch_shift_count(const StoreView& s, const ParkView& pv, int set, const DirWindow& nw, int2* d_counts, int n_lists, cudaStream_t st);
+size_t shift_smem_bytes(int dir_dim);
+cudaError_t launch_shift_apply(const StoreView& s, const ParkView& pv, int set, const DirWindow& nw, ParkEntry* d_out, const int2* d_out_ol, int32_t* d_scratch, int n_lists,
+                               cudaStream_t st);
+// resampling: parked lists (kinds 0 and 1) of dst particle k = shared copies of those of src particle d_from[k] (-1: empty)
+void launch_copy_parked(const StoreView& s, const ParkEntry* d_src, const int2* d_src_ol, ParkEntry* d_dst, const int2* d_dst_ol, const int32_t* d_from,
+                        int count, cudaStream_t st);
+// drops the references held by the parked lists of particles [first, first + count) of `set`
+void launch_release_parked(const StoreView& s, const ParkView& pv, int first, int count, cudaStream_t st);
+// drops one reference per listed directory entry
+void launch_release_entries(const StoreView& s, const int32_t* d_entries, int n, cudaStream_t st);
 // sharded exchange: kShardFields doubles per particle out of the match results (state, likelihood, evaluation / iteration counts) + one digest
 constexpr int kShardFields = 7;
 void launch_pack_results(const MatchResult* d_results, int n, double digest, double* d_out, cudaStream_t st);
-void launch_gather_cells(const StoreView& s, int set, int particle, int kind, const uint32_t* d_cells, int n, uint32_t* d_words, uint8_t* d_flags,
+void launch_gather_cells(const StoreView& s, const ParkView& pv, int set, int particle, int kind, const uint32_t* d_cells, int n, uint32_t* d_words, uint8_t* d_flags,
                          cudaStream_t st);
 void launch_delete_patches(const StoreView& s, int set, int particle, const int32_t* d_list, int count, cudaStream_t st);
 void launch_init_store(const StoreView& s, int n_sets, cudaStream_t st);
 // dense window of one bit plane (0 = obstacle mirror, 1 = known bits of log-odds maps) of an occupancy map, one byte per cell
-void launch_export_bits(const StoreView& s, int plane, int set, int particle, uint32_t x0, uint32_t y0, int w, int h, uint8_t* d_out, cudaStream_t st);
+void launch_export_bits(const StoreView& s, const ParkView& pv, int plane, int set, int particle, uint32_t x0, uint32_t y0, int w, int h, uint8_t* d_out, cudaStream_t st);
 // dense window export: out[j * w + i] = cell word or 0; present[..] = 1 when the patch exists
-void launch_export(const StoreView& s, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, uint32_t* d_out,
+void launch_export(const StoreView& s, const ParkView& pv, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, uint32_t* d_out,
                    uint8_t* d_present, cudaStream_t st);
 // dense, patch-aligned window import (x0,y0 multiples of 32; w,h multiples of 32); all-zero patches are skipped
 void launch_import(const StoreView& s, int set, int particle, int kind, uint32_t x0, uint32_t y0, int w, int h, const uint32_t* d_in,
@@ -134,22 +149,25 @@ struct CkptScratch {
     uint32_t* bad;      // bit 0: a directory entry points outside the pool, bit 1: a reference count differs from the directory references
     void* temp;         // CUB scan temporary storage
     size_t temp_bytes;
+    const int32_t* parked;   // the parked directory entries of the saved particles (n_parked), counted and remapped into parked_out
+    int32_t* parked_out;
+    size_t n_parked;
 };
 size_t ckpt_scan_temp_bytes(int n_slots);
-// k_ckpt_count (cnt must be zero) -> [after_count recorded] -> k_ckpt_mark -> exclusive scan of `used` -> k_ckpt_list -> k_ckpt_remap
-// over the directories of the first `particles` particles; the used slots in ascending order get the ids 0 .. K-1,
+// k_ckpt_count + k_ckpt_count_list (cnt must be zero) -> [after_count recorded] -> k_ckpt_mark -> exclusive scan of `used` -> k_ckpt_list -> k_ckpt_remap
+// (and k_ckpt_remap_list) over the directories and parked entries of the first `particles` particles; the used slots in ascending order get the ids 0 .. K-1,
 // K = new_id[n_slots - 1] + used[n_slots - 1]
 void launch_ckpt_compact(const StoreView& s, int set, int particles, const CkptScratch& c, cudaStream_t st, cudaEvent_t after_count);
 void launch_scatter_patches(const StoreView& s, int set, int particle, int kind, const int32_t* d_entries, int n, const uint32_t* d_in,
                             const uint32_t* d_in_fbits, cudaStream_t st);
 // Loc2D::addSamplingCovariance likelihoods: out[i] for offset i (offsets = n x 2 doubles)
-void launch_sampling(const StoreView& s, int set, int particle, const double* d_points, const ScanParams& scan, const SE2& pose, const double* d_offsets,
+void launch_sampling(const StoreView& s, const ParkView& pv, int set, int particle, const double* d_points, const ScanParams& scan, const SE2& pose, const double* d_offsets,
                      int n_offsets, int stride, double resolution, uint32_t max_sqdist, double* d_out, cudaStream_t st);
 // MatchSurface2D::error() of `count` states (block k on the map of particle0 + k, or all on particle0's with shared_map)
-void launch_match_error(const StoreView& s, int set, int particle0, bool shared_map, const double* d_points, const ScanParams& scan, const SE2* d_states, int count,
+void launch_match_error(const StoreView& s, const ParkView& pv, int set, int particle0, bool shared_map, const double* d_points, const ScanParams& scan, const SE2* d_states, int count,
                         double resolution, uint32_t max_sqdist, double* d_out, cudaStream_t st);
 // batched DistanceMap::distance(point, &grad) on one particle's distance map (SDM grid interface)
-void launch_distance(const StoreView& s, int set, int particle, const double* d_pts, int n, double resolution, uint32_t max_sqdist, double* d_dist,
+void launch_distance(const StoreView& s, const ParkView& pv, int set, int particle, const double* d_pts, int n, double resolution, uint32_t max_sqdist, double* d_dist,
                      double* d_grad, cudaStream_t st);
 
 // GraphSlam2D::generateOccupancyMap's cast of posed scans into particle 0's frequency map (the map needs the `known` plane)
