@@ -8,7 +8,8 @@
 // starts with the 8-byte marker "LAMAPARK", and every engine section carries, between its directories and its slots, the parked lists:
 // particles x kinds u32 lengths, then the entries {i32 patch x, i32 patch y, i32 directory entry} list after list.
 // The byte-exact layout is in DESIGN.md §13; tests/test_checkpoint.py, tests/test_graph_checkpoint.py and tests/test_shard_checkpoint.py
-// write it independently.
+// write it independently.  checkpoint.cpp states every section once, as a template over CkptWriter / CkptReader that save and load
+// share, and holds the save / load entry points of PFSlam2D, Slam2D and GraphSlam2D.
 #pragma once
 
 #include <cstdint>
@@ -36,29 +37,48 @@ struct CheckpointStats {
     uint64_t used_slots = 0, references = 0, file_bytes = 0;
 };
 
+// The field vocabulary a section is written in once, as a template over CkptWriter and CkptReader: every method takes its field by
+// reference, writes it (writer) or reads it into place (reader).  check(bad, message) is a reader's refusal and does nothing in a writer;
+// kLoad tells the few places where the two directions differ apart.
 class CkptWriter {
 public:
+    static constexpr bool kLoad = false;
     std::vector<uint8_t> buf = std::vector<uint8_t>(kCkptHeaderBytes, 0);
     uint32_t version = kCkptVersion;   // ckpt_put_engine raises it to kCkptVersionParked for an image with parked entries
+    bool ok() const { return true; }
+    size_t pos() const { return buf.size(); }
+    void check(bool, const char*, const char* = nullptr) {}
     void bytes(const void* p, size_t n) { const uint8_t* b = (const uint8_t*)p; buf.insert(buf.end(), b, b + n); }
     template <typename T> void put(T v) { bytes(&v, sizeof(T)); }   // the hosts this builds for are little endian
-    void u8(bool v) { put<uint8_t>(v ? 1 : 0); }
-    void u32(uint32_t v) { put(v); }
-    void i32(int32_t v) { put(v); }
-    void u64(uint64_t v) { put(v); }
-    void f64(double v) { put(v); }
-    void se2(const SE2& s) { f64(s.c); f64(s.s); f64(s.tx); f64(s.ty); }
-    void str(const std::string& s) { u32((uint32_t)s.size()); bytes(s.data(), s.size()); }
+    void u8(bool v, const char* = nullptr) { put<uint8_t>(v ? 1 : 0); }
+    void u32(uint32_t v, const char* = nullptr) { put(v); }
+    void i32(int32_t v, const char* = nullptr) { put(v); }
+    void u64(uint64_t v, const char* = nullptr) { put(v); }
+    void f64(double v, const char* = nullptr) { put(v); }
+    void se2(const SE2& s, const char* = nullptr) { f64(s.c); f64(s.s); f64(s.tx); f64(s.ty); }
+    void str(const std::string& s, const char* = nullptr) { u32((uint32_t)s.size()); bytes(s.data(), s.size()); }
+    // n elements of v in one copy
+    template <typename T> void array(const std::vector<T>& v, size_t n, const char*) { bytes(v.data(), n * sizeof(T)); }
+    // u32 v.size() / group, then all of v in one copy
+    template <typename T> void vec(const std::vector<T>& v, const char*, size_t group = 1) { u32((uint32_t)(v.size() / group)); array(v, v.size(), nullptr); }
+    // u32 v.size(): the length of a list whose elements follow field by field
+    template <typename T> void length(const std::vector<T>& v, size_t, const char*) { u32((uint32_t)v.size()); }
 };
 
-// Bounds-checked reads: a read past the end sets the error and returns zeros, so a parser can check once per section.
+// Bounds-checked reads: a read past the end sets the error and reads zeros, so a parser can check once per section.
 class CkptReader {
 public:
+    static constexpr bool kLoad = true;
     CkptReader(const uint8_t* p, size_t n, uint32_t version = kCkptVersion) : version(version), p_(p), n_(n) {}
     uint32_t version;
     bool ok() const { return err_.empty(); }
     const std::string& error() const { return err_; }
     void fail(const std::string& m) { if (err_.empty()) err_ = m; }
+    // the first refusal wins; `what` is appended in parentheses
+    void check(bool bad, const char* m, const char* what = nullptr)
+    {
+        if (ok() && bad) fail(what ? std::string(m) + " (" + what + ")" : std::string(m));
+    }
     size_t left() const { return n_ - off_; }
     size_t pos() const { return off_; }
     const uint8_t* take(size_t n, const char* what)
@@ -68,13 +88,27 @@ public:
         off_ += n;
         return q;
     }
-    template <typename T> T get(const char* what) { T v{}; if (const uint8_t* q = take(sizeof(T), what)) std::memcpy(&v, q, sizeof(T)); return v; }
-    bool u8(const char* what) { const uint8_t v = get<uint8_t>(what); if (v > 1) fail(std::string("bad flag byte (") + what + ")"); return v == 1; }
-    uint32_t u32(const char* what) { return get<uint32_t>(what); }
-    int32_t i32(const char* what) { return get<int32_t>(what); }
-    uint64_t u64(const char* what) { return get<uint64_t>(what); }
-    double f64(const char* what) { return get<double>(what); }
-    SE2 se2(const char* what) { SE2 s; s.c = f64(what); s.s = f64(what); s.tx = f64(what); s.ty = f64(what); return s; }
+    template <typename T> void get(T& v, const char* what) { v = T{}; if (const uint8_t* q = take(sizeof(T), what)) std::memcpy(&v, q, sizeof(T)); }
+    void u8(bool& v, const char* what)
+    {
+        uint8_t b;
+        get(b, what);
+        if (b > 1) fail(std::string("bad flag byte (") + what + ")");
+        v = b == 1;
+    }
+    void u32(uint32_t& v, const char* what) { get(v, what); }
+    void i32(int32_t& v, const char* what) { get(v, what); }
+    void u64(uint64_t& v, const char* what) { get(v, what); }
+    void f64(double& v, const char* what) { get(v, what); }
+    void se2(SE2& s, const char* what) { f64(s.c, what); f64(s.s, what); f64(s.tx, what); f64(s.ty, what); }
+    void str(std::string& s, const char* what)
+    {
+        uint32_t n;
+        u32(n, what);
+        const size_t m = count(n, 1, what);
+        const uint8_t* q = take(m, what);
+        s = q ? std::string((const char*)q, m) : std::string();
+    }
     // an element count whose elements (elem bytes each) must still fit in the file: checked before anything is allocated
     size_t count(uint64_t n, size_t elem, const char* what)
     {
@@ -87,11 +121,17 @@ public:
         v.assign(n, T{});
         if (const uint8_t* q = take(n * sizeof(T), what)) std::memcpy(v.data(), q, n * sizeof(T));
     }
-    std::string str(const char* what)
+    template <typename T> void vec(std::vector<T>& v, const char* what, size_t group = 1)
     {
-        const size_t n = count(u32(what), 1, what);
-        const uint8_t* q = take(n, what);
-        return q ? std::string((const char*)q, n) : std::string();
+        uint32_t n;
+        u32(n, what);
+        array(v, group * count(n, group * sizeof(T), what), what);
+    }
+    template <typename T> void length(std::vector<T>& v, size_t elem, const char* what)
+    {
+        uint32_t n;
+        u32(n, what);
+        v.assign(count(n, elem, what), T{});
     }
 
 private:

@@ -1,6 +1,5 @@
 // frontend.cpp -- host orchestration of PFSlam2D / Slam2D / Loc2D over the device Engine.
 #include "frontend.h"
-#include "checkpoint.h"
 #include "rng_skip.h"
 #include "sdm_io.h"
 #include "window_guard.h"
@@ -14,7 +13,6 @@
 #include <cmath>
 #include <cstring>
 #include <limits>
-#include <sstream>
 #include <unordered_set>
 
 namespace lama_b200 {
@@ -69,29 +67,40 @@ static int follow_window(Engine* e, const SE2* poses, int count, const double* o
 // =====================================================================================================
 // PFSlam2D
 // =====================================================================================================
-PFSlam2D* PFSlam2D::create(const PFOptions& o, std::string& err)
+bool PFSlam2D::valid_options(const PFOptions& o, std::string& err)
 {
-    if (o.particles < 1) { err = "PFSlam2D: Options::particles must be set (>= 1)"; return nullptr; }
-    if (o.patch_size != 32) { err = "PFSlam2D: only patch_size 32 is supported on the device"; return nullptr; }
-    { uint32_t r; if (!Engine::reach_fits(o.resolution, o.l2_max, &r, err)) { err = "PFSlam2D: " + err; return nullptr; } }
+    if (o.particles < 1) { err = "PFSlam2D: Options::particles must be set (>= 1)"; return false; }
+    if (o.patch_size != 32) { err = "PFSlam2D: only patch_size 32 is supported on the device"; return false; }
+    { uint32_t r; if (!Engine::reach_fits(o.resolution, o.l2_max, &r, err)) { err = "PFSlam2D: " + err; return false; } }
     if (o.shard_count < 1 || o.shard_rank >= o.shard_count || o.particles % o.shard_count != 0) {
         err = "PFSlam2D: particles must divide evenly over shard_count";
-        return nullptr;
+        return false;
     }
     if (o.shard_count > 1 && o.seed == 0) {
         // seed 0 means "take one from random_device" (pf_slam2d.cpp:131-132): every rank would draw its own, the ranks' odometry
         // noise and resampling indices would differ and the map migration would pair up the wrong particles
-        err = "PFSlam2D: sharded operation needs an explicit (non-zero) seed shared by all ranks";
-        return nullptr;
+        err = "PFSlam2D: sharded operation needs an explicit (non-zero) seed shared by all ranks (with seed 0 each rank draws its own)";
+        return false;
     }
+    return true;
+}
+
+void PFSlam2D::place()
+{
+    P_ = opt_.particles;
+    const int per = (int)(opt_.particles / opt_.shard_count);
+    lo_ = (int)opt_.shard_rank * per;
+    hi_ = lo_ + per;
+    if (opt_.seed == 0) opt_.seed = std::random_device{}();  // pf_slam2d.cpp:131-132
+}
+
+PFSlam2D* PFSlam2D::create(const PFOptions& o, std::string& err)
+{
+    if (!valid_options(o, err)) return nullptr;
     if (cuda_device_count() < 1) { err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
     PFSlam2D* p = new PFSlam2D();
     p->opt_ = o;
-    p->P_   = o.particles;
-    const int per = (int)(o.particles / o.shard_count);
-    p->lo_ = (int)o.shard_rank * per;
-    p->hi_ = p->lo_ + per;
-    if (p->opt_.seed == 0) p->opt_.seed = std::random_device{}();  // pf_slam2d.cpp:131-132
+    p->place();
     p->gen_.seed(p->opt_.seed);                                    // random::setSeed, pf_slam2d.cpp:134
     p->pose_.assign(p->P_, SE2{1, 0, 0, 0});
     p->weight_.assign(p->P_, 0.0);
@@ -1015,15 +1024,14 @@ int GraphSlam2D::optimize_pose_graph()
     return LAMA_OK;
 }
 
-// the inner Slam2D's window centre (its engine is created at the first update, centred on the pose of that moment)
-static void slam_window_center(Slam2D* s, double c[2])
+void Slam2D::window_center(double c[2])
 {
-    if (s->engine()) {
-        c[0] = s->engine()->config().center_x;
-        c[1] = s->engine()->config().center_y;
+    if (eng_) {
+        c[0] = eng_->config().center_x;
+        c[1] = eng_->config().center_y;
     } else {
-        c[0] = s->pose().tx;
-        c[1] = s->pose().ty;
+        c[0] = pose_.tx;
+        c[1] = pose_.ty;
     }
 }
 
@@ -1031,7 +1039,7 @@ int GraphSlam2D::generate_occupancy_map(bool full, OccupancyMapDev** out)
 {
     if (mapping_keyid_ == 0 || !occ_) {   // :132-133
         double c[2];
-        slam_window_center(slam_.get(), c);
+        slam_->window_center(c);
         OccupancyMapDev* m = OccupancyMapDev::create(full ? opt_.slam.resolution : 0.1, 32, c[0], c[1], slam_->device_options(), err_);
         if (!m) return LAMA_ERR_CUDA;
         occ_.reset(m);   // borrowed handles never see a null map
@@ -1062,7 +1070,7 @@ int GraphSlam2D::generate_coarse_distance_map(DistanceMapDev** out, uint32_t* pr
     Engine* e = slam_->engine();
     if (!e) { err_ = "no map yet (update() has not been called)"; return LAMA_ERR_STATE; }
     double c[2];
-    slam_window_center(slam_.get(), c);
+    slam_->window_center(c);
     {   // centred where the inner map's window now is: the creation centre moved by the patches between the window the engine was
         // created with around it and the window it has now
         const EngineConfig& ec = e->config();
@@ -1126,10 +1134,16 @@ int GraphSlam2D::generate_coarse_distance_map(DistanceMapDev** out, uint32_t* pr
 // =====================================================================================================
 // Slam2D
 // =====================================================================================================
+bool Slam2D::valid_options(const SlamOptions& o, std::string& err)
+{
+    if (o.patch_size != 32) { err = "Slam2D: only patch_size 32 is supported on the device"; return false; }
+    { uint32_t r; if (!Engine::reach_fits(o.resolution, o.l2_max, &r, err)) { err = "Slam2D: " + err; return false; } }
+    return true;
+}
+
 Slam2D* Slam2D::create(const SlamOptions& o, std::string& err)
 {
-    if (o.patch_size != 32) { err = "Slam2D: only patch_size 32 is supported on the device"; return nullptr; }
-    { uint32_t r; if (!Engine::reach_fits(o.resolution, o.l2_max, &r, err)) { err = "Slam2D: " + err; return nullptr; } }
+    if (!valid_options(o, err)) return nullptr;
     if (cuda_device_count() < 1) { err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
     Slam2D* s = new Slam2D();
     s->opt_ = o;
@@ -1521,807 +1535,6 @@ void unpack_distance_words(const uint32_t* words, const uint8_t* occ_known, size
         if (oy) oy[i] = (int16_t)dm_oy(w);
         if (queued) queued[i] = (w & kDmQueued) ? 1 : 0;
     }
-}
-
-// =====================================================================================================
-// Checkpoints (format: checkpoint.h, DESIGN.md §13)
-// =====================================================================================================
-namespace {
-using clk = std::chrono::steady_clock;
-double ms_since(clk::time_point a) { return std::chrono::duration<double, std::milli>(clk::now() - a).count(); }
-
-void put_counters(CkptWriter& w, const Counters& c)
-{
-    w.u64(c.evals); w.u64(c.ray_cells); w.u64(c.dm_pops); w.u64(c.detached); w.u64(c.gn_iters); w.u64(c.resampled);
-}
-Counters get_counters(CkptReader& r)
-{
-    Counters c;
-    c.evals = r.u64("counters"); c.ray_cells = r.u64("counters"); c.dm_pops = r.u64("counters");
-    c.detached = r.u64("counters"); c.gn_iters = r.u64("counters"); c.resampled = r.u64("counters");
-    return c;
-}
-void put_geometry(CkptWriter& w, const DeviceOptions& d) { w.i32(d.dir_dim); w.i32(d.pool_slots); w.i32(d.max_beams); }
-void get_geometry(CkptReader& r, DeviceOptions& d) { d.dir_dim = r.i32("dir_dim"); d.pool_slots = r.i32("pool_slots"); d.max_beams = r.i32("max_beams"); }
-// the caller's dir_dim / pool_slots / max_beams: 0, or the file's (its options, or the engine it holds)
-bool geometry_matches(const DeviceOptions& call, const DeviceOptions& file, const EngineImage* img, std::string& err)
-{
-    auto ok = [](int v, int opt, int eng) { return v == 0 || v == opt || v == eng; };
-    if (ok(call.dir_dim, file.dir_dim, img ? img->dir_dim : file.dir_dim) && ok(call.pool_slots, file.pool_slots, img ? img->pool_slots : file.pool_slots) &&
-        ok(call.max_beams, file.max_beams, img ? img->max_beams : file.max_beams))
-        return true;
-    err = "device options differ from the checkpoint's geometry (dir_dim, pool_slots and max_beams must be 0 or the saved values)";
-    return false;
-}
-bool finite_se2(const SE2& s) { return std::isfinite(s.c) && std::isfinite(s.s) && std::isfinite(s.tx) && std::isfinite(s.ty); }
-uint64_t sum_refs(const EngineImage& img)
-{
-    uint64_t n = 0;
-    for (int32_t v : img.refcount) n += (uint64_t)v;
-    return n;
-}
-// the refusal of a loader called on another handle kind's file
-std::string wrong_kind(uint32_t kind, const char* want)
-{
-    const char* held = kind == kCkptPFSlam2D ? "PFSlam2D"
-                       : kind == kCkptPFSlam2DShard ? "PFSlam2D shard"
-                       : kind == kCkptSlam2D || kind == kCkptLidarOdometry2D ? "Slam2D"
-                       : kind == kCkptGraphSlam2D ? "GraphSlam2D" : nullptr;
-    return held ? std::string("the checkpoint holds a ") + held + ", not a " + want : std::string("unknown checkpoint handle kind");
-}
-void add_times(CheckpointTimes& a, const CheckpointTimes& b)
-{
-    a.count_ms += b.count_ms; a.compact_ms += b.compact_ms; a.gather_ms += b.gather_ms;
-    a.copy_ms += b.copy_ms; a.create_ms += b.create_ms; a.tables_ms += b.tables_ms;
-}
-}  // namespace
-
-int PFSlam2D::save(const std::string& path, CheckpointStats* st)
-{
-    CheckpointStats local;
-    CheckpointStats& s = st ? *st : local;
-    s = CheckpointStats();
-    if (opt_.shard_count > 1) return fail("saveState: a sharded handle cannot be saved (each rank holds only its part of the filter)", LAMA_ERR_STATE);
-    return write_checkpoint(path, false, s);
-}
-
-int PFSlam2D::save_shard(const std::string& path, CheckpointStats* st)
-{
-    CheckpointStats local;
-    CheckpointStats& s = st ? *st : local;
-    s = CheckpointStats();
-    if (opt_.shard_count < 2) return fail("saveShardState: the handle is not sharded; save it with lama_pf_save_state", LAMA_ERR_STATE);
-    if (pending_maps_)
-        return fail("saveShardState: the handle is inside a split-phase step (between shard_begin and shard_map_update); save after shard_map_update",
-                    LAMA_ERR_STATE);
-    return write_checkpoint(path, true, s);
-}
-
-int PFSlam2D::write_checkpoint(const std::string& path, bool shard, CheckpointStats& s)
-{
-    const auto t0 = clk::now();
-    EngineImage img;
-    if (eng_) {
-        int rc = settle_counters();   // the pending map update and its counters, as the getters would book them
-        if (rc != LAMA_OK) return rc;
-        rc = eng_->snapshot(&img, &s.dev, hi_ - lo_);   // the local particles; a sharded engine's staging particles are not saved
-        if (rc != LAMA_OK) return engine_fail(rc);
-    }
-    const auto t1 = clk::now();
-    CkptWriter w;
-    size_t id_at = 0;
-    if (shard) {
-        w.u32(opt_.shard_rank); w.u32(opt_.shard_count);
-        id_at = w.buf.size();
-        w.u64(0);
-    }
-    const size_t shared = w.buf.size();
-    size_t marks[3];
-    ckpt_put(w, marks);
-    if (shard) {   // the session id: FNV-1a-64 of the options and state sections without the rank-local fields
-        uint64_t id = fnv1a64(w.buf.data() + shared, marks[1] - shared);
-        id = fnv1a64(w.buf.data() + marks[2], w.buf.size() - marks[2], id);
-        std::memcpy(w.buf.data() + id_at, &id, 8);
-    }
-    ckpt_put_engine(w, eng_ ? &img : nullptr);
-    s.encode_ms = ms_since(t1);
-    std::string err;
-    const int rc = ckpt_write_file(path, shard ? kCkptPFSlam2DShard : kCkptPFSlam2D, w, {{img.slot_bytes, (size_t)img.used * img.slot_stride()}}, err, &s);
-    if (rc != LAMA_OK) return fail(err, rc);
-    s.used_slots = img.used;
-    s.references = sum_refs(img);
-    s.total_ms   = ms_since(t0);
-    return LAMA_OK;
-}
-
-void PFSlam2D::ckpt_put(CkptWriter& w, size_t marks[3]) const
-{
-    // options
-    w.u32(opt_.particles);
-    for (double v : {opt_.srr, opt_.str, opt_.stt, opt_.srt, opt_.meas_sigma, opt_.meas_sigma_gain, opt_.trans_thresh, opt_.rot_thresh, opt_.l2_max,
-                     opt_.truncated_ray, opt_.truncated_range, opt_.resolution})
-        w.f64(v);
-    w.u32(opt_.patch_size); w.u32(opt_.max_iter); w.i32(opt_.strategy); w.i32(opt_.threads); w.u32(opt_.seed);
-    put_geometry(w, opt_.dev);
-    marks[0] = w.buf.size();
-    // front-end state
-    w.se2(prior_); w.se2(odom_); w.u8(has_first_);
-    w.f64(acc_trans_); w.f64(acc_rot_); w.f64(neff_);
-    for (uint32_t i = 0; i < P_; ++i) w.se2(pose_[i]);
-    for (const std::vector<double>* v : {&weight_, &nweight_, &wsum_}) w.bytes(v->data(), (size_t)P_ * 8);
-    w.u32((uint32_t)last_idx_.size());
-    w.bytes(last_idx_.data(), last_idx_.size() * 4);
-    w.u64(resample_count_); w.u64(resample_hash_); w.u64(scans_seen_);
-    w.u32((uint32_t)timestamps_.size());
-    w.bytes(timestamps_.data(), timestamps_.size() * 8);
-    marks[1] = w.buf.size();
-    put_counters(w, last_); put_counters(w, total_);
-    w.u64(detached_seen_);
-    w.f64(t_sample_); w.f64(t_solve_); w.f64(t_norm_); w.f64(t_resample_);
-    marks[2] = w.buf.size();
-    // the trajectory nodes reachable from the particles, renumbered in their old order (a parent precedes its children)
-    std::vector<int> renum(nodes_.size(), -1);
-    for (uint32_t i = 0; i < P_; ++i)
-        for (int n = node_of_[i]; n >= 0 && renum[(size_t)n] < 0; n = nodes_[(size_t)n].parent) renum[(size_t)n] = 0;
-    uint32_t kept = 0;
-    for (int& v : renum)
-        if (v == 0) v = (int)kept++;
-    w.u32(kept);
-    for (size_t n = 0; n < nodes_.size(); ++n)
-        if (renum[n] >= 0) {
-            w.se2(nodes_[n].pose);
-            w.i32(nodes_[n].parent < 0 ? -1 : renum[(size_t)nodes_[n].parent]);
-        }
-    for (uint32_t i = 0; i < P_; ++i) w.i32(node_of_[i] < 0 ? -1 : renum[(size_t)node_of_[i]]);
-    std::ostringstream rng;
-    rng << gen_;
-    w.str(rng.str());
-}
-
-void PFSlam2D::ckpt_get(CkptReader& r, Saved& s, size_t marks[3])
-{
-    PFOptions& o = s.opt;
-    o.particles = r.u32("options");
-    double* f[] = {&o.srr, &o.str, &o.stt, &o.srt, &o.meas_sigma, &o.meas_sigma_gain, &o.trans_thresh, &o.rot_thresh, &o.l2_max, &o.truncated_ray,
-                   &o.truncated_range, &o.resolution};
-    for (double* v : f) *v = r.f64("options");
-    o.patch_size = r.u32("options"); o.max_iter = r.u32("options"); o.strategy = r.i32("options"); o.threads = r.i32("options"); o.seed = r.u32("options");
-    get_geometry(r, o.dev);
-    if (r.ok() && (o.particles < 1 || o.patch_size != 32 || !(o.resolution > 0) || o.dev.dir_dim < 8 || o.dev.max_beams < 1 || o.dev.pool_slots < 0))
-        r.fail("bad options");
-    marks[0] = r.pos();
-    const uint32_t P = r.ok() ? o.particles : 0;
-    // front-end state
-    s.prior = r.se2("state"); s.odom = r.se2("state");
-    s.has_first = r.u8("state");
-    s.acc_trans = r.f64("state"); s.acc_rot = r.f64("state"); s.neff = r.f64("state");
-    s.pose.assign(r.count(P, 4 * 8, "poses"), SE2{});
-    for (SE2& p : s.pose) p = r.se2("poses");
-    r.array(s.weight, P, "weights");
-    r.array(s.nweight, P, "weights");
-    r.array(s.wsum, P, "weights");
-    r.array(s.last_idx, r.u32("resample indices"), "resample indices");
-    s.rs_count = r.u64("resample digest"); s.rs_hash = r.u64("resample digest"); s.scans_seen = r.u64("resample digest");
-    r.array(s.stamps, r.u32("timestamps"), "timestamps");
-    marks[1] = r.pos();
-    s.last = get_counters(r); s.total = get_counters(r);
-    s.detached_seen = r.u64("counters");
-    for (double& v : s.summary) v = r.f64("summary");
-    marks[2] = r.pos();
-    s.nodes.assign(r.count(r.u32("nodes"), 4 * 8 + 4, "nodes"), Node{});
-    for (size_t n = 0; n < s.nodes.size(); ++n) {
-        s.nodes[n].pose   = r.se2("nodes");
-        s.nodes[n].parent = r.i32("nodes");
-        if (r.ok() && (s.nodes[n].parent < -1 || s.nodes[n].parent >= (int)n)) r.fail("a trajectory node does not follow its parent");
-    }
-    r.array(s.node_of, P, "trajectory heads");
-    s.rng = r.str("random generator");
-    if (r.ok()) {
-        for (int32_t v : s.last_idx)
-            if (v < 0 || v >= (int32_t)P) r.fail("resample index out of range");
-        if (!s.last_idx.empty() && s.last_idx.size() != P) r.fail("resample indices of the wrong length");
-        for (int32_t v : s.node_of)
-            if (v < -1 || v >= (int32_t)s.nodes.size() || (s.has_first && v < 0)) r.fail("trajectory head out of range");
-        if (!ckpt_check_rng(s.rng)) r.fail("malformed random generator state");
-        if (!finite_se2(s.prior) || !finite_se2(s.odom)) r.fail("non-finite pose");
-    }
-}
-
-PFSlam2D* PFSlam2D::load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st)
-{
-    return load_sharded({path}, 0, 1, dev, err, code, st, true);
-}
-
-namespace {
-// what one file contributes to the new rank: its kept slots (ascending old ids) and the directories of the particles it gives
-struct ShardSource {
-    bool seen = false;
-    std::vector<uint32_t> kept;              // old slot ids
-    std::vector<int32_t> remap;              // old slot -> position in `kept` (-1: not kept)
-    std::vector<int32_t> dirs;               // the directories of the particles this file gives, in global particle order
-    std::vector<uint8_t> file;               // the whole file, kept when every slot is needed
-    std::vector<uint8_t> slots;              // otherwise the kept slots only, laid out as a payload of kept.size() slots
-    const uint8_t* payload = nullptr;
-    uint32_t payload_count = 0;
-    std::vector<int32_t> park_len;           // the parked lists of a whole-session file (never of a set of shards)
-    std::vector<ParkEntry> parked;
-};
-bool same_engine_geometry(const EngineImage& a, const EngineImage& b)
-{
-    return a.dir_dim == b.dir_dim && a.pool_slots == b.pool_slots && a.max_beams == b.max_beams && a.occupancy_kind == b.occupancy_kind &&
-           a.known_plane == b.known_plane && a.resolution == b.resolution && a.l2_max == b.l2_max;
-}
-}  // namespace
-
-PFSlam2D* PFSlam2D::load_sharded(const std::vector<std::string>& paths, uint32_t shard_rank, uint32_t shard_count, const DeviceOptions& dev,
-                                 std::string& err, int* code, CheckpointStats* st, bool whole_only)
-{
-    const auto t0 = clk::now();
-    CheckpointStats local;
-    CheckpointStats& s = st ? *st : local;
-    s = CheckpointStats();
-    *code = LAMA_ERR_ARG;
-    if (paths.empty()) { err = "no checkpoint files"; return nullptr; }
-    if (shard_count < 1 || shard_rank >= shard_count) { err = "shard_rank must be below shard_count (>= 1)"; return nullptr; }
-    Saved sv;                                   // the shared sections (the first file's) and, at the saved world size, this rank's local fields
-    std::vector<uint8_t> options0;              // the first file's options section, byte for byte
-    EngineImage geo;                            // the first file's engine geometry and window
-    bool present = false;
-    uint32_t G = 0, per_src = 0, per = 0, lo = 0;
-    uint64_t session = 0, file_bytes = 0;
-    std::vector<ShardSource> src;
-    for (size_t f = 0; f < paths.size(); ++f) {
-        std::vector<uint8_t> file;
-        uint32_t kind = 0;
-        *code = ckpt_read_file(paths[f], file, &kind, err, &s);
-        if (*code != LAMA_OK) return nullptr;
-        *code = LAMA_ERR_ARG;
-        file_bytes += file.size();
-        if (kind == kCkptPFSlam2DShard && whole_only) {
-            err = "the checkpoint holds one shard of a sharded PFSlam2D: load the complete set of shard files with lama_pf_load_state_sharded";
-            return nullptr;
-        }
-        if (kind != kCkptPFSlam2D && kind != kCkptPFSlam2DShard) { err = wrong_kind(kind, "PFSlam2D"); return nullptr; }
-        if (kind == kCkptPFSlam2D && paths.size() > 1) { err = "a whole-filter checkpoint (kind 1) cannot be mixed with other files: load it alone"; return nullptr; }
-        const auto t1 = clk::now();
-        CkptReader r = ckpt_body(file);
-        uint32_t rank = 0, count = 1;
-        uint64_t id = 0;
-        if (kind == kCkptPFSlam2DShard) {
-            rank = r.u32("shard record"); count = r.u32("shard record"); id = r.u64("shard record");
-            if (r.ok() && (count < 2 || rank >= count)) r.fail("bad shard record (shard_rank must be below shard_count >= 2)");
-        }
-        const size_t shared = r.pos();
-        Saved fs;
-        size_t marks[3];
-        ckpt_get(r, fs, marks);
-        const uint32_t P = r.ok() ? fs.opt.particles : 0;
-        if (r.ok() && P % count != 0) r.fail("the particles do not divide evenly over the file's shard count");
-        if (r.ok() && kind == kCkptPFSlam2DShard) {
-            const uint8_t* b = file.data() + kCkptHeaderBytes;
-            uint64_t h = fnv1a64(b + shared, marks[1] - shared);
-            h = fnv1a64(b + marks[2], marks[2] <= r.pos() ? r.pos() - marks[2] : 0, h);
-            if (h != id) r.fail("session id differs from the file's shared sections");
-        }
-        EngineImage img;
-        bool has_engine = false;
-        if (r.ok()) ckpt_get_engine(r, &has_engine, img, (int)(P / count), 0);
-        if (r.ok() && !img.parked.empty() && !whole_only)
-            r.fail("the session's maps have parked entries (its window moved with the robot); sharded sessions keep a fixed window, load it with lama_pf_load_state");
-        if (r.ok() && fs.has_first && !has_engine) r.fail("a filter past its first scan without device state");
-        if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
-        if (!r.ok()) { err = r.error(); return nullptr; }
-        const uint8_t* opts = file.data() + kCkptHeaderBytes + shared;
-        if (f == 0) {
-            G = count; per_src = P / count;
-            options0.assign(opts, opts + (marks[0] - shared));
-            geo = img; geo.dirs.clear(); geo.refcount.clear(); geo.slot_bytes = nullptr; geo.park_len.clear(); geo.parked.clear();
-            present = has_engine;
-            session = id;
-            sv = fs;
-            if (P % shard_count != 0) { err = "the particles do not divide evenly over shard_count"; return nullptr; }
-            if (shard_count > 1 && fs.opt.seed == 0) { err = "a session with seed 0 cannot be loaded on several ranks (sharded operation needs an explicit seed)"; return nullptr; }
-            per = P / shard_count;
-            lo = shard_rank * per;
-            src.resize(G);
-        } else {
-            if (count != G) { err = "the shard files disagree about the shard count"; return nullptr; }
-            if (marks[0] - shared != options0.size() || std::memcmp(opts, options0.data(), options0.size()) != 0) { err = "the shard files hold different options"; return nullptr; }
-            if (has_engine != present || (present && !same_engine_geometry(img, geo))) { err = "the shard files hold different engine geometry"; return nullptr; }
-            if (present && (img.window.base_px != geo.window.base_px || img.window.base_py != geo.window.base_py)) { err = "the shard files hold different directory windows"; return nullptr; }
-            if (id != session) { err = "the shard files come from different saves (session ids differ)"; return nullptr; }
-        }
-        ShardSource& so = src[rank];
-        if (so.seen) { err = "shard rank " + std::to_string(rank) + " appears twice"; return nullptr; }
-        so.seen = true;
-        if (count == shard_count && rank == shard_rank) {   // the saved world size: this rank's own values come back
-            sv.last = fs.last; sv.total = fs.total; sv.detached_seen = fs.detached_seen;
-            std::copy(fs.summary, fs.summary + 4, sv.summary);
-            for (int k = 0; k < 3; ++k) geo.counters[k] = img.counters[k];
-        }
-        // the particles of the new rank this file holds: global [a, b)
-        const uint32_t a = std::max(lo, rank * per_src), b = std::min(lo + per, (rank + 1) * per_src);
-        if (has_engine && a < b) {
-            const size_t dir_n = (size_t)img.n_kinds() * img.dir_dim * img.dir_dim;
-            so.dirs.assign(img.dirs.begin() + (size_t)(a - rank * per_src) * dir_n, img.dirs.begin() + (size_t)(b - rank * per_src) * dir_n);
-            so.remap.assign(img.used, -1);
-            for (int32_t e : so.dirs)
-                if (e != -1) so.remap[(size_t)(e & kDirSlotMask)] = 0;
-            for (const ParkEntry& pe : img.parked) so.remap[(size_t)(pe.entry & kDirSlotMask)] = 0;   // whole-session files only
-            so.park_len = img.park_len;
-            so.parked = img.parked;
-            for (uint32_t k = 0; k < img.used; ++k)
-                if (so.remap[k] == 0) { so.remap[k] = (int32_t)so.kept.size(); so.kept.push_back(k); }
-            const size_t stride = img.slot_stride(), n = so.kept.size();
-            if (n == img.used) {   // every slot: keep the file instead of copying its slots
-                so.payload_count = img.used;
-                const size_t at = (size_t)(img.slot_bytes - file.data());
-                so.file.swap(file);
-                so.payload = so.file.data() + at;
-            } else {               // only the kept slots, as a payload of n slots: cells, then mirror bits, then known bits
-                so.slots.resize(n * stride);
-                const size_t planes[3] = {0, (size_t)img.used * kPatchBytes, (size_t)img.used * (kPatchBytes + 128)};
-                const size_t pieces[3] = {(size_t)kPatchBytes, 128, 128}, out[3] = {0, n * kPatchBytes, n * (kPatchBytes + 128)};
-                for (int p = 0; p < (img.has_kbits() ? 3 : 2); ++p)
-                    for (size_t j = 0; j < n; ++j)
-                        std::memcpy(so.slots.data() + out[p] + j * pieces[p], img.slot_bytes + planes[p] + (size_t)so.kept[j] * pieces[p], pieces[p]);
-                so.payload = so.slots.data();
-                so.payload_count = (uint32_t)n;
-            }
-        }
-        s.encode_ms += ms_since(t1);
-    }
-    for (uint32_t k = 0; k < G; ++k)
-        if (!src[k].seen) { err = "shard rank " + std::to_string(k) + " is missing from the set"; return nullptr; }
-    // the device options: dir_dim and max_beams 0 or the saved values; pool_slots too at the saved world size, any value at another
-    const bool same_world = G == shard_count;
-    DeviceOptions check = dev;
-    if (!same_world) check.pool_slots = 0;
-    if (!geometry_matches(check, sv.opt.dev, present ? &geo : nullptr, err)) return nullptr;
-    // assembly: kept slots numbered in ascending (source rank, old slot) order, directories remapped, reference counts recounted
-    const int capacity = shard_count > 1 ? 2 * (int)per : (int)per;
-    EngineImage img = geo;
-    if (present) {
-        img.particles = (int)per;
-        if (!same_world) {
-            img.pool_slots = dev.pool_slots > 0 ? dev.pool_slots : Engine::auto_pool_slots(capacity);
-            for (uint64_t& c : img.counters) c = 0;
-        }
-        std::vector<uint32_t> base(G, 0);
-        uint32_t K = 0;
-        for (uint32_t k = 0; k < G; ++k) {
-            base[k] = K;
-            K += (uint32_t)src[k].kept.size();
-        }
-        if (img.pool_slots >= (int)kDirSlotMask || K > (uint32_t)img.pool_slots) {
-            err = "the " + std::to_string(K) + " slots this rank keeps do not fit a pool of " + std::to_string(img.pool_slots) + " slots (raise pool_slots)";
-            return nullptr;
-        }
-        img.used = K;
-        img.refcount.assign(K, 0);
-        img.dirs.clear();
-        img.dirs.reserve((size_t)per * img.n_kinds() * img.dir_dim * img.dir_dim);
-        img.slot_src.resize(K);
-        for (uint32_t k = 0; k < G; ++k) {
-            const ShardSource& so = src[k];
-            for (int32_t e : so.dirs) {
-                if (e == -1) { img.dirs.push_back(-1); continue; }
-                const uint32_t id = base[k] + (uint32_t)so.remap[(size_t)(e & kDirSlotMask)];
-                ++img.refcount[id];
-                img.dirs.push_back((int32_t)id | (e & ~kDirSlotMask));
-            }
-            if (!so.parked.empty()) img.park_len = so.park_len;
-            for (const ParkEntry& pe : so.parked) {
-                const uint32_t id = base[k] + (uint32_t)so.remap[(size_t)(pe.entry & kDirSlotMask)];
-                ++img.refcount[id];
-                img.parked.push_back(ParkEntry{pe.px, pe.py, (int32_t)id | (pe.entry & ~kDirSlotMask)});
-            }
-            for (size_t j = 0; j < so.kept.size(); ++j)
-                img.slot_src[base[k] + j] = EngineImage::SlotRef{so.payload, so.payload_count, so.payload == so.slots.data() ? (uint32_t)j : so.kept[j]};
-            if (K > 0 && so.kept.size() == K && so.payload_count == K) {   // one file gives every slot, in its own order: one contiguous copy
-                img.slot_bytes = so.payload;
-                img.slot_src.clear();
-            }
-        }
-    } else if (!same_world) {
-        if (dev.pool_slots > 0) sv.opt.dev.pool_slots = dev.pool_slots;
-    }
-    if (!same_world) {
-        sv.last = Counters(); sv.total = Counters(); sv.detached_seen = 0;
-        std::fill(sv.summary, sv.summary + 4, 0.0);
-    }
-    // the set is valid: from here on the device
-    if (cuda_device_count() < 1) { *code = LAMA_ERR_NO_DEVICE; err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
-    PFOptions o = sv.opt;
-    o.shard_rank = shard_rank; o.shard_count = shard_count;
-    o.dev.device = dev.device; o.dev.stream = dev.stream; o.dev.timing = dev.timing;
-    std::unique_ptr<PFSlam2D> p(create(o, err));
-    if (!p) return nullptr;
-    p->prior_ = sv.prior; p->odom_ = sv.odom; p->has_first_ = sv.has_first;
-    p->acc_trans_ = sv.acc_trans; p->acc_rot_ = sv.acc_rot; p->neff_ = sv.neff;
-    p->pose_ = sv.pose; p->weight_ = sv.weight; p->nweight_ = sv.nweight; p->wsum_ = sv.wsum;
-    p->last_idx_ = sv.last_idx;
-    p->resample_count_ = sv.rs_count; p->resample_hash_ = sv.rs_hash; p->scans_seen_ = sv.scans_seen;
-    p->timestamps_ = sv.stamps;
-    p->last_ = sv.last; p->total_ = sv.total; p->detached_seen_ = sv.detached_seen;
-    p->t_sample_ = sv.summary[0]; p->t_solve_ = sv.summary[1]; p->t_norm_ = sv.summary[2]; p->t_resample_ = sv.summary[3];
-    p->nodes_ = sv.nodes; p->node_of_.assign(sv.node_of.begin(), sv.node_of.end());
-    std::istringstream in(sv.rng);
-    in >> p->gen_;
-    if (present) {
-        Engine* e = Engine::restore(img, dev.device, dev.stream, err, &s.dev, capacity);
-        if (!e) { *code = LAMA_ERR_CUDA; return nullptr; }
-        p->eng_.reset(e);
-        e->enable_timing(dev.timing != 0);
-    }
-    s.used_slots = img.used;
-    s.references = sum_refs(img);
-    s.file_bytes = file_bytes;
-    s.total_ms   = ms_since(t0);
-    *code = LAMA_OK;
-    return p.release();
-}
-
-int Slam2D::save(const std::string& path, CheckpointStats* st)
-{
-    const auto t0 = clk::now();
-    CheckpointStats local;
-    CheckpointStats& s = st ? *st : local;
-    s = CheckpointStats();
-    EngineImage img;
-    if (eng_) {
-        const int rc = eng_->snapshot(&img, &s.dev);
-        if (rc != LAMA_OK) { err_ = eng_->last_error(); return rc; }
-    }
-    const auto t1 = clk::now();
-    CkptWriter w;
-    ckpt_put(w);
-    ckpt_put_engine(w, eng_ ? &img : nullptr);
-    s.encode_ms = ms_since(t1);
-    std::string err;
-    const int rc = ckpt_write_file(path, opt_.lidar_odometry ? kCkptLidarOdometry2D : kCkptSlam2D, w, {{img.slot_bytes, (size_t)img.used * img.slot_stride()}}, err, &s);
-    if (rc != LAMA_OK) { err_ = err; return rc; }
-    s.used_slots = img.used;
-    s.references = sum_refs(img);
-    s.total_ms   = ms_since(t0);
-    return LAMA_OK;
-}
-
-Slam2D* Slam2D::load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st)
-{
-    const auto t0 = clk::now();
-    CheckpointStats local;
-    CheckpointStats& s = st ? *st : local;
-    s = CheckpointStats();
-    std::vector<uint8_t> file;
-    uint32_t kind = 0;
-    *code = ckpt_read_file(path, file, &kind, err, &s);
-    if (*code != LAMA_OK) return nullptr;
-    *code = LAMA_ERR_ARG;
-    if (kind != kCkptSlam2D && kind != kCkptLidarOdometry2D) {
-        err = wrong_kind(kind, "Slam2D");
-        return nullptr;
-    }
-    const auto t1 = clk::now();
-    CkptReader r = ckpt_body(file);
-    SlamSaved sv;
-    ckpt_get(r, kind == kCkptLidarOdometry2D, sv);
-    EngineImage img;
-    bool present = false;
-    if (r.ok()) ckpt_get_engine(r, &present, img, 1, sv.opt.occupancy == 1 ? 1 : 0);
-    if (r.ok() && sv.has_first && !present) r.fail("a Slam2D past its first scan without device state");
-    if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
-    if (!r.ok()) { err = r.error(); return nullptr; }
-    if (!geometry_matches(dev, sv.opt.dev, present ? &img : nullptr, err)) return nullptr;
-    s.encode_ms += ms_since(t1);
-    if (cuda_device_count() < 1) { *code = LAMA_ERR_NO_DEVICE; err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
-    std::unique_ptr<Slam2D> p(ckpt_restore(sv, present ? &img : nullptr, dev, err, code, &s.dev));
-    if (!p) return nullptr;
-    s.used_slots = img.used;
-    s.references = sum_refs(img);
-    s.total_ms   = ms_since(t0);
-    *code = LAMA_OK;
-    return p.release();
-}
-
-void Slam2D::ckpt_put(CkptWriter& w) const
-{
-    for (double v : {opt_.trans_thresh, opt_.rot_thresh, opt_.l2_max, opt_.truncated_ray, opt_.truncated_range, opt_.resolution}) w.f64(v);
-    w.u32(opt_.patch_size); w.u32(opt_.max_iter); w.i32(opt_.strategy); w.i32(opt_.occupancy);
-    w.u8(opt_.transient_map); w.u8(opt_.lidar_odometry);
-    put_geometry(w, opt_.dev);
-    w.se2(pose_); w.se2(odom_); w.se2(map_update_pose_);
-    w.u8(has_first_); w.u8(engine_ready_);
-    w.u32(processed_); w.u64(removed_); w.u64(map_updates_);
-    put_counters(w, last_); put_counters(w, total_);
-}
-
-void Slam2D::ckpt_get(CkptReader& r, bool lidar_odometry, SlamSaved& s)
-{
-    SlamOptions& o = s.opt;
-    for (double* v : {&o.trans_thresh, &o.rot_thresh, &o.l2_max, &o.truncated_ray, &o.truncated_range, &o.resolution}) *v = r.f64("options");
-    o.patch_size = r.u32("options"); o.max_iter = r.u32("options"); o.strategy = r.i32("options"); o.occupancy = r.i32("options");
-    o.transient_map = r.u8("options"); o.lidar_odometry = r.u8("options");
-    get_geometry(r, o.dev);
-    if (r.ok() && (o.patch_size != 32 || !(o.resolution > 0) || o.occupancy < 0 || o.occupancy > 1 || o.dev.dir_dim < 8 || o.dev.max_beams < 1 ||
-                   o.dev.pool_slots < 0 || o.lidar_odometry != lidar_odometry))
-        r.fail("bad options");
-    s.pose = r.se2("state"); s.odom = r.se2("state"); s.map_update_pose = r.se2("state");
-    s.has_first = r.u8("state"); s.engine_ready = r.u8("state");
-    s.processed = r.u32("state");
-    s.removed = r.u64("state"); s.map_updates = r.u64("state");
-    s.last = get_counters(r); s.total = get_counters(r);
-    if (r.ok() && (!finite_se2(s.pose) || !finite_se2(s.odom) || !finite_se2(s.map_update_pose))) r.fail("non-finite pose");
-}
-
-Slam2D* Slam2D::ckpt_restore(const SlamSaved& s, const EngineImage* img, const DeviceOptions& dev, std::string& err, int* code, CheckpointTimes* t)
-{
-    SlamOptions o = s.opt;
-    o.dev.device = dev.device; o.dev.stream = dev.stream; o.dev.timing = dev.timing;
-    std::unique_ptr<Slam2D> p(create(o, err));
-    if (!p) return nullptr;
-    p->pose_ = s.pose; p->odom_ = s.odom; p->map_update_pose_ = s.map_update_pose;
-    p->has_first_ = s.has_first; p->engine_ready_ = s.engine_ready;
-    p->processed_ = s.processed; p->removed_ = s.removed; p->map_updates_ = s.map_updates;
-    p->last_ = s.last; p->total_ = s.total;
-    if (img) {
-        Engine* e = Engine::restore(*img, dev.device, dev.stream, err, t);
-        if (!e) { *code = LAMA_ERR_CUDA; return nullptr; }
-        p->eng_.reset(e);
-        e->enable_timing(dev.timing != 0);
-        e->set_lidar_odometry_rays(o.lidar_odometry);
-    }
-    return p.release();
-}
-
-// ---- GraphSlam2D (kind 4) ---------------------------------------------------------------------------------------------------------------
-namespace {
-void put_loss(CkptWriter& w, const PgoLoss& l)
-{
-    for (double v : l.sigma) w.f64(v);
-    w.f64(l.huber_k);
-}
-PgoLoss get_loss(CkptReader& r, const char* what)
-{
-    PgoLoss l;
-    for (double& v : l.sigma) v = r.f64(what);
-    l.huber_k = r.f64(what);
-    bool ok = l.huber_k >= 0 && std::isfinite(l.huber_k);
-    for (double v : l.sigma) ok = ok && v > 0 && std::isfinite(v);   // GraphSlam2D's sigmas are finite constants; inf would drop a factor
-    if (r.ok() && !ok) r.fail(std::string("bad loss (") + what + ")");
-    return l;
-}
-void put_betweens(CkptWriter& w, const std::vector<PgoBetween>& v)
-{
-    w.u32((uint32_t)v.size());
-    for (const PgoBetween& b : v) {
-        w.i32(b.from); w.i32(b.to); w.se2(b.measured);
-        put_loss(w, b.loss);
-    }
-}
-void get_betweens(CkptReader& r, std::vector<PgoBetween>& v, size_t n_keys, const char* what)
-{
-    v.resize(r.count(r.u32(what), 2 * 4 + 4 * 8 + 4 * 8, what));
-    for (PgoBetween& b : v) {
-        b.from = r.i32(what); b.to = r.i32(what); b.measured = r.se2(what);
-        b.loss = get_loss(r, what);
-        if (r.ok() && (b.from < 0 || (size_t)b.from >= n_keys || b.to < 0 || (size_t)b.to >= n_keys)) r.fail(std::string("a factor names no key (") + what + ")");
-        if (r.ok() && !finite_se2(b.measured)) r.fail(std::string("non-finite factor (") + what + ")");
-    }
-}
-bool finite3(const double* v, int n)
-{
-    for (int k = 0; k < n; ++k)
-        if (!std::isfinite(v[k])) return false;
-    return true;
-}
-}  // namespace
-
-int GraphSlam2D::save(const std::string& path, CheckpointStats* st)
-{
-    const auto t0 = clk::now();
-    CheckpointStats local;
-    CheckpointStats& s = st ? *st : local;
-    s = CheckpointStats();
-    Engine* ie = slam_->engine();
-    const bool global = mapping_keyid_ > 0 && occ_;   // only then does the next generate_occupancy_map draw on occ_
-    EngineImage inner, gimg;
-    if (ie) {
-        const int rc = ie->snapshot(&inner, &s.dev);
-        if (rc != LAMA_OK) { err_ = ie->last_error(); return rc; }
-    }
-    if (global) {
-        CheckpointTimes t;
-        const int rc = occ_->engine()->snapshot(&gimg, &t);
-        if (rc != LAMA_OK) { err_ = occ_->engine()->last_error(); return rc; }
-        add_times(s.dev, t);
-    }
-    const auto t1 = clk::now();
-    CkptWriter w;
-    // graph options
-    w.f64(opt_.key_pose_distance); w.f64(opt_.key_pose_angular_distance); w.i32(opt_.key_pose_head_delay);
-    w.f64(opt_.loop_search_max_distance); w.f64(opt_.loop_search_min_distance); w.i32(opt_.loop_max_candidates);
-    w.f64(opt_.loop_closure_scan_rmse); w.i32(opt_.loop_closure_max_candidates); w.i32(opt_.ignore_n_chain_poses);
-    // the inner Slam2D: the bytes of a kind-2 file's options and state
-    slam_->ckpt_put(w);
-    // graph state
-    w.se2(correction_); w.se2(prev_);
-    w.f64(accdist_); w.f64(factordist_);
-    w.u64(mapping_keyid_);
-    w.u64(stats_.loop_factors); w.u64(stats_.optimizations); w.u64(stats_.optimizations_ok);
-    const PgoReport& rep = stats_.last;
-    w.i32(rep.status); w.u32(rep.iterations); w.u32(rep.lambda_tries); w.u64(rep.cg_iterations);
-    w.f64(rep.initial_error); w.f64(rep.final_error); w.f64(rep.device_ms);
-    w.u32((uint32_t)last_candidates_.size());
-    for (int c : last_candidates_) w.i32(c);
-    double c[2];
-    slam_window_center(slam_.get(), c);   // a restored engine does not know its centre (Engine::set_center)
-    w.f64(c[0]); w.f64(c[1]);
-    // key poses
-    w.u32((uint32_t)keys_.size());
-    for (const KeyPose& k : keys_) {
-        w.i32(k.id); w.se2(k.pose); w.se2(k.original);
-        for (double v : k.origin) w.f64(v);
-        for (double v : k.quat) w.f64(v);
-        w.f64(k.stamp);
-        w.u32((uint32_t)(k.pts.size() / 3));
-        w.bytes(k.pts.data(), k.pts.size() * 8);
-    }
-    w.u32((uint32_t)links_.size());
-    for (const auto& l : links_) { w.i32(l.first); w.i32(l.second); }
-    // the pose graph
-    w.u32((uint32_t)priors_.size());
-    for (const PgoPrior& p : priors_) {
-        w.i32(p.node); w.se2(p.measured);
-        put_loss(w, p.loss);
-    }
-    put_betweens(w, factors_);
-    put_betweens(w, queue_);
-    // the inner engine, its slots, the global map's engine and its slots
-    ckpt_put_engine(w, ie ? &inner : nullptr);
-    CkptWriter g;
-    g.buf.clear();
-    g.version = w.version;   // the global map's section is framed like the inner one
-    ckpt_put_engine(g, global ? &gimg : nullptr);
-    s.encode_ms = ms_since(t1);
-    std::string err;
-    const int rc = ckpt_write_file(path, kCkptGraphSlam2D, w,
-                                   {{inner.slot_bytes, (size_t)inner.used * inner.slot_stride()}, {g.buf.data(), g.buf.size()},
-                                    {gimg.slot_bytes, (size_t)gimg.used * gimg.slot_stride()}},
-                                   err, &s);
-    if (rc != LAMA_OK) { err_ = err; return rc; }
-    s.used_slots = (uint64_t)inner.used + gimg.used;
-    s.references = sum_refs(inner) + sum_refs(gimg);
-    s.total_ms   = ms_since(t0);
-    return LAMA_OK;
-}
-
-GraphSlam2D* GraphSlam2D::load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st)
-{
-    const auto t0 = clk::now();
-    CheckpointStats local;
-    CheckpointStats& s = st ? *st : local;
-    s = CheckpointStats();
-    std::vector<uint8_t> file;
-    uint32_t kind = 0;
-    *code = ckpt_read_file(path, file, &kind, err, &s);
-    if (*code != LAMA_OK) return nullptr;
-    *code = LAMA_ERR_ARG;
-    if (kind != kCkptGraphSlam2D) {
-        err = wrong_kind(kind, "GraphSlam2D");
-        return nullptr;
-    }
-    const auto t1 = clk::now();
-    CkptReader r = ckpt_body(file);
-    GraphOptions g;
-    g.key_pose_distance = r.f64("graph options"); g.key_pose_angular_distance = r.f64("graph options"); g.key_pose_head_delay = r.i32("graph options");
-    g.loop_search_max_distance = r.f64("graph options"); g.loop_search_min_distance = r.f64("graph options"); g.loop_max_candidates = r.i32("graph options");
-    g.loop_closure_scan_rmse = r.f64("graph options"); g.loop_closure_max_candidates = r.i32("graph options"); g.ignore_n_chain_poses = r.i32("graph options");
-    // an infinite threshold is a user's way to switch a test off (key_pose_angular_distance = inf: keys by distance only), so only NaN is refused
-    bool nan = false;
-    for (double v : {g.key_pose_distance, g.key_pose_angular_distance, g.loop_search_max_distance, g.loop_search_min_distance, g.loop_closure_scan_rmse})
-        nan = nan || std::isnan(v);
-    if (r.ok() && (nan || g.key_pose_head_delay < 0 || g.ignore_n_chain_poses < 0 || g.loop_max_candidates < 0)) r.fail("bad graph options");
-    SlamSaved sv;
-    Slam2D::ckpt_get(r, false, sv);
-    if (r.ok() && (!sv.opt.transient_map || sv.opt.truncated_ray != 1.0 || sv.opt.occupancy != 0))
-        r.fail("the inner Slam2D's options are not the ones GraphSlam2D forces (transient map, truncated_ray 1, frequency map, no lidar odometry)");
-    // graph state
-    const SE2 correction = r.se2("graph state"), prev = r.se2("graph state");
-    const double accdist = r.f64("graph state"), factordist = r.f64("graph state");
-    const uint64_t mapping_keyid = r.u64("graph state");
-    Stats stats;
-    stats.loop_factors = r.u64("graph stats"); stats.optimizations = r.u64("graph stats"); stats.optimizations_ok = r.u64("graph stats");
-    stats.last.status = r.i32("last report"); stats.last.iterations = r.u32("last report"); stats.last.lambda_tries = r.u32("last report");
-    stats.last.cg_iterations = r.u64("last report");
-    stats.last.initial_error = r.f64("last report"); stats.last.final_error = r.f64("last report"); stats.last.device_ms = r.f64("last report");
-    std::vector<int32_t> cands;
-    r.array(cands, r.u32("last candidates"), "last candidates");
-    double center[2];
-    center[0] = r.f64("window centre"); center[1] = r.f64("window centre");
-    if (r.ok() && (!finite_se2(correction) || !finite_se2(prev) || !std::isfinite(accdist) || !std::isfinite(factordist) || !finite3(center, 2)))
-        r.fail("non-finite graph state");
-    // key poses: every one at least 136 bytes before its points
-    std::vector<KeyPose> keys(r.count(r.u32("key poses"), 4 + 2 * 32 + 7 * 8 + 8 + 4, "key poses"));
-    for (size_t i = 0; i < keys.size() && r.ok(); ++i) {
-        KeyPose& k = keys[i];
-        k.id = r.i32("key pose"); k.pose = r.se2("key pose"); k.original = r.se2("key pose");
-        for (double& v : k.origin) v = r.f64("key pose");
-        for (double& v : k.quat) v = r.f64("key pose");
-        k.stamp = r.f64("key pose");
-        const size_t m = r.count(r.u32("key points"), 24, "key points");
-        r.array(k.pts, 3 * m, "key points");
-        if (r.ok() && k.id != (int)i) r.fail("a key pose id differs from its index");
-        if (r.ok() && (!finite_se2(k.pose) || !finite_se2(k.original) || !finite3(k.origin, 3) || !finite3(k.quat, 4))) r.fail("non-finite key pose");
-    }
-    const size_t n = keys.size();
-    auto is_key = [n](int32_t v) { return v >= 0 && (size_t)v < n; };
-    std::vector<int32_t> link_ids;
-    r.array(link_ids, 2 * (uint64_t)r.count(r.u32("links"), 8, "links"), "links");
-    std::vector<PgoPrior> priors(r.count(r.u32("priors"), 4 + 4 * 8 + 4 * 8, "priors"));
-    for (PgoPrior& p : priors) {
-        p.node = r.i32("priors"); p.measured = r.se2("priors");
-        p.loss = get_loss(r, "priors");
-        if (r.ok() && !is_key(p.node)) r.fail("a prior names no key");
-        if (r.ok() && !finite_se2(p.measured)) r.fail("non-finite prior");
-    }
-    std::vector<PgoBetween> factors, queue;
-    get_betweens(r, factors, n, "factors");
-    get_betweens(r, queue, n, "loop-factor queue");
-    if (r.ok()) {
-        for (int32_t v : link_ids)
-            if (!is_key(v)) r.fail("a link names no key");
-        for (int32_t v : cands)
-            if (!is_key(v)) r.fail("a loop candidate names no key");
-        if (mapping_keyid > n) r.fail("mapping key id past the key poses");
-    }
-    EngineImage inner, gimg;
-    bool inner_present = false, global_present = false;
-    if (r.ok()) ckpt_get_engine(r, &inner_present, inner, 1, 0, false);
-    if (r.ok() && inner_present && inner.known_plane) r.fail("the inner engine has a known plane");
-    if (r.ok() && (sv.has_first || n > 0) && !inner_present) r.fail("a GraphSlam2D past its first scan without device state");
-    if (r.ok()) ckpt_get_engine(r, &global_present, gimg, 1, 0, true);
-    if (r.ok() && global_present && !gimg.known_plane) r.fail("the global map's engine has no known plane");
-    if (r.ok() && global_present != (mapping_keyid > 0)) r.fail("a global map section must be present exactly when the mapping key id is above 0");
-    if (r.ok() && r.left() != 0) r.fail("bytes after the last section");
-    if (!r.ok()) { err = r.error(); return nullptr; }
-    if (!geometry_matches(dev, sv.opt.dev, inner_present ? &inner : nullptr, err)) return nullptr;
-    s.encode_ms += ms_since(t1);
-    // the file is valid: from here on the device
-    if (cuda_device_count() < 1) { *code = LAMA_ERR_NO_DEVICE; err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
-    std::unique_ptr<Slam2D> slam(Slam2D::ckpt_restore(sv, inner_present ? &inner : nullptr, dev, err, code, &s.dev));
-    if (!slam) return nullptr;
-    if (slam->engine()) slam->engine()->set_center(center[0], center[1]);
-    std::unique_ptr<GraphSlam2D> p(new GraphSlam2D());
-    g.slam = sv.opt;
-    g.slam.dev.device = dev.device; g.slam.dev.stream = dev.stream; g.slam.dev.timing = dev.timing;   // pgo_optimize_graph runs there
-    p->opt_ = g;
-    p->slam_ = std::move(slam);
-    if (global_present) {
-        CheckpointTimes t;
-        Engine* e = Engine::restore(gimg, dev.device, dev.stream, err, &t);
-        if (!e) { *code = LAMA_ERR_CUDA; return nullptr; }
-        e->enable_timing(dev.timing != 0);
-        p->occ_.reset(OccupancyMapDev::adopt(e));
-        add_times(s.dev, t);
-    }
-    p->mapping_keyid_ = (size_t)mapping_keyid;
-    p->keys_ = std::move(keys);
-    for (size_t i = 0; i < link_ids.size(); i += 2) p->links_.push_back({link_ids[i], link_ids[i + 1]});
-    p->priors_ = std::move(priors);
-    p->factors_ = std::move(factors);
-    p->queue_ = std::move(queue);
-    p->last_candidates_.assign(cands.begin(), cands.end());
-    p->correction_ = correction;
-    p->accdist_ = accdist;
-    p->prev_ = prev;
-    p->factordist_ = factordist;
-    p->stats_ = stats;
-    s.used_slots = (uint64_t)inner.used + gimg.used;
-    s.references = sum_refs(inner) + sum_refs(gimg);
-    s.total_ms   = ms_since(t0);
-    *code = LAMA_OK;
-    return p.release();
 }
 
 }  // namespace lama_b200

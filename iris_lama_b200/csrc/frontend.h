@@ -18,8 +18,7 @@ namespace lama_b200 {
 
 struct ShardComm;
 struct CheckpointStats;
-class CkptWriter;
-class CkptReader;
+struct Ckpt;   // checkpoint.cpp: the sections and the save / load frames
 
 struct DeviceOptions {
     int device = 0, dir_dim = 64, pool_slots = 0, max_beams = 2048, timing = 0;
@@ -117,26 +116,6 @@ public:
     static PFSlam2D* load_sharded(const std::vector<std::string>& paths, uint32_t shard_rank, uint32_t shard_count, const DeviceOptions& dev,
                                   std::string& err, int* code, CheckpointStats* st = nullptr, bool whole_only = false);
     struct Node { SE2 pose; int parent; };
-    // the options and state sections of a kind-1 / kind-5 file, as read and checked
-    struct Saved {
-        PFOptions opt;
-        SE2 prior{1, 0, 0, 0}, odom{1, 0, 0, 0};
-        bool has_first = false;
-        double acc_trans = 0, acc_rot = 0, neff = 0;
-        std::vector<SE2> pose;
-        std::vector<double> weight, nweight, wsum, stamps;
-        std::vector<int32_t> last_idx, node_of;
-        uint64_t rs_count = 0, rs_hash = 0, scans_seen = 0;
-        Counters last, total;                 // rank-local: with detached_seen and summary, the only fields the ranks of one
-        uint64_t detached_seen = 0;           // filter hold differently (the session id of a shard file skips them)
-        double summary[4] = {0, 0, 0, 0};
-        std::vector<Node> nodes;
-        std::string rng;
-    };
-    // The options and state sections.  marks = {end of the options, start and end of the rank-local fields}, as offsets into w.buf /
-    // from the reader's start.
-    void ckpt_put(CkptWriter& w, size_t marks[3]) const;
-    static void ckpt_get(CkptReader& r, Saved& s, size_t marks[3]);
     bool maps_enqueued_ = false;   // sharded ranks: this scan's map update was enqueued together with its match
     int settle_counters();
     int pipelined_begin(const double* pts, int n, const double* origin, const double* quat, bool moved, bool* did_update, double* local_out);
@@ -144,7 +123,12 @@ public:
     void collect_map_stats(Counters& c);
 
 private:
-    PFSlam2D() = default;
+    friend struct Ckpt;
+    PFSlam2D() = default;   // a handle without a device: create() and the checkpoint loader fill it in
+    // the checks create() applies to its options (everything but the device)
+    static bool valid_options(const PFOptions& o, std::string& err);
+    // rank opt_.shard_rank of opt_.shard_count: the particle count, the local particles [lo_, hi_) and, for seed 0, a seed of its own
+    void place();
     PFOptions opt_;
     std::unique_ptr<Engine> eng_;
     std::vector<double> timestamps_;
@@ -175,7 +159,6 @@ private:
     double digest_ = 0.0;           // of the previous scan's resampling decision, compared across ranks one scan later
     uint64_t shard_collectives_ = 0, shard_migrated_bytes_ = 0;
     int update_sharded(const double* pts, int n, const double* origin, const double* quat, const double odom_xyr[3], bool* did_update);
-    int write_checkpoint(const std::string& path, bool shard, CheckpointStats& s);
     int migrate_and_apply(const std::vector<int32_t>& idx);
     std::vector<double> staged_host_;  // the staged scans on the host too: the window guard reads them
     int staged_scans_ = 0, staged_beams_ = 0, staged_index_ = -1;
@@ -208,16 +191,6 @@ struct SlamOptions {  // include/lama/slam2d.h:91-125
     DeviceOptions dev;
 };
 
-// the options and host state of a Slam2D checkpoint (every section of a kind-2 / kind-3 file but the engine), as read and checked
-struct SlamSaved {
-    SlamOptions opt;
-    SE2 pose{1, 0, 0, 0}, odom{1, 0, 0, 0}, map_update_pose{1, 0, 0, 0};
-    bool has_first = false, engine_ready = false;
-    uint32_t processed = 0;
-    uint64_t removed = 0, map_updates = 0;
-    Counters last, total;
-};
-
 class Slam2D {
 public:
     static Slam2D* create(const SlamOptions& o, std::string& err);
@@ -233,17 +206,17 @@ public:
     const DeviceOptions& device_options() const { return opt_.dev; }
     const std::string& error() const { return err_; }
     bool lidar_odometry() const { return opt_.lidar_odometry; }
-    // checkpoints, as PFSlam2D::save / load; a handle saved before its first scan has no engine section
+    // the window centre: the engine's, or before the first update (the engine is created then, centred on the pose) the pose
+    void window_center(double c[2]);
+    // checkpoints, as PFSlam2D::save / load; a handle saved before its first scan has no engine section.  A GraphSlam2D file holds the
+    // same options and state sections for its inner Slam2D.
     int save(const std::string& path, CheckpointStats* st = nullptr);
     static Slam2D* load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st = nullptr);
-    // The options and state sections, shared by Slam2D files and the inner Slam2D of a GraphSlam2D file.  ckpt_get reads and checks them
-    // (lidar_odometry must match the file kind); ckpt_restore builds the handle on dev.device / dev.stream with dev.timing and, when
-    // `img` is given, restores its engine (*code = LAMA_ERR_CUDA when that fails).
-    void ckpt_put(CkptWriter& w) const;
-    static void ckpt_get(CkptReader& r, bool lidar_odometry, SlamSaved& s);
-    static Slam2D* ckpt_restore(const SlamSaved& s, const EngineImage* img, const DeviceOptions& dev, std::string& err, int* code, CheckpointTimes* t);
 
 private:
+    friend struct Ckpt;
+    friend class GraphSlam2D;   // its checkpoint loader restores the inner Slam2D
+    static bool valid_options(const SlamOptions& o, std::string& err);   // the checks create() applies (everything but the device)
     SlamOptions opt_;
     std::unique_ptr<Engine> eng_;
     SE2 pose_{1, 0, 0, 0}, odom_{1, 0, 0, 0};
@@ -361,6 +334,7 @@ public:
     static GraphSlam2D* load(const std::string& path, const DeviceOptions& dev, std::string& err, int* code, CheckpointStats* st = nullptr);
 
 private:
+    friend struct Ckpt;
     GraphOptions opt_;
     std::unique_ptr<Slam2D> slam_;
     size_t mapping_keyid_ = 0;                      // graph_slam2d.h: the first key not yet cast into occ_
