@@ -390,12 +390,12 @@ int lama_graph_slam(lama_graph* h, lama_slam** slam);
 
 /* ------------------------------------------------------------------------------------------------
  * FrequencyOccupancyMap -- include/lama/sdm/frequency_occupancy_map.h: a device-resident {occupied, visited} map with its own
- * 'known' plane (a pruned cell is {0, 0} and still known).  Cells outside the directory window make a call fail with
- * LAMA_ERR_WINDOW; the map is then partly updated.
+ * 'known' plane (a pruned cell is {0, 0} and still known).  By default the directory window is fixed: cells outside it make a call fail
+ * with LAMA_ERR_WINDOW, and the map is then partly updated.  A following map (lama_om_set_follow) moves the window over its scans instead.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct lama_om lama_om;
 /* FrequencyOccupancyMap(resolution, patch_size), window of dev->dir_dim^2 patches centred on center_xy (NULL: origin); dev->pool_slots
- * 0 = dir_dim^2 patches, so a full window cannot run out */
+ * 0 = dir_dim^2 patches, so a full window cannot run out, and a following map grows them; dev->pool_slots > 0 = a fixed pool */
 int lama_om_create(double resolution, uint32_t patch_size, const double center_xy[2], const lama_device_options* dev, lama_om** out);
 int lama_om_destroy(lama_om* om);   /* does nothing on a borrowed handle */
 /* the loop of GraphSlam2D::generateOccupancyMap (graph_slam2d.cpp:135-160) for any posed scans: scan k = points [offsets[k],
@@ -414,6 +414,16 @@ int lama_om_write(lama_om* om, const char* path);                               
 int lama_om_export_image(lama_om* om, uint8_t* pixels, size_t cap, int dims[2]);   /* sdm::export_to_png(OccupancyMap), export.cpp:46-73 */
 /* with dev->timing: ms[1] = device time of the casts (lama_om_insert_scans), launches as lama_slam_kernel_times */
 int lama_om_kernel_times(lama_om* om, double ms[4], uint64_t launches[5]);
+/* follow != 0: every later lama_om_insert_scans splits its scans, in order, into groups that each fit one window, and moves the window to
+ * each group (patches it leaves are parked and come back when it returns; exports, queries, bounds and files see them all).  A scan
+ * whose cells span more than dir_dim patches on an axis is refused with LAMA_ERR_WINDOW before anything is written.  With
+ * dev->pool_slots 0 the pool doubles before a group while fewer than dir_dim^2 slots may be free, up to 2^24 - 2 slots; an explicit
+ * pool_slots stays a hard cap (LAMA_ERR_POOL).  follow == 0 (the default) keeps the window fixed. */
+int lama_om_set_follow(lama_om* om, int follow);
+/* the working window as lama_slam_get_window: base (patch coordinates), dir_dim, counts = {shifts, parked entries, entries restored} */
+int lama_om_get_window(lama_om* om, int32_t base[2], int32_t* dim, uint64_t counts[3]);
+/* out = {pool slots, slots in use} */
+int lama_om_get_pool(lama_om* om, uint64_t out[2]);
 /* GraphSlam2D::generateOccupancyMap(full) (graph_slam2d.cpp:131-164): after an optimisation (or on the first call) a new map at
  * (full ? resolution : 0.1 m), then the key scans not yet cast, at their corrected poses, then prune over the whole map.  The handle
  * is BORROWED: owned by the lama_graph, and the map behind it is replaced in place when it is recreated (possibly at another

@@ -53,6 +53,17 @@ inline MapWindow map_window(int rc, const int32_t base[2], int32_t dim, const ui
     return w;
 }
 
+// a device FrequencyOccupancyMap (lama_om, stand-alone or the global map GraphSlam2D::generateOccupancyMap returns): following on or off
+// (lama_om_set_follow; a GraphSlam2D's map always follows), its working window and its pool {slots, slots in use}
+inline void occupancyMapSetFollow(lama_om* m, bool on) { check(lama_om_set_follow(m, on ? 1 : 0)); }
+inline MapWindow occupancyMapWindow(lama_om* m)
+{
+    int32_t b[2], d = 0;
+    uint64_t c[3];
+    return map_window(lama_om_get_window(m, b, &d, c), b, d, c);
+}
+inline void occupancyMapPool(lama_om* m, uint64_t out[2]) { check(lama_om_get_pool(m, out)); }
+
 class PFSlam2D {
 public:
     using Options = lama_pf_options;

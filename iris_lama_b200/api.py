@@ -87,7 +87,7 @@ EXPORTED_SYMBOLS = [
     "lama_graph_get_pose", "lama_graph_get_key_poses", "lama_graph_get_key_cloud", "lama_graph_get_links", "lama_graph_get_last_candidates",
     "lama_graph_get_stats", "lama_graph_slam", "lama_graph_generate_occupancy_map", "lama_graph_generate_coarse_distance_map",
     "lama_om_create", "lama_om_destroy", "lama_om_insert_scans", "lama_om_prune", "lama_om_resolution", "lama_om_bounds", "lama_om_query",
-    "lama_om_export", "lama_om_write", "lama_om_export_image", "lama_om_kernel_times",
+    "lama_om_export", "lama_om_write", "lama_om_export_image", "lama_om_kernel_times", "lama_om_set_follow", "lama_om_get_window", "lama_om_get_pool",
     "lama_tsdm_create", "lama_tsdm_destroy", "lama_tsdm_set_max_distance", "lama_tsdm_max_distance", "lama_tsdm_insert_point_clouds",
     "lama_tsdm_distance", "lama_tsdm_bounds", "lama_tsdm_export", "lama_tsdm_to_mesh", "lama_tsdm_write_ply", "lama_tsdm_kernel_times",
     "lama_om3_create", "lama_om3_destroy", "lama_om3_insert_point_clouds", "lama_om3_apply", "lama_om3_query", "lama_om3_prune",
@@ -911,9 +911,11 @@ def _graph_options_of_checkpoint(path, device, stream, timing) -> GraphOptions:
 
 class FrequencyOccupancyMap:
     """Device-resident lama::FrequencyOccupancyMap (include/lama/sdm/frequency_occupancy_map.h), stand-alone or borrowed from a
-    GraphSlam2D (handle= / owner=, as DynamicDistanceMap)."""
+    GraphSlam2D (handle= / owner=, as DynamicDistanceMap).  follow=True: every insertScans moves the directory window over its scans
+    group by group instead of failing at the window's edge, and with pool_slots 0 the pool grows (lama_om_set_follow).  A GraphSlam2D's
+    map always follows."""
 
-    def __init__(self, resolution=0.05, patch_size=32, center=(0.0, 0.0), handle=None, owner=None, **dev):
+    def __init__(self, resolution=0.05, patch_size=32, center=(0.0, 0.0), handle=None, owner=None, follow=False, **dev):
         self.owner = owner
         if handle is not None:
             self.h = handle
@@ -926,6 +928,8 @@ class FrequencyOccupancyMap:
         self.h = C.c_void_p()
         self.owned = True
         _chk(lib().lama_om_create(C.c_double(resolution), C.c_uint32(patch_size), cp, C.byref(d), C.byref(self.h)))
+        if follow:
+            _chk(lib().lama_om_set_follow(self.h, C.c_int(1)))
 
     def __del__(self):
         if getattr(self, "owned", False) and getattr(self, "h", None) and _lib is not None:
@@ -985,6 +989,16 @@ class FrequencyOccupancyMap:
 
     def kernelTimes(self):
         return _times(lib().lama_om_kernel_times, self.h)
+
+    def window(self):
+        """The working window: base (patch coordinates), dim (dir_dim), shifts so far, entries parked now, entries restored so far."""
+        return _window(lib().lama_om_get_window, self.h)
+
+    def pool(self):
+        """(pool slots, slots in use)"""
+        out = np.zeros(2, np.uint64)
+        _chk(lib().lama_om_get_pool(self.h, _vp(out)))
+        return int(out[0]), int(out[1])
 
 
 def _clouds(clouds):

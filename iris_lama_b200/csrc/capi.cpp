@@ -1526,6 +1526,29 @@ try {
     return times_out(om_engine(om), ms, launches);
 }
 LAMA_CATCH
+int lama_om_set_follow(lama_om* om, int follow)
+try {
+    if (!om) return set_err("null handle", LAMA_ERR_ARG);
+    if (!om->m) return set_err("no map yet (generateOccupancyMap has not been called)", LAMA_ERR_STATE);
+    om->m->set_follow(follow != 0);
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_om_get_window(lama_om* om, int32_t base[2], int32_t* dim, uint64_t counts[3])
+try {
+    if (!om) return set_err("null handle", LAMA_ERR_ARG);
+    return window_out(om_engine(om), base, dim, counts);
+}
+LAMA_CATCH
+int lama_om_get_pool(lama_om* om, uint64_t out[2])
+try {
+    if (!om || !out) return set_err("null argument", LAMA_ERR_ARG);
+    Engine* e = om_engine(om);
+    if (!e) return set_err("no map yet (generateOccupancyMap has not been called)", LAMA_ERR_STATE);
+    const int rc = e->pool_info(out);
+    return rc == LAMA_OK ? rc : set_err(e->last_error(), rc);
+}
+LAMA_CATCH
 
 // ---- TruncatedSignedDistanceMap (include/lama/sdm/truncated_signed_distance_map.h) -------------------------------------------------
 struct lama_tsdm { TsdmDev* t; };

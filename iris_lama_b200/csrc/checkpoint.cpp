@@ -311,6 +311,10 @@ public:
         std::vector<CkptWriter> more(imgs_.size());   // the engine sections after the first: own buffers, framed like the first
         std::vector<CkptSegment> tail;
         uint64_t used = 0, refs = 0;
+        // one version for the whole file: every engine section carries parked lists when any of them has parked entries (a GraphSlam2D
+        // whose global map has moved and whose inner map has not)
+        for (size_t i = 0; i < imgs_.size(); ++i)
+            if (present_[i] && !imgs_[i].parked.empty()) w.version = kCkptVersionParked;
         for (size_t i = 0; i < imgs_.size(); ++i) {
             const EngineImage& img = imgs_[i];
             CkptWriter& to = i == 0 ? w : more[i];
@@ -938,7 +942,8 @@ GraphSlam2D* GraphSlam2D::load(const std::string& path, const DeviceOptions& dev
     if (global_present) {
         Engine* e = f.restore(gimg, dev);
         if (!e) return nullptr;
-        p->occ_.reset(OccupancyMapDev::adopt(e));
+        p->occ_.reset(OccupancyMapDev::adopt(e, s.opt_.dev.pool_slots <= 0));
+        p->occ_->set_follow(true);
     }
     return f.done(p);
 }

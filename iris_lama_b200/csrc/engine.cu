@@ -8,6 +8,7 @@
 #include <memory>
 
 #include "kernels.cuh"
+#include "render_plan.h"
 
 namespace lama_b200 {
 
@@ -50,6 +51,8 @@ struct Engine::Impl {
     bool scan_flat = false;     // the current scan has z == 0 everywhere and a sensor that keeps z planes: every beam is planar
     bool staged_flat = false;   // the same for the staged scans
     cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+    cudaEvent_t ev_render[2] = {nullptr, nullptr};   // around one group of a following render (shift_window takes ev[0] / ev[1] between groups)
+    void* pool_raw = nullptr;                          // the allocation view.pool was aligned out of (grow_pool replaces it)
     // timing of the pipelined step (step_enqueue): per report buffer {before match, after match, after the ray stage, after the brushfire}; read when
     // that step is collected, so no host synchronisation is added
     cudaEvent_t evp[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};
@@ -57,6 +60,9 @@ struct Engine::Impl {
     // scratch for import/export/distance
     void* d_scratch = nullptr;
     size_t scratch_bytes = 0;
+    // scratch of shift_window, apart from d_scratch: a following render shifts the window between groups while its scans sit in d_scratch
+    void* d_shift_scratch = nullptr;
+    size_t shift_scratch_bytes = 0;
     // device arena of a migration round (pack_device / migration_alloc): bump allocation out of chunks that are kept between rounds, so that a resampling
     // scan costs no cudaMalloc / cudaFree once the arena has grown to its working size
     std::vector<std::pair<char*, size_t>> mig_chunks;
@@ -205,6 +211,8 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     CU_NEW(cudaEventCreate(&d->ev[0]));
     CU_NEW(cudaEventCreate(&d->ev[1]));
     CU_NEW(cudaEventCreate(&d->ev[2]));
+    CU_NEW(cudaEventCreate(&d->ev_render[0]));
+    CU_NEW(cudaEventCreate(&d->ev_render[1]));
     for (int b = 0; b < 2; ++b)
         for (int k = 0; k < 4; ++k) CU_NEW(cudaEventCreate(&d->evp[b][k]));
 
@@ -227,8 +235,8 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
         return r;
     };
     // k_raycast ORs cell offsets into patch base addresses: the pool starts on a 4 KiB boundary (cudaMalloc only promises 256 B)
-    CU_NEW(dalloc((void**)&v.pool, ((size_t)v.n_slots + 1) * kPatchBytes));
-    v.pool = reinterpret_cast<uint32_t*>(((uintptr_t)v.pool + (kPatchBytes - 1)) & ~(uintptr_t)(kPatchBytes - 1));
+    CU_NEW(dalloc(&d->pool_raw, ((size_t)v.n_slots + 1) * kPatchBytes));
+    v.pool = reinterpret_cast<uint32_t*>(((uintptr_t)d->pool_raw + (kPatchBytes - 1)) & ~(uintptr_t)(kPatchBytes - 1));
     CU_NEW(dalloc((void**)&v.fbits, (size_t)v.n_slots * 128));
     if (cfg.occupancy_kind == 1 || cfg.known_plane) CU_NEW(dalloc((void**)&v.kbits, (size_t)v.n_slots * 128));
     CU_NEW(dalloc((void**)&v.refcount, (size_t)v.n_slots * 4));
@@ -349,10 +357,13 @@ Engine::~Engine()
     if (d_->h_scan) cudaFreeHost(d_->h_scan);
     if (d_->ev_match) cudaEventDestroy(d_->ev_match);
     if (d_->ev_sync) cudaEventDestroy(d_->ev_sync);
+    for (cudaEvent_t ev : d_->ev_render)
+        if (ev) cudaEventDestroy(ev);
     for (auto& c : d_->mig_chunks) cudaFree(c.first);
     if (d_->h_idx) cudaFreeHost(d_->h_idx);
     if (d_->h_status) cudaFreeHost(d_->h_status);
     if (d_->d_scratch) cudaFree(d_->d_scratch);
+    if (d_->d_shift_scratch) cudaFree(d_->d_shift_scratch);
     if (d_->d_staged) cudaFree(d_->d_staged);
     for (int b = 0; b < 2; ++b)
         for (int k = 0; k < 4; ++k)
@@ -846,15 +857,17 @@ int Engine::resample(const int32_t* idx)
     return LAMA_OK;
 }
 
-static int ensure_scratch(Engine::Impl* d, size_t bytes)
+static int ensure_buffer(void** buf, size_t* cap, size_t bytes)
 {
-    if (bytes <= d->scratch_bytes) return 0;
-    if (d->d_scratch) cudaFree(d->d_scratch);
-    d->scratch_bytes = 0;
-    if (cudaMalloc(&d->d_scratch, bytes) != cudaSuccess) return -1;
-    d->scratch_bytes = bytes;
+    if (bytes <= *cap) return 0;
+    if (*buf) cudaFree(*buf);
+    *buf = nullptr;
+    *cap = 0;
+    if (cudaMalloc(buf, bytes) != cudaSuccess) return -1;
+    *cap = bytes;
     return 0;
 }
+static int ensure_scratch(Engine::Impl* d, size_t bytes) { return ensure_buffer(&d->d_scratch, &d->scratch_bytes, bytes); }
 
 bool Engine::has_parked(int particle) const
 {
@@ -882,8 +895,8 @@ int Engine::shift_window(int32_t base_px, int32_t base_py)
     // scratch: counts | new {offset, length} | enter prefixes (window_shift_core.h: the arena may have gaps after a prune)
     const size_t b_cnt = (size_t)n_lists * sizeof(int2);
     const size_t b_enter = shift_scratch_ints(reinterpret_cast<const int32_t*>(d_->park_ol[set].data()), n_lists) * 4;
-    if (ensure_scratch(d_, 2 * b_cnt + b_enter)) return fail("shift_window: out of device memory", LAMA_ERR_CUDA);
-    int2* d_cnt = (int2*)d_->d_scratch;
+    if (ensure_buffer(&d_->d_shift_scratch, &d_->shift_scratch_bytes, 2 * b_cnt + b_enter)) return fail("shift_window: out of device memory", LAMA_ERR_CUDA);
+    int2* d_cnt = (int2*)d_->d_shift_scratch;
     int2* d_new_ol = d_cnt + n_lists;
     int32_t* d_enter = (int32_t*)(d_new_ol + n_lists);
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
@@ -943,6 +956,21 @@ int Engine::render_scans(const double* pts, const int64_t* offsets, int n_scans,
     CU_TRY(cudaSetDevice(cfg_.device));
     std::vector<MovingTf> moving((size_t)n_scans);
     for (int k = 0; k < n_scans; ++k) moving[k] = moving_tf(origins ? origins + 3 * (size_t)k : nullptr, quats ? quats + 4 * (size_t)k : nullptr);
+    // the groups and their windows, every scan checked before anything is written (render_plan.h); without following, one group in the
+    // current window, whose kernels report a beam outside it
+    std::vector<RenderGroup> groups;
+    if (follow_) {
+        std::vector<CellBox> boxes((size_t)n_scans);
+        for (int k = 0; k < n_scans; ++k)
+            boxes[k] = render_scan_box(compose_tf(states[k], moving[k]), 1.0 / cfg_.resolution, pts + 3 * offsets[k], offsets[k + 1] - offsets[k]);
+        const int bad = plan_render(window_, boxes.data(), n_scans, groups);
+        if (bad >= 0)
+            return fail("render_scans: scan " + std::to_string(bad) + " reaches over more than one directory window (" + std::to_string(cfg_.dir_dim) +
+                            " x " + std::to_string(cfg_.dir_dim) + " patches)",
+                        LAMA_ERR_WINDOW);
+    } else {
+        groups.push_back(RenderGroup{0, n_scans, window_});
+    }
     // scratch: points | offsets | moving | states | marks (dim^2 bytes) | cell counter
     auto up = [](size_t b) { return (b + 15) & ~(size_t)15; };
     const size_t dim2 = (size_t)cfg_.dir_dim * cfg_.dir_dim;
@@ -965,22 +993,130 @@ int Engine::render_scans(const double* pts, const int64_t* offsets, int n_scans,
     CU_TRY(cudaMemcpyAsync((void*)p.states, states, (size_t)n_scans * sizeof(SE2), cudaMemcpyHostToDevice, d_->stream));
     CU_TRY(cudaMemsetAsync(p.marks, 0, b_marks + 16, d_->stream));   // marks and the cell counter
     h2d_bytes_ += (uint64_t)n_pts * 24;
-    if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
-    launch_render_scans(d_->view, cur_set_, p, n_scans, d_->stream);
-    CU_TRY(cudaGetLastError());
-    if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
+    // The cell counters are sums, so the grouping changes no cell; `known` is ORed per group; the cell count adds up over the groups.
+    float ms = 0.f;
+    bool timed = false;
+    for (const RenderGroup& g : groups) {
+        if (g.window.base_px != window_.base_px || g.window.base_py != window_.base_py) {
+            const int rc = shift_window(g.window.base_px, g.window.base_py);   // parked patches the window covers return before the marks
+            if (rc != LAMA_OK) return rc;
+        }
+        if (grow_) {
+            // every slot of a one-particle render-only map is one directory entry or one parked entry, so a group, which can fill at most
+            // the empty entries of its window, always has room when the pool holds the parked entries and a whole window: no read-back
+            const int64_t n_slots = d_->view.n_slots, want = pool_growth(n_slots, (int64_t)d_->parked(cur_set_), (int64_t)dim2, true);
+            if (want != n_slots) {
+                const int rc = grow_pool((int)want);
+                if (rc != LAMA_OK) return rc;
+            }
+        }
+        if (timed) {   // the previous group: every later group opens with a shift, which has synchronised the stream since
+            float g_ms = 0.f;
+            CU_TRY(cudaEventSynchronize(d_->ev_render[1]));
+            CU_TRY(cudaEventElapsedTime(&g_ms, d_->ev_render[0], d_->ev_render[1]));
+            ms += g_ms;
+            timed = false;
+        }
+        RenderParams q = p;
+        q.offsets += g.first;
+        q.moving += g.first;
+        q.states += g.first;
+        if (timing_) CU_TRY(cudaEventRecord(d_->ev_render[0], d_->stream));
+        launch_render_scans(d_->view, cur_set_, q, g.count, d_->stream);
+        CU_TRY(cudaGetLastError());
+        if (timing_) {
+            CU_TRY(cudaEventRecord(d_->ev_render[1], d_->stream));
+            timed = true;
+        }
+        times_.raycast_launches += 4;
+    }
     unsigned long long n_cells = 0;
     CU_TRY(cudaMemcpyAsync(&n_cells, p.cells, 8, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
-    if (timing_) {
-        float ms = 0.f;
-        CU_TRY(cudaEventElapsedTime(&ms, d_->ev[0], d_->ev[1]));
-        times_.raycast_ms += ms;
+    if (timed) {
+        float g_ms = 0.f;
+        CU_TRY(cudaEventElapsedTime(&g_ms, d_->ev_render[0], d_->ev_render[1]));
+        ms += g_ms;
     }
-    times_.raycast_launches += 4;
+    times_.raycast_ms += ms;
     if (cells) *cells = n_cells;
     return check_device_status();
+}
+
+int Engine::pool_info(uint64_t out[2])
+{
+    { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
+    CU_TRY(cudaSetDevice(cfg_.device));
+    int32_t free_count = 0;
+    CU_TRY(cudaMemcpyAsync(&free_count, d_->view.free_count, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaStreamSynchronize(d_->stream));
+    out[0] = (uint64_t)d_->view.n_slots;
+    out[1] = (uint64_t)(d_->view.n_slots - free_count);
+    return LAMA_OK;
+}
+
+int Engine::grow_pool(int new_slots)
+{
+    { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
+    StoreView& v = d_->view;
+    if (cfg_.particles != 1) return fail("grow_pool: only a one-particle engine's pool grows", LAMA_ERR_STATE);
+    if (new_slots <= v.n_slots) return LAMA_OK;
+    if ((int64_t)new_slots > kPoolSlotCap) return fail("grow_pool: more than 2^24 - 2 slots (the slot field of a directory entry)", LAMA_ERR_POOL);
+    CU_TRY(cudaSetDevice(cfg_.device));
+    int32_t counts[2] = {0, 0};   // free, freed (released slots not yet merged)
+    CU_TRY(cudaMemcpyAsync(counts, v.free_count, 8, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaStreamSynchronize(d_->stream));
+    const size_t n_old = (size_t)v.n_slots, n_new = (size_t)new_slots, n_add = n_new - n_old;
+    // everything is allocated before anything is changed
+    StoreView nv = v;
+    void* pool_raw = nullptr;
+    std::vector<void*> fresh;
+    auto grab = [&](void** ptr, size_t bytes) -> bool {
+        if (cudaMalloc(ptr, bytes) != cudaSuccess) return false;
+        fresh.push_back(*ptr);
+        return true;
+    };
+    bool ok = grab(&pool_raw, (n_new + 1) * kPatchBytes) && grab((void**)&nv.fbits, n_new * 128) && (!v.kbits || grab((void**)&nv.kbits, n_new * 128)) &&
+              grab((void**)&nv.refcount, n_new * 4) && grab((void**)&nv.free_slots, n_new * 4) && grab((void**)&nv.freed, n_new * 4);
+    auto give_up = [&](const std::string& why) {
+        cudaStreamSynchronize(d_->stream);
+        for (void* q : fresh) cudaFree(q);
+        cudaGetLastError();   // a failed cudaMalloc is not sticky; clear it for the next call
+        return fail("grow_pool: " + why + " (the pool keeps its " + std::to_string(n_old) + " slots)", LAMA_ERR_CUDA);
+    };
+    if (!ok) return give_up("out of device memory for " + std::to_string(n_new) + " slots");
+    nv.pool = reinterpret_cast<uint32_t*>(((uintptr_t)pool_raw + (kPatchBytes - 1)) & ~(uintptr_t)(kPatchBytes - 1));
+    nv.n_slots = new_slots;
+    // slots keep their ids; the free stack gets the new slots below the old free entries, the lowest new slot deepest of them, so the
+    // old free slots are handed out first, then n_old, n_old + 1, ...
+    cudaError_t e = cudaMemcpyAsync(nv.pool, v.pool, n_old * kPatchBytes, cudaMemcpyDeviceToDevice, d_->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(nv.fbits, v.fbits, n_old * 128, cudaMemcpyDeviceToDevice, d_->stream);
+    if (e == cudaSuccess && v.kbits) e = cudaMemcpyAsync(nv.kbits, v.kbits, n_old * 128, cudaMemcpyDeviceToDevice, d_->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(nv.refcount, v.refcount, n_old * 4, cudaMemcpyDeviceToDevice, d_->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(nv.refcount + n_old, 0, n_add * 4, d_->stream);
+    if (e == cudaSuccess) e = launch_fill_descending(nv.free_slots, (int)n_add, new_slots - 1, d_->stream);
+    if (e == cudaSuccess && counts[0] > 0)
+        e = cudaMemcpyAsync(nv.free_slots + n_add, v.free_slots, (size_t)counts[0] * 4, cudaMemcpyDeviceToDevice, d_->stream);
+    if (e == cudaSuccess && counts[1] > 0) e = cudaMemcpyAsync(nv.freed, v.freed, (size_t)counts[1] * 4, cudaMemcpyDeviceToDevice, d_->stream);
+    counts[0] += (int32_t)n_add;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(v.free_count, counts, 4, cudaMemcpyHostToDevice, d_->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(d_->stream);
+    if (e != cudaSuccess) return give_up(cudaGetErrorString(e));   // the old arrays are untouched; only the free count is written in place, last
+    const void* old[] = {d_->pool_raw, v.fbits, v.kbits, v.refcount, v.free_slots, v.freed};
+    for (const void* q : old) {
+        if (!q) continue;
+        auto it = std::find(d_->allocs.begin(), d_->allocs.end(), q);
+        if (it != d_->allocs.end()) d_->allocs.erase(it);
+        cudaFree(const_cast<void*>(q));
+    }
+    d_->allocs.insert(d_->allocs.end(), fresh.begin(), fresh.end());
+    d_->pool_raw = pool_raw;
+    v = nv;
+    cfg_.pool_slots = new_slots;
+    pool_growths_ += 1;
+    times_.misc_launches += 1;
+    return LAMA_OK;
 }
 
 int Engine::prune_frequency()
@@ -989,10 +1125,12 @@ int Engine::prune_frequency()
     if (!d_->view.kbits || cfg_.occupancy_kind != 0) return fail("prune_frequency: needs a frequency map with a known plane", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
     launch_prune_freq(d_->view, cur_set_, d_->stream);
+    const int n_parked = d_->park_ol[cur_set_][kMapOcc].y;   // particle 0's occupancy list
+    if (n_parked) launch_prune_freq_parked(d_->view, d_->pv(cur_set_), n_parked, d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
-    times_.misc_launches += 1;
+    times_.misc_launches += n_parked ? 2 : 1;
     return check_device_status();
 }
 

@@ -163,8 +163,20 @@ public:
     // *cells = number of cell updates.
     int render_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states, bool full,
                      uint64_t* cells);
-    // FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158) of particle 0's map
+    // FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158) of particle 0's map, parked patches included
     int prune_frequency();
+    // Following renders (off by default): render_scans splits its scans into consecutive groups that each fit one window
+    // (render_plan.h), moves the window to each group's window with shift_window and, with `grow`, grows the pool before a group
+    // until it holds the parked entries and a whole window (pool_growth).  A scan no window holds is refused before anything is written.
+    void set_render_follow(bool follow, bool grow) { follow_ = follow; grow_ = follow && grow; }
+    bool render_follow() const { return follow_; }
+    bool pool_grows() const { return grow_; }
+    // A larger pool for a one-particle engine: the slots in use keep their ids, contents, bits and reference counts, the new slots
+    // are free.  Allocates everything first; on failure the engine is unchanged (LAMA_ERR_CUDA, or LAMA_ERR_POOL past the 24-bit cap).
+    int grow_pool(int new_slots);
+    // {pool slots, slots in use}; synchronises
+    int pool_info(uint64_t out[2]);
+    uint64_t pool_growths() const { return pool_growths_; }
 
     // Direct DynamicDistanceMap::addObstacle / removeObstacle calls in list order, then update().
     int dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_add, int n, uint32_t* processed);
@@ -246,6 +258,8 @@ private:
     KernelTimes times_;
     std::string err_;
     uint64_t h2d_bytes_ = 0, d2h_bytes_ = 0;
+    bool follow_ = false, grow_ = false;
+    uint64_t pool_growths_ = 0;
     int pending_maps_ = 0;
     int pending_buf_ = 0;                 // which half of the ping-pong host buffers the pending map update reports into
     uint64_t settled_counters_[4] = {0, 0, 0, 0};

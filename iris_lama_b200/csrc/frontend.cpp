@@ -1,5 +1,6 @@
 // frontend.cpp -- host orchestration of PFSlam2D / Slam2D / Loc2D over the device Engine.
 #include "frontend.h"
+#include "render_plan.h"
 #include "rng_skip.h"
 #include "sdm_io.h"
 #include "window_guard.h"
@@ -1040,8 +1041,12 @@ int GraphSlam2D::generate_occupancy_map(bool full, OccupancyMapDev** out)
     if (mapping_keyid_ == 0 || !occ_) {   // :132-133
         double c[2];
         slam_->window_center(c);
-        OccupancyMapDev* m = OccupancyMapDev::create(full ? opt_.slam.resolution : 0.1, 32, c[0], c[1], slam_->device_options(), err_);
+        const double res = full ? opt_.slam.resolution : 0.1;
+        // a rebuild after an optimisation casts every key again: start at the pool the previous map of this resolution grew to
+        const int start = occ_ && occ_->engine()->config().resolution == res ? occ_->engine()->config().pool_slots : 0;
+        OccupancyMapDev* m = OccupancyMapDev::create(res, 32, c[0], c[1], slam_->device_options(), err_, start);
         if (!m) return LAMA_ERR_CUDA;
+        m->set_follow(true);
         occ_.reset(m);   // borrowed handles never see a null map
         mapping_keyid_ = 0;
     }
@@ -1317,25 +1322,29 @@ int DistanceMapDev::flush_if_pending()
     return update(nullptr);
 }
 
-OccupancyMapDev* OccupancyMapDev::create(double resolution, uint32_t patch_size, double cx, double cy, const DeviceOptions& dev, std::string& err)
+OccupancyMapDev* OccupancyMapDev::create(double resolution, uint32_t patch_size, double cx, double cy, const DeviceOptions& dev, std::string& err,
+                                         int start_slots)
 {
     if (patch_size != 32) { err = "FrequencyOccupancyMap: only patch_size 32 is supported on the device"; return nullptr; }
     if (cuda_device_count() < 1) { err = "no CUDA device available: the lama_b200 hot path has no CPU fallback"; return nullptr; }
     EngineConfig cfg = engine_config(dev, 1, resolution, resolution, cx, cy);   // no distance map is kept: the smallest reach
-    if (cfg.pool_slots <= 0) cfg.pool_slots = cfg.dir_dim * cfg.dir_dim;
+    const bool growable = cfg.pool_slots <= 0;
+    if (growable) cfg.pool_slots = std::max(cfg.dir_dim * cfg.dir_dim, (int)std::min<int64_t>(start_slots, kPoolSlotCap));
     cfg.known_plane = true;
     Engine* en = Engine::create(cfg, err);
     if (!en) return nullptr;
     OccupancyMapDev* m = new OccupancyMapDev();
     m->eng_.reset(en);
+    m->growable_ = growable;
     en->enable_timing(dev.timing != 0);
     return m;
 }
 
-OccupancyMapDev* OccupancyMapDev::adopt(Engine* e)
+OccupancyMapDev* OccupancyMapDev::adopt(Engine* e, bool growable)
 {
     OccupancyMapDev* m = new OccupancyMapDev();
     m->eng_.reset(e);
+    m->growable_ = growable;
     return m;
 }
 

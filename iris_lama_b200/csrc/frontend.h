@@ -252,9 +252,15 @@ private:
 // ---- device FrequencyOccupancyMap that keeps its own known plane: GraphSlam2D's global map ---------------------------------------------
 class OccupancyMapDev {
 public:
-    // one-particle engine; dev.pool_slots 0 = dir_dim^2 slots, so a full window cannot run out of patches
-    static OccupancyMapDev* create(double resolution, uint32_t patch_size, double cx, double cy, const DeviceOptions& dev, std::string& err);
-    static OccupancyMapDev* adopt(Engine* e);   // a map around a restored engine (one particle, frequency, known plane); takes ownership
+    // one-particle engine; dev.pool_slots 0 = max(dir_dim^2, start_slots) slots that may grow when the map follows (a full window cannot
+    // run out of patches), dev.pool_slots > 0 = a fixed pool
+    static OccupancyMapDev* create(double resolution, uint32_t patch_size, double cx, double cy, const DeviceOptions& dev, std::string& err,
+                                   int start_slots = 0);
+    // a map around a restored engine (one particle, frequency, known plane); takes ownership.  `growable`: dev.pool_slots was 0
+    static OccupancyMapDev* adopt(Engine* e, bool growable = true);
+    // Following (off by default): each insert_scans moves the window over its scans group by group (Engine::set_render_follow), and a
+    // map created with an automatic pool grows it
+    void set_follow(bool on) { eng_->set_render_follow(on, growable_); }
     // GraphSlam2D::generateOccupancyMap's loop body (graph_slam2d.cpp:136-160) for any posed scans (Engine::render_scans)
     int insert_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states, bool full,
                      uint64_t* cells);
@@ -265,6 +271,7 @@ public:
 private:
     std::unique_ptr<Engine> eng_;
     std::string err_;
+    bool growable_ = true;
 };
 
 // ---- GraphSlam2D's loop-closure front end (src/graph_slam2d.cpp:283-355) on a device distance map -------------------------------------
@@ -321,6 +328,7 @@ public:
     const std::string& error() const { return err_; }
     // generateOccupancyMap (:131-164): a new map at (full ? resolution : 0.1) when mapping_keyid is 0, the key scans from mapping_keyid on
     // cast at their corrected poses, prune, mapping_keyid = number of keys.  The map is owned here and replaced on the next recreation.
+    // It follows its scans (OccupancyMapDev::set_follow); a recreated map starts with the pool of the map it replaces at that resolution.
     int generate_occupancy_map(bool full, OccupancyMapDev** out);
     // generateCoarseDistanceMap (:166-186): a new 0.1 m distance map (reach 5 m) with an obstacle at every occupied cell of the inner
     // Slam2D, visited in ascending directory index, then cell index; *processed = its update() return value

@@ -2043,8 +2043,17 @@ __global__ void k_render_known(StoreView s, int set, uint8_t* __restrict__ marks
     if (lane == 0) marks[di] = 0;
 }
 
-// FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158) over every patch: cells visited once and occupied at most
+// FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158) of one patch by one warp: cells visited once and occupied at most
 // once go back to {0, 0}; their known bit stays
+__device__ __forceinline__ void prune_freq_patch(uint32_t* cells, int lane)
+{
+    for (int row = 0; row < kPatchLen; ++row) {
+        const uint32_t w = cells[row * kPatchLen + lane];
+        if (occ_visited(w) == 1u && occ_occupied(w) <= 1u) cells[row * kPatchLen + lane] = 0u;
+    }
+}
+
+// the prune over every patch of the window: one warp per directory entry
 __global__ void k_prune_freq(StoreView s, int set)
 {
     const int lane = threadIdx.x & 31;
@@ -2052,11 +2061,23 @@ __global__ void k_prune_freq(StoreView s, int set)
     if (di >= s.window.dim * s.window.dim) return;
     const int e = dir_of(s, set, 0, kMapOcc)[di];
     if (e < 0) return;
-    uint32_t* cells = patch_ptr(s, e & kDirSlotMask);
-    for (int row = 0; row < kPatchLen; ++row) {
-        const uint32_t w = cells[row * kPatchLen + lane];
-        if (occ_visited(w) == 1u && occ_occupied(w) <= 1u) cells[row * kPatchLen + lane] = 0u;
-    }
+    prune_freq_patch(patch_ptr(s, e & kDirSlotMask), lane);
+}
+
+// the prune over the parked patches of particle 0's occupancy map: one warp per entry of its list (a parked entry always holds a patch)
+__global__ void k_prune_freq_parked(StoreView s, ParkView pv)
+{
+    const int lane = threadIdx.x & 31;
+    const int i    = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int2 ol  = pv.ol[kMapOcc];
+    if (i >= ol.y) return;
+    prune_freq_patch(patch_ptr(s, pv.park[ol.x + i].entry & kDirSlotMask), lane);
+}
+
+__global__ void k_fill_descending(int32_t* __restrict__ out, int n, int32_t top)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = top - i;
 }
 
 }  // namespace
@@ -2295,6 +2316,17 @@ void launch_prune_freq(const StoreView& s, int set, cudaStream_t st)
 {
     const int dim2 = s.window.dim * s.window.dim;
     k_prune_freq<<<(dim2 + 7) / 8, 256, 0, st>>>(s, set);
+}
+void launch_prune_freq_parked(const StoreView& s, const ParkView& pv, int n, cudaStream_t st)
+{
+    if (n <= 0) return;
+    k_prune_freq_parked<<<(n + 7) / 8, 256, 0, st>>>(s, pv);
+}
+cudaError_t launch_fill_descending(int32_t* d_out, int n, int32_t top, cudaStream_t st)
+{
+    if (n <= 0) return cudaSuccess;
+    k_fill_descending<<<(n + 255) / 256, 256, 0, st>>>(d_out, n, top);
+    return cudaGetLastError();
 }
 
 }  // namespace lama_b200

@@ -183,7 +183,11 @@ struct RenderParams {
 };
 // mark pass -> allocation of the marked patches -> counting pass -> known bits of the touched patches
 void launch_render_scans(const StoreView& s, int set, const RenderParams& p, int n_scans, cudaStream_t st);
-// FrequencyOccupancyMap::prune over the whole map of particle 0
+// FrequencyOccupancyMap::prune over the patches in the window of particle 0's map
 void launch_prune_freq(const StoreView& s, int set, cudaStream_t st);
+// the same rule over the n entries of particle 0's parked occupancy list
+void launch_prune_freq_parked(const StoreView& s, const ParkView& pv, int n, cudaStream_t st);
+// out[i] = top - i, i in [0, n) (the new free slots of a grown pool)
+cudaError_t launch_fill_descending(int32_t* d_out, int n, int32_t top, cudaStream_t st);
 
 }  // namespace lama_b200
