@@ -529,6 +529,8 @@ int Engine::match(const SE2* states, int count, int first_particle, bool shared_
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(d_->h_results, d_->d_results, (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
+    // with parked entries a read outside the window sets kErrWindow (k_match reads it as absent): the caller must not get that result
+    if (mp.parked_any) CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     if (timing_) {
         float ms = 0;
@@ -536,6 +538,7 @@ int Engine::match(const SE2* states, int count, int first_particle, bool shared_
         times_.match_ms += ms;
     }
     times_.match_launches += 1;
+    if (mp.parked_any && *d_->h_status) return check_device_status();
     static_assert(sizeof(HostMatchResult) == sizeof(MatchResult), "layout");
     std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
     h2d_bytes_ += (uint64_t)count * sizeof(SE2);

@@ -510,6 +510,7 @@ void orc_lo_counters(void* h, uint64_t* out)
 void* orc_lo_occ_handle(void* h) { return &((LidarOdometry2D*)h)->occ; }
 void* orc_lo_dm_handle(void* h) { return &((LidarOdometry2D*)h)->dm; }
 uint64_t orc_slam_removed_patches(void* h) { return ((Slam2D*)h)->removed_patches; }
+uint64_t orc_slamp_removed_patches(void* h) { return ((Slam2DProb*)h)->removed_patches; }
 
 
 void orc_freq_query(void* d, const uint32_t* cells, int n, double* prob, uint8_t* flags) { occ_query(*(FrequencyOccupancyMap*)d, cells, n, prob, flags); }
