@@ -265,6 +265,8 @@ int lama_loc_global_localization_active(lama_loc* h, int* active);
 /* ------------------------------------------------------------------------------------------------
  * SDM grid interface on a device-resident DynamicDistanceMap
  * include/lama/sdm/distance_map.h:66-70, dynamic_distance_map.h:55-66
+ * By default the directory window (dev->dir_dim^2 patches) is fixed: cells outside it make a call fail with LAMA_ERR_WINDOW.  A
+ * following map (lama_dm_set_follow) moves the window instead, for lama_dm_read, lama_dm_update and a Loc2D on the map; see there.
  * ------------------------------------------------------------------------------------------------ */
 int lama_dm_create(double resolution, uint32_t patch_size, double l2_max, const double center_xy[2], const lama_device_options* dev, lama_dm** out);
 int lama_dm_destroy(lama_dm* dm);
@@ -285,6 +287,27 @@ int lama_dm_export(lama_dm* dm, uint32_t x0, uint32_t y0, int w, int hgt, uint16
 /* upload distance_t fields for a patch-aligned window (x0, y0, w, hgt multiples of 32); cells with known == 0 are left absent */
 int lama_dm_import(lama_dm* dm, uint32_t x0, uint32_t y0, int w, int hgt, const uint16_t* sqdist, const uint8_t* valid, const uint8_t* known,
                    const int16_t* ox, const int16_t* oy, const uint8_t* queued);
+/* follow != 0 (off by default; a Loc2D follows exactly when its lama_loc_distance_map does):
+ * - lama_dm_read loads a file of any size: the patches inside the window go into it, the others are parked (kept, and brought back
+ *   when the window returns).  distance, export, bounds, write, export_image and memory use see every patch.  With dev->pool_slots 0
+ *   the pool grows to hold the file; an explicit pool_slots is a hard cap: LAMA_ERR_POOL before anything is written.
+ * - lama_dm_update applies its list in chunks of one brushfire each (2 048 cells by default), in order, as a fixed map does.  Before a
+ *   chunk's brushfire the window moves to the one centred on the chunk's cells grown by the brushfire's reach (twice the map's reach in
+ *   cells) unless the current window holds them; cells and *processed are those of a window that never moves.  Every chunk is checked
+ *   first: one spanning more than dir_dim patches on an axis fails the call with LAMA_ERR_WINDOW and leaves the map untouched.  With
+ *   dev->pool_slots 0 the pool grows before a chunk until every patch the chunk can touch has a slot.
+ * - a Loc2D moves the window over each scan before it reads the map, and its global localisation scores its candidates over the whole
+ *   map in one launch; a map wider than 4 096 patches on an axis fails it with LAMA_ERR_WINDOW.
+ * lama_dm_import, lama_dm_match_normal_equations, lama_dm_match_solve, lama_dm_match_error and the lama_dm_*correlate_candidate_scan
+ * calls do not move the window: they are exact inside it and fail with LAMA_ERR_WINDOW when they reach a parked patch. */
+int lama_dm_set_follow(lama_dm* dm, int follow);
+/* the working window as lama_slam_get_window: base (patch coordinates), dir_dim, counts = {shifts, parked entries, entries restored} */
+int lama_dm_get_window(lama_dm* dm, int32_t base[2], int32_t* dim, uint64_t counts[3]);
+/* out = {pool slots, slots in use} */
+int lama_dm_get_pool(lama_dm* dm, uint64_t out[2]);
+/* with dev->timing: ms[0] = device time of the scan-match launches (a Loc2D's, including global localisation), ms[2] of the brushfires;
+ * launches as lama_slam_kernel_times */
+int lama_dm_kernel_times(lama_dm* dm, double ms[4], uint64_t launches[5]);
 
 /* Solver plug point: the weighted normal equations of MatchSurface2D at `count` SE2 states on one distance
  * map, so that a host nlls::Strategy (nlls/strategy.h:43-82) can drive the device evaluation.

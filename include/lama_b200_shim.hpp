@@ -64,6 +64,17 @@ inline MapWindow occupancyMapWindow(lama_om* m)
 }
 inline void occupancyMapPool(lama_om* m, uint64_t out[2]) { check(lama_om_get_pool(m, out)); }
 
+// a device DynamicDistanceMap (lama_dm, stand-alone or a Loc2D's distance_map()): following on or off (lama_dm_set_follow; a Loc2D
+// follows exactly when its distance map does), its working window and its pool {slots, slots in use}
+inline void distanceMapSetFollow(lama_dm* m, bool on) { check(lama_dm_set_follow(m, on ? 1 : 0)); }
+inline MapWindow distanceMapWindow(lama_dm* m)
+{
+    int32_t b[2], d = 0;
+    uint64_t c[3];
+    return map_window(lama_dm_get_window(m, b, &d, c), b, d, c);
+}
+inline void distanceMapPool(lama_dm* m, uint64_t out[2]) { check(lama_dm_get_pool(m, out)); }
+
 class PFSlam2D {
 public:
     using Options = lama_pf_options;
@@ -296,6 +307,9 @@ public:
     void triggerGlobalLocalization() { check(lama_loc_trigger_global_localization(h_)); }   // loc2d.cpp:194-197
     void readOccupancyMap(const std::string& path) { check(lama_loc_occupancy_read(h_, path.c_str())); }    // occupancy_map->read(path)
     void readDistanceMap(const std::string& path) { check(lama_dm_read(distance_map(), path.c_str())); }    // distance_map->read(path)
+    // following on or off, through the distance map (lama_dm_set_follow); turn it on before readDistanceMap for a map larger than the window
+    void setFollow(bool on) { distanceMapSetFollow(distance_map(), on); }
+    MapWindow window() { return distanceMapWindow(distance_map()); }
 
 private:
     lama_loc* h_ = nullptr;

@@ -83,6 +83,7 @@ EXPORTED_SYMBOLS = [
     "lama_loc_occupancy_set", "lama_loc_set_seed", "lama_loc_trigger_global_localization", "lama_loc_global_localization_active",
     "lama_dm_create", "lama_dm_destroy", "lama_dm_max_sqdist", "lama_dm_add_obstacles", "lama_dm_remove_obstacles", "lama_dm_update",
     "lama_dm_distance", "lama_dm_bounds", "lama_dm_export", "lama_dm_import", "lama_dm_match_normal_equations", "lama_dm_match_solve",
+    "lama_dm_set_follow", "lama_dm_get_window", "lama_dm_get_pool", "lama_dm_kernel_times",
     "lama_pgo_optimize_graph", "lama_graph_options_default", "lama_graph_create", "lama_graph_destroy", "lama_graph_set_pose", "lama_graph_update",
     "lama_graph_get_pose", "lama_graph_get_key_poses", "lama_graph_get_key_cloud", "lama_graph_get_links", "lama_graph_get_last_candidates",
     "lama_graph_get_stats", "lama_graph_slam", "lama_graph_generate_occupancy_map", "lama_graph_generate_coarse_distance_map",
@@ -1319,9 +1320,11 @@ def dm3_fields(words, known):
 
 
 class DynamicDistanceMap:
-    """Device-resident lama::DynamicDistanceMap (include/lama/sdm/dynamic_distance_map.h:55-66)."""
+    """Device-resident lama::DynamicDistanceMap (include/lama/sdm/dynamic_distance_map.h:55-66).  follow=True (setFollow): read()
+    loads a file of any size and update() moves the directory window over its obstacles instead of failing at the window's edge, and
+    with pool_slots 0 the pool grows (lama_dm_set_follow).  A Loc2D follows exactly when its distance_map does."""
 
-    def __init__(self, resolution=0.05, patch_size=32, l2_max=0.5, center=(0.0, 0.0), handle=None, owner=None, **dev):
+    def __init__(self, resolution=0.05, patch_size=32, l2_max=0.5, center=(0.0, 0.0), handle=None, owner=None, follow=False, **dev):
         self.owner = owner
         if handle is not None:
             self.h = handle
@@ -1334,6 +1337,8 @@ class DynamicDistanceMap:
         self.h = C.c_void_p()
         self.owned = True
         _chk(lib().lama_dm_create(C.c_double(resolution), C.c_uint32(patch_size), C.c_double(l2_max), cp, C.byref(d), C.byref(self.h)))
+        if follow:
+            self.setFollow(True)
 
     def __del__(self):
         if getattr(self, "owned", False) and getattr(self, "h", None) and _lib is not None:
@@ -1390,6 +1395,22 @@ class DynamicDistanceMap:
 
     def exportImage(self):
         return _image(lib().lama_dm_export_image, (self.h,))
+
+    def setFollow(self, on=True):
+        _chk(lib().lama_dm_set_follow(self.h, C.c_int(1 if on else 0)))
+
+    def window(self):
+        """The working window: base (patch coordinates), dim (dir_dim), shifts so far, entries parked now, entries restored so far."""
+        return _window(lib().lama_dm_get_window, self.h)
+
+    def pool(self):
+        """(pool slots, slots in use)"""
+        out = np.zeros(2, np.uint64)
+        _chk(lib().lama_dm_get_pool(self.h, _vp(out)))
+        return int(out[0]), int(out[1])
+
+    def kernelTimes(self):
+        return _times(lib().lama_dm_kernel_times, self.h)
 
     def matchNormalEquations(self, pts, states, robust=(1, 0.15), meas_sigma=0.05, origin=_ID3, quat=_IDQ):
         p, pp = _d(pts)

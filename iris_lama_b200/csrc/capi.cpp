@@ -3,6 +3,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <map>
 #include <new>
 #include <stdexcept>
 #include <string>
@@ -12,6 +13,7 @@
 // headers must come first.
 #include "checkpoint.h"
 #include "frontend.h"
+#include "render_plan.h"
 #include "sdm_io.h"
 #include "shard_comm.h"
 #include "pgo.h"
@@ -884,6 +886,80 @@ try {
     return export_image(dm->d->engine(), 0, 1, false, pixels, cap, dims);
 }
 LAMA_CATCH
+// The packed cell holds 12 bits of sqdist and 7-bit offsets, and the scan matcher's distance table has max_sqdist + 1 entries:
+// a cell outside those ranges would be stored truncated, or read past the table.  The reference keeps every valid cell below
+// max_sqdist (an obstacle's wave stops there).  An empty string: the known cell can be stored.
+static std::string dm_cell_problem(uint32_t max_sqdist, uint16_t sqdist, bool valid, int ox, int oy)
+{
+    if (sqdist > kDmSqMask || (valid && sqdist >= max_sqdist))
+        return "has sqdist " + std::to_string(sqdist) + " (valid cells stay below max_sqdist " + std::to_string(max_sqdist) + ")";
+    if (ox < -64 || ox > 63 || oy < -64 || oy > 63) return "has an obstacle offset outside [-64, 63]";
+    return std::string();
+}
+
+// Map::read of a file larger than the window, into a following map: every cell is checked and the pool sized first, then the file
+// goes in one window-sized tile at a time, each through lama_dm_import with the window moved over it, and the window returns to
+// where it was.  The patches outside it end up parked (Engine::shift_window), as if the map had been built there.
+static int read_following(lama_dm* dm, const SdmFile& f)
+{
+    constexpr size_t kMaskWords = kPatchCells / 64;   // mask words of one patch in SdmFile::masks
+    Engine* e = dm->d->engine();
+    const uint32_t max_sqdist = e->max_sqdist();
+    for (size_t i = 0; i < f.ids.size(); ++i) {
+        const SdmDistanceCell* c = reinterpret_cast<const SdmDistanceCell*>(f.cells.data() + i * (size_t)kPatchCells * sizeof(SdmDistanceCell));
+        const uint64_t* mask = f.masks.data() + i * kMaskWords;
+        for (uint32_t ci = 0; ci < (uint32_t)kPatchCells; ++ci) {
+            if (!((mask[ci >> 6] >> (ci & 63)) & 1ull)) continue;
+            const std::string why = dm_cell_problem(max_sqdist, c[ci].sqdist, c[ci].valid_obstacle != 0, c[ci].obstacle[0], c[ci].obstacle[1]);
+            if (!why.empty()) return set_err("lama_dm_read: cell " + std::to_string(ci) + " of patch " + std::to_string(i) + " " + why, LAMA_ERR_ARG);
+        }
+    }
+    uint64_t pool[2];
+    int rc = e->pool_info(pool);
+    if (rc != LAMA_OK) return set_err(e->last_error(), rc);
+    const int64_t n_file = (int64_t)f.ids.size();
+    if ((int64_t)pool[0] - (int64_t)pool[1] < n_file) {   // every patch of the file may need a slot
+        if (!e->pool_grows())
+            return set_err("lama_dm_read: the file's " + std::to_string(n_file) + " patches do not fit the " + std::to_string(pool[0] - pool[1]) +
+                               " free slots of the pool (pool_slots)",
+                           LAMA_ERR_POOL);
+        const int64_t want = pool_growth((int64_t)pool[0], (int64_t)pool[1], n_file, true);
+        if (want - (int64_t)pool[1] < n_file) return set_err("lama_dm_read: the file has more patches than the largest pool holds", LAMA_ERR_POOL);
+        rc = e->grow_pool((int)want);
+        if (rc != LAMA_OK) return set_err(e->last_error(), rc);
+    }
+    // tiles of dim x dim patches on a grid anchored at patch 0, in (y, x) order
+    const DirWindow w0 = e->window();
+    const int64_t dim = w0.dim, max_base = ((int64_t)1 << (32 - kPatchLog2)) - dim;
+    std::map<std::pair<int64_t, int64_t>, std::vector<size_t>> tiles;
+    for (size_t i = 0; i < f.ids.size(); ++i) {
+        const int64_t px = (int64_t)(f.ids[i] / kUniversalConstant), py = (int64_t)(f.ids[i] % kUniversalConstant);
+        tiles[{std::min(py / dim * dim, max_base), std::min(px / dim * dim, max_base)}].push_back(i);
+    }
+    for (const auto& t : tiles) {
+        rc = e->shift_window((int32_t)t.first.second, (int32_t)t.first.first);
+        if (rc != LAMA_OK) return set_err(e->last_error(), rc);
+        SdmFile sub;
+        sub.header = f.header;
+        for (size_t i : t.second) {
+            sub.ids.push_back(f.ids[i]);
+            const size_t cb = (size_t)kPatchCells * sizeof(SdmDistanceCell);
+            sub.cells.insert(sub.cells.end(), f.cells.begin() + i * cb, f.cells.begin() + (i + 1) * cb);
+            sub.masks.insert(sub.masks.end(), f.masks.begin() + i * kMaskWords, f.masks.begin() + (i + 1) * kMaskWords);
+        }
+        SdmWindow win;
+        sdm_window_of(sub, win);
+        DmPlanes p;
+        const size_t cells = (size_t)win.w * win.h;
+        p.sqdist.resize(cells); p.valid.resize(cells); p.known.resize(cells); p.queued.resize(cells); p.ox.resize(cells); p.oy.resize(cells);
+        sdm_to_distance(sub, win, p.sqdist.data(), p.valid.data(), p.known.data(), p.ox.data(), p.oy.data(), p.queued.data());
+        rc = lama_dm_import(dm, win.x0, win.y0, win.w, win.h, p.sqdist.data(), p.valid.data(), p.known.data(), p.ox.data(), p.oy.data(), p.queued.data());
+        if (rc != LAMA_OK) return rc;
+    }
+    rc = e->shift_window(w0.base_px, w0.base_py);
+    return rc == LAMA_OK ? rc : set_err(e->last_error(), rc);
+}
+
 // Map::read into an EMPTY device distance map (map.cpp:531-575).  The file must have been written at this map's
 // resolution and maximum distance (the reference adopts the file's values; the device map's are fixed at creation).
 int lama_dm_read(lama_dm* dm, const char* path)
@@ -902,8 +978,10 @@ try {
     {   // the patch ids come from the file: the window they span must lie inside this map's directory window before it is sized
         const DirWindow dw = e->window();
         const int64_t px0 = (int64_t)(win.x0 >> kPatchLog2) - dw.base_px, py0 = (int64_t)(win.y0 >> kPatchLog2) - dw.base_py;
-        if (px0 < 0 || py0 < 0 || px0 + (win.w >> kPatchLog2) > dw.dim || py0 + (win.h >> kPatchLog2) > dw.dim)
+        if (px0 < 0 || py0 < 0 || px0 + (win.w >> kPatchLog2) > dw.dim || py0 + (win.h >> kPatchLog2) > dw.dim) {
+            if (e->follows()) return read_following(dm, f);
             return set_err("the file's patches lie outside this map's directory window", LAMA_ERR_WINDOW);
+        }
     }
     DmPlanes p;
     const size_t cells = (size_t)win.w * win.h;
@@ -916,18 +994,11 @@ int lama_dm_import(lama_dm* dm, uint32_t x0, uint32_t y0, int w, int hgt, const 
                    const int16_t* ox, const int16_t* oy, const uint8_t* queued)
 try {
     if (!dm || !sqdist || !valid || !known) return set_err("null argument", LAMA_ERR_ARG);
-    // The packed cell holds 12 bits of sqdist and 7-bit offsets, and the scan matcher's distance table has max_sqdist + 1 entries:
-    // a cell outside those ranges would be stored truncated, or read past the table.  The reference keeps every valid cell below
-    // max_sqdist (an obstacle's wave stops there).
     const uint32_t max_sqdist = dm->d->engine()->max_sqdist();
     for (size_t i = 0; i < (size_t)w * hgt; ++i) {
         if (!known[i]) continue;
-        if (sqdist[i] > kDmSqMask || (valid[i] && sqdist[i] >= max_sqdist))
-            return set_err("lama_dm_import: cell " + std::to_string(i) + " has sqdist " + std::to_string(sqdist[i]) + " (valid cells stay below max_sqdist " +
-                               std::to_string(max_sqdist) + ")",
-                           LAMA_ERR_ARG);
-        if ((ox && (ox[i] < -64 || ox[i] > 63)) || (oy && (oy[i] < -64 || oy[i] > 63)))
-            return set_err("lama_dm_import: cell " + std::to_string(i) + " has an obstacle offset outside [-64, 63]", LAMA_ERR_ARG);
+        const std::string why = dm_cell_problem(max_sqdist, sqdist[i], valid[i] != 0, ox ? ox[i] : 0, oy ? oy[i] : 0);
+        if (!why.empty()) return set_err("lama_dm_import: cell " + std::to_string(i) + " " + why, LAMA_ERR_ARG);
     }
     std::vector<uint32_t> words((size_t)w * hgt);
     for (size_t i = 0; i < words.size(); ++i) {
@@ -936,6 +1007,32 @@ try {
     }
     int rc = dm->d->engine()->import_window(0, 1, x0, y0, w, hgt, words.data());
     return rc == LAMA_OK ? rc : set_err(dm->d->engine()->last_error(), rc);
+}
+LAMA_CATCH
+int lama_dm_set_follow(lama_dm* dm, int follow)
+try {
+    if (!dm) return set_err("null handle", LAMA_ERR_ARG);
+    dm->d->set_follow(follow != 0);
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_dm_get_window(lama_dm* dm, int32_t base[2], int32_t* dim, uint64_t counts[3])
+try {
+    if (!dm) return set_err("null handle", LAMA_ERR_ARG);
+    return window_out(dm->d->engine(), base, dim, counts);
+}
+LAMA_CATCH
+int lama_dm_get_pool(lama_dm* dm, uint64_t out[2])
+try {
+    if (!dm || !out) return set_err("null argument", LAMA_ERR_ARG);
+    const int rc = dm->d->engine()->pool_info(out);
+    return rc == LAMA_OK ? rc : set_err(dm->d->engine()->last_error(), rc);
+}
+LAMA_CATCH
+int lama_dm_kernel_times(lama_dm* dm, double ms[4], uint64_t launches[5])
+try {
+    if (!dm) return set_err("null handle", LAMA_ERR_ARG);
+    return times_out(dm->d->engine(), ms, launches);
 }
 LAMA_CATCH
 int lama_dm_match_normal_equations(lama_dm* dm, const double* pts, int n, const double* origin, const double* quat, const double* states, int count,

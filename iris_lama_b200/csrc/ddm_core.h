@@ -79,6 +79,13 @@ LAMA_HD uint64_t heap_pop(Heap& h)
     return top;
 }
 
+// How far from the cells of its batch one update() reaches, in cells on each axis, with R = ceil(l2_max * scale), the reach of the map
+// (a valid cell lies less than R from its obstacle, so at most R - 1 on each axis).  On a map that update() left consistent, every cell
+// it writes or queues lies within R of a batch cell: the cells of an added obstacle, the cells whose removed obstacle raise() clears,
+// and the neighbours of those.  lower() and raise() also read the obstacle of the cells they visit and of their neighbours (one more
+// cell out), which lie up to R - 1 further: 2R covers every cell one update() touches.
+LAMA_HD uint32_t brushfire_reach(uint32_t radius) { return 2 * radius; }
+
 // Map policy requirements:
 //   uint32_t* cell(uint32_t x, uint32_t y)  -- the MUTABLE Map::get (map.cpp:371-412): allocates the
 //        patch on first touch, detaches a shared patch, marks the cell known; never returns null

@@ -7,6 +7,7 @@
 #include <cstring>
 #include <memory>
 
+#include "dm_follow.h"
 #include "kernels.cuh"
 #include "render_plan.h"
 
@@ -63,6 +64,9 @@ struct Engine::Impl {
     // scratch of shift_window, apart from d_scratch: a following render shifts the window between groups while its scans sit in d_scratch
     void* d_shift_scratch = nullptr;
     size_t shift_scratch_bytes = 0;
+    // the dense directory of match_extent (Engine::extent_)
+    void* d_extent = nullptr;
+    size_t extent_bytes = 0;
     // device arena of a migration round (pack_device / migration_alloc): bump allocation out of chunks that are kept between rounds, so that a resampling
     // scan costs no cudaMalloc / cudaFree once the arena has grown to its working size
     std::vector<std::pair<char*, size_t>> mig_chunks;
@@ -364,6 +368,7 @@ Engine::~Engine()
     if (d_->h_status) cudaFreeHost(d_->h_status);
     if (d_->d_scratch) cudaFree(d_->d_scratch);
     if (d_->d_shift_scratch) cudaFree(d_->d_shift_scratch);
+    if (d_->d_extent) cudaFree(d_->d_extent);
     if (d_->d_staged) cudaFree(d_->d_staged);
     for (int b = 0; b < 2; ++b)
         for (int k = 0; k < 4; ++k)
@@ -584,6 +589,7 @@ static int brush_debug_flag()
 // synchronises, collects the per-particle statistics and surfaces device errors.
 int Engine::update_maps_async(const SE2* states, int first_particle, int count)
 {
+    extent_stale_ = true;
     if (count < 1 || first_particle < 0 || first_particle + count > cfg_.particles) return fail("update_maps: particle range out of bounds", LAMA_ERR_ARG);
     if (d_->scan.n_beams < 1) return fail("update_maps: no scan uploaded", LAMA_ERR_STATE);
     { int rc = settle(nullptr); if (rc != LAMA_OK) return rc; }
@@ -642,6 +648,7 @@ int Engine::step_enqueue(const double* pts, int n, const double origin[3], const
                          const SE2* predicted, int count, const SolverOptions& so, double meas_sigma)
 {
     if (count < 1 || count > cfg_.particles) return fail("step_enqueue: particle range out of bounds", LAMA_ERR_ARG);
+    extent_stale_ = true;
     CU_TRY(cudaSetDevice(cfg_.device));
     // the previous scan's map update may still be running: nothing below waits for it on the host
     enq_had_pending_ = pending_maps_ != 0;
@@ -793,6 +800,7 @@ int Engine::settle(HostMapStats* out, bool already_complete)
 int Engine::share_from(int src_particle, int dst_first, int count)
 {
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
+    extent_stale_ = true;
     if (count == 0) return LAMA_OK;
     if (src_particle < 0 || src_particle >= cfg_.particles || dst_first < 0 || dst_first + count > cfg_.particles ||
         (src_particle >= dst_first && src_particle < dst_first + count))
@@ -813,6 +821,7 @@ int Engine::share_from(int src_particle, int dst_first, int count)
 int Engine::resample(const int32_t* idx)
 {
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
+    extent_stale_ = true;
     CU_TRY(cudaSetDevice(cfg_.device));
     const int P = cfg_.particles;
     for (int i = 0; i < P; ++i) {
@@ -952,6 +961,7 @@ int Engine::render_scans(const double* pts, const int64_t* offsets, int n_scans,
     if (cells) *cells = 0;
     if (n_scans == 0) return LAMA_OK;
     if (offsets[0] != 0) return fail("render_scans: offsets[0] must be 0", LAMA_ERR_ARG);
+    extent_stale_ = true;
     for (int k = 0; k < n_scans; ++k)
         if (offsets[k + 1] < offsets[k]) return fail("render_scans: offsets must not decrease", LAMA_ERR_ARG);
     const int64_t n_pts = offsets[n_scans];
@@ -1127,6 +1137,7 @@ int Engine::prune_frequency()
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
     if (!d_->view.kbits || cfg_.occupancy_kind != 0) return fail("prune_frequency: needs a frequency map with a known plane", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
+    extent_stale_ = true;
     launch_prune_freq(d_->view, cur_set_, d_->stream);
     const int n_parked = d_->park_ol[cur_set_][kMapOcc].y;   // particle 0's occupancy list
     if (n_parked) launch_prune_freq_parked(d_->view, d_->pv(cur_set_), n_parked, d_->stream);
@@ -1144,12 +1155,43 @@ int Engine::dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_a
     CU_TRY(cudaSetDevice(cfg_.device));
     uint32_t total = 0;
     const int cap = d_->ray.event_cap;
+    // A following map runs each chunk's brushfire in a window that holds every cell it touches (dm_follow.h); every chunk is checked
+    // before the first brushfire.  A fixed map runs every chunk in its window and refuses a cell outside it.
+    std::vector<CellBox> boxes;
+    std::vector<RenderGroup> groups;
+    if (follow_ && n > 0) {
+        const uint32_t reach = brushfire_reach((uint32_t)std::lround(std::sqrt((double)max_sqdist_)));
+        const int bad = plan_dm_chunks(window_, cells_xy, n, cap, reach, boxes, groups);
+        if (bad >= 0)
+            return fail("dm_apply: cells " + std::to_string((int64_t)bad * cap) + " .. " + std::to_string(std::min<int64_t>(((int64_t)bad + 1) * cap, n) - 1) +
+                            " of the list, grown by the brushfire's reach of " + std::to_string(reach) + " cells, span more than one directory window (" +
+                            std::to_string(cfg_.dir_dim) + " x " + std::to_string(cfg_.dir_dim) + " patches)",
+                        LAMA_ERR_WINDOW);
+    }
+    extent_stale_ = true;
     std::vector<uint64_t> ev;
     int done = 0;
+    size_t g = 0;
     do {  // One brushfire over the whole list reproduces the reference (all cells queued, then ONE update()).  Lists longer than the
           // per-particle event buffer (2 048 cells) are applied in pieces with a brushfire after each, which gives a valid distance map but not necessarily the
           // reference's tie order -- big maps are loaded with lama_dm_read / lama_dm_import instead (DESIGN.md 10).
         int m = std::min(cap, n - done);
+        if (!groups.empty()) {   // following: this chunk's window and, with a growing pool, a slot for every patch of its box
+            const int chunk = done / cap;
+            while (chunk >= groups[g].first + groups[g].count) ++g;
+            const DirWindow& w = groups[g].window;
+            if (w.base_px != window_.base_px || w.base_py != window_.base_py) {
+                const int rc = shift_window(w.base_px, w.base_py);
+                if (rc != LAMA_OK) return rc;
+            }
+            if (grow_) {
+                uint64_t pool[2];
+                int rc = pool_info(pool);
+                const int64_t want = pool_growth((int64_t)pool[0], (int64_t)pool[1], box_patches(boxes[(size_t)chunk]), true);
+                if (rc == LAMA_OK && want != (int64_t)pool[0]) rc = grow_pool((int)want);
+                if (rc != LAMA_OK) return rc;
+            }
+        }
         ev.resize((size_t)std::max(m, 1));
         for (int i = 0; i < m; ++i) {
             uint32_t x = cells_xy[2 * (done + i)], y = cells_xy[2 * (done + i) + 1];
@@ -1179,6 +1221,62 @@ int Engine::dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_a
         if (rc != LAMA_OK) return rc;
     } while (done < n);
     if (processed) *processed = total;
+    return LAMA_OK;
+}
+
+int Engine::match_extent(const SE2* states, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out)
+{
+    { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
+    if (count < 1) return fail("match_extent: no states", LAMA_ERR_ARG);
+    if (d_->scan.n_beams < 1) return fail("match_extent: no scan uploaded", LAMA_ERR_STATE);
+    CU_TRY(cudaSetDevice(cfg_.device));
+    if (extent_stale_) {   // a shift moves entries between the window and the parked list, never between slots: it keeps the directory
+        uint32_t mn[2], mx[2];
+        const int n_patches = bounds(0, kMapDm, mn, mx);
+        if (n_patches < 0) return fail("match_extent: reading the map's bounds failed", LAMA_ERR_CUDA);
+        DirWindow xw{0, 0, 0};   // dim 0: no patch, every cell reads as absent
+        if (extent_window(mn, mx, n_patches, &xw) < 0)
+            return fail("match_extent: the map spans more than " + std::to_string(kExtentMaxPatches) + " patches on an axis", LAMA_ERR_WINDOW);
+        if (xw.dim) {
+            const size_t bytes = (size_t)xw.dim * xw.dim * 4;
+            if (ensure_buffer(&d_->d_extent, &d_->extent_bytes, bytes)) return fail("match_extent: out of device memory", LAMA_ERR_CUDA);
+            CU_TRY(cudaMemsetAsync(d_->d_extent, 0xFF, bytes, d_->stream));
+            launch_extent_dir(d_->view, d_->pv(cur_set_), cur_set_, xw, d_->park_ol[cur_set_][kMapDm].y, (int32_t*)d_->d_extent, d_->stream);
+            CU_TRY(cudaGetLastError());
+            times_.misc_launches += 1;
+        }
+        extent_ = xw;
+        extent_stale_ = false;
+    }
+    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
+    std::memcpy(d_->h_states, states, (size_t)count * sizeof(SE2));
+    CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d_->stream));
+    MatchParams mp{};
+    mp.points = d_->d_points;
+    mp.scan = d_->scan;
+    mp.solver = so;
+    mp.meas_sigma = meas_sigma;
+    mp.resolution = cfg_.resolution;
+    mp.max_sqdist = max_sqdist_;
+    mp.set = cur_set_;
+    mp.particle_offset = 0;
+    mp.shared_map = 1;
+    mp.mode = 1;
+    if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
+    launch_match_extent(d_->view, mp, (const int32_t*)d_->d_extent, extent_, d_->d_states, d_->d_results, count, d_->stream);
+    if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(d_->h_results, d_->d_results, (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaStreamSynchronize(d_->stream));
+    if (timing_) {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, d_->ev[0], d_->ev[1]);
+        times_.match_ms += ms;
+    }
+    times_.match_launches += 1;
+    std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
+    h2d_bytes_ += (uint64_t)count * sizeof(SE2);
+    d2h_bytes_ += (uint64_t)count * sizeof(MatchResult);
     return LAMA_OK;
 }
 
@@ -1276,6 +1374,7 @@ int Engine::import_window(int particle, int kind, uint32_t x0, uint32_t y0, int 
     if (particle < 0 || particle >= cfg_.particles || kind < 0 || kind > 1 || w < 1 || h < 1 || (x0 | y0 | (uint32_t)w | (uint32_t)h) % kPatchLen)
         return fail("import_window: window must be patch aligned", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
+    extent_stale_ = true;
     const size_t bw = (size_t)w * h * 4;
     if (ensure_scratch(d_, bw)) return fail("import_window: out of device memory", LAMA_ERR_CUDA);
     CU_TRY(cudaMemcpyAsync(d_->d_scratch, words, bw, cudaMemcpyHostToDevice, d_->stream));
@@ -1380,6 +1479,7 @@ int Engine::pack_device(int particle, DeviceBlob* out)
 int Engine::unpack_device(int particle, const DeviceBlob& blob, bool check)
 {
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
+    extent_stale_ = true;
     const size_t n = (size_t)blob.n_occ + blob.n_dm, ne = blob_entry_bytes(n);
     if (particle < 0 || particle >= cfg_.particles || blob.bytes < ne + n * (size_t)(kPatchBytes + 128)) return fail("unpack: bad arguments", LAMA_ERR_ARG);
     if (has_parked(particle)) return fail("unpack: the slot's maps have parked entries (the window has moved)", LAMA_ERR_STATE);
@@ -1427,6 +1527,7 @@ int Engine::pack(int particle, void* buf, size_t cap, size_t* used)
 int Engine::unpack(int particle, const void* buf, size_t bytes)
 {
     if (particle < 0 || particle >= cfg_.particles || bytes < 16) return fail("unpack: bad arguments", LAMA_ERR_ARG);
+    extent_stale_ = true;
     const uint32_t* hdr = (const uint32_t*)buf;
     if (hdr[0] != kPackMagic || hdr[1] != pack_window_word(cfg_.dir_dim, window_)) return fail("unpack: incompatible buffer (directory window differs)", LAMA_ERR_ARG);
     DeviceBlob blob;
@@ -1451,6 +1552,7 @@ int Engine::prune_outside(int particle, const double center[2], const double hwi
     { int rc = settle(nullptr); if (rc != LAMA_OK) return rc; }
     if (particle < 0 || particle >= cfg_.particles) return fail("prune_outside: no such particle", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
+    extent_stale_ = true;
     const size_t dim2 = (size_t)cfg_.dir_dim * cfg_.dir_dim;
     std::vector<int32_t> dirs(2 * dim2);   // kinds 0 (occupancy) and 1 (distance) are adjacent
     const int32_t* src = d_->view.dirs + (((size_t)cur_set_ * cfg_.particles + particle) * d_->view.n_kinds) * dim2;

@@ -165,11 +165,13 @@ public:
                      uint64_t* cells);
     // FrequencyOccupancyMap::prune (frequency_occupancy_map.cpp:149-158) of particle 0's map, parked patches included
     int prune_frequency();
-    // Following renders (off by default): render_scans splits its scans into consecutive groups that each fit one window
-    // (render_plan.h), moves the window to each group's window with shift_window and, with `grow`, grows the pool before a group
-    // until it holds the parked entries and a whole window (pool_growth).  A scan no window holds is refused before anything is written.
-    void set_render_follow(bool follow, bool grow) { follow_ = follow; grow_ = follow && grow; }
-    bool render_follow() const { return follow_; }
+    // Following (off by default).  render_scans splits its scans into consecutive groups that each fit one window (render_plan.h),
+    // moves the window to each group's window with shift_window and, with `grow`, grows the pool before a group until it holds the
+    // parked entries and a whole window (pool_growth).  dm_apply does the same with its chunks (dm_follow.h) and, with `grow`, grows
+    // the pool before a chunk until every patch of the chunk's box has a slot.  A scan or chunk no window holds is refused before
+    // anything is written.
+    void set_follow(bool follow, bool grow) { follow_ = follow; grow_ = follow && grow; }
+    bool follows() const { return follow_; }
     bool pool_grows() const { return grow_; }
     // A larger pool for a one-particle engine: the slots in use keep their ids, contents, bits and reference counts, the new slots
     // are free.  Allocates everything first; on failure the engine is unchanged (LAMA_ERR_CUDA, or LAMA_ERR_POOL past the 24-bit cap).
@@ -180,6 +182,10 @@ public:
 
     // Direct DynamicDistanceMap::addObstacle / removeObstacle calls in list order, then update().
     int dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_add, int n, uint32_t* processed);
+    // Single evaluations (match mode 1) of `count` states on particle 0's distance map, parked patches included: k_match_extent reads
+    // a dense directory over every allocated patch (k_extent_dir), built when a call allocated or deleted patches since the last one.
+    // One k_match_extent launch; a map wider than kExtentMaxPatches patches is refused with LAMA_ERR_WINDOW before any launch.
+    int match_extent(const SE2* states, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out);
     // Likelihoods of Loc2D::addSamplingCovariance for n offsets (x, y pairs) around `pose` on the current scan.
     int sampling_likelihood(int particle, const SE2& pose, const double* offsets_xy, int n, int stride, double* out);
     // Batched DistanceMap::distance(p, &grad).
@@ -260,6 +266,8 @@ private:
     uint64_t h2d_bytes_ = 0, d2h_bytes_ = 0;
     bool follow_ = false, grow_ = false;
     uint64_t pool_growths_ = 0;
+    bool extent_stale_ = true;            // a patch was allocated or deleted since match_extent built its directory
+    DirWindow extent_{};                  // that directory's window (dim 0: the map had no patch)
     int pending_maps_ = 0;
     int pending_buf_ = 0;                 // which half of the ping-pong host buffers the pending map update reports into
     uint64_t settled_counters_[4] = {0, 0, 0, 0};

@@ -52,13 +52,17 @@ static EngineConfig engine_config(const DeviceOptions& dev, int particles, doubl
 static double xy_norm(const SE2& s) { return std::sqrt(s.tx * s.tx + s.ty * s.ty); }
 
 // Before an update of `count` particles at predicted poses `poses`: moves the engine's window so that every cell the update can touch
-// lies inside it (window_guard.h), or leaves it where it is when no window holds that box
-static int follow_window(Engine* e, const SE2* poses, int count, const double* origin, const double* quat, const double* pts, int n)
+// lies inside it (window_guard.h), or leaves it where it is when no window holds that box.  `grow` (m) widens the box on every side.
+static int follow_window(Engine* e, const SE2* poses, int count, const double* origin, const double* quat, const double* pts, int n, double grow = 0.0)
 {
     const EngineConfig& c = e->config();
     const uint32_t reach = (uint32_t)std::lround(std::sqrt((double)e->max_sqdist()));
     double mn[2], mx[2];
     guard_box(poses, count, moving_tf(origin, quat), pts, n, c.resolution, reach, mn, mx);
+    for (int k = 0; k < 2; ++k) {
+        mn[k] -= grow;
+        mx[k] += grow;
+    }
     const double robot[2] = {poses[0].tx, poses[0].ty};
     int32_t base[2];
     if (window_guard(e->window(), mn, mx, robot, 1.0 / c.resolution, base) != kGuardShift) return LAMA_OK;
@@ -1287,6 +1291,7 @@ DistanceMapDev* DistanceMapDev::create(double resolution, uint32_t patch_size, d
     if (!en) return nullptr;
     DistanceMapDev* d = new DistanceMapDev();
     d->eng_.reset(en);
+    d->growable_ = dev.pool_slots <= 0;
     en->enable_timing(dev.timing != 0);
     return d;
 }
@@ -1416,6 +1421,9 @@ Loc2D* Loc2D::create(const LocOptions& o, std::string& err)
 // Loc2D::globalLocalization (loc2d.cpp:249-286): candidates are drawn on the host with the reference's rejection
 // sampling (same generator calls in the same order), evaluated in ONE device launch (the same evaluation kernel as
 // scan matching, every block on the same map) and the best is chosen with the reference's strict `<` in index order.
+// The candidates cover the whole SimpleOccupancyMap, which has no window.  When the distance map follows and has parked patches the
+// launch is k_match_extent, which reads every patch (Engine::match_extent).  With nothing parked every patch is in the window, and
+// k_match reads a cell outside it as absent, as the reference's const get does.
 int Loc2D::global_localization(int n)
 {
     double mn[2], mx[2];
@@ -1436,8 +1444,10 @@ int Loc2D::global_localization(int n)
     }
     std::vector<HostMatchResult> res(cand.size());
     SolverOptions so = make_solver(0, 0);
-    int rc = dm_->engine()->match(cand.data(), (int)cand.size(), 0, true, so, 0.05, 1, res.data());
-    if (rc != LAMA_OK) { err_ = dm_->engine()->last_error(); return rc; }
+    Engine* eng = dm_->engine();
+    int rc = eng->follows() && eng->has_parked() ? eng->match_extent(cand.data(), (int)cand.size(), so, 0.05, res.data())
+                                                 : eng->match(cand.data(), (int)cand.size(), 0, true, so, 0.05, 1, res.data());
+    if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
     double best = std::numeric_limits<double>::max();
     for (size_t i = 0; i < cand.size(); ++i)
         if (res[i].sums[10] < best) {  // residuals.squaredNorm()
@@ -1448,13 +1458,26 @@ int Loc2D::global_localization(int n)
     return LAMA_OK;
 }
 
+// A Loc2D follows exactly when its distance map does: before a device read at pose_, the window moves over the guarded box of the scan
+// at pose_ (window_guard.h), grown by the reach of the sampling covariance's offsets (20 steps of one resolution, Loc2D::create).  On a
+// static map a shift only moves directory entries to and from the parked lists.
+int Loc2D::follow(const double* pts, int n, const double* origin, const double* quat)
+{
+    Engine* eng = dm_->engine();
+    if (!eng->follows()) return LAMA_OK;
+    const int rc = follow_window(eng, &pose_, 1, origin, quat, pts, n, 20.0 * opt_.resolution);
+    if (rc != LAMA_OK) err_ = eng->last_error();
+    return rc;
+}
+
 // Loc2D::addSamplingCovariance (loc2d.cpp:199-247)
-int Loc2D::add_sampling_covariance(int n)
+int Loc2D::add_sampling_covariance(const double* pts, int n, const double* origin, const double* quat)
 {
     const int n_off = (int)(sampling_steps_.size() / 2);
     const int stride = (int)std::max((size_t)n / 100, (size_t)1);
     std::vector<double> l((size_t)n_off);
-    int rc = dm_->engine()->sampling_likelihood(0, pose_, sampling_steps_.data(), n_off, stride, l.data());
+    int rc = follow(pts, n, origin, quat);
+    if (rc == LAMA_OK) rc = dm_->engine()->sampling_likelihood(0, pose_, sampling_steps_.data(), n_off, stride, l.data());
     if (rc != LAMA_OK) { err_ = dm_->engine()->last_error(); return rc; }
     double K[4] = {0, 0, 0, 0}, u[2] = {0, 0}, sl = 0;
     for (int i = 0; i < n_off; ++i) {
@@ -1488,7 +1511,8 @@ int Loc2D::update(const double* pts, int n, const double* origin, const double* 
         if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
         scan_set = true;
         HostMatchResult r;
-        rc = eng->match(&pose_, 1, 0, false, so, 0.05, 1, &r);
+        rc = follow(pts, n, origin, quat);
+        if (rc == LAMA_OK) rc = eng->match(&pose_, 1, 0, false, so, 0.05, 1, &r);
         if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
         rmse_ = std::sqrt(r.sums[10] / ((double)((size_t)n - 1)));
     }
@@ -1513,14 +1537,15 @@ int Loc2D::update(const double* pts, int n, const double* origin, const double* 
         }
     }
     HostMatchResult r;
-    rc = eng->match(&pose_, 1, 0, false, so, 0.05, 0, &r);
+    rc = follow(pts, n, origin, quat);
+    if (rc == LAMA_OK) rc = eng->match(&pose_, 1, 0, false, so, 0.05, 0, &r);
     if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
     pose_  = r.state;
     iters_ = r.iterations;
     evals_ = r.evals_ref + 2;  // + the covariance and rmse evaluations of solver.cpp:110 / loc2d.cpp:178
     covariance_from_sums(r.sums, (size_t)n, cov_);
     if (cov_blend_ > 0.0) {     // loc2d.cpp:175-176
-        rc = add_sampling_covariance(n);
+        rc = add_sampling_covariance(pts, n, origin, quat);
         if (rc != LAMA_OK) return rc;
     }
     rmse_ = std::sqrt(r.sums[10] / ((double)((size_t)n - 1)));  // loc2d.cpp:178-180

@@ -241,12 +241,17 @@ public:
     Engine* engine() { return eng_.get(); }
     const std::string& error() const { return err_; }
     int flush_if_pending();
+    // Following (off by default): update() moves the window over each chunk of its list (Engine::dm_apply), a file of any size can be
+    // read, and a Loc2D on this map moves the window with the robot and localises globally over the whole map; a map created with an
+    // automatic pool (dev.pool_slots 0) grows it
+    void set_follow(bool on) { eng_->set_follow(on, growable_); }
 
 private:
     std::unique_ptr<Engine> eng_;
     std::vector<uint32_t> pend_cells_;
     std::vector<uint8_t> pend_kind_;
     std::string err_;
+    bool growable_ = true;
 };
 
 // ---- device FrequencyOccupancyMap that keeps its own known plane: GraphSlam2D's global map ---------------------------------------------
@@ -258,9 +263,9 @@ public:
                                    int start_slots = 0);
     // a map around a restored engine (one particle, frequency, known plane); takes ownership.  `growable`: dev.pool_slots was 0
     static OccupancyMapDev* adopt(Engine* e, bool growable = true);
-    // Following (off by default): each insert_scans moves the window over its scans group by group (Engine::set_render_follow), and a
+    // Following (off by default): each insert_scans moves the window over its scans group by group (Engine::set_follow), and a
     // map created with an automatic pool grows it
-    void set_follow(bool on) { eng_->set_render_follow(on, growable_); }
+    void set_follow(bool on) { eng_->set_follow(on, growable_); }
     // GraphSlam2D::generateOccupancyMap's loop body (graph_slam2d.cpp:136-160) for any posed scans (Engine::render_scans)
     int insert_scans(const double* pts, const int64_t* offsets, int n_scans, const double* origins, const double* quats, const SE2* states, bool full,
                      uint64_t* cells);
@@ -427,7 +432,8 @@ private:
     double cov_blend_ = 0.0;
     std::vector<double> sampling_steps_;         // 161 (x, y) offsets, loc2d.cpp:93-107
     int global_localization(int n);               // loc2d.cpp:249-286
-    int add_sampling_covariance(int n);           // loc2d.cpp:199-247
+    int add_sampling_covariance(const double* pts, int n, const double* origin, const double* quat);   // loc2d.cpp:199-247
+    int follow(const double* pts, int n, const double* origin, const double* quat);
 };
 
 // shared helpers

@@ -1,7 +1,8 @@
 // kernels.cu -- the hand-written sm_90a kernels of the LaMa particle-filter hot path.
 //
 //   k_match      one CTA per particle: the whole Gauss-Newton / LM scan-matching loop
-//                (MatchSurface2D::eval + Solver::solve + GaussNewton, see match_core.h)
+//                (MatchSurface2D::eval + Solver::solve + GaussNewton, see match_core.h); k_match_extent, the same over a
+//                dense directory of the whole map (global localisation on a following map, k_extent_dir builds it)
 //   k_raycast    one CTA per particle: beam ray-cast into the frequency occupancy map with packed
 //                atomics + ordered replay of threshold crossings (see ray_core.h)
 //   k_brushfire  one warp per particle: DynamicDistanceMap::update() in exact heap order (ddm_core.h)
@@ -99,18 +100,25 @@ __device__ __forceinline__ void eval_beam(double s[kNumSums], const Affine& tf, 
     accumulate(s, e, so.robust_kind, so.robust_param, meas_sigma);
 }
 
-__global__ void __launch_bounds__(kMatchThreads, 2)
-k_match(StoreView s, MatchParams mp, const SE2* __restrict__ states_in, MatchResult* __restrict__ results)
+// The body of k_match and k_match_extent.  kExtent (global localisation over a following map): directory entries come from the dense
+// directory xdir over window xwin in global memory (k_extent_dir) instead of the working window staged in shared memory, and a patch
+// outside xwin is absent.  Every other line, the reductions included, is shared, so each state's sums are those k_match gives on a
+// window that holds the whole map.
+template <bool kExtent>
+__device__ __forceinline__ void match_body(const StoreView& s, const MatchParams& mp, const SE2* __restrict__ states_in, MatchResult* __restrict__ results,
+                                           const int32_t* xdir, const DirWindow& xwin)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int dim2      = s.window.dim * s.window.dim;
-    int32_t* dir        = reinterpret_cast<int32_t*>(smem_raw);
+    const int dim2      = kExtent ? 0 : s.window.dim * s.window.dim;
+    int32_t* sdir       = reinterpret_cast<int32_t*>(smem_raw);
     double* dtab        = reinterpret_cast<double*>(smem_raw + (size_t)dim2 * 4);
     MatchShared& sh     = *reinterpret_cast<MatchShared*>(smem_raw + (size_t)dim2 * 4 + (size_t)(mp.max_sqdist + 1) * 8);
     double* part        = reinterpret_cast<double*>(smem_raw + (size_t)dim2 * 4 + (size_t)(mp.max_sqdist + 1) * 8 + ((sizeof(MatchShared) + 15) & ~(size_t)15));
     const int tid       = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int particle  = mp.shared_map ? mp.particle_offset : mp.particle_offset + blockIdx.x;
-    const int32_t* gdir = dir_of(s, mp.set, particle, kMapDm);
+    const int32_t* dir  = kExtent ? xdir : sdir;
+    const DirWindow& win = kExtent ? xwin : s.window;
+    const int parked    = kExtent ? 0 : mp.parked_any;
 
     if (tid == 0) {
         mbar_init(&sh.bar, 1);
@@ -123,7 +131,7 @@ k_match(StoreView s, MatchParams mp, const SE2* __restrict__ states_in, MatchRes
     // dynamic_distance_map.cpp:143-146, so table entries are bit-identical to the reference's values)
     for (uint32_t k = tid; k <= mp.max_sqdist; k += blockDim.x) dtab[k] = mul_rn(sqrt((double)k), mp.resolution);
     __syncthreads();
-    block_stage_tma(dir, gdir, (uint32_t)dim2 * 4u, &sh.bar, 0);
+    if (!kExtent) block_stage_tma(sdir, dir_of(s, mp.set, particle, kMapDm), (uint32_t)dim2 * 4u, &sh.bar, 0);
 
     const int n = mp.scan.n_beams;
     const bool single = mp.mode == 1;
@@ -135,8 +143,8 @@ k_match(StoreView s, MatchParams mp, const SE2* __restrict__ states_in, MatchRes
         for (int k = 0; k < kNumSums; ++k) acc[k] = 0.0;
         const Affine tf = sh.tf;
         for (int b = tid; b < n; b += blockDim.x)
-            eval_beam(acc, tf, mp.points + 3 * (size_t)b, mp.scan.scale, s.pool, dir, s.window, dtab, mp.max_sqdist, mp.solver, mp.meas_sigma,
-                      mp.parked_any, s.status);
+            eval_beam(acc, tf, mp.points + 3 * (size_t)b, mp.scan.scale, s.pool, dir, win, dtab, mp.max_sqdist, mp.solver, mp.meas_sigma,
+                      parked, s.status);
         // Block reduction through shared memory, fixed order (deterministic): every thread parks its 12 partial sums, then warp k adds
         // up sum k over all threads (a strided pass + one warp shuffle tree) -- 12 stores per thread instead of 60 shuffles per value.
 #pragma unroll
@@ -175,6 +183,40 @@ k_match(StoreView s, MatchParams mp, const SE2* __restrict__ states_in, MatchRes
         r.evals_ref  = sh.ctl.evals_ref;
         r.evals_done = sh.evals_done;
         r.pad        = 0;
+    }
+}
+
+__global__ void __launch_bounds__(kMatchThreads, 2)
+k_match(StoreView s, MatchParams mp, const SE2* __restrict__ states_in, MatchResult* __restrict__ results)
+{
+    match_body<false>(s, mp, states_in, results, nullptr, s.window);
+}
+
+__global__ void __launch_bounds__(kMatchThreads, 2)
+k_match_extent(StoreView s, MatchParams mp, const SE2* __restrict__ states_in, MatchResult* __restrict__ results, const int32_t* __restrict__ xdir,
+               DirWindow xwin)
+{
+    match_body<true>(s, mp, states_in, results, xdir, xwin);
+}
+
+// The dense directory of particle 0's distance map over window xw (xw.dim^2 entries, all -1 on entry): the working window's entries and
+// the n_parked entries of its parked list, each at its patch.  Patches outside xw are left out.
+__global__ void k_extent_dir(StoreView s, ParkView pv, int set, DirWindow xw, int n_parked, int32_t* __restrict__ xdir)
+{
+    const int dim2 = s.window.dim * s.window.dim;
+    const int32_t* dir = dir_of(s, set, 0, kMapDm);
+    const ParkEntry* parked = pv.park + (n_parked ? pv.ol[kMapDm].x : 0);   // list of particle 0, kind kMapDm
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < dim2 + n_parked; i += gridDim.x * blockDim.x) {
+        int32_t px, py, e;
+        if (i < dim2) {
+            e = dir[i];
+            px = s.window.base_px + i % s.window.dim;
+            py = s.window.base_py + i / s.window.dim;
+        } else {
+            const ParkEntry a = parked[i - dim2];
+            e = a.entry; px = a.px; py = a.py;
+        }
+        if (e >= 0 && patch_in_window(xw, px, py)) xdir[(size_t)(py - xw.base_py) * xw.dim + (px - xw.base_px)] = e;
     }
 }
 
@@ -2121,6 +2163,8 @@ cudaError_t configure_kernels(int dir_dim, uint32_t max_sqdist_limit, const RayP
     cudaError_t e;
     e = raise_smem_limit(k_match, match_smem_bytes(dir_dim, max_sqdist_limit));
     if (e != cudaSuccess) return e;
+    e = raise_smem_limit(k_match_extent, match_smem_bytes(0, max_sqdist_limit));
+    if (e != cudaSuccess) return e;
     if (rp.prob_mode) e = raise_smem_limit(k_raycast<true>, raycast_smem_bytes(dir_dim, rp));
     else e = raise_smem_limit(k_raycast<false>, raycast_smem_bytes(dir_dim, rp));
     if (e != cudaSuccess) return e;
@@ -2134,14 +2178,28 @@ cudaError_t configure_kernels(int dir_dim, uint32_t max_sqdist_limit, const RayP
     return e;
 }
 
+// every thread evaluates ceil(n / threads) beams: choose the block so that the last round is (almost) full
+static int match_threads(int n)
+{
+    const int rounds = (n + kMatchThreads - 1) / kMatchThreads;
+    const int threads = (((n + rounds - 1) / rounds) + 31) & ~31;
+    return threads < 128 ? 128 : threads;
+}
 void launch_match(const StoreView& s, const MatchParams& mp, const SE2* d_states, MatchResult* d_results, int count, cudaStream_t st)
 {
     if (count <= 0) return;
-    // every thread evaluates ceil(n / threads) beams: choose the block so that the last round is (almost) full
-    const int n = mp.scan.n_beams, rounds = (n + kMatchThreads - 1) / kMatchThreads;
-    int threads = (((n + rounds - 1) / rounds) + 31) & ~31;
-    threads = threads < 128 ? 128 : threads;
-    k_match<<<count, threads, match_smem_bytes(s.window.dim, mp.max_sqdist), st>>>(s, mp, d_states, d_results);
+    k_match<<<count, match_threads(mp.scan.n_beams), match_smem_bytes(s.window.dim, mp.max_sqdist), st>>>(s, mp, d_states, d_results);
+}
+void launch_match_extent(const StoreView& s, const MatchParams& mp, const int32_t* d_xdir, const DirWindow& xw, const SE2* d_states, MatchResult* d_results,
+                         int count, cudaStream_t st)
+{
+    if (count <= 0) return;
+    k_match_extent<<<count, match_threads(mp.scan.n_beams), match_smem_bytes(0, mp.max_sqdist), st>>>(s, mp, d_states, d_results, d_xdir, xw);
+}
+void launch_extent_dir(const StoreView& s, const ParkView& pv, int set, const DirWindow& xw, int n_parked, int32_t* d_xdir, cudaStream_t st)
+{
+    const int n = s.window.dim * s.window.dim + n_parked;
+    k_extent_dir<<<(n + 255) / 256, 256, 0, st>>>(s, pv, set, xw, n_parked, d_xdir);
 }
 void launch_raycast(const StoreView& s, const RayParams& rp, const SE2* d_states, uint64_t* d_events, MapUpdateStats* d_stats, int count,
                     cudaStream_t st)

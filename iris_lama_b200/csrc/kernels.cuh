@@ -96,6 +96,13 @@ size_t brushfire_smem_bytes(int dir_dim, const BrushParams& bp);
 cudaError_t configure_kernels(int dir_dim, uint32_t max_sqdist_limit, const RayParams& rp, const BrushParams& bp);
 
 void launch_match(const StoreView& s, const MatchParams& mp, const SE2* d_states, MatchResult* d_results, int count, cudaStream_t st);
+// k_match_extent: k_match (mp.shared_map, mp.mode 1) reading the dense directory d_xdir over window xw (launch_extent_dir) instead of the
+// working window; a patch outside xw is absent
+void launch_match_extent(const StoreView& s, const MatchParams& mp, const int32_t* d_xdir, const DirWindow& xw, const SE2* d_states, MatchResult* d_results,
+                         int count, cudaStream_t st);
+// d_xdir (xw.dim^2 entries, all -1 on entry) = the entries of particle 0's distance map, its window and the n_parked entries of its parked
+// list, at their patches
+void launch_extent_dir(const StoreView& s, const ParkView& pv, int set, const DirWindow& xw, int n_parked, int32_t* d_xdir, cudaStream_t st);
 void launch_raycast(const StoreView& s, const RayParams& rp, const SE2* d_states, uint64_t* d_events, MapUpdateStats* d_stats, int count,
                     cudaStream_t st);
 // the pull form (every beam planar and starting in the same cell): k_ray_setup + k_ray_pull; particles it cannot take are left to
