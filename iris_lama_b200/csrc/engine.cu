@@ -58,6 +58,24 @@ struct Engine::Impl {
     // that step is collected, so no host synchronisation is added
     cudaEvent_t evp[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};
     bool evp_used[2] = {false, false};
+    // particle groups of the grouped step (Engine::step_groups): group g owns the particles [g * P / G, (g + 1) * P / G) and a stream of
+    // its own; an upload stream carries the scan and the predicted states.  Each group's kernels count patches into a counter block
+    // of their own (d_gcnt[g]), so that a report holds that group's work of one scan exactly; settle() folds the blocks into
+    // view.counters.  h_grep[half][g] = {status, allocated, detached, freed, free slots, ...}, slot G = view.counters at the step.
+    int groups = 1;
+    bool ray_order = false;                     // ray(g + 1) after ray(g), ray(0) of the next scan after ray(G - 1) (measured slower, DESIGN.md 7a)
+    cudaStream_t gstream[kMaxGroups] = {};
+    cudaStream_t up_stream = nullptr;
+    cudaEvent_t ev_gmatch[kMaxGroups] = {}, ev_gray[kMaxGroups] = {}, ev_gdone[kMaxGroups] = {};
+    cudaEvent_t ev_up = nullptr, ev_fork = nullptr;
+    uint64_t* d_gcnt = nullptr;                 // [kMaxGroups][4]
+    uint64_t* h_grep = nullptr;                 // pinned [2][kMaxGroups + 1][8]
+    int report_groups[2] = {0, 0};              // groups of the step that reported into each half (0: a single-stream report)
+    int last_groups = 0;                        // groups of the last grouped step (its ev_gray[last_groups - 1] orders the next ray(0))
+    bool fork = true;                           // the group streams must wait for the launching stream before their next work
+    bool groups_ran = false;                    // grouped steps since the last fold: d_gcnt and the deferred k_merge_free are pending
+    int scan_half = 0;                          // half of d_scan_buf the last grouped host scan went to
+    uint64_t scan_alloc = 0, prev_alloc = 0;    // patches the last booked grouped scan allocated (allocated + detached), and the sum at its booking
     // scratch for import/export/distance
     void* d_scratch = nullptr;
     size_t scratch_bytes = 0;
@@ -105,6 +123,8 @@ struct Engine::Impl {
 
 
 constexpr int kPullMaxBeams = 4096;   // k_ray_setup sorts the beams of a scan in shared memory
+constexpr int kGroupMinParticles = 256;   // particle groups of step_async from this many particles per device on: measured at 256 only
+constexpr int kDefaultGroups     = 4;     // scripts/pf_groups_rate.py, DESIGN.md 7a
 
 static bool points_flat(const double* pts, size_t n)
 {
@@ -256,7 +276,8 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
         CU_NEW(dalloc((void**)&d->d_park_ol[set], d->park_ol[set].size() * sizeof(int2)));
         CU_NEW(cudaMemset(d->d_park_ol[set], 0, d->park_ol[set].size() * sizeof(int2)));
     }
-    CU_NEW(dalloc((void**)&d->d_scan_buf, (size_t)cfg.max_beams * 3 * 8));
+    // two halves: a grouped step uploads the next host scan into one while the other groups' ray casts may still read the other
+    CU_NEW(dalloc((void**)&d->d_scan_buf, 2 * (size_t)cfg.max_beams * 3 * 8));
     d->d_points = d->d_scan_buf;
 
     d->ray.log_cap   = next_pow2_host(std::max(4096, 3 * cfg.max_beams));
@@ -332,6 +353,33 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     CU_NEW(cudaMallocHost((void**)&d->h_idx, idx_ints * 4));
     CU_NEW(cudaMallocHost((void**)&d->h_status, 64));
 
+    // Particle groups of step_async (DESIGN.md 7a): a scan of G groups overlaps one group's brushfire and next match with other groups'
+    // ray casts.  One group when the pull ray cast may be selected (its task list is shared by every particle of a launch); otherwise
+    // kDefaultGroups from kGroupMinParticles particles on, measured by scripts/pf_groups_rate.py.  Developer hooks, read here:
+    // LAMA_PF_GROUPS sets G, LAMA_PF_RAY_ORDER=1 adds the edge that serialises the groups' ray casts.
+    {
+        int g = cfg.particles >= kGroupMinParticles ? kDefaultGroups : 1;
+        if (const char* pg = std::getenv("LAMA_PF_GROUPS")) g = std::atoi(pg);
+        if (d->pull_max_particles > 0) g = 1;
+        d->groups = std::max(1, std::min(std::min(g, kMaxGroups), cfg.particles));
+        if (const char* ro = std::getenv("LAMA_PF_RAY_ORDER")) d->ray_order = std::atoi(ro) != 0;
+        if (d->groups > 1) {
+            for (int k = 0; k < d->groups; ++k) {
+                CU_NEW(cudaStreamCreateWithFlags(&d->gstream[k], cudaStreamNonBlocking));
+                CU_NEW(cudaEventCreateWithFlags(&d->ev_gmatch[k], cudaEventDisableTiming));
+                CU_NEW(cudaEventCreateWithFlags(&d->ev_gray[k], cudaEventDisableTiming));
+                CU_NEW(cudaEventCreateWithFlags(&d->ev_gdone[k], cudaEventDisableTiming));
+            }
+            CU_NEW(cudaStreamCreateWithFlags(&d->up_stream, cudaStreamNonBlocking));
+            CU_NEW(cudaEventCreateWithFlags(&d->ev_up, cudaEventDisableTiming));
+            CU_NEW(cudaEventCreateWithFlags(&d->ev_fork, cudaEventDisableTiming));
+            CU_NEW(dalloc((void**)&d->d_gcnt, (size_t)kMaxGroups * 4 * sizeof(uint64_t)));
+            CU_NEW(cudaMemset(d->d_gcnt, 0, (size_t)kMaxGroups * 4 * sizeof(uint64_t)));
+            CU_NEW(cudaMallocHost((void**)&d->h_grep, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t)));
+            std::memset(d->h_grep, 0, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t));
+        }
+    }
+
     const size_t need_ray = raycast_smem_bytes(cfg.dir_dim, d->ray), need_match = match_smem_bytes(cfg.dir_dim, e->max_sqdist_),
                  need_brush = brushfire_smem_bytes(cfg.dir_dim, d->brush);
     if (need_ray > 227 * 1024 || need_match > 227 * 1024 || need_brush > 227 * 1024) return bail("shared memory budget exceeded (reduce max_beams / dir_dim)");
@@ -349,6 +397,15 @@ Engine::~Engine()
     if (!d_) return;
     cudaSetDevice(cfg_.device);
     if (d_->stream) cudaStreamSynchronize(d_->stream);
+    for (int k = 0; k < kMaxGroups; ++k) {
+        if (d_->gstream[k]) { cudaStreamSynchronize(d_->gstream[k]); cudaStreamDestroy(d_->gstream[k]); }
+        for (cudaEvent_t ev : {d_->ev_gmatch[k], d_->ev_gray[k], d_->ev_gdone[k]})
+            if (ev) cudaEventDestroy(ev);
+    }
+    if (d_->up_stream) { cudaStreamSynchronize(d_->up_stream); cudaStreamDestroy(d_->up_stream); }
+    if (d_->ev_up) cudaEventDestroy(d_->ev_up);
+    if (d_->ev_fork) cudaEventDestroy(d_->ev_fork);
+    if (d_->h_grep) cudaFreeHost(d_->h_grep);
     for (void* p : d_->allocs) cudaFree(p);
     for (int set = 0; set < 2; ++set)
         if (d_->park[set]) cudaFree(d_->park[set]);
@@ -649,6 +706,7 @@ int Engine::step_enqueue(const double* pts, int n, const double origin[3], const
 {
     if (count < 1 || count > cfg_.particles) return fail("step_enqueue: particle range out of bounds", LAMA_ERR_ARG);
     extent_stale_ = true;
+    d_->fork = true;   // a grouped step after this one waits for it
     CU_TRY(cudaSetDevice(cfg_.device));
     // the previous scan's map update may still be running: nothing below waits for it on the host
     enq_had_pending_ = pending_maps_ != 0;
@@ -733,14 +791,166 @@ int Engine::collect_previous()
     return rc;
 }
 
+int Engine::particle_groups() const { return d_->groups; }
+
 int Engine::step_async(const double* pts, int n, const double origin[3], const double quat[4], double truncated_ray, double truncated_range,
                        const SE2* predicted, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out)
 {
+    // timing mode keeps one stream, so that kernelTimes() still times single kernels
+    if (d_->groups > 1 && count > 1 && !timing_) return step_groups(pts, n, origin, quat, truncated_ray, truncated_range, predicted, count, so, meas_sigma, out);
     { int rc = step_enqueue(pts, n, origin, quat, truncated_ray, truncated_range, predicted, count, so, meas_sigma); if (rc != LAMA_OK) return rc; }
     CU_TRY(cudaEventSynchronize(d_->ev_match));
     static_assert(sizeof(HostMatchResult) == sizeof(MatchResult), "layout");
     std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
     return collect_previous();
+}
+
+// step_async over G particle groups (DESIGN.md 7a).  Group g's stream runs match -> copy of its results -> ray cast -> brushfire -> report of
+// its particles; its particles' chain match(t) -> ray(t) -> brushfire(t) -> match(t + 1) depends on no other group, because the map update
+// runs before the resampling decision, so the groups drift apart and one group's brushfire and next match run beside another group's
+// ray cast.  (LAMA_PF_RAY_ORDER=1 serialises the ray casts across groups -- ray(g + 1) after ray(g), ray(0) of the next scan after
+// ray(G - 1) -- which measured slower.)  The launching stream waits for every group at the end (its events keep meaning "this scan's
+// map update has completed"); the groups wait for the launching stream only after settle(), which every other entry point calls first:
+// that is the barrier behind which resampling, window shifts, checkpoints, exports and k_merge_free run.  Patches freed by a grouped
+// scan go back to the free stack at the next barrier (k_merge_free is not safe beside a running alloc_slot), and a barrier is forced
+// when the free stack drops under twice what the last booked scan allocated (at least one patch per particle and kind), so that
+// freed patches waiting for the merge never make a scan run out of patches that one stream would have had.
+int Engine::step_groups(const double* pts, int n, const double origin[3], const double quat[4], double truncated_ray, double truncated_range,
+                        const SE2* predicted, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out)
+{
+    if (count < 1 || count > cfg_.particles) return fail("step_async: particle range out of bounds", LAMA_ERR_ARG);
+    if (pts && (n < 1 || n > cfg_.max_beams)) return fail("step_async: number of beams out of range", LAMA_ERR_ARG);
+    if (!pts && d_->scan.n_beams < 1) return fail("step_async: no scan selected", LAMA_ERR_STATE);
+    Impl* d = d_;
+    if (d->groups_ran) {
+        const uint64_t reserve = 2 * std::max<uint64_t>(d->scan_alloc, (uint64_t)count * d->view.n_kinds);
+        if (settled_counters_[3] < reserve) {
+            int rc = settle(nullptr);   // a barrier: the frees are merged, the groups fork again
+            if (rc != LAMA_OK) return rc;
+        }
+    }
+    extent_stale_ = true;
+    CU_TRY(cudaSetDevice(cfg_.device));
+    enq_had_pending_ = pending_maps_ != 0;
+    enq_prev_count_  = pending_maps_;
+    enq_prev_buf_    = pending_buf_;
+    const int G = std::min(d->groups, count);
+    if (d->fork) {   // work the engine put on the launching stream since the last grouped step comes first
+        CU_TRY(cudaEventRecord(d->ev_fork, d->stream));
+        CU_TRY(cudaStreamWaitEvent(d->up_stream, d->ev_fork, 0));
+        for (int g = 0; g < d->groups; ++g) CU_TRY(cudaStreamWaitEvent(d->gstream[g], d->ev_fork, 0));
+        d->fork = false;
+    }
+    // uploads: the host buffers are free (the previous call waited for every match, which follows its upload); the scan goes to the half of
+    // d_scan_buf the previous scan did not use, since that scan's later ray casts may still be reading it
+    if (pts) {
+        set_moving(origin, quat, truncated_ray, truncated_range, n);
+        std::memcpy(d->h_scan, pts, (size_t)n * 24);
+        d->scan_half ^= 1;
+        d->d_points = d->d_scan_buf + (size_t)d->scan_half * cfg_.max_beams * 3;
+        d->scan_flat = points_flat(pts, (size_t)n);
+        CU_TRY(cudaMemcpyAsync(d->d_points, d->h_scan, (size_t)n * 24, cudaMemcpyHostToDevice, d->up_stream));
+        h2d_bytes_ += (uint64_t)n * 24;
+    }
+    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
+    std::memcpy(d->h_states, predicted, (size_t)count * sizeof(SE2));
+    CU_TRY(cudaMemcpyAsync(d->d_states, d->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d->up_stream));
+    CU_TRY(cudaEventRecord(d->ev_up, d->up_stream));
+
+    MatchParams mp{};
+    mp.points = d->d_points;
+    mp.scan = d->scan;
+    mp.solver = so;
+    mp.meas_sigma = meas_sigma;
+    mp.resolution = cfg_.resolution;
+    mp.max_sqdist = max_sqdist_;
+    mp.set = cur_set_;
+    mp.shared_map = 0;
+    mp.mode = 0;
+    mp.parked_any = d->parked(cur_set_) != 0;
+    RayParams rp = d->ray;
+    rp.points = d->d_points;
+    rp.scan = d->scan;
+    rp.set = cur_set_;
+    rp.state_stride = (int)sizeof(MatchResult);
+    const int nb = d->scan.n_beams;
+    rp.log_cap   = std::min(d->ray.log_cap, next_pow2_host(std::max(1024, 3 * nb)));
+    rp.event_cap = std::min(d->ray.event_cap, next_pow2_host(std::max(512, nb)));
+    BrushParams bp = d->brush;
+    bp.set = cur_set_;
+    bp.event_cap = rp.event_cap;
+    bp.debug = brush_debug_flag();
+    const int half = 1 - pending_buf_;
+    MapUpdateStats* hs = d->h_stats + (size_t)half * cfg_.particles;
+    uint64_t* hr = d->h_grep + (size_t)half * (kMaxGroups + 1) * 8;
+    cudaEvent_t ray_before = d->ray_order && d->last_groups ? d->ev_gray[d->last_groups - 1] : nullptr;
+    for (int g = 0; g < G; ++g) {
+        const int lo = (int)((int64_t)g * count / G), cnt = (int)((int64_t)(g + 1) * count / G) - lo;
+        cudaStream_t st = d->gstream[g];
+        StoreView v = d->view;
+        v.counters = d->d_gcnt + (size_t)g * 4;
+        CU_TRY(cudaStreamWaitEvent(st, d->ev_up, 0));
+        mp.particle_offset = lo;
+        launch_match(v, mp, d->d_states + lo, d->d_results + lo, cnt, st);
+        CU_TRY(cudaMemcpyAsync(d->h_results + lo, d->d_results + lo, (size_t)cnt * sizeof(MatchResult), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaEventRecord(d->ev_gmatch[g], st));
+        if (ray_before) CU_TRY(cudaStreamWaitEvent(st, ray_before, 0));
+        rp.particle_offset = lo;
+        launch_raycast(v, rp, reinterpret_cast<const SE2*>(d->d_results + lo), d->d_events + (size_t)lo * d->ray.event_cap, d->d_stats + lo, cnt, st);
+        CU_TRY(cudaEventRecord(d->ev_gray[g], st));
+        ray_before = d->ray_order ? d->ev_gray[g] : nullptr;
+        bp.particle_offset = lo;
+        bp.lower_spill = d->brush.lower_spill + (size_t)lo * (d->brush.lower_total + 2);
+        bp.raise_spill = d->brush.raise_spill + (size_t)lo * (d->brush.raise_total + 2);
+        launch_brushfire(v, bp, d->d_events + (size_t)lo * d->ray.event_cap, d->d_stats + lo, cnt, st);
+        CU_TRY(cudaGetLastError());
+        // this group's report: its statistics, its counter block, status and free slots; group 0 also copies view.counters, which no kernel
+        // of a grouped step writes
+        uint64_t* r = hr + (size_t)g * 8;
+        CU_TRY(cudaMemcpyAsync(hs + lo, d->d_stats + lo, (size_t)cnt * sizeof(MapUpdateStats), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(r, d->view.status, 4, cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(r + 1, v.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(r + 4, d->view.free_count, 4, cudaMemcpyDeviceToHost, st));
+        if (g == 0) CU_TRY(cudaMemcpyAsync(hr + (size_t)G * 8 + 1, d->view.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaEventRecord(d->ev_gdone[g], st));
+        d2h_bytes_ += (uint64_t)cnt * sizeof(MapUpdateStats) + 4 + 28 + (g == 0 ? 24 : 0);
+    }
+    for (int g = 0; g < G; ++g) CU_TRY(cudaStreamWaitEvent(d->stream, d->ev_gdone[g], 0));   // the launching stream joins every group
+    d->last_groups = G;
+    d->groups_ran = true;
+    d->report_groups[half] = G;
+    pending_buf_  = half;
+    pending_maps_ = count;
+    times_.match_launches += G;
+    times_.raycast_launches += G;
+    times_.brushfire_launches += G;
+    h2d_bytes_ += (uint64_t)count * sizeof(SE2);
+    d2h_bytes_ += (uint64_t)count * sizeof(MatchResult);
+    for (int g = 0; g < G; ++g) CU_TRY(cudaEventSynchronize(d->ev_gmatch[g]));
+    static_assert(sizeof(HostMatchResult) == sizeof(MatchResult), "layout");
+    std::memcpy(out, d->h_results, (size_t)count * sizeof(MatchResult));
+    return collect_previous();
+}
+
+// Folds the groups' counter blocks into view.counters and returns the patches freed by grouped scans to the free stack.  The engine's
+// streams must have completed (settle() calls it after synchronising the launching stream, which has joined every group).
+int Engine::fold_groups()
+{
+    Impl* d = d_;
+    d->groups_ran = false;
+    uint64_t g[kMaxGroups * 4], m[3];
+    CU_TRY(cudaMemcpyAsync(g, d->d_gcnt, sizeof(g), cudaMemcpyDeviceToHost, d->stream));
+    CU_TRY(cudaMemcpyAsync(m, d->view.counters, sizeof(m), cudaMemcpyDeviceToHost, d->stream));
+    CU_TRY(cudaStreamSynchronize(d->stream));
+    for (int k = 0; k < kMaxGroups; ++k)
+        for (int c = 0; c < 3; ++c) m[c] += g[k * 4 + c];
+    CU_TRY(cudaMemcpyAsync(d->view.counters, m, sizeof(m), cudaMemcpyHostToDevice, d->stream));
+    CU_TRY(cudaMemsetAsync(d->d_gcnt, 0, sizeof(g), d->stream));
+    launch_merge_free(d->view, d->stream);
+    CU_TRY(cudaGetLastError());
+    CU_TRY(cudaStreamSynchronize(d->stream));   // `m` is on this stack
+    times_.misc_launches += 1;
+    return LAMA_OK;
 }
 
 void* Engine::stream_handle() const { return d_->stream; }
@@ -765,7 +975,14 @@ int Engine::pack_results(int count, double digest, double* d_out, void* stream)
 
 int Engine::settle(HostMapStats* out, bool already_complete)
 {
-    if (pending_maps_ == 0) return LAMA_OK;
+    if (!already_complete) d_->fork = true;   // whatever the caller enqueues next on the launching stream precedes the next grouped step
+    if (pending_maps_ == 0) {
+        if (!already_complete && d_->groups_ran) {
+            CU_TRY(cudaSetDevice(cfg_.device));
+            return fold_groups();
+        }
+        return LAMA_OK;
+    }
     const int count = pending_maps_;
     pending_maps_ = 0;
     CU_TRY(cudaSetDevice(cfg_.device));
@@ -788,12 +1005,32 @@ int Engine::settle(HostMapStats* out, bool already_complete)
     }
     static_assert(sizeof(HostMapStats) == sizeof(MapUpdateStats), "layout");
     const MapUpdateStats* hs = d_->h_stats + (size_t)pending_buf_ * cfg_.particles;
-    const uint64_t* hr = d_->h_report + (size_t)pending_buf_ * 8;
     last_map_stats_.assign((const HostMapStats*)hs, (const HostMapStats*)hs + count);
     if (out) std::memcpy(out, hs, (size_t)count * sizeof(MapUpdateStats));
-    settled_counters_[0] = hr[1]; settled_counters_[1] = hr[2]; settled_counters_[2] = hr[3];
-    settled_counters_[3] = (uint64_t)(uint32_t)hr[4];
-    *d_->h_status = (uint32_t)hr[0];
+    if (const int G = d_->report_groups[pending_buf_]) {   // a grouped step: view.counters plus every group's block
+        d_->report_groups[pending_buf_] = 0;
+        const uint64_t* hr = d_->h_grep + (size_t)pending_buf_ * (kMaxGroups + 1) * 8;
+        uint32_t status = 0;
+        for (int c = 0; c < 3; ++c) settled_counters_[c] = hr[(size_t)G * 8 + 1 + c];
+        for (int g = 0; g < G; ++g) {
+            status |= (uint32_t)hr[g * 8];
+            for (int c = 0; c < 3; ++c) settled_counters_[c] += hr[g * 8 + 1 + c];
+        }
+        settled_counters_[3] = (uint64_t)(uint32_t)hr[(G - 1) * 8 + 4];
+        *d_->h_status = status;
+        const uint64_t alloc = settled_counters_[0] + settled_counters_[1];
+        d_->scan_alloc = d_->prev_alloc && alloc > d_->prev_alloc ? alloc - d_->prev_alloc : 0;
+        d_->prev_alloc = alloc;
+    } else {
+        const uint64_t* hr = d_->h_report + (size_t)pending_buf_ * 8;
+        settled_counters_[0] = hr[1]; settled_counters_[1] = hr[2]; settled_counters_[2] = hr[3];
+        settled_counters_[3] = (uint64_t)(uint32_t)hr[4];
+        *d_->h_status = (uint32_t)hr[0];
+    }
+    if (!already_complete && d_->groups_ran) {
+        int rc = fold_groups();
+        if (rc != LAMA_OK) return rc;
+    }
     return check_device_status();
 }
 

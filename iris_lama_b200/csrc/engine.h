@@ -30,6 +30,9 @@ struct EngineConfig {
                                 // after a prune, `known` can no longer be derived from a non-zero cell
 };
 
+// Most particle groups Engine::step_async pipelines a scan over (LAMA_PF_GROUPS is clamped to it)
+constexpr int kMaxGroups = 8;
+
 struct HostMatchResult {
     SE2 state;
     double sums[kNumSums];
@@ -125,6 +128,7 @@ public:
     // resampling applied afterwards copies the updated maps, which gives the same maps as the reference's resample-then-update
     // (update(copy(m), pose) == copy(update(m, pose)), DESIGN.md 12).  Returns when the match results are on the host; the map
     // update keeps running and is collected by the next settle().  `pts` != nullptr: upload that scan first (no synchronisation).
+    // Outside timing mode the particles run in particle_groups() groups with a stream each (DESIGN.md 7a); the results do not change.
     int step_async(const double* pts, int n, const double origin[3], const double quat[4], double truncated_ray, double truncated_range,
                    const SE2* predicted, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out);
     // The same without waiting for anything (sharded ranks): the match results stay on the device, where pack_results() turns them into
@@ -133,6 +137,7 @@ public:
                      const SE2* predicted, int count, const SolverOptions& so, double meas_sigma);
     int pack_results(int count, double digest, double* d_out, void* stream);   // `stream` (cudaStream_t) first waits for the match
     int collect_previous();                                                     // call after the match is known to have completed
+    int particle_groups() const;                                                // groups step_async pipelines a scan over (1: one stream)
     void* stream_handle() const;                                                // cudaStream_t of the engine
     int wait_for_stream(void* other_stream);                                    // `other_stream` waits for everything enqueued on the engine's stream so far
     bool map_update_pending() const { return pending_maps_ != 0; }
@@ -274,6 +279,9 @@ private:
     std::vector<HostMapStats> last_map_stats_;
     bool enq_had_pending_ = false;        // step_enqueue: the previous scan's map update still has to be booked (collect_previous)
     int enq_prev_count_ = 0, enq_prev_buf_ = 0;
+    int step_groups(const double* pts, int n, const double origin[3], const double quat[4], double truncated_ray, double truncated_range,
+                    const SE2* predicted, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out);
+    int fold_groups();
     void set_moving(const double origin[3], const double quat[4], double truncated_ray, double truncated_range, int n);
     int enqueue_report(int count);
     int fail(const std::string& what, int code);
