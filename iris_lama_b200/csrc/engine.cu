@@ -36,7 +36,6 @@ struct Engine::Impl {
     MatchResult* h_results = nullptr;  // pinned
     MapUpdateStats* d_stats = nullptr;
     MapUpdateStats* h_stats = nullptr;  // pinned; two halves (ping-pong between consecutive map updates)
-    uint64_t* h_report = nullptr;       // pinned; per half: {status, allocated, detached, freed, free slots}
     double* h_scan = nullptr;           // pinned staging of a host scan (step_async)
     cudaEvent_t ev_match = nullptr, ev_sync = nullptr;
     uint64_t* d_events = nullptr;
@@ -51,27 +50,26 @@ struct Engine::Impl {
                                   // count, see launch_ray_stage); LAMA_PULL_MAX_PARTICLES overrides
     bool scan_flat = false;     // the current scan has z == 0 everywhere and a sensor that keeps z planes: every beam is planar
     bool staged_flat = false;   // the same for the staged scans
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+    cudaEvent_t ev[2] = {nullptr, nullptr};
     cudaEvent_t ev_render[2] = {nullptr, nullptr};   // around one group of a following render (shift_window takes ev[0] / ev[1] between groups)
     void* pool_raw = nullptr;                          // the allocation view.pool was aligned out of (grow_pool replaces it)
-    // timing of the pipelined step (step_enqueue): per report buffer {before match, after match, after the ray stage, after the brushfire}; read when
-    // that step is collected, so no host synchronisation is added
+    // timing of a map update: per report buffer {before the match, after the match, after the ray stage, after the brushfire}; read when
+    // that update is collected, so no host synchronisation is added.  evp_match: the update recorded a match (evp[half][0] is set).
     cudaEvent_t evp[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};
-    bool evp_used[2] = {false, false};
+    bool evp_used[2] = {false, false}, evp_match[2] = {false, false};
     // particle groups of the grouped step (Engine::step_groups): group g owns the particles [g * P / G, (g + 1) * P / G) and a stream of
     // its own; an upload stream carries the scan and the predicted states.  Each group's kernels count patches into a counter block
     // of their own (d_gcnt[g]), so that a report holds that group's work of one scan exactly; settle() folds the blocks into
-    // view.counters.  h_grep[half][g] = {status, allocated, detached, freed, free slots, ...}, slot G = view.counters at the step.
+    // view.counters.  A map update on one stream is the one-group case, counting into view.counters itself.
+    // h_grep[half][g] = {status, allocated, detached, freed, free slots, ...}; with G > 1 slot G = view.counters at the step.
     int groups = 1;
-    bool ray_order = false;                     // ray(g + 1) after ray(g), ray(0) of the next scan after ray(G - 1) (measured slower, DESIGN.md 7a)
     cudaStream_t gstream[kMaxGroups] = {};
     cudaStream_t up_stream = nullptr;
-    cudaEvent_t ev_gmatch[kMaxGroups] = {}, ev_gray[kMaxGroups] = {}, ev_gdone[kMaxGroups] = {};
+    cudaEvent_t ev_gmatch[kMaxGroups] = {}, ev_gdone[kMaxGroups] = {};
     cudaEvent_t ev_up = nullptr, ev_fork = nullptr;
     uint64_t* d_gcnt = nullptr;                 // [kMaxGroups][4]
     uint64_t* h_grep = nullptr;                 // pinned [2][kMaxGroups + 1][8]
-    int report_groups[2] = {0, 0};              // groups of the step that reported into each half (0: a single-stream report)
-    int last_groups = 0;                        // groups of the last grouped step (its ev_gray[last_groups - 1] orders the next ray(0))
+    int report_groups[2] = {0, 0};              // groups of the map update that reported into each half
     bool fork = true;                           // the group streams must wait for the launching stream before their next work
     bool groups_ran = false;                    // grouped steps since the last fold: d_gcnt and the deferred k_merge_free are pending
     int scan_half = 0;                          // half of d_scan_buf the last grouped host scan went to
@@ -119,6 +117,7 @@ struct Engine::Impl {
         std::fill(park_ol[set].begin(), park_ol[set].end(), make_int2(0, 0));
         cudaMemsetAsync(d_park_ol[set], 0, park_ol[set].size() * sizeof(int2), stream);
     }
+    int launch_ray_stage(const StoreView& v, RayParams rp, const SE2* states, uint64_t* events, MapUpdateStats* stats, int count, cudaStream_t st) const;
 };
 
 
@@ -136,22 +135,23 @@ static bool points_flat(const double* pts, size_t n)
 // The occupancy ray cast of `count` particles.  Scans whose beams all start in the same cell (no per-beam ray truncation) go through
 // the pull form (k_ray_setup + k_ray_pull); k_raycast, the per-beam walk, takes everything else: LidarOdometry2D's and truncated rays,
 // and -- decided per particle on the device -- scans of a tilted sensor (`flat` false: the beams may leave the z plane).
-static int launch_ray_stage(Engine::Impl* d, RayParams rp, const SE2* states, int count)   // returns the number of kernels launched
+int Engine::Impl::launch_ray_stage(const StoreView& v, RayParams rp, const SE2* states, uint64_t* events, MapUpdateStats* stats, int count,
+                                   cudaStream_t st) const   // returns the number of kernels launched
 {
     const ScanParams& sp = rp.scan;
     // The walk runs one CTA per particle, the pull form spreads the patches of all particles over every SM.  Measured on an H100 (scripts/pull_variants.py,
     // revisit regime): walk 0.152 / 0.200 / 0.318 / 0.636 ms, pull 0.227 / 0.287 / 0.393 / 0.632 ms at 32 / 64 / 128 / 256 particles -- the walk wins
     // up to 128 and ties at 256, so pull_max_particles defaults to 0; LAMA_PULL_MAX_PARTICLES (read when the engine is created) selects the pull
     // form up to that many particles per device.
-    const bool no_pull = count > d->pull_max_particles;
-    const bool flat = d->scan_flat && sp.moving.l[6] == 0.0 && sp.moving.l[7] == 0.0;
+    const bool no_pull = count > pull_max_particles;
+    const bool flat = scan_flat && sp.moving.l[6] == 0.0 && sp.moving.l[7] == 0.0;
     rp.pull_fallback = 0;
     if (!no_pull && !sp.lo_ray && sp.truncated_ray == 0.0 && sp.n_beams <= kPullMaxBeams) {
-        launch_raycast_pull(d->view, rp, states, d->d_events, d->d_stats, count, d->n_sms, d->stream);
+        launch_raycast_pull(v, rp, states, events, stats, count, n_sms, st);
         if (flat) return 2;   // hit.z == start.z exactly for every beam: k_ray_setup takes every particle
         rp.pull_fallback = 1;
     }
-    launch_raycast(d->view, rp, states, d->d_events, d->d_stats, count, d->stream);
+    launch_raycast(v, rp, states, events, stats, count, st);
     return rp.pull_fallback ? 3 : 1;
 }
 
@@ -234,7 +234,6 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     }
     CU_NEW(cudaEventCreate(&d->ev[0]));
     CU_NEW(cudaEventCreate(&d->ev[1]));
-    CU_NEW(cudaEventCreate(&d->ev[2]));
     CU_NEW(cudaEventCreate(&d->ev_render[0]));
     CU_NEW(cudaEventCreate(&d->ev_render[1]));
     for (int b = 0; b < 2; ++b)
@@ -345,8 +344,8 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     const size_t idx_ints = std::max((size_t)cfg.particles, (size_t)cfg.dir_dim * cfg.dir_dim);   // resample indices / directory entries to delete
     CU_NEW(dalloc((void**)&d->d_idx, idx_ints * 4));
     CU_NEW(cudaMallocHost((void**)&d->h_stats, 2 * (size_t)cfg.particles * sizeof(MapUpdateStats)));
-    CU_NEW(cudaMallocHost((void**)&d->h_report, 2 * 8 * sizeof(uint64_t)));
-    std::memset(d->h_report, 0, 2 * 8 * sizeof(uint64_t));
+    CU_NEW(cudaMallocHost((void**)&d->h_grep, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t)));
+    std::memset(d->h_grep, 0, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t));
     CU_NEW(cudaMallocHost((void**)&d->h_scan, (size_t)cfg.max_beams * 24));
     CU_NEW(cudaEventCreateWithFlags(&d->ev_match, cudaEventDisableTiming));
     CU_NEW(cudaEventCreateWithFlags(&d->ev_sync, cudaEventDisableTiming));
@@ -355,19 +354,17 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
 
     // Particle groups of step_async (DESIGN.md 7a): a scan of G groups overlaps one group's brushfire and next match with other groups'
     // ray casts.  One group when the pull ray cast may be selected (its task list is shared by every particle of a launch); otherwise
-    // kDefaultGroups from kGroupMinParticles particles on, measured by scripts/pf_groups_rate.py.  Developer hooks, read here:
-    // LAMA_PF_GROUPS sets G, LAMA_PF_RAY_ORDER=1 adds the edge that serialises the groups' ray casts.
+    // kDefaultGroups from kGroupMinParticles particles on, measured by scripts/pf_groups_rate.py.  Developer hook, read here:
+    // LAMA_PF_GROUPS sets G.
     {
         int g = cfg.particles >= kGroupMinParticles ? kDefaultGroups : 1;
         if (const char* pg = std::getenv("LAMA_PF_GROUPS")) g = std::atoi(pg);
         if (d->pull_max_particles > 0) g = 1;
         d->groups = std::max(1, std::min(std::min(g, kMaxGroups), cfg.particles));
-        if (const char* ro = std::getenv("LAMA_PF_RAY_ORDER")) d->ray_order = std::atoi(ro) != 0;
         if (d->groups > 1) {
             for (int k = 0; k < d->groups; ++k) {
                 CU_NEW(cudaStreamCreateWithFlags(&d->gstream[k], cudaStreamNonBlocking));
                 CU_NEW(cudaEventCreateWithFlags(&d->ev_gmatch[k], cudaEventDisableTiming));
-                CU_NEW(cudaEventCreateWithFlags(&d->ev_gray[k], cudaEventDisableTiming));
                 CU_NEW(cudaEventCreateWithFlags(&d->ev_gdone[k], cudaEventDisableTiming));
             }
             CU_NEW(cudaStreamCreateWithFlags(&d->up_stream, cudaStreamNonBlocking));
@@ -375,8 +372,6 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
             CU_NEW(cudaEventCreateWithFlags(&d->ev_fork, cudaEventDisableTiming));
             CU_NEW(dalloc((void**)&d->d_gcnt, (size_t)kMaxGroups * 4 * sizeof(uint64_t)));
             CU_NEW(cudaMemset(d->d_gcnt, 0, (size_t)kMaxGroups * 4 * sizeof(uint64_t)));
-            CU_NEW(cudaMallocHost((void**)&d->h_grep, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t)));
-            std::memset(d->h_grep, 0, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t));
         }
     }
 
@@ -399,7 +394,7 @@ Engine::~Engine()
     if (d_->stream) cudaStreamSynchronize(d_->stream);
     for (int k = 0; k < kMaxGroups; ++k) {
         if (d_->gstream[k]) { cudaStreamSynchronize(d_->gstream[k]); cudaStreamDestroy(d_->gstream[k]); }
-        for (cudaEvent_t ev : {d_->ev_gmatch[k], d_->ev_gray[k], d_->ev_gdone[k]})
+        for (cudaEvent_t ev : {d_->ev_gmatch[k], d_->ev_gdone[k]})
             if (ev) cudaEventDestroy(ev);
     }
     if (d_->up_stream) { cudaStreamSynchronize(d_->up_stream); cudaStreamDestroy(d_->up_stream); }
@@ -414,7 +409,6 @@ Engine::~Engine()
     if (d_->h_states) cudaFreeHost(d_->h_states);
     if (d_->h_results) cudaFreeHost(d_->h_results);
     if (d_->h_stats) cudaFreeHost(d_->h_stats);
-    if (d_->h_report) cudaFreeHost(d_->h_report);
     if (d_->h_scan) cudaFreeHost(d_->h_scan);
     if (d_->ev_match) cudaEventDestroy(d_->ev_match);
     if (d_->ev_sync) cudaEventDestroy(d_->ev_sync);
@@ -432,7 +426,6 @@ Engine::~Engine()
             if (d_->evp[b][k]) cudaEventDestroy(d_->evp[b][k]);
     if (d_->ev[0]) cudaEventDestroy(d_->ev[0]);
     if (d_->ev[1]) cudaEventDestroy(d_->ev[1]);
-    if (d_->ev[2]) cudaEventDestroy(d_->ev[2]);
     if (d_->stream && d_->own_stream) cudaStreamDestroy(d_->stream);
     delete d_;
 }
@@ -525,6 +518,77 @@ int Engine::ensure_states(int count)
     return LAMA_OK;
 }
 
+// The predicted states through the pinned staging buffer into d_states, on `stream`
+int Engine::upload_states(const SE2* states, int count, void* stream)
+{
+    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
+    std::memcpy(d_->h_states, states, (size_t)count * sizeof(SE2));
+    CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    h2d_bytes_ += (uint64_t)count * sizeof(SE2);
+    return LAMA_OK;
+}
+
+// A host scan through the pinned staging buffer into `dst`, on `stream`; it becomes the current scan.  The staging buffer is free: the
+// previous step returned after its match, which follows its upload.
+int Engine::upload_scan(const double* pts, int n, double* dst, void* stream)
+{
+    std::memcpy(d_->h_scan, pts, (size_t)n * 24);
+    d_->d_points = dst;
+    d_->scan_flat = points_flat(pts, (size_t)n);
+    CU_TRY(cudaMemcpyAsync(dst, d_->h_scan, (size_t)n * 24, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    h2d_bytes_ += (uint64_t)n * 24;
+    return LAMA_OK;
+}
+
+MatchParams Engine::match_params(const SolverOptions& so, double meas_sigma, int first_particle, bool shared_map, int mode) const
+{
+    MatchParams mp{};
+    mp.points = d_->d_points;
+    mp.scan = d_->scan;
+    mp.solver = so;
+    mp.meas_sigma = meas_sigma;
+    mp.resolution = cfg_.resolution;
+    mp.max_sqdist = max_sqdist_;
+    mp.set = cur_set_;
+    mp.particle_offset = first_particle;
+    mp.shared_map = shared_map ? 1 : 0;
+    mp.mode = mode;
+    mp.parked_any = d_->parked(cur_set_) != 0;
+    return mp;
+}
+
+// developer builds (LAMA_PHASE_TIMING): LAMA_BF_DEBUG = ordinal of the map update whose k_brushfire prints its per-particle phase cycles
+static int brush_debug_flag()
+{
+    static int launch_no = 0;
+    const char* dbg = std::getenv("LAMA_BF_DEBUG");
+    return dbg && std::atoi(dbg) == launch_no++;
+}
+
+// The brushfire of a map update with block 0 on `particle_offset` and, with `rp`, the ray cast of the current scan before it, reading
+// poses `state_stride` bytes apart.  The ray cast's shared-memory scratch and the event lists are sized for this scan (two CTAs per SM
+// at 1080 beams; the maxima were registered at create); a brushfire alone (dm_apply) takes lists of the full capacity.
+BrushParams Engine::map_update_params(int state_stride, int particle_offset, RayParams* rp) const
+{
+    BrushParams bp = d_->brush;
+    bp.set = cur_set_;
+    bp.particle_offset = particle_offset;
+    bp.debug = brush_debug_flag();
+    if (!rp) return bp;
+    *rp = d_->ray;
+    rp->points = d_->d_points;
+    rp->scan = d_->scan;
+    rp->set = cur_set_;
+    rp->particle_offset = particle_offset;
+    rp->state_stride = state_stride;
+    { const char* dbg = std::getenv("LAMA_RAY_DEBUG"); rp->debug = dbg ? std::atoi(dbg) : 0; }  // see RayParams::debug
+    const int nb = d_->scan.n_beams;
+    rp->log_cap   = std::min(d_->ray.log_cap, next_pow2_host(std::max(1024, 3 * nb)));
+    rp->event_cap = std::min(d_->ray.event_cap, next_pow2_host(std::max(512, nb)));
+    bp.event_cap = rp->event_cap;
+    return bp;
+}
+
 int Engine::check_device_status()
 {
     uint32_t st = *d_->h_status;
@@ -571,27 +635,20 @@ int Engine::match(const SE2* states, int count, int first_particle, bool shared_
         return fail("match: particle range out of bounds", LAMA_ERR_ARG);
     if (d_->scan.n_beams < 1) return fail("match: no scan uploaded", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
-    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
-    std::memcpy(d_->h_states, states, (size_t)count * sizeof(SE2));
-    CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d_->stream));
-    MatchParams mp{};
-    mp.points = d_->d_points;
-    mp.scan = d_->scan;
-    mp.solver = so;
-    mp.meas_sigma = meas_sigma;
-    mp.resolution = cfg_.resolution;
-    mp.max_sqdist = max_sqdist_;
-    mp.set = cur_set_;
-    mp.particle_offset = first_particle;
-    mp.shared_map = shared_map ? 1 : 0;
-    mp.mode = mode;
-    mp.parked_any = d_->parked(cur_set_) != 0;
+    return match_sync(states, count, match_params(so, meas_sigma, first_particle, shared_map, mode), false, out);
+}
+
+// The synchronous match of match() and, with `extent`, of match_extent() (k_match_extent over its directory).  With parked entries a read
+// outside the window sets kErrWindow (k_match reads it as absent): the caller must not get that result.
+int Engine::match_sync(const SE2* states, int count, const MatchParams& mp, bool extent, HostMatchResult* out)
+{
+    { int rc = upload_states(states, count, d_->stream); if (rc != LAMA_OK) return rc; }
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
-    launch_match(d_->view, mp, d_->d_states, d_->d_results, count, d_->stream);
+    if (extent) launch_match_extent(d_->view, mp, (const int32_t*)d_->d_extent, extent_, d_->d_states, d_->d_results, count, d_->stream);
+    else launch_match(d_->view, mp, d_->d_states, d_->d_results, count, d_->stream);
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(d_->h_results, d_->d_results, (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
-    // with parked entries a read outside the window sets kErrWindow (k_match reads it as absent): the caller must not get that result
     if (mp.parked_any) CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     if (timing_) {
@@ -603,7 +660,6 @@ int Engine::match(const SE2* states, int count, int first_particle, bool shared_
     if (mp.parked_any && *d_->h_status) return check_device_status();
     static_assert(sizeof(HostMatchResult) == sizeof(MatchResult), "layout");
     std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
-    h2d_bytes_ += (uint64_t)count * sizeof(SE2);
     d2h_bytes_ += (uint64_t)count * sizeof(MatchResult);
     return LAMA_OK;
 }
@@ -615,9 +671,7 @@ int Engine::match_error(const SE2* states, int count, int first_particle, bool s
         return fail("match_error: particle range out of bounds", LAMA_ERR_ARG);
     if (d_->scan.n_beams < 1) return fail("match_error: no scan uploaded", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
-    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
-    std::memcpy(d_->h_states, states, (size_t)count * sizeof(SE2));
-    CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d_->stream));
+    { int rc = upload_states(states, count, d_->stream); if (rc != LAMA_OK) return rc; }
     double* d_out = reinterpret_cast<double*>(d_->d_results);   // count doubles fit in count MatchResults
     launch_match_error(d_->view, d_->pv(cur_set_), cur_set_, first_particle, shared_map, d_->d_points, d_->scan, d_->d_states, count, cfg_.resolution, max_sqdist_, d_out, d_->stream);
     CU_TRY(cudaGetLastError());
@@ -634,14 +688,6 @@ int Engine::update_maps(const SE2* states, int first_particle, int count, HostMa
     return settle(out);
 }
 
-// developer builds (LAMA_PHASE_TIMING): LAMA_BF_DEBUG = ordinal of the map update whose k_brushfire prints its per-particle phase cycles
-static int brush_debug_flag()
-{
-    static int launch_no = 0;
-    const char* dbg = std::getenv("LAMA_BF_DEBUG");
-    return dbg && std::atoi(dbg) == launch_no++;
-}
-
 // Launches ray cast + brushfire and returns without waiting; settle() (called by every later entry point)
 // synchronises, collects the per-particle statistics and surfaces device errors.
 int Engine::update_maps_async(const SE2* states, int first_particle, int count)
@@ -651,60 +697,86 @@ int Engine::update_maps_async(const SE2* states, int first_particle, int count)
     if (d_->scan.n_beams < 1) return fail("update_maps: no scan uploaded", LAMA_ERR_STATE);
     { int rc = settle(nullptr); if (rc != LAMA_OK) return rc; }
     CU_TRY(cudaSetDevice(cfg_.device));
-    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
-    std::memcpy(d_->h_states, states, (size_t)count * sizeof(SE2));
-    CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d_->stream));
-    RayParams rp = d_->ray;
-    rp.points = d_->d_points;
-    rp.scan = d_->scan;
-    rp.set = cur_set_;
-    rp.particle_offset = first_particle;
-    rp.state_stride = (int)sizeof(SE2);
-    { const char* dbg = std::getenv("LAMA_RAY_DEBUG"); rp.debug = dbg ? std::atoi(dbg) : 0; }  // see RayParams::debug
-    // shared-memory scratch sized for THIS scan (two CTAs per SM at 1080 beams); the maxima were registered at create
-    const int nb = d_->scan.n_beams;
-    rp.log_cap   = std::min(d_->ray.log_cap, next_pow2_host(std::max(1024, 3 * nb)));
-    rp.event_cap = std::min(d_->ray.event_cap, next_pow2_host(std::max(512, nb)));
-    BrushParams bp = d_->brush;
-    bp.set = cur_set_;
-    bp.particle_offset = first_particle;
-    bp.event_cap = rp.event_cap;
-    bp.debug = brush_debug_flag();
-    if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
-    const int ray_kernels = launch_ray_stage(d_, rp, d_->d_states, count);
-    if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
-    launch_brushfire(d_->view, bp, d_->d_events, d_->d_stats, count, d_->stream);
-    if (timing_) CU_TRY(cudaEventRecord(d_->ev[2], d_->stream));
-    launch_merge_free(d_->view, d_->stream);
-    CU_TRY(cudaGetLastError());
-    { int rc = enqueue_report(count); if (rc != LAMA_OK) return rc; }
-    times_.raycast_launches += ray_kernels;
-    times_.brushfire_launches += 1;
-    times_.misc_launches += 1;
-    h2d_bytes_ += (uint64_t)count * sizeof(SE2);
+    { int rc = upload_states(states, count, d_->stream); if (rc != LAMA_OK) return rc; }
+    RayParams rp;
+    const BrushParams bp = map_update_params((int)sizeof(SE2), first_particle, &rp);
+    { int rc = enqueue_group(nullptr, rp, bp, 0, count, d_->stream, d_->view.counters, 0, nullptr); if (rc != LAMA_OK) return rc; }
+    const int half = 1 - pending_buf_;
+    d_->report_groups[half] = 1;
+    pending_buf_  = half;
+    pending_maps_ = count;
     return LAMA_OK;
 }
 
-// device -> host report of a map update into the other half of the ping-pong buffers (the previous half may not have been read yet)
-int Engine::enqueue_report(int count)
+// Particles [lo, lo + cnt) of a map update on `stream`, their kernels counting patches into `counters` (view.counters on one stream, a
+// group's block of d_gcnt in a grouped step): with `mp`, the match of their predicted states, the copy of its results to the host and
+// `ev_match`, then the map update on the matched poses; without, the map update on the poses in d_states.  Then the ray stage, the
+// brushfire, on one stream k_merge_free, and report g (statistics, status, counter block, free slots) into the half of the host buffers
+// that the pending update does not use.  Timing mode (always one stream) records evp[half] around the kernels.
+int Engine::enqueue_group(const MatchParams* mp, RayParams rp, BrushParams bp, int lo, int cnt, void* stream, uint64_t* counters, int g, void* ev_match)
 {
+    Impl* d = d_;
+    cudaStream_t st = (cudaStream_t)stream;
     const int half = 1 - pending_buf_;
-    MapUpdateStats* hs = d_->h_stats + (size_t)half * cfg_.particles;
-    uint64_t* hr = d_->h_report + (size_t)half * 8;
-    CU_TRY(cudaMemcpyAsync(hs, d_->d_stats, (size_t)count * sizeof(MapUpdateStats), cudaMemcpyDeviceToHost, d_->stream));
-    CU_TRY(cudaMemcpyAsync(hr, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
-    CU_TRY(cudaMemcpyAsync(hr + 1, d_->view.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, d_->stream));
-    CU_TRY(cudaMemcpyAsync(hr + 4, d_->view.free_count, 4, cudaMemcpyDeviceToHost, d_->stream));
-    d2h_bytes_ += (uint64_t)count * sizeof(MapUpdateStats) + 4 + 28;
-    pending_buf_  = half;
-    pending_maps_ = count;
+    cudaEvent_t* ev = timing_ ? d->evp[half] : nullptr;
+    StoreView v = d->view;
+    v.counters = counters;
+    const SE2* poses = d->d_states + lo;
+    if (mp) {
+        MatchParams m = *mp;
+        m.particle_offset += lo;
+        if (ev) CU_TRY(cudaEventRecord(ev[0], st));
+        launch_match(v, m, d->d_states + lo, d->d_results + lo, cnt, st);
+        if (ev) CU_TRY(cudaEventRecord(ev[1], st));
+        CU_TRY(cudaMemcpyAsync(d->h_results + lo, d->d_results + lo, (size_t)cnt * sizeof(MatchResult), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaEventRecord((cudaEvent_t)ev_match, st));
+        poses = reinterpret_cast<const SE2*>(d->d_results + lo);
+        times_.match_launches += 1;
+        d2h_bytes_ += (uint64_t)cnt * sizeof(MatchResult);
+    } else if (ev) {
+        CU_TRY(cudaEventRecord(ev[1], st));
+    }
+    uint64_t* events = d->d_events + (size_t)lo * d->ray.event_cap;
+    rp.particle_offset += lo;
+    const int ray_kernels = d->launch_ray_stage(v, rp, poses, events, d->d_stats + lo, cnt, st);
+    if (ev) CU_TRY(cudaEventRecord(ev[2], st));
+    bp.particle_offset += lo;
+    bp.lower_spill += (size_t)lo * (d->brush.lower_total + 2);
+    bp.raise_spill += (size_t)lo * (d->brush.raise_total + 2);
+    launch_brushfire(v, bp, events, d->d_stats + lo, cnt, st);
+    if (ev) {
+        CU_TRY(cudaEventRecord(ev[3], st));
+        d->evp_used[half]  = true;
+        d->evp_match[half] = mp != nullptr;
+    }
+    // a grouped step returns freed patches at the next barrier: k_merge_free is not safe beside another group's alloc_slot
+    const bool one_stream = counters == d->view.counters;
+    if (one_stream) launch_merge_free(d->view, st);
+    CU_TRY(cudaGetLastError());
+    uint64_t* r = d->h_grep + ((size_t)half * (kMaxGroups + 1) + g) * 8;
+    CU_TRY(cudaMemcpyAsync(d->h_stats + (size_t)half * cfg_.particles + lo, d->d_stats + lo, (size_t)cnt * sizeof(MapUpdateStats), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(r, d->view.status, 4, cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(r + 1, counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    CU_TRY(cudaMemcpyAsync(r + 4, d->view.free_count, 4, cudaMemcpyDeviceToHost, st));
+    times_.raycast_launches += ray_kernels;
+    times_.brushfire_launches += 1;
+    times_.misc_launches += one_stream ? 1 : 0;
+    d2h_bytes_ += (uint64_t)cnt * sizeof(MapUpdateStats) + 4 + 28;
+    return LAMA_OK;
+}
+
+int Engine::check_step(const double* pts, int n, int count)
+{
+    if (count < 1 || count > cfg_.particles) return fail("step: particle range out of bounds", LAMA_ERR_ARG);
+    if (pts && (n < 1 || n > cfg_.max_beams)) return fail("step: number of beams out of range", LAMA_ERR_ARG);
+    if (!pts && d_->scan.n_beams < 1) return fail("step: no scan selected", LAMA_ERR_STATE);
     return LAMA_OK;
 }
 
 int Engine::step_enqueue(const double* pts, int n, const double origin[3], const double quat[4], double truncated_ray, double truncated_range,
                          const SE2* predicted, int count, const SolverOptions& so, double meas_sigma)
 {
-    if (count < 1 || count > cfg_.particles) return fail("step_enqueue: particle range out of bounds", LAMA_ERR_ARG);
+    { int rc = check_step(pts, n, count); if (rc != LAMA_OK) return rc; }
     extent_stale_ = true;
     d_->fork = true;   // a grouped step after this one waits for it
     CU_TRY(cudaSetDevice(cfg_.device));
@@ -713,67 +785,19 @@ int Engine::step_enqueue(const double* pts, int n, const double origin[3], const
     enq_prev_count_  = pending_maps_;
     enq_prev_buf_    = pending_buf_;
     if (pts) {
-        if (n < 1 || n > cfg_.max_beams) return fail("step_enqueue: number of beams out of range", LAMA_ERR_ARG);
         set_moving(origin, quat, truncated_ray, truncated_range, n);
-        std::memcpy(d_->h_scan, pts, (size_t)n * 24);   // free again: the previous call returned after its match, which follows its upload
-        d_->d_points = d_->d_scan_buf;
-        d_->scan_flat = points_flat(pts, (size_t)n);
-        CU_TRY(cudaMemcpyAsync(d_->d_points, d_->h_scan, (size_t)n * 24, cudaMemcpyHostToDevice, d_->stream));
-        h2d_bytes_ += (uint64_t)n * 24;
+        int rc = upload_scan(pts, n, d_->d_scan_buf, d_->stream);
+        if (rc != LAMA_OK) return rc;
     }
-    if (d_->scan.n_beams < 1) return fail("step_enqueue: no scan selected", LAMA_ERR_STATE);
-    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
-    std::memcpy(d_->h_states, predicted, (size_t)count * sizeof(SE2));
-    CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d_->stream));
-    MatchParams mp{};
-    mp.points = d_->d_points;
-    mp.scan = d_->scan;
-    mp.solver = so;
-    mp.meas_sigma = meas_sigma;
-    mp.resolution = cfg_.resolution;
-    mp.max_sqdist = max_sqdist_;
-    mp.set = cur_set_;
-    mp.particle_offset = 0;
-    mp.shared_map = 0;
-    mp.mode = 0;
-    mp.parked_any = d_->parked(cur_set_) != 0;
-    const int tbuf = 1 - pending_buf_;   // the report buffer enqueue_report() will hand to this step
-    if (timing_) CU_TRY(cudaEventRecord(d_->evp[tbuf][0], d_->stream));
-    launch_match(d_->view, mp, d_->d_states, d_->d_results, count, d_->stream);
-    if (timing_) CU_TRY(cudaEventRecord(d_->evp[tbuf][1], d_->stream));
-    CU_TRY(cudaMemcpyAsync(d_->h_results, d_->d_results, (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
-    CU_TRY(cudaEventRecord(d_->ev_match, d_->stream));
-    // map update on the matched poses, read from the match results on the device
-    RayParams rp = d_->ray;
-    rp.points = d_->d_points;
-    rp.scan = d_->scan;
-    rp.set = cur_set_;
-    rp.particle_offset = 0;
-    rp.state_stride = (int)sizeof(MatchResult);
-    const int nb = d_->scan.n_beams;
-    rp.log_cap   = std::min(d_->ray.log_cap, next_pow2_host(std::max(1024, 3 * nb)));
-    rp.event_cap = std::min(d_->ray.event_cap, next_pow2_host(std::max(512, nb)));
-    BrushParams bp = d_->brush;
-    bp.set = cur_set_;
-    bp.particle_offset = 0;
-    bp.event_cap = rp.event_cap;
-    bp.debug = brush_debug_flag();
-    const int ray_kernels = launch_ray_stage(d_, rp, reinterpret_cast<const SE2*>(d_->d_results), count);
-    if (timing_) CU_TRY(cudaEventRecord(d_->evp[tbuf][2], d_->stream));
-    launch_brushfire(d_->view, bp, d_->d_events, d_->d_stats, count, d_->stream);
-    if (timing_) {
-        CU_TRY(cudaEventRecord(d_->evp[tbuf][3], d_->stream));
-        d_->evp_used[tbuf] = true;
-    }
-    launch_merge_free(d_->view, d_->stream);
-    CU_TRY(cudaGetLastError());
-    { int rc = enqueue_report(count); if (rc != LAMA_OK) return rc; }
-    times_.match_launches += 1;
-    times_.raycast_launches += ray_kernels;
-    times_.brushfire_launches += 1;
-    times_.misc_launches += 1;
-    h2d_bytes_ += (uint64_t)count * sizeof(SE2);
-    d2h_bytes_ += (uint64_t)count * sizeof(MatchResult);
+    { int rc = upload_states(predicted, count, d_->stream); if (rc != LAMA_OK) return rc; }
+    const MatchParams mp = match_params(so, meas_sigma, 0, false, 0);
+    RayParams rp;
+    const BrushParams bp = map_update_params((int)sizeof(MatchResult), 0, &rp);
+    { int rc = enqueue_group(&mp, rp, bp, 0, count, d_->stream, d_->view.counters, 0, d_->ev_match); if (rc != LAMA_OK) return rc; }
+    const int half = 1 - pending_buf_;
+    d_->report_groups[half] = 1;
+    pending_buf_  = half;
+    pending_maps_ = count;
     return LAMA_OK;
 }
 
@@ -796,6 +820,7 @@ int Engine::particle_groups() const { return d_->groups; }
 int Engine::step_async(const double* pts, int n, const double origin[3], const double quat[4], double truncated_ray, double truncated_range,
                        const SE2* predicted, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out)
 {
+    { int rc = check_step(pts, n, count); if (rc != LAMA_OK) return rc; }
     // timing mode keeps one stream, so that kernelTimes() still times single kernels
     if (d_->groups > 1 && count > 1 && !timing_) return step_groups(pts, n, origin, quat, truncated_ray, truncated_range, predicted, count, so, meas_sigma, out);
     { int rc = step_enqueue(pts, n, origin, quat, truncated_ray, truncated_range, predicted, count, so, meas_sigma); if (rc != LAMA_OK) return rc; }
@@ -808,8 +833,7 @@ int Engine::step_async(const double* pts, int n, const double origin[3], const d
 // step_async over G particle groups (DESIGN.md 7a).  Group g's stream runs match -> copy of its results -> ray cast -> brushfire -> report of
 // its particles; its particles' chain match(t) -> ray(t) -> brushfire(t) -> match(t + 1) depends on no other group, because the map update
 // runs before the resampling decision, so the groups drift apart and one group's brushfire and next match run beside another group's
-// ray cast.  (LAMA_PF_RAY_ORDER=1 serialises the ray casts across groups -- ray(g + 1) after ray(g), ray(0) of the next scan after
-// ray(G - 1) -- which measured slower.)  The launching stream waits for every group at the end (its events keep meaning "this scan's
+// ray cast.  The launching stream waits for every group at the end (its events keep meaning "this scan's
 // map update has completed"); the groups wait for the launching stream only after settle(), which every other entry point calls first:
 // that is the barrier behind which resampling, window shifts, checkpoints, exports and k_merge_free run.  Patches freed by a grouped
 // scan go back to the free stack at the next barrier (k_merge_free is not safe beside a running alloc_slot), and a barrier is forced
@@ -818,9 +842,6 @@ int Engine::step_async(const double* pts, int n, const double origin[3], const d
 int Engine::step_groups(const double* pts, int n, const double origin[3], const double quat[4], double truncated_ray, double truncated_range,
                         const SE2* predicted, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out)
 {
-    if (count < 1 || count > cfg_.particles) return fail("step_async: particle range out of bounds", LAMA_ERR_ARG);
-    if (pts && (n < 1 || n > cfg_.max_beams)) return fail("step_async: number of beams out of range", LAMA_ERR_ARG);
-    if (!pts && d_->scan.n_beams < 1) return fail("step_async: no scan selected", LAMA_ERR_STATE);
     Impl* d = d_;
     if (d->groups_ran) {
         const uint64_t reserve = 2 * std::max<uint64_t>(d->scan_alloc, (uint64_t)count * d->view.n_kinds);
@@ -841,91 +862,35 @@ int Engine::step_groups(const double* pts, int n, const double origin[3], const 
         for (int g = 0; g < d->groups; ++g) CU_TRY(cudaStreamWaitEvent(d->gstream[g], d->ev_fork, 0));
         d->fork = false;
     }
-    // uploads: the host buffers are free (the previous call waited for every match, which follows its upload); the scan goes to the half of
-    // d_scan_buf the previous scan did not use, since that scan's later ray casts may still be reading it
+    // uploads: the scan goes to the half of d_scan_buf the previous scan did not use, since that scan's later ray casts may still be reading it
     if (pts) {
         set_moving(origin, quat, truncated_ray, truncated_range, n);
-        std::memcpy(d->h_scan, pts, (size_t)n * 24);
         d->scan_half ^= 1;
-        d->d_points = d->d_scan_buf + (size_t)d->scan_half * cfg_.max_beams * 3;
-        d->scan_flat = points_flat(pts, (size_t)n);
-        CU_TRY(cudaMemcpyAsync(d->d_points, d->h_scan, (size_t)n * 24, cudaMemcpyHostToDevice, d->up_stream));
-        h2d_bytes_ += (uint64_t)n * 24;
+        int rc = upload_scan(pts, n, d->d_scan_buf + (size_t)d->scan_half * cfg_.max_beams * 3, d->up_stream);
+        if (rc != LAMA_OK) return rc;
     }
-    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
-    std::memcpy(d->h_states, predicted, (size_t)count * sizeof(SE2));
-    CU_TRY(cudaMemcpyAsync(d->d_states, d->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d->up_stream));
+    { int rc = upload_states(predicted, count, d->up_stream); if (rc != LAMA_OK) return rc; }
     CU_TRY(cudaEventRecord(d->ev_up, d->up_stream));
-
-    MatchParams mp{};
-    mp.points = d->d_points;
-    mp.scan = d->scan;
-    mp.solver = so;
-    mp.meas_sigma = meas_sigma;
-    mp.resolution = cfg_.resolution;
-    mp.max_sqdist = max_sqdist_;
-    mp.set = cur_set_;
-    mp.shared_map = 0;
-    mp.mode = 0;
-    mp.parked_any = d->parked(cur_set_) != 0;
-    RayParams rp = d->ray;
-    rp.points = d->d_points;
-    rp.scan = d->scan;
-    rp.set = cur_set_;
-    rp.state_stride = (int)sizeof(MatchResult);
-    const int nb = d->scan.n_beams;
-    rp.log_cap   = std::min(d->ray.log_cap, next_pow2_host(std::max(1024, 3 * nb)));
-    rp.event_cap = std::min(d->ray.event_cap, next_pow2_host(std::max(512, nb)));
-    BrushParams bp = d->brush;
-    bp.set = cur_set_;
-    bp.event_cap = rp.event_cap;
-    bp.debug = brush_debug_flag();
+    const MatchParams mp = match_params(so, meas_sigma, 0, false, 0);
+    RayParams rp;
+    const BrushParams bp = map_update_params((int)sizeof(MatchResult), 0, &rp);
     const int half = 1 - pending_buf_;
-    MapUpdateStats* hs = d->h_stats + (size_t)half * cfg_.particles;
-    uint64_t* hr = d->h_grep + (size_t)half * (kMaxGroups + 1) * 8;
-    cudaEvent_t ray_before = d->ray_order && d->last_groups ? d->ev_gray[d->last_groups - 1] : nullptr;
     for (int g = 0; g < G; ++g) {
         const int lo = (int)((int64_t)g * count / G), cnt = (int)((int64_t)(g + 1) * count / G) - lo;
         cudaStream_t st = d->gstream[g];
-        StoreView v = d->view;
-        v.counters = d->d_gcnt + (size_t)g * 4;
         CU_TRY(cudaStreamWaitEvent(st, d->ev_up, 0));
-        mp.particle_offset = lo;
-        launch_match(v, mp, d->d_states + lo, d->d_results + lo, cnt, st);
-        CU_TRY(cudaMemcpyAsync(d->h_results + lo, d->d_results + lo, (size_t)cnt * sizeof(MatchResult), cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaEventRecord(d->ev_gmatch[g], st));
-        if (ray_before) CU_TRY(cudaStreamWaitEvent(st, ray_before, 0));
-        rp.particle_offset = lo;
-        launch_raycast(v, rp, reinterpret_cast<const SE2*>(d->d_results + lo), d->d_events + (size_t)lo * d->ray.event_cap, d->d_stats + lo, cnt, st);
-        CU_TRY(cudaEventRecord(d->ev_gray[g], st));
-        ray_before = d->ray_order ? d->ev_gray[g] : nullptr;
-        bp.particle_offset = lo;
-        bp.lower_spill = d->brush.lower_spill + (size_t)lo * (d->brush.lower_total + 2);
-        bp.raise_spill = d->brush.raise_spill + (size_t)lo * (d->brush.raise_total + 2);
-        launch_brushfire(v, bp, d->d_events + (size_t)lo * d->ray.event_cap, d->d_stats + lo, cnt, st);
-        CU_TRY(cudaGetLastError());
-        // this group's report: its statistics, its counter block, status and free slots; group 0 also copies view.counters, which no kernel
-        // of a grouped step writes
-        uint64_t* r = hr + (size_t)g * 8;
-        CU_TRY(cudaMemcpyAsync(hs + lo, d->d_stats + lo, (size_t)cnt * sizeof(MapUpdateStats), cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaMemcpyAsync(r, d->view.status, 4, cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaMemcpyAsync(r + 1, v.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-        CU_TRY(cudaMemcpyAsync(r + 4, d->view.free_count, 4, cudaMemcpyDeviceToHost, st));
-        if (g == 0) CU_TRY(cudaMemcpyAsync(hr + (size_t)G * 8 + 1, d->view.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        { int rc = enqueue_group(&mp, rp, bp, lo, cnt, st, d->d_gcnt + (size_t)g * 4, g, d->ev_gmatch[g]); if (rc != LAMA_OK) return rc; }
+        if (g == 0) {   // view.counters, which no kernel of a grouped step writes, into slot G of the report
+            CU_TRY(cudaMemcpyAsync(d->h_grep + ((size_t)half * (kMaxGroups + 1) + G) * 8 + 1, d->view.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+            d2h_bytes_ += 24;
+        }
         CU_TRY(cudaEventRecord(d->ev_gdone[g], st));
-        d2h_bytes_ += (uint64_t)cnt * sizeof(MapUpdateStats) + 4 + 28 + (g == 0 ? 24 : 0);
     }
     for (int g = 0; g < G; ++g) CU_TRY(cudaStreamWaitEvent(d->stream, d->ev_gdone[g], 0));   // the launching stream joins every group
-    d->last_groups = G;
     d->groups_ran = true;
     d->report_groups[half] = G;
     pending_buf_  = half;
     pending_maps_ = count;
-    times_.match_launches += G;
-    times_.raycast_launches += G;
-    times_.brushfire_launches += G;
-    h2d_bytes_ += (uint64_t)count * sizeof(SE2);
-    d2h_bytes_ += (uint64_t)count * sizeof(MatchResult);
     for (int g = 0; g < G; ++g) CU_TRY(cudaEventSynchronize(d->ev_gmatch[g]));
     static_assert(sizeof(HostMatchResult) == sizeof(MatchResult), "layout");
     std::memcpy(out, d->h_results, (size_t)count * sizeof(MatchResult));
@@ -983,49 +948,40 @@ int Engine::settle(HostMapStats* out, bool already_complete)
         }
         return LAMA_OK;
     }
-    const int count = pending_maps_;
+    const int count = pending_maps_, half = pending_buf_;
     pending_maps_ = 0;
     CU_TRY(cudaSetDevice(cfg_.device));
     if (!already_complete) CU_TRY(cudaStreamSynchronize(d_->stream));
-    if (timing_ && d_->evp_used[pending_buf_]) {   // a pipelined step: its four events have completed (the stream is past them, or was just synchronised)
+    if (timing_ && d_->evp_used[half]) {   // the update's events have completed (the stream is past them, or was just synchronised)
+        const cudaEvent_t* e = d_->evp[half];
         float m = 0, a = 0, b = 0;
-        cudaEventElapsedTime(&m, d_->evp[pending_buf_][0], d_->evp[pending_buf_][1]);
-        cudaEventElapsedTime(&a, d_->evp[pending_buf_][1], d_->evp[pending_buf_][2]);
-        cudaEventElapsedTime(&b, d_->evp[pending_buf_][2], d_->evp[pending_buf_][3]);
+        if (d_->evp_match[half]) cudaEventElapsedTime(&m, e[0], e[1]);
+        cudaEventElapsedTime(&a, e[1], e[2]);
+        cudaEventElapsedTime(&b, e[2], e[3]);
         times_.match_ms += m;
         times_.raycast_ms += a;
         times_.brushfire_ms += b;
-        d_->evp_used[pending_buf_] = false;
-    } else if (timing_ && !already_complete) {
-        float a = 0, b = 0;
-        cudaEventElapsedTime(&a, d_->ev[0], d_->ev[1]);
-        cudaEventElapsedTime(&b, d_->ev[1], d_->ev[2]);
-        times_.raycast_ms += a;
-        times_.brushfire_ms += b;
+        d_->evp_used[half] = false;
     }
     static_assert(sizeof(HostMapStats) == sizeof(MapUpdateStats), "layout");
-    const MapUpdateStats* hs = d_->h_stats + (size_t)pending_buf_ * cfg_.particles;
+    const MapUpdateStats* hs = d_->h_stats + (size_t)half * cfg_.particles;
     last_map_stats_.assign((const HostMapStats*)hs, (const HostMapStats*)hs + count);
     if (out) std::memcpy(out, hs, (size_t)count * sizeof(MapUpdateStats));
-    if (const int G = d_->report_groups[pending_buf_]) {   // a grouped step: view.counters plus every group's block
-        d_->report_groups[pending_buf_] = 0;
-        const uint64_t* hr = d_->h_grep + (size_t)pending_buf_ * (kMaxGroups + 1) * 8;
-        uint32_t status = 0;
-        for (int c = 0; c < 3; ++c) settled_counters_[c] = hr[(size_t)G * 8 + 1 + c];
-        for (int g = 0; g < G; ++g) {
-            status |= (uint32_t)hr[g * 8];
-            for (int c = 0; c < 3; ++c) settled_counters_[c] += hr[g * 8 + 1 + c];
-        }
-        settled_counters_[3] = (uint64_t)(uint32_t)hr[(G - 1) * 8 + 4];
-        *d_->h_status = status;
+    // view.counters plus every group's block; one group is a map update on one stream, whose block is view.counters itself
+    const int G = d_->report_groups[half];
+    const uint64_t* hr = d_->h_grep + (size_t)half * (kMaxGroups + 1) * 8;
+    uint32_t status = 0;
+    for (int c = 0; c < 3; ++c) settled_counters_[c] = G > 1 ? hr[(size_t)G * 8 + 1 + c] : 0;
+    for (int g = 0; g < G; ++g) {
+        status |= (uint32_t)hr[g * 8];
+        for (int c = 0; c < 3; ++c) settled_counters_[c] += hr[g * 8 + 1 + c];
+    }
+    settled_counters_[3] = (uint64_t)(uint32_t)hr[(G - 1) * 8 + 4];
+    *d_->h_status = status;
+    if (G > 1) {
         const uint64_t alloc = settled_counters_[0] + settled_counters_[1];
         d_->scan_alloc = d_->prev_alloc && alloc > d_->prev_alloc ? alloc - d_->prev_alloc : 0;
         d_->prev_alloc = alloc;
-    } else {
-        const uint64_t* hr = d_->h_report + (size_t)pending_buf_ * 8;
-        settled_counters_[0] = hr[1]; settled_counters_[1] = hr[2]; settled_counters_[2] = hr[3];
-        settled_counters_[3] = (uint64_t)(uint32_t)hr[4];
-        *d_->h_status = (uint32_t)hr[0];
     }
     if (!already_complete && d_->groups_ran) {
         int rc = fold_groups();
@@ -1440,9 +1396,7 @@ int Engine::dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_a
         uint64_t* dev_ev = d_->d_events + (size_t)particle * cap;
         CU_TRY(cudaMemcpyAsync(dev_ev, ev.data(), (size_t)m * 8, cudaMemcpyHostToDevice, d_->stream));
         CU_TRY(cudaMemcpyAsync(d_->d_stats + particle, &st, sizeof(st), cudaMemcpyHostToDevice, d_->stream));
-        BrushParams bp = d_->brush;
-        bp.set = cur_set_;
-        bp.particle_offset = particle;
+        const BrushParams bp = map_update_params(0, particle, nullptr);
         // block 0 of this launch must read the event list / stats of `particle`
         launch_brushfire(d_->view, bp, dev_ev, d_->d_stats + particle, 1, d_->stream);
         launch_merge_free(d_->view, d_->stream);
@@ -1485,36 +1439,9 @@ int Engine::match_extent(const SE2* states, int count, const SolverOptions& so, 
         extent_ = xw;
         extent_stale_ = false;
     }
-    { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
-    std::memcpy(d_->h_states, states, (size_t)count * sizeof(SE2));
-    CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, d_->stream));
-    MatchParams mp{};
-    mp.points = d_->d_points;
-    mp.scan = d_->scan;
-    mp.solver = so;
-    mp.meas_sigma = meas_sigma;
-    mp.resolution = cfg_.resolution;
-    mp.max_sqdist = max_sqdist_;
-    mp.set = cur_set_;
-    mp.particle_offset = 0;
-    mp.shared_map = 1;
-    mp.mode = 1;
-    if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
-    launch_match_extent(d_->view, mp, (const int32_t*)d_->d_extent, extent_, d_->d_states, d_->d_results, count, d_->stream);
-    if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
-    CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(d_->h_results, d_->d_results, (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
-    CU_TRY(cudaStreamSynchronize(d_->stream));
-    if (timing_) {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, d_->ev[0], d_->ev[1]);
-        times_.match_ms += ms;
-    }
-    times_.match_launches += 1;
-    std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
-    h2d_bytes_ += (uint64_t)count * sizeof(SE2);
-    d2h_bytes_ += (uint64_t)count * sizeof(MatchResult);
-    return LAMA_OK;
+    MatchParams mp = match_params(so, meas_sigma, 0, true, 1);
+    mp.parked_any = 0;   // k_match_extent reads parked patches through its directory: no read sets kErrWindow
+    return match_sync(states, count, mp, true, out);
 }
 
 int Engine::sampling_likelihood(int particle, const SE2& pose, const double* offsets_xy, int n, int stride, double* out)

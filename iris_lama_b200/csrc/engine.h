@@ -13,6 +13,10 @@
 
 namespace lama_b200 {
 
+struct MatchParams;   // kernels.cuh
+struct RayParams;
+struct BrushParams;
+
 struct EngineConfig {
     int device        = 0;
     int particles     = 1;      // particles resident on THIS device
@@ -260,6 +264,13 @@ private:
     Engine() = default;
     Impl* d_ = nullptr;
     int ensure_states(int count);
+    int upload_states(const SE2* states, int count, void* stream);        // `stream`: cudaStream_t
+    int upload_scan(const double* pts, int n, double* dst, void* stream);
+    MatchParams match_params(const SolverOptions& so, double meas_sigma, int first_particle, bool shared_map, int mode) const;
+    BrushParams map_update_params(int state_stride, int particle_offset, RayParams* rp) const;
+    int match_sync(const SE2* states, int count, const MatchParams& mp, bool extent, HostMatchResult* out);
+    int enqueue_group(const MatchParams* mp, RayParams rp, BrushParams bp, int lo, int cnt, void* stream, uint64_t* counters, int g, void* ev_match);
+    int check_step(const double* pts, int n, int count);
     EngineConfig cfg_;
     DirWindow window_{};
     uint32_t max_sqdist_ = 0;
@@ -283,7 +294,6 @@ private:
                     const SE2* predicted, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out);
     int fold_groups();
     void set_moving(const double origin[3], const double quat[4], double truncated_ray, double truncated_range, int n);
-    int enqueue_report(int count);
     int fail(const std::string& what, int code);
     int check_device_status();
 };

@@ -326,6 +326,34 @@ void PFSlam2D::finish_counters()
     total_.add(last_);
 }
 
+// Start of a pipelined scan.  `moved` false = motion gate (pf_slam2d.cpp:215-222): the previous scan's counters are booked and nothing else
+// happens for this scan.  Otherwise the previous scan's counters go to *prev (*prev_pending: its map update is still to be collected)
+// and a staged scan is selected (*staged: the step uploads no scan).
+int PFSlam2D::begin_step(const double* origin, const double* quat, bool moved, bool* did_update, Counters* prev, bool* prev_pending, bool* staged)
+{
+    if (!moved) {
+        int rcs = settle_counters();
+        last_ = Counters();
+        last_idx_.clear();
+        staged_index_ = -1;
+        return rcs;
+    }
+    *did_update = true;
+    *prev = last_;
+    *prev_pending = counters_pending_;
+    counters_pending_ = false;
+    last_ = Counters();
+    last_idx_.clear();
+    const int index = staged_index_;
+    staged_index_ = -1;
+    *staged = index >= 0;
+    if (*staged) {
+        int rc = eng_->select_staged(index, origin, quat, opt_.truncated_ray, opt_.truncated_range);
+        if (rc != LAMA_OK) return engine_fail(rc);
+    }
+    return LAMA_OK;
+}
+
 // The whole scan enqueued at once (Engine::step_async): odometry sampling on the host, then match -> ray cast -> brushfire
 // back to back on the device.  The map update runs on the matched poses BEFORE the resampling decision; a resampling of
 // this scan then shares the UPDATED maps, which is the reference's resample-then-update with the two steps commuted
@@ -336,29 +364,13 @@ void PFSlam2D::finish_counters()
 int PFSlam2D::pipelined_begin(const double* pts, int n, const double* origin, const double* quat, bool moved, bool* did_update, double* local_out)
 {
     pending_maps_ = false;
-    if (!moved) {
-        int rcs = settle_counters();
-        last_ = Counters();
-        last_idx_.clear();
-        staged_index_ = -1;
-        return rcs;
-    }
-    *did_update = true;
-    Counters prev = last_;
-    const bool prev_pending = counters_pending_;
-    counters_pending_ = false;
-    last_ = Counters();
-    last_idx_.clear();
-    const int staged = staged_index_;
-    staged_index_ = -1;
-    int rc = LAMA_OK;
-    if (staged >= 0) {
-        rc = eng_->select_staged(staged, origin, quat, opt_.truncated_ray, opt_.truncated_range);
-        if (rc != LAMA_OK) return engine_fail(rc);
-    }
+    Counters prev;
+    bool prev_pending = false, staged = false;
+    int rc = begin_step(origin, quat, moved, did_update, &prev, &prev_pending, &staged);
+    if (rc != LAMA_OK || !moved) return rc;
     const int nl = hi_ - lo_;
     std::vector<HostMatchResult> res((size_t)nl);
-    rc = eng_->step_async(staged >= 0 ? nullptr : pts, n, origin, quat, opt_.truncated_ray, opt_.truncated_range, &pose_[lo_], nl,
+    rc = eng_->step_async(staged ? nullptr : pts, n, origin, quat, opt_.truncated_ray, opt_.truncated_range, &pose_[lo_], nl,
                           make_solver(0, opt_.max_iter), opt_.meas_sigma, res.data());   // GaussNewton + CauchyWeight(0.15), pf_slam2d.cpp:423-427
     if (prev_pending) {
         collect_map_stats(prev);
@@ -468,28 +480,12 @@ int PFSlam2D::update_sharded(const double* pts, int n, const double* origin, con
     const bool moved = predict_and_gate(odom_xyr);
     const auto t1 = clk::now();
     t_sample_ += ms(t0, t1);
-    if (!moved) {
-        int rcs = settle_counters();
-        last_ = Counters();
-        last_idx_.clear();
-        staged_index_ = -1;
-        return rcs;
-    }
-    *did_update = true;
-    Counters prev = last_;
-    const bool prev_pending = counters_pending_;
-    counters_pending_ = false;
-    last_ = Counters();
-    last_idx_.clear();
-    const int staged = staged_index_;
-    staged_index_ = -1;
-    int rc = LAMA_OK;
-    if (staged >= 0) {
-        rc = eng_->select_staged(staged, origin, quat, opt_.truncated_ray, opt_.truncated_range);
-        if (rc != LAMA_OK) return engine_fail(rc);
-    }
+    Counters prev;
+    bool prev_pending = false, staged = false;
+    int rc = begin_step(origin, quat, moved, did_update, &prev, &prev_pending, &staged);
+    if (rc != LAMA_OK || !moved) return rc;
     const int nl = hi_ - lo_, G = (int)opt_.shard_count;
-    rc = eng_->step_enqueue(staged >= 0 ? nullptr : pts, n, origin, quat, opt_.truncated_ray, opt_.truncated_range, &pose_[lo_], nl, make_solver(0, opt_.max_iter),
+    rc = eng_->step_enqueue(staged ? nullptr : pts, n, origin, quat, opt_.truncated_ray, opt_.truncated_range, &pose_[lo_], nl, make_solver(0, opt_.max_iter),
                             opt_.meas_sigma);
     if (rc != LAMA_OK) return engine_fail(rc);
     const size_t payload = (size_t)nl * kShardF + 1;

@@ -118,6 +118,7 @@ public:
     struct Node { SE2 pose; int parent; };
     bool maps_enqueued_ = false;   // sharded ranks: this scan's map update was enqueued together with its match
     int settle_counters();
+    int begin_step(const double* origin, const double* quat, bool moved, bool* did_update, Counters* prev, bool* prev_pending, bool* staged);
     int pipelined_begin(const double* pts, int n, const double* origin, const double* quat, bool moved, bool* did_update, double* local_out);
     int update_pipelined(const double* pts, int n, const double* origin, const double* quat, const double odom_xyr[3], bool* did_update);
     void collect_map_stats(Counters& c);

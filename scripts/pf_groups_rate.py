@@ -1,13 +1,12 @@
 """Scans/s of PFSlam2D at the benchmark size with the step pipelined over G particle groups (Engine::step_groups, DESIGN.md 7a), for
-G = 1 .. 4 (or the --settings given), with and without the edge that serialises the groups' ray casts; then, in a separate profiled run per setting, the mean
-duration of each kernel launch, which shows how much the groups stretch each other's kernels.
+G = 1 .. 4 (or the --groups given); then, in a separate profiled run per setting, the mean duration of each kernel launch, which shows how much the groups stretch each other's kernels.
 
-  python scripts/pf_groups_rate.py [--particles 256] [--rounds 3] [--settings 1:1,2:1,2:0,...] [--regime revisit|forced] [--out FILE]
+  python scripts/pf_groups_rate.py [--particles 256] [--rounds 3] [--groups 1,2,3,4] [--regime revisit|forced] [--out FILE]
 
 Timing as in bench.py's `value` (--regime revisit: scans 306 .. 405 after 300 map-building scans) or its `resample_forced` regime
 (--regime forced: meas_sigma_gain 0.0008, scans 60 .. 139): staged scans, one CUDA event pair per step on the launching stream, scans/s = steps / sum of the
-steps.  The settings are alternated round by round; the table gives the median and the spread over the rounds.  LAMA_PF_GROUPS and
-LAMA_PF_RAY_ORDER are read when an engine is created (on the first update), so each setting gets a fresh filter."""
+steps.  The settings are alternated round by round; the table gives the median and the spread over the rounds.  LAMA_PF_GROUPS is read
+when an engine is created (on the first update), so each setting gets a fresh filter."""
 import argparse
 import json
 import os
@@ -23,9 +22,8 @@ sys.path.insert(0, ROOT)
 KERNELS = ("k_match", "k_raycast", "k_brushfire")
 
 
-def make_filter(api, ds, stream, P, groups, order, gain):
+def make_filter(api, ds, stream, P, groups, gain):
     os.environ["LAMA_PF_GROUPS"] = str(groups)
-    os.environ["LAMA_PF_RAY_ORDER"] = "1" if order else "0"
     try:
         kw = {"meas_sigma_gain": gain} if gain else {}
         pf = api.PFSlam2D(api.PFSlam2D.Options(P, trans_thresh=0.05, rot_thresh=0.05, seed=42, stream=stream.cuda_stream, **kw))
@@ -34,12 +32,11 @@ def make_filter(api, ds, stream, P, groups, order, gain):
         pf.updateStaged(0, ds.odom[0])   # creates the engine
     finally:
         os.environ.pop("LAMA_PF_GROUPS", None)
-        os.environ.pop("LAMA_PF_RAY_ORDER", None)
     return pf
 
 
-def timed(torch, api, ds, stream, P, groups, order, first, steps, gain):
-    pf = make_filter(api, ds, stream, P, groups, order, gain)
+def timed(torch, api, ds, stream, P, groups, first, steps, gain):
+    pf = make_filter(api, ds, stream, P, groups, gain)
     for t in range(1, first):
         pf.updateStaged(t, ds.odom[t])
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(steps + 1)]
@@ -54,10 +51,10 @@ def timed(torch, api, ds, stream, P, groups, order, first, steps, gain):
     return steps / (sum(ms) * 1e-3), float(np.median(ms)), (st.tobytes(), w.tobytes(), pf.resampleDigest())
 
 
-def profiled(torch, api, ds, stream, P, groups, order, first, steps, gain):
+def profiled(torch, api, ds, stream, P, groups, first, steps, gain):
     """mean device duration of each kernel over `steps` scans, from the profiler's CUDA activity records"""
     from torch.profiler import ProfilerActivity, profile
-    pf = make_filter(api, ds, stream, P, groups, order, gain)
+    pf = make_filter(api, ds, stream, P, groups, gain)
     for t in range(1, first):
         pf.updateStaged(t, ds.odom[t])
     torch.cuda.synchronize()
@@ -85,7 +82,7 @@ def main():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--prebuild", type=int, default=300)
     ap.add_argument("--profile-steps", type=int, default=30)
-    ap.add_argument("--settings", default="1:1,2:1,2:0,3:1,3:0,4:1,4:0", help="G:ray_order pairs")
+    ap.add_argument("--groups", default="1,2,3,4", help="comma-separated G")
     ap.add_argument("--regime", default="revisit", choices=["revisit", "forced"])
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
@@ -98,23 +95,23 @@ def main():
     a.steps = steps
     ds = synth.make_dataset("loop", first + a.steps, n_beams=1080)
     stream = torch.cuda.Stream()
-    settings = [(int(x.split(":")[0]), x.split(":")[1] == "1") for x in a.settings.split(",")]
+    settings = [int(x) for x in a.groups.split(",")]
     rates = {s: [] for s in settings}
     med = {s: [] for s in settings}
     ref = None
     for r in range(a.rounds):
         for s in (settings if r % 2 == 0 else settings[::-1]):
-            v, m, res = timed(torch, api, ds, stream, a.particles, s[0], s[1], first, a.steps, gain)
+            v, m, res = timed(torch, api, ds, stream, a.particles, s, first, a.steps, gain)
             if ref is None:
                 ref = res
             assert res[0] == ref[0] and res[1] == ref[1] and res[2] == ref[2], ("results differ from G = 1", s)
             rates[s].append(v)
             med[s].append(m)
-            print(f"round {r} G={s[0]} ray_order={int(s[1])}: {v:8.1f} scans/s  median step {m:.4f} ms", flush=True)
+            print(f"round {r} G={s}: {v:8.1f} scans/s  median step {m:.4f} ms", flush=True)
     prof = {}
     for s in settings:
         try:
-            prof[s] = profiled(torch, api, ds, stream, a.particles, s[0], s[1], first, min(a.profile_steps, a.steps), gain)
+            prof[s] = profiled(torch, api, ds, stream, a.particles, s, first, min(a.profile_steps, a.steps), gain)
         except Exception as e:   # the profiler is a diagnostic: its absence does not void the rates
             prof[s] = {"error": repr(e)}
     name = torch.cuda.get_device_name(0)
@@ -125,16 +122,16 @@ def main():
         pl = "unknown"
     print(f"\n{name}, power limit / max SM clock: {pl}; {a.particles} particles x 1080 beams, scans {first} .. {first + a.steps - 1} ({a.regime}), "
           f"{a.rounds} alternated rounds")
-    print("G  ray order   scans/s median   min .. max        median step ms   k_match  k_raycast  k_brushfire (ms per scan, profiled)")
+    print("G  scans/s median   min .. max        median step ms   k_match  k_raycast  k_brushfire (ms per scan, profiled)")
     base = float(np.median(rates[settings[0]]))
     rows = []
     for s in settings:
         v = np.asarray(rates[s])
         p = prof[s]
         ks = "  ".join(f"{p[k]['ms_per_scan']:.3f}" if k in p else "  -  " for k in KERNELS)
-        print(f"{s[0]}  {'on ' if s[1] else 'off'}        {np.median(v):9.1f}   {v.min():7.1f} .. {v.max():7.1f}   {np.median(med[s]):.4f}"
+        print(f"{s}  {np.median(v):9.1f}   {v.min():7.1f} .. {v.max():7.1f}   {np.median(med[s]):.4f}"
               f"          {ks}   ({np.median(v) / base - 1:+.1%})")
-        rows.append({"groups": s[0], "ray_order": s[1], "scans_per_s": v.tolist(), "median_step_ms": med[s], "kernels": p})
+        rows.append({"groups": s, "scans_per_s": v.tolist(), "median_step_ms": med[s], "kernels": p})
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, "w") as f:
