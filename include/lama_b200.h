@@ -262,6 +262,29 @@ int lama_loc_set_seed(lama_loc* h, uint32_t seed);                            /*
 int lama_loc_trigger_global_localization(lama_loc* h);                        /* Loc2D::triggerGlobalLocalization, loc2d.cpp:194-197 */
 int lama_loc_global_localization_active(lama_loc* h, int* active);
 
+/* ---- Loc2DFleet: many robots localising on one shared map ----
+ * Robot r gives what a lama_loc with the same options, map contents and seed gives when it is fed only r's calls in the same order,
+ * whatever the other robots of a call.  One update round makes one device launch per step for all its robots (the global-localisation
+ * candidates, the tracking matches, the sampling likelihoods) and one read-back.  The window never moves: on a following map with
+ * parked patches (lama_dm_set_follow) every read goes through a directory of the whole map, which may span at most 4 096 patches. */
+typedef struct lama_locf lama_locf;
+int lama_locf_create(const lama_loc_options* o, int n_robots, lama_locf** out);
+int lama_locf_destroy(lama_locf* h);
+int lama_locf_distance_map(lama_locf* h, lama_dm** dm);                       /* borrowed, shared by every robot */
+int lama_locf_occupancy_set(lama_locf* h, const uint32_t* cells_xy, int n, int state);
+int lama_locf_occupancy_read(lama_locf* h, const char* path);
+int lama_locf_set_pose(lama_locf* h, int robot, const double xyr[3]);
+int lama_locf_set_seed(lama_locf* h, int robot, uint32_t seed);
+int lama_locf_trigger_global_localization(lama_locf* h, int robot);
+int lama_locf_global_localization_active(lama_locf* h, int robot, int* active);
+/* robots[k] (distinct, in [0, n_robots)) takes scan k: the next n_points[k] (1 .. max_beams) points of pts_xyz, sensor origin
+ * origins + 3k and quaternion quats + 4k (NULL: identity for all), odometry odom_xyr + 3k, force[k] (NULL: none).  did_update[k] as
+ * lama_loc_update.  Bad arguments return LAMA_ERR_ARG with no robot changed. */
+int lama_locf_update(lama_locf* h, int count, const int* robots, const double* pts_xyz, const int* n_points, const double* origins, const double* quats,
+                     const double* odom_xyr, const int* force, int* did_update);
+/* every robot: state[r*4] {cos, sin, x, y}, cov[r*9], rmse[r], stats[r*2] {iterations, residual evaluations}; NULL outputs are skipped */
+int lama_locf_get(lama_locf* h, double* state, double* cov, double* rmse, uint32_t* stats);
+
 /* ------------------------------------------------------------------------------------------------
  * SDM grid interface on a device-resident DynamicDistanceMap
  * include/lama/sdm/distance_map.h:66-70, dynamic_distance_map.h:55-66

@@ -98,6 +98,8 @@ EXPORTED_SYMBOLS = [
     "lama_dm3_export_image", "lama_dm3_kernel_times", "lama_dm3_run_stats", "lama_om3_insert_point_clouds_dm3",
     "lama_pf_save_state", "lama_pf_load_state", "lama_slam_save_state", "lama_slam_load_state", "lama_checkpoint_last_stats",
     "lama_graph_save_state", "lama_graph_load_state", "lama_pf_save_shard_state", "lama_pf_load_state_sharded",
+    "lama_locf_create", "lama_locf_destroy", "lama_locf_distance_map", "lama_locf_occupancy_set", "lama_locf_occupancy_read", "lama_locf_set_pose",
+    "lama_locf_set_seed", "lama_locf_trigger_global_localization", "lama_locf_global_localization_active", "lama_locf_update", "lama_locf_get",
 ]
 
 
@@ -1537,3 +1539,92 @@ class Loc2D:
         s = np.zeros(2, np.uint32)
         _chk(lib().lama_loc_get_solve_stats(self.h, s.ctypes.data_as(c_u32p)))
         return s
+
+
+def _fleet_update_args(robots, scans, odoms, force=None, origins=None, quats=None):
+    """the arrays of lama_locf_update: robot indices, the scans' points back to back (xyz), points per scan, sensor origins (k x 3) and
+    quaternions (k x 4, xyzw) or None, odometry (k x 3), force flags or None"""
+    rb = np.ascontiguousarray(robots, dtype=np.int32).reshape(-1)
+    k = rb.size
+    if len(scans) != k:
+        raise ValueError("one scan per robot")
+    sc = [np.asarray(p, dtype=np.float64).reshape(-1, 3) for p in scans]
+    pts = np.ascontiguousarray(np.concatenate(sc) if k else np.zeros((0, 3)))
+    n = np.array([p.shape[0] for p in sc], np.int32)
+    od = np.ascontiguousarray(odoms, dtype=np.float64).reshape(k, 3)
+    fo = None if force is None else np.ascontiguousarray(force, dtype=np.int32).reshape(k)
+    org = None if origins is None else np.ascontiguousarray(origins, dtype=np.float64).reshape(k, 3)
+    qt = None if quats is None else np.ascontiguousarray(quats, dtype=np.float64).reshape(k, 4)
+    return rb, pts, n, org, qt, od, fo
+
+
+class Loc2DFleet:
+    """Many robots localising on one shared map (lama_locf_*).  Robot r gives what a Loc2D with the same options, map and seed gives
+    when it is fed only r's calls in the same order.  update() matches every robot of a call in one device launch per step."""
+
+    Options = Loc2D.Options
+
+    def __init__(self, options: LocOptions, robots: int):
+        self.options = options
+        self.robots = int(robots)
+        self.h = C.c_void_p()
+        _chk(lib().lama_locf_create(C.byref(options), C.c_int(self.robots), C.byref(self.h)))
+        dm = C.c_void_p()
+        _chk(lib().lama_locf_distance_map(self.h, C.byref(dm)))
+        self.distance_map = DynamicDistanceMap(handle=dm, owner=self)
+
+    def __del__(self):
+        if getattr(self, "h", None) and _lib is not None:
+            _lib.lama_locf_destroy(self.h)
+            self.h = None
+
+    def update(self, robots, scans, odoms, force=None, origins=None, quats=None):
+        """robots[k] takes scans[k] (n x 3) with odometry odoms[k] (x, y, rotation); per-robot force flags and sensor origins / quaternions
+        (xyzw) are optional.  Returns the did_update flags (bool array, in call order)."""
+        rb, pts, n, org, qt, od, fo = _fleet_update_args(robots, scans, odoms, force, origins, quats)
+        did = np.zeros(rb.size, np.int32)
+        _chk(lib().lama_locf_update(self.h, C.c_int(rb.size), _vp(rb), _vp(pts), _vp(n), _vp(org), _vp(qt), _vp(od), _vp(fo), _vp(did)))
+        return did.astype(bool)
+
+    def _get(self):
+        st, cov, rmse, stats = np.zeros((self.robots, 4)), np.zeros((self.robots, 3, 3)), np.zeros(self.robots), np.zeros((self.robots, 2), np.uint32)
+        _chk(lib().lama_locf_get(self.h, _vp(st), _vp(cov), _vp(rmse), _vp(stats)))
+        return st, cov, rmse, stats
+
+    def states(self):
+        """(robots, 4): cos, sin, x, y of every robot"""
+        return self._get()[0]
+
+    def covars(self):
+        return self._get()[1]
+
+    def rmses(self):
+        return self._get()[2]
+
+    def solveStats(self):
+        """(robots, 2): iterations and residual evaluations of every robot's last tracking match"""
+        return self._get()[3]
+
+    def setPose(self, robot, x, y, r):
+        a, ap = _d([x, y, r])
+        _chk(lib().lama_locf_set_pose(self.h, C.c_int(robot), ap))
+
+    def setSeed(self, robot, seed):
+        _chk(lib().lama_locf_set_seed(self.h, C.c_int(robot), C.c_uint32(seed)))
+
+    def triggerGlobalLocalization(self, robot):
+        _chk(lib().lama_locf_trigger_global_localization(self.h, C.c_int(robot)))
+
+    def globalLocalizationActive(self, robot) -> bool:
+        a = C.c_int(0)
+        _chk(lib().lama_locf_global_localization_active(self.h, C.c_int(robot), C.byref(a)))
+        return bool(a.value)
+
+    def occupancyRead(self, path):
+        """the shared SimpleOccupancyMap from a .sdm file"""
+        _chk(lib().lama_locf_occupancy_read(self.h, str(path).encode()))
+
+    def occupancySet(self, cells, state):
+        """the shared SimpleOccupancyMap: state -1 setFree, 0 setUnknown, 1 setOccupied"""
+        c, cp = _u32(cells)
+        _chk(lib().lama_locf_occupancy_set(self.h, cp, C.c_int(c.size // 2), C.c_int(state)))

@@ -279,6 +279,7 @@ struct lama_slam { Slam2D* s; bool owned = true; };   // borrowed (owned = false
 struct lama_dm { DistanceMapDev* d; bool owned; };
 struct lama_om { OccupancyMapDev* m; bool owned; };
 struct lama_loc { Loc2D* l; lama_dm dm; };
+struct lama_locf { Loc2DFleet* f; lama_dm dm; };
 // om / coarse: the borrowed handles of the generated maps; the graph recreates a map in place, so a handle it returned earlier
 // follows the newest map
 struct lama_graph { GraphSlam2D* g; lama_slam slam; lama_om om{nullptr, false}; lama_dm coarse{nullptr, false}; };
@@ -1239,14 +1240,41 @@ try {
     return LAMA_OK;
 }
 LAMA_CATCH
-int lama_loc_create(const lama_loc_options* o, lama_loc** out)
-try {
-    if (!o || !out) return set_err("null argument", LAMA_ERR_ARG);
+}  // extern "C"
+namespace {
+LocOptions loc_options_from(const lama_loc_options* o)
+{
     LocOptions l;
     l.trans_thresh = o->trans_thresh; l.rot_thresh = o->rot_thresh; l.l2_max = o->l2_max; l.resolution = o->resolution;
     l.patch_size = o->patch_size; l.max_iter = o->max_iter; l.strategy = o->strategy; l.center_x = o->center_xy[0]; l.center_y = o->center_xy[1];
     l.gloc_particles = o->gloc_particles; l.gloc_iters = o->gloc_iters; l.gloc_thresh = o->gloc_thresh; l.cov_blend = o->cov_blend;
     l.dev = dev_from(o->dev);
+    return l;
+}
+// SimpleOccupancyMap::read (Map::read, map.cpp:531-575; int8 cells: -1 free, 0 unknown, 1 occupied)
+int occupancy_read(SimpleOccupancyHost* occ, const char* path)
+{
+    SdmFile f;
+    std::string err;
+    if (!sdm_read(path, 1, 0, f, err)) return set_err(err, LAMA_ERR_ARG);
+    // Map::read adopts the file's resolution (map.cpp:549-558); this map's scale is fixed at Init, so a different one is refused
+    if (f.header.resolution != (float)occ->resolution()) return set_err("the file's resolution differs from this map's", LAMA_ERR_ARG);
+    for (size_t i = 0; i < f.ids.size(); ++i) {
+        uint32_t ax, ay;
+        p2m(f.ids[i], ax, ay);
+        const int8_t* c = reinterpret_cast<const int8_t*>(f.cells.data() + i * (size_t)kPatchCells);
+        const uint64_t* mask = f.masks.data() + i * (kPatchCells / 64);
+        for (uint32_t ci = 0; ci < (uint32_t)kPatchCells; ++ci)
+            if ((mask[ci >> 6] >> (ci & 63)) & 1ull) occ->set(ax + (ci & (kPatchLen - 1)), ay + (ci >> kPatchLog2), c[ci]);
+    }
+    return LAMA_OK;
+}
+}  // namespace
+extern "C" {
+int lama_loc_create(const lama_loc_options* o, lama_loc** out)
+try {
+    if (!o || !out) return set_err("null argument", LAMA_ERR_ARG);
+    const LocOptions l = loc_options_from(o);
     std::string err;
     Loc2D* loc = Loc2D::create(l, err);
     if (!loc) return set_err(err, lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_ARG);
@@ -1322,24 +1350,10 @@ try {
     return LAMA_OK;
 }
 LAMA_CATCH
-// SimpleOccupancyMap::read (Map::read, map.cpp:531-575; int8 cells: -1 free, 0 unknown, 1 occupied)
 int lama_loc_occupancy_read(lama_loc* h, const char* path)
 try {
     if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
-    SdmFile f;
-    std::string err;
-    if (!sdm_read(path, 1, 0, f, err)) return set_err(err, LAMA_ERR_ARG);
-    // Map::read adopts the file's resolution (map.cpp:549-558); this map's scale is fixed at Init, so a different one is refused
-    if (f.header.resolution != (float)h->l->occupancy_map()->resolution()) return set_err("the file's resolution differs from this map's", LAMA_ERR_ARG);
-    for (size_t i = 0; i < f.ids.size(); ++i) {
-        uint32_t ax, ay;
-        p2m(f.ids[i], ax, ay);
-        const int8_t* c = reinterpret_cast<const int8_t*>(f.cells.data() + i * (size_t)kPatchCells);
-        const uint64_t* mask = f.masks.data() + i * (kPatchCells / 64);
-        for (uint32_t ci = 0; ci < (uint32_t)kPatchCells; ++ci)
-            if ((mask[ci >> 6] >> (ci & 63)) & 1ull) h->l->occupancy_map()->set(ax + (ci & (kPatchLen - 1)), ay + (ci >> kPatchLog2), c[ci]);
-    }
-    return LAMA_OK;
+    return occupancy_read(h->l->occupancy_map(), path);
 }
 LAMA_CATCH
 int lama_loc_set_seed(lama_loc* h, uint32_t seed)
@@ -1368,6 +1382,114 @@ try {
     if (!h || !stats) return set_err("null argument", LAMA_ERR_ARG);
     stats[0] = h->l->iterations();
     stats[1] = h->l->evals();
+    return LAMA_OK;
+}
+LAMA_CATCH
+
+// ---- Loc2DFleet -----------------------------------------------------------------------------------------------------------------------
+int lama_locf_create(const lama_loc_options* o, int n_robots, lama_locf** out)
+try {
+    if (!o || !out) return set_err("null argument", LAMA_ERR_ARG);
+    if (n_robots < 1) return set_err("a fleet needs at least one robot", LAMA_ERR_ARG);
+    std::string err;
+    Loc2DFleet* f = Loc2DFleet::create(loc_options_from(o), n_robots, err);
+    if (!f) return set_err(err, lama_b200::cuda_device_count() < 1 ? LAMA_ERR_NO_DEVICE : LAMA_ERR_ARG);
+    *out = new lama_locf{f, lama_dm{f->distance_map(), false}};
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_locf_destroy(lama_locf* h)
+try {
+    if (!h) return LAMA_OK;
+    delete h->f;
+    delete h;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_locf_distance_map(lama_locf* h, lama_dm** dm)
+try {
+    if (!h || !dm) return set_err("null argument", LAMA_ERR_ARG);
+    *dm = &h->dm;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_locf_occupancy_set(lama_locf* h, const uint32_t* cells, int n, int state)
+try {
+    if (!h || (!cells && n)) return set_err("null argument", LAMA_ERR_ARG);
+    for (int i = 0; i < n; ++i) h->f->occupancy_map()->set(cells[2 * i], cells[2 * i + 1], state);
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_locf_occupancy_read(lama_locf* h, const char* path)
+try {
+    if (!h || !path) return set_err("null argument", LAMA_ERR_ARG);
+    return occupancy_read(h->f->occupancy_map(), path);
+}
+LAMA_CATCH
+}  // extern "C"
+namespace {
+// the robot of a per-robot call, or null (the error set) when the handle is null or the robot out of range
+LocRobot* fleet_robot(lama_locf* h, int robot)
+{
+    if (!h) { set_err("null handle", LAMA_ERR_ARG); return nullptr; }
+    if (robot < 0 || robot >= h->f->robots()) { set_err("robot " + std::to_string(robot) + " out of range", LAMA_ERR_ARG); return nullptr; }
+    return &h->f->robot(robot);
+}
+}  // namespace
+extern "C" {
+int lama_locf_set_pose(lama_locf* h, int robot, const double xyr[3])
+try {
+    LocRobot* r = fleet_robot(h, robot);
+    if (!r) return LAMA_ERR_ARG;
+    if (!xyr) return set_err("null argument", LAMA_ERR_ARG);
+    r->pose      = se2_from_xyr(xyr[0], xyr[1], xyr[2]);   // Loc2D::set_pose
+    r->has_first = false;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_locf_set_seed(lama_locf* h, int robot, uint32_t seed)
+try {
+    LocRobot* r = fleet_robot(h, robot);
+    if (!r) return LAMA_ERR_ARG;
+    r->gen.seed(seed);
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_locf_trigger_global_localization(lama_locf* h, int robot)
+try {
+    LocRobot* r = fleet_robot(h, robot);
+    if (!r) return LAMA_ERR_ARG;
+    r->do_gloc = true;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_locf_global_localization_active(lama_locf* h, int robot, int* active)
+try {
+    LocRobot* r = fleet_robot(h, robot);
+    if (!r) return LAMA_ERR_ARG;
+    if (!active) return set_err("null argument", LAMA_ERR_ARG);
+    *active = r->do_gloc ? 1 : 0;
+    return LAMA_OK;
+}
+LAMA_CATCH
+int lama_locf_update(lama_locf* h, int count, const int* robots, const double* pts, const int* n_points, const double* origins, const double* quats,
+                     const double* odom, const int* force, int* did_update)
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    int rc = h->f->update(count, robots, pts, n_points, origins, quats, odom, force, did_update);
+    return rc == LAMA_OK ? rc : set_err(h->f->error(), rc);
+}
+LAMA_CATCH
+int lama_locf_get(lama_locf* h, double* state, double* cov, double* rmse, uint32_t* stats)
+try {
+    if (!h) return set_err("null handle", LAMA_ERR_ARG);
+    for (int i = 0; i < h->f->robots(); ++i) {
+        const LocRobot& r = h->f->robot(i);
+        if (state) { state[4 * i] = r.pose.c; state[4 * i + 1] = r.pose.s; state[4 * i + 2] = r.pose.tx; state[4 * i + 3] = r.pose.ty; }
+        if (cov) std::memcpy(cov + 9 * (size_t)i, r.cov, sizeof(double) * 9);
+        if (rmse) rmse[i] = r.rmse;
+        if (stats) { stats[2 * i] = r.iters; stats[2 * i + 1] = r.evals; }
+    }
     return LAMA_OK;
 }
 LAMA_CATCH

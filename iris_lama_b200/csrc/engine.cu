@@ -83,6 +83,20 @@ struct Engine::Impl {
     // the dense directory of match_extent (Engine::extent_)
     void* d_extent = nullptr;
     size_t extent_bytes = 0;
+    // fleet rounds (fleet_reserve): room for fleet_cap scans of max_beams beams; the pinned staging h_fleet holds the descriptors, then
+    // the points, in the layout of d_fleet; the per-block scan indices (upload_states' growth) and the sampling offsets and likelihoods
+    void* d_fleet = nullptr;
+    void* h_fleet = nullptr;
+    int fleet_cap = 0, fleet_max_beams = 0;
+    int32_t* d_fleet_blocks = nullptr;
+    int32_t* h_fleet_blocks = nullptr;
+    int fleet_block_cap = 0;
+    double* d_fleet_off = nullptr;
+    double* d_fleet_lik = nullptr;
+    double* h_fleet_lik = nullptr;
+    int fleet_n_off = 0;
+    FleetScan* fleet_scans() const { return (FleetScan*)d_fleet; }
+    double* fleet_points() const { return (double*)((char*)d_fleet + (size_t)fleet_cap * sizeof(FleetScan)); }
     // device arena of a migration round (pack_device / migration_alloc): bump allocation out of chunks that are kept between rounds, so that a resampling
     // scan costs no cudaMalloc / cudaFree once the arena has grown to its working size
     std::vector<std::pair<char*, size_t>> mig_chunks;
@@ -420,6 +434,10 @@ Engine::~Engine()
     if (d_->d_scratch) cudaFree(d_->d_scratch);
     if (d_->d_shift_scratch) cudaFree(d_->d_shift_scratch);
     if (d_->d_extent) cudaFree(d_->d_extent);
+    for (void* p : {d_->d_fleet, (void*)d_->d_fleet_blocks, (void*)d_->d_fleet_off, (void*)d_->d_fleet_lik})
+        if (p) cudaFree(p);
+    for (void* p : {d_->h_fleet, (void*)d_->h_fleet_blocks, (void*)d_->h_fleet_lik})
+        if (p) cudaFreeHost(p);
     if (d_->d_staged) cudaFree(d_->d_staged);
     for (int b = 0; b < 2; ++b)
         for (int k = 0; k < 4; ++k)
@@ -1415,33 +1433,148 @@ int Engine::dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_a
     return LAMA_OK;
 }
 
+// The dense directory of match_extent and match_fleet, built when a call allocated or deleted patches since the last one
+int Engine::ensure_extent()
+{
+    if (!extent_stale_) return LAMA_OK;   // a shift moves entries between the window and the parked list, never between slots: it keeps the directory
+    uint32_t mn[2], mx[2];
+    const int n_patches = bounds(0, kMapDm, mn, mx);
+    if (n_patches < 0) return fail("match_extent: reading the map's bounds failed", LAMA_ERR_CUDA);
+    DirWindow xw{0, 0, 0};   // dim 0: no patch, every cell reads as absent
+    if (extent_window(mn, mx, n_patches, &xw) < 0)
+        return fail("match_extent: the map spans more than " + std::to_string(kExtentMaxPatches) + " patches on an axis", LAMA_ERR_WINDOW);
+    if (xw.dim) {
+        const size_t bytes = (size_t)xw.dim * xw.dim * 4;
+        if (ensure_buffer(&d_->d_extent, &d_->extent_bytes, bytes)) return fail("match_extent: out of device memory", LAMA_ERR_CUDA);
+        CU_TRY(cudaMemsetAsync(d_->d_extent, 0xFF, bytes, d_->stream));
+        launch_extent_dir(d_->view, d_->pv(cur_set_), cur_set_, xw, d_->park_ol[cur_set_][kMapDm].y, (int32_t*)d_->d_extent, d_->stream);
+        CU_TRY(cudaGetLastError());
+        times_.misc_launches += 1;
+    }
+    extent_ = xw;
+    extent_stale_ = false;
+    return LAMA_OK;
+}
+
 int Engine::match_extent(const SE2* states, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out)
 {
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
     if (count < 1) return fail("match_extent: no states", LAMA_ERR_ARG);
     if (d_->scan.n_beams < 1) return fail("match_extent: no scan uploaded", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
-    if (extent_stale_) {   // a shift moves entries between the window and the parked list, never between slots: it keeps the directory
-        uint32_t mn[2], mx[2];
-        const int n_patches = bounds(0, kMapDm, mn, mx);
-        if (n_patches < 0) return fail("match_extent: reading the map's bounds failed", LAMA_ERR_CUDA);
-        DirWindow xw{0, 0, 0};   // dim 0: no patch, every cell reads as absent
-        if (extent_window(mn, mx, n_patches, &xw) < 0)
-            return fail("match_extent: the map spans more than " + std::to_string(kExtentMaxPatches) + " patches on an axis", LAMA_ERR_WINDOW);
-        if (xw.dim) {
-            const size_t bytes = (size_t)xw.dim * xw.dim * 4;
-            if (ensure_buffer(&d_->d_extent, &d_->extent_bytes, bytes)) return fail("match_extent: out of device memory", LAMA_ERR_CUDA);
-            CU_TRY(cudaMemsetAsync(d_->d_extent, 0xFF, bytes, d_->stream));
-            launch_extent_dir(d_->view, d_->pv(cur_set_), cur_set_, xw, d_->park_ol[cur_set_][kMapDm].y, (int32_t*)d_->d_extent, d_->stream);
-            CU_TRY(cudaGetLastError());
-            times_.misc_launches += 1;
-        }
-        extent_ = xw;
-        extent_stale_ = false;
-    }
+    { int rc = ensure_extent(); if (rc != LAMA_OK) return rc; }
     MatchParams mp = match_params(so, meas_sigma, 0, true, 1);
     mp.parked_any = 0;   // k_match_extent reads parked patches through its directory: no read sets kErrWindow
     return match_sync(states, count, mp, true, out);
+}
+
+int Engine::fleet_reserve(int robots, const double* offsets_xy, int n_off)
+{
+    if (d_->d_fleet) return fail("fleet_reserve: already reserved", LAMA_ERR_STATE);
+    if (robots < 1 || n_off < 1 || !offsets_xy) return fail("fleet_reserve: bad arguments", LAMA_ERR_ARG);
+    CU_TRY(cudaSetDevice(cfg_.device));
+    const size_t bytes = (size_t)robots * (sizeof(FleetScan) + (size_t)cfg_.max_beams * 24);
+    d_->fleet_cap = robots;
+    d_->fleet_n_off = n_off;
+    CU_TRY(cudaMalloc(&d_->d_fleet, bytes));
+    CU_TRY(cudaMallocHost(&d_->h_fleet, bytes));
+    CU_TRY(cudaMalloc((void**)&d_->d_fleet_off, (size_t)n_off * 16));
+    CU_TRY(cudaMalloc((void**)&d_->d_fleet_lik, (size_t)robots * n_off * 8));
+    CU_TRY(cudaMallocHost((void**)&d_->h_fleet_lik, (size_t)robots * n_off * 8));
+    CU_TRY(cudaMemcpy(d_->d_fleet_off, offsets_xy, (size_t)n_off * 16, cudaMemcpyHostToDevice));
+    return LAMA_OK;
+}
+
+int Engine::fleet_scans(const double* pts, const int* n_points, int count, const double* origins, const double* quats)
+{
+    { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
+    if (count < 1 || count > d_->fleet_cap || !pts || !n_points) return fail("fleet_scans: bad arguments", LAMA_ERR_ARG);
+    for (int k = 0; k < count; ++k)
+        if (n_points[k] < 1 || n_points[k] > cfg_.max_beams) return fail("fleet_scans: number of beams out of range", LAMA_ERR_ARG);
+    CU_TRY(cudaSetDevice(cfg_.device));
+    FleetScan* desc = (FleetScan*)d_->h_fleet;
+    double* hp = (double*)((char*)d_->h_fleet + (size_t)d_->fleet_cap * sizeof(FleetScan));
+    int64_t off = 0;
+    int max_n = 0;
+    for (int k = 0; k < count; ++k) {
+        desc[k] = FleetScan{off, n_points[k], 0, moving_tf(origins ? origins + 3 * k : nullptr, quats ? quats + 4 * k : nullptr)};
+        off += n_points[k];
+        max_n = std::max(max_n, n_points[k]);
+    }
+    std::memcpy(hp, pts, (size_t)off * 24);
+    // descriptors and points in one copy: everything from the first descriptor to the last point
+    const size_t bytes = (size_t)d_->fleet_cap * sizeof(FleetScan) + (size_t)off * 24;
+    CU_TRY(cudaMemcpyAsync(d_->d_fleet, d_->h_fleet, bytes, cudaMemcpyHostToDevice, d_->stream));
+    h2d_bytes_ += bytes;
+    d_->fleet_max_beams = max_n;
+    return LAMA_OK;
+}
+
+int Engine::match_fleet(const int32_t* scan_of_block, const SE2* states, int count, int mode, const SolverOptions& so, double meas_sigma)
+{
+    { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
+    if (count < 1 || !scan_of_block || !states || (mode != 0 && mode != 1)) return fail("match_fleet: bad arguments", LAMA_ERR_ARG);
+    if (d_->fleet_max_beams < 1) return fail("match_fleet: no fleet scans uploaded", LAMA_ERR_STATE);
+    CU_TRY(cudaSetDevice(cfg_.device));
+    const bool extent = follow_ && has_parked();
+    if (extent) { int rc = ensure_extent(); if (rc != LAMA_OK) return rc; }
+    if (count > d_->fleet_block_cap) {
+        if (d_->d_fleet_blocks) { cudaFree(d_->d_fleet_blocks); cudaFreeHost(d_->h_fleet_blocks); }
+        d_->d_fleet_blocks = nullptr; d_->h_fleet_blocks = nullptr; d_->fleet_block_cap = 0;
+        CU_TRY(cudaMalloc((void**)&d_->d_fleet_blocks, (size_t)count * 4));
+        CU_TRY(cudaMallocHost((void**)&d_->h_fleet_blocks, (size_t)count * 4));
+        d_->fleet_block_cap = count;
+    }
+    std::memcpy(d_->h_fleet_blocks, scan_of_block, (size_t)count * 4);
+    CU_TRY(cudaMemcpyAsync(d_->d_fleet_blocks, d_->h_fleet_blocks, (size_t)count * 4, cudaMemcpyHostToDevice, d_->stream));
+    { int rc = upload_states(states, count, d_->stream); if (rc != LAMA_OK) return rc; }
+    MatchParams mp = match_params(so, meas_sigma, 0, true, mode);
+    mp.points = d_->fleet_points();
+    mp.scan.scale = 1.0 / cfg_.resolution;
+    if (extent) mp.parked_any = 0;   // the dense directory holds the parked patches
+    if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
+    launch_match_fleet(d_->view, mp, d_->fleet_scans(), d_->d_fleet_blocks, d_->fleet_max_beams, extent ? (const int32_t*)d_->d_extent : nullptr, extent_,
+                       d_->d_states, d_->d_results, count, d_->stream);
+    if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
+    CU_TRY(cudaGetLastError());
+    times_.match_launches += 1;
+    fleet_count_ = count;
+    fleet_parked_ = mp.parked_any != 0;
+    fleet_sampled_ = false;
+    return LAMA_OK;
+}
+
+int Engine::sampling_fleet()
+{
+    if (fleet_count_ < 1 || fleet_count_ > d_->fleet_cap) return fail("sampling_fleet: no fleet match of at most one block per robot", LAMA_ERR_STATE);
+    launch_sampling_fleet(d_->view, d_->pv(cur_set_), cur_set_, d_->fleet_points(), d_->fleet_scans(), d_->d_fleet_blocks, d_->d_results, fleet_count_,
+                          1.0 / cfg_.resolution, d_->d_fleet_off, d_->fleet_n_off, cfg_.resolution, max_sqdist_, d_->d_fleet_lik, d_->stream);
+    CU_TRY(cudaGetLastError());
+    times_.misc_launches += 1;
+    fleet_sampled_ = true;
+    return LAMA_OK;
+}
+
+int Engine::fleet_results(HostMatchResult* out, double* lik)
+{
+    const int count = fleet_count_;
+    if (count < 1) return fail("fleet_results: no fleet match", LAMA_ERR_STATE);
+    fleet_count_ = 0;
+    CU_TRY(cudaMemcpyAsync(d_->h_results, d_->d_results, (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
+    const size_t lik_n = fleet_sampled_ ? (size_t)count * d_->fleet_n_off : 0;
+    if (lik_n) CU_TRY(cudaMemcpyAsync(d_->h_fleet_lik, d_->d_fleet_lik, lik_n * 8, cudaMemcpyDeviceToHost, d_->stream));
+    if (fleet_parked_) CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaStreamSynchronize(d_->stream));
+    if (timing_) {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, d_->ev[0], d_->ev[1]);
+        times_.match_ms += ms;
+    }
+    if (fleet_parked_ && *d_->h_status) return check_device_status();
+    std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
+    if (lik && lik_n) std::memcpy(lik, d_->h_fleet_lik, lik_n * 8);
+    d2h_bytes_ += (uint64_t)count * sizeof(MatchResult) + lik_n * 8;
+    return LAMA_OK;
 }
 
 int Engine::sampling_likelihood(int particle, const SE2& pose, const double* offsets_xy, int n, int stride, double* out)

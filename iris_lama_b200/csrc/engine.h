@@ -197,6 +197,23 @@ public:
     int match_extent(const SE2* states, int count, const SolverOptions& so, double meas_sigma, HostMatchResult* out);
     // Likelihoods of Loc2D::addSamplingCovariance for n offsets (x, y pairs) around `pose` on the current scan.
     int sampling_likelihood(int particle, const SE2& pose, const double* offsets_xy, int n, int stride, double* out);
+
+    // Fleet rounds (Loc2DFleet): the scans of many robots matched on particle 0's map in one launch per step.  fleet_reserve allocates,
+    // once, room for the scans of `robots` robots of up to max_beams beams each and keeps the n_off sampling offsets (x, y pairs).
+    int fleet_reserve(int robots, const double* offsets_xy, int n_off);
+    // The scans of a round: scan k = the next n_points[k] points of pts (xyz), sensor origin / quaternion xyzw origins + 3k / quats + 4k
+    // (null: identity); 1 <= n_points[k] <= max_beams.  One host -> device copy of the descriptors and points through pinned staging.
+    int fleet_scans(const double* pts, const int* n_points, int count, const double* origins, const double* quats);
+    // Enqueues the scan matching of `count` states, block k on scan scan_of_block[k] of the round, mode 0 = solve, 1 = single
+    // evaluation.  The read path is global localisation's: the dense directory of match_extent when the map follows and has parked
+    // patches (a map wider than kExtentMaxPatches patches is refused with LAMA_ERR_WINDOW before any launch), the working window
+    // otherwise.  The window never moves.
+    int match_fleet(const int32_t* scan_of_block, const SE2* states, int count, int mode, const SolverOptions& so, double meas_sigma);
+    // Enqueues the sampling likelihoods of every block of the last match_fleet around its result state (mode 0: the solved pose).
+    int sampling_fleet();
+    // One read-back and one synchronise: the results of the last match_fleet and, when sampling_fleet followed it, its likelihoods
+    // (lik[k * n_off + i] for block k, offset i).
+    int fleet_results(HostMatchResult* out, double* lik);
     // Batched DistanceMap::distance(p, &grad).
     int dm_distance(int particle, const double* pts, int n, double* dist, double* grad);
 
@@ -296,6 +313,9 @@ private:
     void set_moving(const double origin[3], const double quat[4], double truncated_ray, double truncated_range, int n);
     int fail(const std::string& what, int code);
     int check_device_status();
+    int ensure_extent();
+    int fleet_count_ = 0;                 // blocks of the last match_fleet
+    bool fleet_parked_ = false, fleet_sampled_ = false;   // ... read with parked_any, followed by sampling_fleet
 };
 
 // error codes returned through the C-ABI

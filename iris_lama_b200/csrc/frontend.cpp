@@ -1395,6 +1395,109 @@ bool SimpleOccupancyHost::bounds_world(double mn[2], double mx[2]) const
     return true;
 }
 
+// ---- per-robot steps of Loc2D ---------------------------------------------------------------------------------------
+std::vector<double> loc_sampling_steps(double resolution)
+{
+    std::vector<double> st;
+    const double sstep = resolution;   // loc2d.cpp:93-107
+    auto add = [&](double x, double y) { st.push_back(x); st.push_back(y); };
+    add(0.0, 0.0);
+    for (int i = 1; i <= 20; ++i) {
+        add(i * sstep, 0.0); add(0.0, i * sstep); add(-i * sstep, 0.0); add(0.0, -i * sstep);
+        add(i * sstep, i * sstep); add(-i * sstep, i * sstep); add(i * sstep, -i * sstep); add(-i * sstep, -i * sstep);
+    }
+    return st;
+}
+
+bool loc_predict(LocRobot& r, const LocOptions& o, const SE2& odometry, bool force)
+{
+    const SE2 odelta = se2_mul(se2_inv(r.odom), odometry);
+    const SE2 ppose  = se2_mul(r.pose, odelta);
+    const bool enough = !(xy_norm(odelta) <= o.trans_thresh && std::abs(se2_rotation(odelta)) <= o.rot_thresh);
+    if (!force && !enough) return false;
+    r.pose = ppose;
+    r.odom = odometry;
+    return true;
+}
+
+bool loc_gloc_step(LocRobot& r, const LocOptions& o)
+{
+    if (!r.do_gloc) return false;
+    if (r.gloc_cur_iter < o.gloc_iters) {
+        r.gloc_cur_iter++;
+        return true;
+    }
+    r.do_gloc       = false;
+    r.gloc_cur_iter = 0;
+    return false;
+}
+
+bool loc_gloc_candidates(LocRobot& r, const LocOptions& o, const SimpleOccupancyHost& occ, std::vector<SE2>& cand)
+{
+    double mn[2], mx[2];
+    if (!occ.bounds_world(mn, mx)) return false;
+    const double diff[2] = {mx[0] - mn[0], mx[1] - mn[1]};
+    cand.resize(o.gloc_particles);
+    auto uniform = [&]() { std::uniform_real_distribution<double> d(0.0, 1.0); return d(r.gen); };
+    for (uint32_t i = 0; i < o.gloc_particles; ++i) {
+        double x, y, a;
+        for (;;) {
+            x = mn[0] + uniform() * diff[0];
+            y = mn[1] + uniform() * diff[1];
+            if (!occ.is_free_world(x, y)) continue;
+            a = uniform() * 2 * M_PI - M_PI;
+            break;
+        }
+        cand[i] = se2_from_xyr(x, y, a);
+    }
+    return true;
+}
+
+void loc_gloc_winner(LocRobot& r, const SE2* cand, const HostMatchResult* res, size_t n)
+{
+    double best = std::numeric_limits<double>::max();
+    for (size_t i = 0; i < n; ++i)
+        if (res[i].sums[10] < best) {  // residuals.squaredNorm()
+            best   = res[i].sums[10];
+            r.pose = cand[i];
+        }
+}
+
+void loc_tracked(LocRobot& r, const HostMatchResult& res, size_t n)
+{
+    r.pose  = res.state;
+    r.iters = res.iterations;
+    r.evals = res.evals_ref + 2;  // + the covariance and rmse evaluations of solver.cpp:110 / loc2d.cpp:178
+    covariance_from_sums(res.sums, n, r.cov);
+}
+
+void loc_sampling_blend(LocRobot& r, const std::vector<double>& steps, const double* l, double alpha)
+{
+    const int n_off = (int)(steps.size() / 2);
+    double K[4] = {0, 0, 0, 0}, u[2] = {0, 0}, sl = 0;
+    for (int i = 0; i < n_off; ++i) {
+        const double x = r.pose.tx + steps[2 * i], y = r.pose.ty + steps[2 * i + 1];
+        K[0] = K[0] + x * x * l[i]; K[1] = K[1] + x * y * l[i]; K[2] = K[2] + y * x * l[i]; K[3] = K[3] + y * y * l[i];
+        u[0] = u[0] + x * l[i]; u[1] = u[1] + y * l[i];
+        sl = sl + l[i];
+    }
+    const double a = 1.0 / sl, b = 1.0 / (sl * sl);
+    const double sc[4] = {a * K[0] - b * u[0] * u[0], a * K[1] - b * u[0] * u[1], a * K[2] - b * u[1] * u[0], a * K[3] - b * u[1] * u[1]};
+    double* cov = r.cov;
+    cov[0] = alpha * sc[0] + (1.0 - alpha) * cov[0]; cov[1] = alpha * sc[1] + (1.0 - alpha) * cov[1];
+    cov[3] = alpha * sc[2] + (1.0 - alpha) * cov[3]; cov[4] = alpha * sc[3] + (1.0 - alpha) * cov[4];
+}
+
+void loc_finish(LocRobot& r, const LocOptions& o, const HostMatchResult& res, size_t n)
+{
+    r.rmse = std::sqrt(res.sums[10] / ((double)(n - 1)));  // loc2d.cpp:178-180
+    if (r.do_gloc && r.rmse < o.gloc_thresh) {             // loc2d.cpp:182-188
+        r.do_gloc       = false;
+        r.gloc_cur_iter = 0;
+    }
+}
+
+// ---- Loc2D -----------------------------------------------------------------------------------------------------------
 Loc2D* Loc2D::create(const LocOptions& o, std::string& err)
 {
     DistanceMapDev* dm = DistanceMapDev::create(o.resolution, o.patch_size, o.l2_max, o.center_x, o.center_y, o.dev, err);
@@ -1404,13 +1507,7 @@ Loc2D* Loc2D::create(const LocOptions& o, std::string& err)
     l->dm_.reset(dm);
     l->occ_.reset(new SimpleOccupancyHost(o.resolution));
     l->cov_blend_ = std::max(std::min(o.cov_blend, 1.0), 0.0);  // loc2d.cpp:90
-    const double sstep = o.resolution;                           // loc2d.cpp:93-107
-    auto add = [&](double x, double y) { l->sampling_steps_.push_back(x); l->sampling_steps_.push_back(y); };
-    add(0.0, 0.0);
-    for (int i = 1; i <= 20; ++i) {
-        add(i * sstep, 0.0); add(0.0, i * sstep); add(-i * sstep, 0.0); add(0.0, -i * sstep);
-        add(i * sstep, i * sstep); add(-i * sstep, i * sstep); add(i * sstep, -i * sstep); add(-i * sstep, -i * sstep);
-    }
+    l->sampling_steps_ = loc_sampling_steps(o.resolution);
     return l;
 }
 
@@ -1422,46 +1519,27 @@ Loc2D* Loc2D::create(const LocOptions& o, std::string& err)
 // k_match reads a cell outside it as absent, as the reference's const get does.
 int Loc2D::global_localization(int n)
 {
-    double mn[2], mx[2];
-    if (!occ_->bounds_world(mn, mx)) return LAMA_OK;
-    const double diff[2] = {mx[0] - mn[0], mx[1] - mn[1]};
-    std::vector<SE2> cand(opt_.gloc_particles);
-    auto uniform = [&]() { std::uniform_real_distribution<double> d(0.0, 1.0); return d(gen_); };
-    for (uint32_t i = 0; i < opt_.gloc_particles; ++i) {
-        double x, y, a;
-        for (;;) {
-            x = mn[0] + uniform() * diff[0];
-            y = mn[1] + uniform() * diff[1];
-            if (!occ_->is_free_world(x, y)) continue;
-            a = uniform() * 2 * M_PI - M_PI;
-            break;
-        }
-        cand[i] = se2_from_xyr(x, y, a);
-    }
+    std::vector<SE2> cand;
+    if (!loc_gloc_candidates(rb_, opt_, *occ_, cand)) return LAMA_OK;
     std::vector<HostMatchResult> res(cand.size());
     SolverOptions so = make_solver(0, 0);
     Engine* eng = dm_->engine();
     int rc = eng->follows() && eng->has_parked() ? eng->match_extent(cand.data(), (int)cand.size(), so, 0.05, res.data())
                                                  : eng->match(cand.data(), (int)cand.size(), 0, true, so, 0.05, 1, res.data());
     if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
-    double best = std::numeric_limits<double>::max();
-    for (size_t i = 0; i < cand.size(); ++i)
-        if (res[i].sums[10] < best) {  // residuals.squaredNorm()
-            best  = res[i].sums[10];
-            pose_ = cand[i];
-        }
+    loc_gloc_winner(rb_, cand.data(), res.data(), cand.size());
     (void)n;
     return LAMA_OK;
 }
 
-// A Loc2D follows exactly when its distance map does: before a device read at pose_, the window moves over the guarded box of the scan
-// at pose_ (window_guard.h), grown by the reach of the sampling covariance's offsets (20 steps of one resolution, Loc2D::create).  On a
-// static map a shift only moves directory entries to and from the parked lists.
+// A Loc2D follows exactly when its distance map does: before a device read at the pose, the window moves over the guarded box of the
+// scan at the pose (window_guard.h), grown by the reach of the sampling covariance's offsets (20 steps of one resolution,
+// loc_sampling_steps).  On a static map a shift only moves directory entries to and from the parked lists.
 int Loc2D::follow(const double* pts, int n, const double* origin, const double* quat)
 {
     Engine* eng = dm_->engine();
     if (!eng->follows()) return LAMA_OK;
-    const int rc = follow_window(eng, &pose_, 1, origin, quat, pts, n, 20.0 * opt_.resolution);
+    const int rc = follow_window(eng, &rb_.pose, 1, origin, quat, pts, n, 20.0 * opt_.resolution);
     if (rc != LAMA_OK) err_ = eng->last_error();
     return rc;
 }
@@ -1473,20 +1551,9 @@ int Loc2D::add_sampling_covariance(const double* pts, int n, const double* origi
     const int stride = (int)std::max((size_t)n / 100, (size_t)1);
     std::vector<double> l((size_t)n_off);
     int rc = follow(pts, n, origin, quat);
-    if (rc == LAMA_OK) rc = dm_->engine()->sampling_likelihood(0, pose_, sampling_steps_.data(), n_off, stride, l.data());
+    if (rc == LAMA_OK) rc = dm_->engine()->sampling_likelihood(0, rb_.pose, sampling_steps_.data(), n_off, stride, l.data());
     if (rc != LAMA_OK) { err_ = dm_->engine()->last_error(); return rc; }
-    double K[4] = {0, 0, 0, 0}, u[2] = {0, 0}, sl = 0;
-    for (int i = 0; i < n_off; ++i) {
-        const double x = pose_.tx + sampling_steps_[2 * i], y = pose_.ty + sampling_steps_[2 * i + 1];
-        K[0] = K[0] + x * x * l[i]; K[1] = K[1] + x * y * l[i]; K[2] = K[2] + y * x * l[i]; K[3] = K[3] + y * y * l[i];
-        u[0] = u[0] + x * l[i]; u[1] = u[1] + y * l[i];
-        sl = sl + l[i];
-    }
-    const double a = 1.0 / sl, b = 1.0 / (sl * sl);
-    const double sc[4] = {a * K[0] - b * u[0] * u[0], a * K[1] - b * u[0] * u[1], a * K[2] - b * u[1] * u[0], a * K[3] - b * u[1] * u[1]};
-    const double alpha = cov_blend_;
-    cov_[0] = alpha * sc[0] + (1.0 - alpha) * cov_[0]; cov_[1] = alpha * sc[1] + (1.0 - alpha) * cov_[1];
-    cov_[3] = alpha * sc[2] + (1.0 - alpha) * cov_[3]; cov_[4] = alpha * sc[3] + (1.0 - alpha) * cov_[4];
+    loc_sampling_blend(rb_, sampling_steps_, l.data(), cov_blend_);
     return LAMA_OK;
 }
 
@@ -1499,57 +1566,162 @@ int Loc2D::update(const double* pts, int n, const double* origin, const double* 
     const SE2 odometry = se2_from_xyr(odom_xyr[0], odom_xyr[1], odom_xyr[2]);
     SolverOptions so = make_solver(opt_.strategy, opt_.max_iter);
     bool scan_set = false;
-    if (!has_first_) {  // loc2d.cpp:128-141
-        odom_      = odometry;
-        has_first_ = true;
+    if (!rb_.has_first) {  // loc2d.cpp:128-141
+        rb_.odom      = odometry;
+        rb_.has_first = true;
         if (!force) { *did_update = true; return LAMA_OK; }
         rc = eng->set_scan(pts, n, origin, quat, 0, 0);
         if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
         scan_set = true;
         HostMatchResult r;
         rc = follow(pts, n, origin, quat);
-        if (rc == LAMA_OK) rc = eng->match(&pose_, 1, 0, false, so, 0.05, 1, &r);
+        if (rc == LAMA_OK) rc = eng->match(&rb_.pose, 1, 0, false, so, 0.05, 1, &r);
         if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
-        rmse_ = std::sqrt(r.sums[10] / ((double)((size_t)n - 1)));
+        rb_.rmse = std::sqrt(r.sums[10] / ((double)((size_t)n - 1)));
     }
-    const SE2 odelta = se2_mul(se2_inv(odom_), odometry);
-    const SE2 ppose  = se2_mul(pose_, odelta);
-    const bool enough = !(xy_norm(odelta) <= opt_.trans_thresh && std::abs(se2_rotation(odelta)) <= opt_.rot_thresh);
-    if (!force && !enough) return LAMA_OK;
-    pose_ = ppose;
-    odom_ = odometry;
+    if (!loc_predict(rb_, opt_, odometry, force)) return LAMA_OK;
     if (!scan_set) {
         rc = eng->set_scan(pts, n, origin, quat, 0, 0);
         if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
     }
-    if (do_gloc_) {  // loc2d.cpp:154-166
-        if (gloc_cur_iter_ < opt_.gloc_iters) {
-            gloc_cur_iter_++;
-            rc = global_localization(n);
-            if (rc != LAMA_OK) return rc;
-        } else {
-            do_gloc_       = false;
-            gloc_cur_iter_ = 0;
-        }
+    if (loc_gloc_step(rb_, opt_)) {  // loc2d.cpp:154-166
+        rc = global_localization(n);
+        if (rc != LAMA_OK) return rc;
     }
     HostMatchResult r;
     rc = follow(pts, n, origin, quat);
-    if (rc == LAMA_OK) rc = eng->match(&pose_, 1, 0, false, so, 0.05, 0, &r);
+    if (rc == LAMA_OK) rc = eng->match(&rb_.pose, 1, 0, false, so, 0.05, 0, &r);
     if (rc != LAMA_OK) { err_ = eng->last_error(); return rc; }
-    pose_  = r.state;
-    iters_ = r.iterations;
-    evals_ = r.evals_ref + 2;  // + the covariance and rmse evaluations of solver.cpp:110 / loc2d.cpp:178
-    covariance_from_sums(r.sums, (size_t)n, cov_);
+    loc_tracked(rb_, r, (size_t)n);
     if (cov_blend_ > 0.0) {     // loc2d.cpp:175-176
         rc = add_sampling_covariance(pts, n, origin, quat);
         if (rc != LAMA_OK) return rc;
     }
-    rmse_ = std::sqrt(r.sums[10] / ((double)((size_t)n - 1)));  // loc2d.cpp:178-180
-    if (do_gloc_ && rmse_ < opt_.gloc_thresh) {                 // loc2d.cpp:182-188
-        do_gloc_       = false;
-        gloc_cur_iter_ = 0;
-    }
+    loc_finish(rb_, opt_, r, (size_t)n);
     *did_update = true;
+    return LAMA_OK;
+}
+
+// ---- Loc2DFleet ------------------------------------------------------------------------------------------------------
+Loc2DFleet* Loc2DFleet::create(const LocOptions& o, int robots, std::string& err)
+{
+    if (robots < 1) { err = "a fleet needs at least one robot"; return nullptr; }
+    DistanceMapDev* dm = DistanceMapDev::create(o.resolution, o.patch_size, o.l2_max, o.center_x, o.center_y, o.dev, err);
+    if (!dm) return nullptr;
+    std::unique_ptr<Loc2DFleet> f(new Loc2DFleet());
+    f->opt_ = o;
+    f->dm_.reset(dm);
+    f->occ_.reset(new SimpleOccupancyHost(o.resolution));
+    f->cov_blend_ = std::max(std::min(o.cov_blend, 1.0), 0.0);
+    f->sampling_steps_ = loc_sampling_steps(o.resolution);
+    f->rb_.resize((size_t)robots);
+    if (dm->engine()->fleet_reserve(robots, f->sampling_steps_.data(), (int)(f->sampling_steps_.size() / 2)) != LAMA_OK) {
+        err = dm->engine()->last_error();
+        return nullptr;
+    }
+    return f.release();
+}
+
+int Loc2DFleet::fail(int rc)
+{
+    err_ = dm_->engine()->last_error();
+    return rc;
+}
+
+// One round.  The stand-alone first forced update also evaluates the RMSE at the pose before the prediction (loc2d.cpp:134-140); the
+// same update overwrites it after the tracking match, so the round leaves that evaluation out.
+int Loc2DFleet::update(int count, const int* robots, const double* pts, const int* n_points, const double* origins, const double* quats, const double* odom_xyr,
+                       const int* force, int* did_update)
+{
+    const int R = (int)rb_.size();
+    const int max_beams = dm_->engine()->config().max_beams;
+    if (count < 1 || count > R || !robots || !pts || !n_points || !odom_xyr || !did_update) { err_ = "null argument or count out of range"; return LAMA_ERR_ARG; }
+    std::vector<uint8_t> seen((size_t)R, 0);
+    for (int k = 0; k < count; ++k) {
+        if (robots[k] < 0 || robots[k] >= R) { err_ = "robot " + std::to_string(robots[k]) + " out of range"; return LAMA_ERR_ARG; }
+        if (seen[(size_t)robots[k]]++) { err_ = "robot " + std::to_string(robots[k]) + " appears twice in one update"; return LAMA_ERR_ARG; }
+        if (n_points[k] < 1 || n_points[k] > max_beams) { err_ = "scan " + std::to_string(k) + ": number of points out of range [1, max_beams]"; return LAMA_ERR_ARG; }
+    }
+    for (int k = 0; k < count; ++k) did_update[k] = 0;
+    int rc = dm_->flush_if_pending();
+    if (rc != LAMA_OK) { err_ = dm_->error(); return rc; }
+    Engine* eng = dm_->engine();
+
+    // the robots that go on (loc2d.cpp:128-152), their scans in call order
+    std::vector<int> go;                 // call index
+    std::vector<size_t> first(count);    // first point of scan k
+    size_t np = 0;
+    for (int k = 0; k < count; ++k) { first[k] = np; np += (size_t)n_points[k]; }
+    for (int k = 0; k < count; ++k) {
+        LocRobot& r = rb_[(size_t)robots[k]];
+        const double* od = odom_xyr + 3 * (size_t)k;
+        const SE2 odometry = se2_from_xyr(od[0], od[1], od[2]);
+        const bool f = force && force[k];
+        if (!r.has_first) {
+            r.odom      = odometry;
+            r.has_first = true;
+            if (!f) { did_update[k] = 1; continue; }
+        }
+        if (loc_predict(r, opt_, odometry, f)) go.push_back(k);
+    }
+    if (go.empty()) return LAMA_OK;
+    const int G = (int)go.size();
+    {
+        std::vector<double> p;
+        std::vector<int> n(G);
+        std::vector<double> o, q;
+        for (int j = 0; j < G; ++j) {
+            const int k = go[j];
+            p.insert(p.end(), pts + 3 * first[k], pts + 3 * (first[k] + n_points[k]));
+            n[j] = n_points[k];
+            if (origins) o.insert(o.end(), origins + 3 * k, origins + 3 * k + 3);
+            if (quats) q.insert(q.end(), quats + 4 * k, quats + 4 * k + 4);
+        }
+        rc = eng->fleet_scans(p.data(), n.data(), G, origins ? o.data() : nullptr, quats ? q.data() : nullptr);
+        if (rc != LAMA_OK) return fail(rc);
+    }
+
+    // global localisation of every robot that runs it this round: one launch over all candidates, winners on the host
+    {
+        std::vector<SE2> cand, c;
+        std::vector<int32_t> blocks;
+        std::vector<std::pair<int, size_t>> owners;   // (go index, first candidate)
+        for (int j = 0; j < G; ++j) {
+            LocRobot& r = rb_[(size_t)robots[go[j]]];
+            if (!loc_gloc_step(r, opt_) || !loc_gloc_candidates(r, opt_, *occ_, c)) continue;
+            owners.emplace_back(j, cand.size());
+            cand.insert(cand.end(), c.begin(), c.end());
+            blocks.insert(blocks.end(), c.size(), j);
+        }
+        if (!cand.empty()) {
+            std::vector<HostMatchResult> res(cand.size());
+            rc = eng->match_fleet(blocks.data(), cand.data(), (int)cand.size(), 1, make_solver(0, 0), 0.05);
+            if (rc == LAMA_OK) rc = eng->fleet_results(res.data(), nullptr);
+            if (rc != LAMA_OK) return fail(rc);
+            for (const auto& ow : owners)
+                loc_gloc_winner(rb_[(size_t)robots[go[ow.first]]], cand.data() + ow.second, res.data() + ow.second, opt_.gloc_particles);
+        }
+    }
+
+    // tracking of every robot that goes on, then the sampling likelihoods at the solved poses: one read-back
+    std::vector<SE2> poses(G);
+    std::vector<int32_t> blocks(G);
+    for (int j = 0; j < G; ++j) { poses[j] = rb_[(size_t)robots[go[j]]].pose; blocks[j] = j; }
+    std::vector<HostMatchResult> res(G);
+    const size_t n_off = sampling_steps_.size() / 2;
+    std::vector<double> lik(cov_blend_ > 0.0 ? (size_t)G * n_off : 0);
+    rc = eng->match_fleet(blocks.data(), poses.data(), G, 0, make_solver(opt_.strategy, opt_.max_iter), 0.05);
+    if (rc == LAMA_OK && cov_blend_ > 0.0) rc = eng->sampling_fleet();
+    if (rc == LAMA_OK) rc = eng->fleet_results(res.data(), lik.data());
+    if (rc != LAMA_OK) return fail(rc);
+    for (int j = 0; j < G; ++j) {
+        const int k = go[j];
+        LocRobot& r = rb_[(size_t)robots[k]];
+        loc_tracked(r, res[j], (size_t)n_points[k]);
+        if (cov_blend_ > 0.0) loc_sampling_blend(r, sampling_steps_, lik.data() + (size_t)j * n_off, cov_blend_);
+        loc_finish(r, opt_, res[j], (size_t)n_points[k]);
+        did_update[k] = 1;
+    }
     return LAMA_OK;
 }
 

@@ -396,45 +396,97 @@ struct LocOptions {  // src/loc2d.cpp:46-58
     DeviceOptions dev;
 };
 
+// What Loc2D keeps per robot (loc2d.h), and its host-side steps (loc_*), shared by Loc2D and Loc2DFleet
+struct LocRobot {
+    SE2 pose{1, 0, 0, 0}, odom{1, 0, 0, 0};
+    bool has_first = false;
+    double cov[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    double rmse = 0;
+    uint32_t iters = 0, evals = 0;
+    std::mt19937 gen{std::random_device{}()};   // the reference's global generator is seeded from random_device (random.cpp:38-39)
+    bool do_gloc = false;
+    uint32_t gloc_cur_iter = 0;
+};
+// Loc2D::Init's sampling offsets (loc2d.cpp:93-107): 161 (x, y) pairs
+std::vector<double> loc_sampling_steps(double resolution);
+// loc2d.cpp:143-152: prediction and motion gate.  False: not enough motion and no force, nothing changes; true: r.pose = the prediction,
+// r.odom = odometry.
+bool loc_predict(LocRobot& r, const LocOptions& o, const SE2& odometry, bool force);
+// loc2d.cpp:154-166: true when this update localises globally (an iteration is counted); false, and the flag cleared after the last one
+bool loc_gloc_step(LocRobot& r, const LocOptions& o);
+// Loc2D::globalLocalization's candidates (loc2d.cpp:249-273): the reference's rejection sampling over the free cells of `occ` with r.gen,
+// same calls in the same order.  False (no candidate drawn, the generator untouched) when the map is empty.
+bool loc_gloc_candidates(LocRobot& r, const LocOptions& o, const SimpleOccupancyHost& occ, std::vector<SE2>& cand);
+// ... and its winner (loc2d.cpp:275-285): the first candidate of least residual norm (strict `<` in index order) becomes r.pose
+void loc_gloc_winner(LocRobot& r, const SE2* cand, const HostMatchResult* res, size_t n);
+// loc2d.cpp:168-174: the solved pose, the solver's counts and the covariance of a tracking match of n beams
+void loc_tracked(LocRobot& r, const HostMatchResult& res, size_t n);
+// Loc2D::addSamplingCovariance's blend (loc2d.cpp:213-247) of the likelihoods l[i] at r.pose + steps[i] into r.cov
+void loc_sampling_blend(LocRobot& r, const std::vector<double>& steps, const double* l, double alpha);
+// loc2d.cpp:178-188: the RMSE of the tracking match and the end of global localisation under gloc_thresh
+void loc_finish(LocRobot& r, const LocOptions& o, const HostMatchResult& res, size_t n);
+
 class Loc2D {
 public:
     static Loc2D* create(const LocOptions& o, std::string& err);
     DistanceMapDev* distance_map() { return dm_.get(); }
     SimpleOccupancyHost* occupancy_map() { return occ_.get(); }
-    void set_seed(uint32_t seed) { gen_.seed(seed); }                 // random::setSeed
-    void trigger_global_localization() { do_gloc_ = true; }          // loc2d.cpp:194-197
-    bool global_localization_active() const { return do_gloc_; }
+    void set_seed(uint32_t seed) { rb_.gen.seed(seed); }             // random::setSeed
+    void trigger_global_localization() { rb_.do_gloc = true; }       // loc2d.cpp:194-197
+    bool global_localization_active() const { return rb_.do_gloc; }
     void set_pose(double x, double y, double r)
     {
-        pose_      = se2_from_xyr(x, y, r);
-        has_first_ = false;
+        rb_.pose      = se2_from_xyr(x, y, r);
+        rb_.has_first = false;
     }
     int update(const double* pts, int n, const double* origin, const double* quat, const double odom_xyr[3], double stamp, bool force, bool* did_update);
-    const SE2& pose() const { return pose_; }
-    const double* cov() const { return cov_; }
-    double rmse() const { return rmse_; }
-    uint32_t iterations() const { return iters_; }
-    uint32_t evals() const { return evals_; }
+    const SE2& pose() const { return rb_.pose; }
+    const double* cov() const { return rb_.cov; }
+    double rmse() const { return rb_.rmse; }
+    uint32_t iterations() const { return rb_.iters; }
+    uint32_t evals() const { return rb_.evals; }
     const std::string& error() const { return err_; }
 
 private:
     LocOptions opt_;
     std::unique_ptr<DistanceMapDev> dm_;
-    SE2 pose_{1, 0, 0, 0}, odom_{1, 0, 0, 0};
-    bool has_first_ = false;
-    double cov_[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-    double rmse_ = 0;
-    uint32_t iters_ = 0, evals_ = 0;
+    LocRobot rb_;
     std::string err_;
     std::unique_ptr<SimpleOccupancyHost> occ_;
-    std::mt19937 gen_{std::random_device{}()};   // the reference's global generator is seeded from random_device (random.cpp:38-39)
-    bool do_gloc_ = false;
-    uint32_t gloc_cur_iter_ = 0;
     double cov_blend_ = 0.0;
-    std::vector<double> sampling_steps_;         // 161 (x, y) offsets, loc2d.cpp:93-107
+    std::vector<double> sampling_steps_;
     int global_localization(int n);               // loc2d.cpp:249-286
     int add_sampling_covariance(const double* pts, int n, const double* origin, const double* quat);   // loc2d.cpp:199-247
     int follow(const double* pts, int n, const double* origin, const double* quat);
+};
+
+// Many robots localising on one shared map.  Robot r gives what a Loc2D with the same options, map and seed gives when it is fed only
+// r's calls in the same order, whatever the other robots of a call.  A round (update) makes one launch per step for all its robots:
+// the global-localisation candidates of every robot that localises globally, the tracking matches, the sampling likelihoods.  The
+// window never moves: on a following map with parked patches every read goes through the dense directory of the whole map.
+class Loc2DFleet {
+public:
+    static Loc2DFleet* create(const LocOptions& o, int robots, std::string& err);
+    DistanceMapDev* distance_map() { return dm_.get(); }
+    SimpleOccupancyHost* occupancy_map() { return occ_.get(); }
+    int robots() const { return (int)rb_.size(); }
+    LocRobot& robot(int r) { return rb_[(size_t)r]; }
+    // robots[k] (distinct, in range) takes scan k: n_points[k] points of pts, after those of scans 0 .. k-1, sensor origin / quaternion
+    // origins + 3k / quats + 4k (null: identity), odometry odom_xyr + 3k, force[k] (null: none); did_update[k] as Loc2D::update.  Bad
+    // arguments are refused with LAMA_ERR_ARG before any robot changes.
+    int update(int count, const int* robots, const double* pts, const int* n_points, const double* origins, const double* quats, const double* odom_xyr,
+               const int* force, int* did_update);
+    const std::string& error() const { return err_; }
+
+private:
+    LocOptions opt_;
+    std::unique_ptr<DistanceMapDev> dm_;
+    std::unique_ptr<SimpleOccupancyHost> occ_;
+    std::vector<LocRobot> rb_;
+    std::vector<double> sampling_steps_;
+    double cov_blend_ = 0.0;
+    std::string err_;
+    int fail(int rc);
 };
 
 // shared helpers

@@ -2,7 +2,8 @@
 //
 //   k_match      one CTA per particle: the whole Gauss-Newton / LM scan-matching loop
 //                (MatchSurface2D::eval + Solver::solve + GaussNewton, see match_core.h); k_match_extent, the same over a
-//                dense directory of the whole map (global localisation on a following map, k_extent_dir builds it)
+//                dense directory of the whole map (global localisation on a following map, k_extent_dir builds it);
+//                k_match_fleet / k_match_fleet_extent, the same with one scan per CTA (Loc2DFleet)
 //   k_raycast    one CTA per particle: beam ray-cast into the frequency occupancy map with packed
 //                atomics + ordered replay of threshold crossings (see ray_core.h)
 //   k_brushfire  one warp per particle: DynamicDistanceMap::update() in exact heap order (ddm_core.h)
@@ -100,13 +101,24 @@ __device__ __forceinline__ void eval_beam(double s[kNumSums], const Affine& tf, 
     accumulate(s, e, so.robust_kind, so.robust_param, meas_sigma);
 }
 
-// The body of k_match and k_match_extent.  kExtent (global localisation over a following map): directory entries come from the dense
-// directory xdir over window xwin in global memory (k_extent_dir) instead of the working window staged in shared memory, and a patch
-// outside xwin is absent.  Every other line, the reductions included, is shared, so each state's sums are those k_match gives on a
-// window that holds the whole map.
-template <bool kExtent>
+// every thread evaluates ceil(n / threads) beams: choose the block so that the last round is (almost) full
+__host__ __device__ __forceinline__ int match_threads(int n)
+{
+    const int rounds = (n + kMatchThreads - 1) / kMatchThreads;
+    const int threads = (((n + rounds - 1) / rounds) + 31) & ~31;
+    return threads < 128 ? 128 : threads;
+}
+
+// The body of k_match, k_match_extent and the two fleet kernels.  kExtent (global localisation over a following map): directory entries
+// come from the dense directory xdir over window xwin in global memory (k_extent_dir) instead of the working window staged in shared
+// memory, and a patch outside xwin is absent.  Every other line, the reductions included, is shared, so each state's sums are those
+// k_match gives on a window that holds the whole map.  kFleet: block b matches scan fleet[scan_of_block[b]] instead of mp.points /
+// mp.scan, and only its first match_threads(n) threads (the block a launch for that scan alone would have) take beams and sum them,
+// so each block's results are those of that launch, whatever the other scans of the launch and the block size they need.
+template <bool kExtent, bool kFleet = false>
 __device__ __forceinline__ void match_body(const StoreView& s, const MatchParams& mp, const SE2* __restrict__ states_in, MatchResult* __restrict__ results,
-                                           const int32_t* xdir, const DirWindow& xwin)
+                                           const int32_t* xdir, const DirWindow& xwin, const FleetScan* fleet = nullptr,
+                                           const int32_t* scan_of_block = nullptr)
 {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int dim2      = kExtent ? 0 : s.window.dim * s.window.dim;
@@ -119,6 +131,11 @@ __device__ __forceinline__ void match_body(const StoreView& s, const MatchParams
     const int32_t* dir  = kExtent ? xdir : sdir;
     const DirWindow& win = kExtent ? xwin : s.window;
     const int parked    = kExtent ? 0 : mp.parked_any;
+    const FleetScan* fs = kFleet ? fleet + scan_of_block[blockIdx.x] : nullptr;
+    const double* points    = kFleet ? mp.points + 3 * fs->offset : mp.points;
+    const MovingTf& moving  = kFleet ? fs->moving : mp.scan.moving;
+    const int n             = kFleet ? fs->n_beams : mp.scan.n_beams;
+    const int nt            = kFleet ? match_threads(n) : (int)blockDim.x;   // the logical block size
 
     if (tid == 0) {
         mbar_init(&sh.bar, 1);
@@ -133,17 +150,16 @@ __device__ __forceinline__ void match_body(const StoreView& s, const MatchParams
     __syncthreads();
     if (!kExtent) block_stage_tma(sdir, dir_of(s, mp.set, particle, kMapDm), (uint32_t)dim2 * 4u, &sh.bar, 0);
 
-    const int n = mp.scan.n_beams;
     const bool single = mp.mode == 1;
-    if (tid == 0) sh.tf = compose_tf_fast(sh.state, mp.scan.moving);
+    if (tid == 0) sh.tf = compose_tf_fast(sh.state, moving);
     __syncthreads();
     for (;;) {
         double acc[kNumSums];
 #pragma unroll
         for (int k = 0; k < kNumSums; ++k) acc[k] = 0.0;
         const Affine tf = sh.tf;
-        for (int b = tid; b < n; b += blockDim.x)
-            eval_beam(acc, tf, mp.points + 3 * (size_t)b, mp.scan.scale, s.pool, dir, win, dtab, mp.max_sqdist, mp.solver, mp.meas_sigma,
+        for (int b = (kFleet && tid >= nt) ? n : tid; b < n; b += nt)
+            eval_beam(acc, tf, points + 3 * (size_t)b, mp.scan.scale, s.pool, dir, win, dtab, mp.max_sqdist, mp.solver, mp.meas_sigma,
                       parked, s.status);
         // Block reduction through shared memory, fixed order (deterministic): every thread parks its 12 partial sums, then warp k adds
         // up sum k over all threads (a strided pass + one warp shuffle tree) -- 12 stores per thread instead of 60 shuffles per value.
@@ -152,7 +168,7 @@ __device__ __forceinline__ void match_body(const StoreView& s, const MatchParams
         __syncthreads();
         for (int k = warp; k < kNumSums; k += (int)(blockDim.x >> 5)) {
             double v = 0.0;
-            for (int t = lane; t < (int)blockDim.x; t += 32) v += part[k * kMatchThreads + t];
+            for (int t = lane; t < nt; t += 32) v += part[k * kMatchThreads + t];
             v = warp_sum(v);
             if (lane == 0) sh.sums[k] = v;
         }
@@ -169,7 +185,7 @@ __device__ __forceinline__ void match_body(const StoreView& s, const MatchParams
                     // one at the final state (likelihood, covariance, rmse); otherwise do one more pass.
                     sh.done = sh.ctl.state_dirty ? 1 : 2;
                 }
-                if (sh.done != 2) sh.tf = compose_tf_fast(sh.state, mp.scan.moving);
+                if (sh.done != 2) sh.tf = compose_tf_fast(sh.state, moving);
             }
         }
         __syncthreads();
@@ -197,6 +213,22 @@ k_match_extent(StoreView s, MatchParams mp, const SE2* __restrict__ states_in, M
                DirWindow xwin)
 {
     match_body<true>(s, mp, states_in, results, xdir, xwin);
+}
+
+// A fleet round (Loc2DFleet): one launch for the scans of many robots on one shared map (mp.shared_map), block b on scan
+// scans[scan_of_block[b]], sized for the largest of them.  k_match_fleet reads the working window, k_match_fleet_extent the dense directory.
+__global__ void __launch_bounds__(kMatchThreads, 2)
+k_match_fleet(StoreView s, MatchParams mp, const FleetScan* __restrict__ scans, const int32_t* __restrict__ scan_of_block, const SE2* __restrict__ states_in,
+              MatchResult* __restrict__ results)
+{
+    match_body<false, true>(s, mp, states_in, results, nullptr, s.window, scans, scan_of_block);
+}
+
+__global__ void __launch_bounds__(kMatchThreads, 2)
+k_match_fleet_extent(StoreView s, MatchParams mp, const FleetScan* __restrict__ scans, const int32_t* __restrict__ scan_of_block, const SE2* __restrict__ states_in,
+                     MatchResult* __restrict__ results, const int32_t* __restrict__ xdir, DirWindow xwin)
+{
+    match_body<true, true>(s, mp, states_in, results, xdir, xwin, scans, scan_of_block);
 }
 
 // The dense directory of particle 0's distance map over window xw (xw.dim^2 entries, all -1 on entry): the working window's entries and
@@ -1870,28 +1902,29 @@ __global__ void k_scatter_patches(StoreView s, int set, int particle, int kind, 
     if (kind == kMapOcc && __any_sync(0xffffffffu, fb != 0u) && lane == 0) d[entries[pi]] |= kDirHot;
 }
 
-// Loc2D::addSamplingCovariance (src/loc2d.cpp:199-236): for every sampling offset the likelihood
-//   l = sum over every `stride`-th beam of exp(-d^2 / 0.01)^3,  d = nearest-cell distance at the offset pose.
-// One block per offset; the host accumulates K, u, s in the reference's order.
-__global__ void k_sampling(StoreView s, ParkView pv, int set, int particle, const double* __restrict__ points, ScanParams scan, SE2 pose, const double* __restrict__ offsets,
-                           int stride, double resolution, uint32_t max_sqdist, double* __restrict__ out)
+// Loc2D::addSamplingCovariance (src/loc2d.cpp:199-236): for sampling offset `oi` the likelihood
+//   l = sum over every `stride`-th beam of exp(-d^2 / 0.01)^3,  d = nearest-cell distance at the offset pose,
+// summed by a block of 128 threads in a fixed order.  The host accumulates K, u, s in the reference's order.
+__device__ __forceinline__ double sampling_body(const StoreView& s, const ParkView& pv, int set, int particle, const double* __restrict__ points, int n_beams,
+                                                double scale, const MovingTf& moving, const SE2& pose, const double* __restrict__ offsets, int oi, int stride,
+                                                double resolution, uint32_t max_sqdist)
 {
     __shared__ Affine tf;
     __shared__ double part[8];
     const int32_t* d = dir_of(s, set, particle, kMapDm);
     if (threadIdx.x == 0) {
         SE2 st = pose;
-        st.tx = add_rn(pose.tx, offsets[2 * blockIdx.x]);
-        st.ty = add_rn(pose.ty, offsets[2 * blockIdx.x + 1]);
-        tf = compose_tf(st, scan.moving);
+        st.tx = add_rn(pose.tx, offsets[2 * oi]);
+        st.ty = add_rn(pose.ty, offsets[2 * oi + 1]);
+        tf = compose_tf(st, moving);
     }
     __syncthreads();
     const double dmax = mul_rn(sqrt((double)max_sqdist), resolution);
     double l = 0.0;
-    for (int k = threadIdx.x * stride; k < scan.n_beams; k += blockDim.x * stride) {
+    for (int k = threadIdx.x * stride; k < n_beams; k += blockDim.x * stride) {
         double hit[3];
         apply_tf(tf, points[3 * k], points[3 * k + 1], points[3 * k + 2], hit);
-        const uint32_t x = w2m(hit[0], scan.scale), y = w2m(hit[1], scan.scale);
+        const uint32_t x = w2m(hit[0], scale), y = w2m(hit[1], scale);
         const int slot = map_entry(s, pv, particle, kMapDm, d, x, y);
         const uint32_t w = slot < 0 ? 0u : __ldcg(patch_ptr(s, slot & kDirSlotMask) + cell_index(x, y));
         const double dist = (w & kDmValid) ? mul_rn(sqrt((double)dm_sqdist(w)), resolution) : dmax;
@@ -1901,11 +1934,31 @@ __global__ void k_sampling(StoreView s, ParkView pv, int set, int particle, cons
     l = warp_sum(l);
     if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = l;
     __syncthreads();
-    if (threadIdx.x == 0) {
-        double v = 0.0;
+    double v = 0.0;
+    if (threadIdx.x == 0)
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v += part[w];
-        out[blockIdx.x] = v;
-    }
+    return v;
+}
+
+// one block per offset
+__global__ void k_sampling(StoreView s, ParkView pv, int set, int particle, const double* __restrict__ points, ScanParams scan, SE2 pose, const double* __restrict__ offsets,
+                           int stride, double resolution, uint32_t max_sqdist, double* __restrict__ out)
+{
+    const double v = sampling_body(s, pv, set, particle, points, scan.n_beams, scan.scale, scan.moving, pose, offsets, blockIdx.x, stride, resolution, max_sqdist);
+    if (threadIdx.x == 0) out[blockIdx.x] = v;
+}
+
+// A fleet round: block (i, r) takes offset i of match block r, around that block's result state, on its scan and particle 0's map, with
+// Loc2D's stride of that scan (every max(n / 100, 1)-th beam).  out[r * gridDim.x + i].
+__global__ void k_sampling_fleet(StoreView s, ParkView pv, int set, const double* __restrict__ points, const FleetScan* __restrict__ scans,
+                                 const int32_t* __restrict__ scan_of_block, const MatchResult* __restrict__ results, double scale, const double* __restrict__ offsets,
+                                 double resolution, uint32_t max_sqdist, double* __restrict__ out)
+{
+    const FleetScan& fs = scans[scan_of_block[blockIdx.y]];
+    const int stride = fs.n_beams / 100 > 1 ? fs.n_beams / 100 : 1;
+    const double v = sampling_body(s, pv, set, 0, points + 3 * fs.offset, fs.n_beams, scale, fs.moving, results[blockIdx.y].state, offsets, blockIdx.x, stride,
+                                   resolution, max_sqdist);
+    if (threadIdx.x == 0) out[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = v;
 }
 
 // MatchSurface2D::error() (src/match_surface_2d.cpp:92-116): sqrt(sum d^2 / N) with d the NEAREST-cell distance (w2m rounding +
@@ -2165,6 +2218,10 @@ cudaError_t configure_kernels(int dir_dim, uint32_t max_sqdist_limit, const RayP
     if (e != cudaSuccess) return e;
     e = raise_smem_limit(k_match_extent, match_smem_bytes(0, max_sqdist_limit));
     if (e != cudaSuccess) return e;
+    e = raise_smem_limit(k_match_fleet, match_smem_bytes(dir_dim, max_sqdist_limit));
+    if (e != cudaSuccess) return e;
+    e = raise_smem_limit(k_match_fleet_extent, match_smem_bytes(0, max_sqdist_limit));
+    if (e != cudaSuccess) return e;
     if (rp.prob_mode) e = raise_smem_limit(k_raycast<true>, raycast_smem_bytes(dir_dim, rp));
     else e = raise_smem_limit(k_raycast<false>, raycast_smem_bytes(dir_dim, rp));
     if (e != cudaSuccess) return e;
@@ -2178,13 +2235,6 @@ cudaError_t configure_kernels(int dir_dim, uint32_t max_sqdist_limit, const RayP
     return e;
 }
 
-// every thread evaluates ceil(n / threads) beams: choose the block so that the last round is (almost) full
-static int match_threads(int n)
-{
-    const int rounds = (n + kMatchThreads - 1) / kMatchThreads;
-    const int threads = (((n + rounds - 1) / rounds) + 31) & ~31;
-    return threads < 128 ? 128 : threads;
-}
 void launch_match(const StoreView& s, const MatchParams& mp, const SE2* d_states, MatchResult* d_results, int count, cudaStream_t st)
 {
     if (count <= 0) return;
@@ -2195,6 +2245,16 @@ void launch_match_extent(const StoreView& s, const MatchParams& mp, const int32_
 {
     if (count <= 0) return;
     k_match_extent<<<count, match_threads(mp.scan.n_beams), match_smem_bytes(0, mp.max_sqdist), st>>>(s, mp, d_states, d_results, d_xdir, xw);
+}
+void launch_match_fleet(const StoreView& s, const MatchParams& mp, const FleetScan* d_scans, const int32_t* d_scan_of_block, int max_beams, const int32_t* d_xdir,
+                        const DirWindow& xw, const SE2* d_states, MatchResult* d_results, int count, cudaStream_t st)
+{
+    if (count <= 0) return;
+    if (d_xdir)
+        k_match_fleet_extent<<<count, match_threads(max_beams), match_smem_bytes(0, mp.max_sqdist), st>>>(s, mp, d_scans, d_scan_of_block, d_states, d_results,
+                                                                                                          d_xdir, xw);
+    else
+        k_match_fleet<<<count, match_threads(max_beams), match_smem_bytes(s.window.dim, mp.max_sqdist), st>>>(s, mp, d_scans, d_scan_of_block, d_states, d_results);
 }
 void launch_extent_dir(const StoreView& s, const ParkView& pv, int set, const DirWindow& xw, int n_parked, int32_t* d_xdir, cudaStream_t st)
 {
@@ -2346,6 +2406,13 @@ void launch_sampling(const StoreView& s, const ParkView& pv, int set, int partic
 {
     if (n_offsets <= 0) return;
     k_sampling<<<n_offsets, 128, 0, st>>>(s, pv, set, particle, d_points, scan, pose, d_offsets, stride, resolution, max_sqdist, d_out);
+}
+void launch_sampling_fleet(const StoreView& s, const ParkView& pv, int set, const double* d_points, const FleetScan* d_scans, const int32_t* d_scan_of_block,
+                           const MatchResult* d_results, int count, double scale, const double* d_offsets, int n_offsets, double resolution, uint32_t max_sqdist,
+                           double* d_out, cudaStream_t st)
+{
+    if (count <= 0 || n_offsets <= 0) return;
+    k_sampling_fleet<<<dim3(n_offsets, count), 128, 0, st>>>(s, pv, set, d_points, d_scans, d_scan_of_block, d_results, scale, d_offsets, resolution, max_sqdist, d_out);
 }
 void launch_match_error(const StoreView& s, const ParkView& pv, int set, int particle0, bool shared_map, const double* d_points, const ScanParams& scan, const SE2* d_states, int count,
                         double resolution, uint32_t max_sqdist, double* d_out, cudaStream_t st)

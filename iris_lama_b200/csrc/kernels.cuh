@@ -19,6 +19,13 @@ struct MatchResult {
     uint32_t pad;
 };
 
+// One robot's scan in a fleet launch (k_match_fleet, k_sampling_fleet): points [offset, offset + n_beams) of the launch's ragged xyz array
+struct FleetScan {
+    int64_t offset;
+    int32_t n_beams, pad;
+    MovingTf moving;   // sensor pose in the base frame
+};
+
 struct MatchParams {
     const double* points;  // device, N x 3
     ScanParams scan;
@@ -100,6 +107,11 @@ void launch_match(const StoreView& s, const MatchParams& mp, const SE2* d_states
 // working window; a patch outside xw is absent
 void launch_match_extent(const StoreView& s, const MatchParams& mp, const int32_t* d_xdir, const DirWindow& xw, const SE2* d_states, MatchResult* d_results,
                          int count, cudaStream_t st);
+// k_match_fleet (d_xdir null: the working window) or k_match_fleet_extent (the dense directory d_xdir over xw): block k matches scan
+// d_scans[d_scan_of_block[k]] from d_states[k] in mode mp.mode on particle mp.particle_offset's map (mp.shared_map); max_beams = the
+// largest n_beams among those scans
+void launch_match_fleet(const StoreView& s, const MatchParams& mp, const FleetScan* d_scans, const int32_t* d_scan_of_block, int max_beams, const int32_t* d_xdir,
+                        const DirWindow& xw, const SE2* d_states, MatchResult* d_results, int count, cudaStream_t st);
 // d_xdir (xw.dim^2 entries, all -1 on entry) = the entries of particle 0's distance map, its window and the n_parked entries of its parked
 // list, at their patches
 void launch_extent_dir(const StoreView& s, const ParkView& pv, int set, const DirWindow& xw, int n_parked, int32_t* d_xdir, cudaStream_t st);
@@ -170,6 +182,10 @@ void launch_scatter_patches(const StoreView& s, int set, int particle, int kind,
 // Loc2D::addSamplingCovariance likelihoods: out[i] for offset i (offsets = n x 2 doubles)
 void launch_sampling(const StoreView& s, const ParkView& pv, int set, int particle, const double* d_points, const ScanParams& scan, const SE2& pose, const double* d_offsets,
                      int n_offsets, int stride, double resolution, uint32_t max_sqdist, double* d_out, cudaStream_t st);
+// the same for the `count` blocks of a fleet match: d_out[k * n_offsets + i] around d_results[k].state on scan d_scans[d_scan_of_block[k]]
+void launch_sampling_fleet(const StoreView& s, const ParkView& pv, int set, const double* d_points, const FleetScan* d_scans, const int32_t* d_scan_of_block,
+                           const MatchResult* d_results, int count, double scale, const double* d_offsets, int n_offsets, double resolution, uint32_t max_sqdist,
+                           double* d_out, cudaStream_t st);
 // MatchSurface2D::error() of `count` states (block k on the map of particle0 + k, or all on particle0's with shared_map)
 void launch_match_error(const StoreView& s, const ParkView& pv, int set, int particle0, bool shared_map, const double* d_points, const ScanParams& scan, const SE2* d_states, int count,
                         double resolution, uint32_t max_sqdist, double* d_out, cudaStream_t st);
