@@ -146,39 +146,30 @@ struct DistMap3Dev::Impl : PatchStore {
     uint32_t max_sqdist = 0;
     Dm3Guard guard;
     Dm3State h_st{};
-    Dm3State* st = nullptr;
-    uint64_t* heap[2] = {nullptr, nullptr};   // raise, lower
-    uint32_t cap[2] = {0, 0};
+    DeviceArray<Dm3State> st;
+    DeviceArray<uint64_t> heap[2];            // raise, lower
     uint64_t budget = kPopBudget;
     uint64_t runs = 0, grows = 0;
     std::vector<uint32_t> pending;            // queued ops, kDm3OpWords words each
     uint32_t pending_kind[2] = {0, 0};        // queued adds, removes
     Buf ops, qin, qout, qgrad, seg;
 
-    ~Impl()
-    {
-        cudaSetDevice(device);
-        if (stream) cudaStreamSynchronize(stream);
-        for (void* p : {(void*)st, (void*)heap[0], (void*)heap[1]})
-            if (p) cudaFree(p);
-    }
+    ~Impl() { quiesce(); }
     View view() const { return View{dir, (uint64_t*)cells, (uint32_t)pool, win}; }
 
     // doubles heap k until it holds `need` entries: allocate, copy the live entries, free
     cudaError_t grow(int k, uint64_t need)
     {
-        while (cap[k] < need) {
-            if (cap[k] >= (1u << 30)) return cudaErrorMemoryAllocation;
-            uint64_t* p = nullptr;
-            cudaError_t e = cudaMalloc((void**)&p, (size_t)cap[k] * 2 * 8);
+        while (heap[k].size() < need) {
+            if (heap[k].size() >= (1u << 30)) return cudaErrorMemoryAllocation;
+            DeviceArray<uint64_t> p;
+            cudaError_t e = p.alloc(heap[k].size() * 2);
             if (e != cudaSuccess) return e;
             const uint32_t live = k == 0 ? h_st.raise_size : h_st.lower_size;
-            if (live) e = cudaMemcpyAsync(p, heap[k], (size_t)live * 8, cudaMemcpyDeviceToDevice, stream);
+            if (live) e = cudaMemcpyAsync(p.get(), heap[k].get(), (size_t)live * 8, cudaMemcpyDeviceToDevice, stream);
             if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-            if (e != cudaSuccess) { cudaFree(p); return e; }
-            cudaFree(heap[k]);
-            heap[k] = p;
-            cap[k] *= 2;
+            if (e != cudaSuccess) return e;
+            heap[k] = std::move(p);
             ++grows;
         }
         return cudaSuccess;
@@ -208,12 +199,9 @@ DistMap3Dev* DistMap3Dev::create(double resolution, uint32_t patch_size, double 
     *code = d.init(dev, win, kDm3Log2Cells, 8, err);
     if (*code != LAMA_OK) { delete t; return nullptr; }
     cudaError_t e = cudaMemsetAsync(d.cells, 0, (size_t)d.pool << kDm3Log2Cells << 3, d.stream);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d.st, sizeof(Dm3State));
-    for (int k = 0; k < 2 && e == cudaSuccess; ++k) {
-        d.cap[k] = (uint32_t)cap0;
-        e = cudaMalloc((void**)&d.heap[k], (size_t)cap0 * 8);
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.st, &d.h_st, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream);
+    if (e == cudaSuccess) e = d.st.alloc(1);
+    for (int k = 0; k < 2 && e == cudaSuccess; ++k) e = d.heap[k].alloc(cap0);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d.st.get(), &d.h_st, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(d.stream);
     if (e != cudaSuccess) {
         err = std::string("DistMap3Dev::create: ") + cudaGetErrorString(e);
@@ -234,8 +222,8 @@ void DistMap3Dev::run_stats(uint64_t out[4]) const
 {
     out[0] = d_->runs;
     out[1] = d_->grows;
-    out[2] = d_->cap[0];
-    out[3] = d_->cap[1];
+    out[2] = d_->heap[0].size();
+    out[3] = d_->heap[1].size();
 }
 
 int DistMap3Dev::add_remove(const uint32_t* cells_xyz, int n, bool remove)
@@ -271,11 +259,11 @@ int DistMap3Dev::run(bool do_update, uint32_t* processed)
     const uint32_t n_ops = (uint32_t)(d.pending.size() / kDm3OpWords);
     PS_TRY(cudaSetDevice(d.device));
     if (n_ops) {
-        PS_TRY(d.ensure(d.ops, d.pending.size() * 4));
-        PS_TRY(cudaMemcpyAsync(d.ops.p, d.pending.data(), d.pending.size() * 4, cudaMemcpyHostToDevice, d.stream));
+        PS_TRY(d.ops.reserve(d.pending.size() * 4));
+        PS_TRY(cudaMemcpyAsync(d.ops.get(), d.pending.data(), d.pending.size() * 4, cudaMemcpyHostToDevice, d.stream));
     }
     if (do_update) d.h_st.processed = 0;
-    const int rc = drive((const uint32_t*)d.ops.p, n_ops, do_update, nullptr, 0, nullptr);
+    const int rc = drive((const uint32_t*)d.ops.get(), n_ops, do_update, nullptr, 0, nullptr);
     if (rc != LAMA_OK) return rc;
     d.pending.clear();
     d.pending_kind[0] = d.pending_kind[1] = 0;
@@ -288,15 +276,15 @@ int DistMap3Dev::run(bool do_update, uint32_t* processed)
 int DistMap3Dev::drive(const uint32_t* ops, uint32_t n_ops, bool do_update, const uint32_t* seg_end, uint32_t n_seg, uint32_t* seg_processed)
 {
     Impl& d = *d_;
-    PS_TRY(cudaMemcpyAsync(d.st, &d.h_st, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream));
+    PS_TRY(cudaMemcpyAsync(d.st.get(), &d.h_st, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream));
     PS_TRY(d.record(0));
     for (;;) {
-        k_dm3_brushfire<<<1, 1, 0, d.stream>>>(d.view(), d.heap[0], d.cap[0], d.heap[1], d.cap[1], ops, n_ops, do_update ? 1 : 0, d.budget, d.max_sqdist,
-                                               d.st, seg_end, n_seg, seg_processed);
+        k_dm3_brushfire<<<1, 1, 0, d.stream>>>(d.view(), d.heap[0].get(), (uint32_t)d.heap[0].size(), d.heap[1].get(), (uint32_t)d.heap[1].size(), ops, n_ops, do_update ? 1 : 0, d.budget, d.max_sqdist,
+                                               d.st.get(), seg_end, n_seg, seg_processed);
         d.launches[0] += 1;
         ++d.runs;
         PS_TRY(cudaGetLastError());
-        PS_TRY(cudaMemcpyAsync(&d.h_st, d.st, sizeof(Dm3State), cudaMemcpyDeviceToHost, d.stream));
+        PS_TRY(cudaMemcpyAsync(&d.h_st, d.st.get(), sizeof(Dm3State), cudaMemcpyDeviceToHost, d.stream));
         PS_TRY(cudaStreamSynchronize(d.stream));
         if (d.h_st.err) {
             err_ = "internal: the brushfire addressed a cell outside the admitted region (error bits " + std::to_string(d.h_st.err) + ")";
@@ -348,7 +336,7 @@ int DistMap3Dev::alloc_entries(const std::vector<uint32_t>& marks, void* done)
     if (fresh) {
         d.used = (int)d.h_st.used;
         PS_TRY(cudaMemcpyAsync(d.dir, d.h_dir.data(), (size_t)d.ndir * 4, cudaMemcpyHostToDevice, d.stream));
-        PS_TRY(cudaMemcpyAsync(d.st, &d.h_st, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream));
+        PS_TRY(cudaMemcpyAsync(d.st.get(), &d.h_st, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream));
     }
     PS_TRY(cudaEventRecord((cudaEvent_t)done, d.stream));
     return LAMA_OK;
@@ -361,8 +349,8 @@ int DistMap3Dev::run_segments(const uint32_t* ops, const std::vector<uint32_t>& 
     if (n_seg == 0) return LAMA_OK;
     PS_TRY(cudaSetDevice(d.device));
     if (wait) PS_TRY(cudaStreamWaitEvent(d.stream, (cudaEvent_t)wait, 0));
-    PS_TRY(d.ensure(d.seg, (size_t)n_seg * 8));
-    uint32_t* dseg = (uint32_t*)d.seg.p;
+    PS_TRY(d.seg.reserve((size_t)n_seg * 8));
+    uint32_t* dseg = (uint32_t*)d.seg.get();
     PS_TRY(cudaMemcpyAsync(dseg, seg_end.data(), (size_t)n_seg * 4, cudaMemcpyHostToDevice, d.stream));
     d.h_st.processed = 0;
     d.h_st.seg = 0;
@@ -388,18 +376,18 @@ int DistMap3Dev::distance(const double* pts_xyz, int n, double* dist, double* gr
     int rc = flush();
     if (rc != LAMA_OK) return rc;
     PS_TRY(cudaSetDevice(d.device));
-    PS_TRY(d.ensure(d.qin, (size_t)n * 24));
-    PS_TRY(d.ensure(d.qout, (size_t)n * 8));
-    if (gradient) PS_TRY(d.ensure(d.qgrad, (size_t)n * 24));
-    PS_TRY(cudaMemcpyAsync(d.qin.p, pts_xyz, (size_t)n * 24, cudaMemcpyHostToDevice, d.stream));
+    PS_TRY(d.qin.reserve((size_t)n * 24));
+    PS_TRY(d.qout.reserve((size_t)n * 8));
+    if (gradient) PS_TRY(d.qgrad.reserve((size_t)n * 24));
+    PS_TRY(cudaMemcpyAsync(d.qin.get(), pts_xyz, (size_t)n * 24, cudaMemcpyHostToDevice, d.stream));
     PS_TRY(d.record(0));
-    k_dm3_distance<<<blocks_for(n), kThreads, 0, d.stream>>>(d.view(), (const double*)d.qin.p, n, d.scale, d.resolution, d.max_sqdist, (double*)d.qout.p,
-                                                             gradient ? (double*)d.qgrad.p : nullptr);
+    k_dm3_distance<<<blocks_for(n), kThreads, 0, d.stream>>>(d.view(), (const double*)d.qin.get(), n, d.scale, d.resolution, d.max_sqdist, (double*)d.qout.get(),
+                                                             gradient ? (double*)d.qgrad.get() : nullptr);
     d.launches[1] += 1;
     PS_TRY(cudaGetLastError());
     PS_TRY(d.record(1));
-    PS_TRY(cudaMemcpyAsync(dist, d.qout.p, (size_t)n * 8, cudaMemcpyDeviceToHost, d.stream));
-    if (gradient) PS_TRY(cudaMemcpyAsync(gradient, d.qgrad.p, (size_t)n * 24, cudaMemcpyDeviceToHost, d.stream));
+    PS_TRY(cudaMemcpyAsync(dist, d.qout.get(), (size_t)n * 8, cudaMemcpyDeviceToHost, d.stream));
+    if (gradient) PS_TRY(cudaMemcpyAsync(gradient, d.qgrad.get(), (size_t)n * 24, cudaMemcpyDeviceToHost, d.stream));
     PS_TRY(d.finish(1));
     return LAMA_OK;
 }
@@ -412,15 +400,15 @@ int DistMap3Dev::cell_distance(const uint32_t* cells_xyz, int n, double* dist)
     int rc = flush();
     if (rc != LAMA_OK) return rc;
     PS_TRY(cudaSetDevice(d.device));
-    PS_TRY(d.ensure(d.qin, (size_t)n * 12));
-    PS_TRY(d.ensure(d.qout, (size_t)n * 8));
-    PS_TRY(cudaMemcpyAsync(d.qin.p, cells_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, d.stream));
+    PS_TRY(d.qin.reserve((size_t)n * 12));
+    PS_TRY(d.qout.reserve((size_t)n * 8));
+    PS_TRY(cudaMemcpyAsync(d.qin.get(), cells_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, d.stream));
     PS_TRY(d.record(0));
-    k_dm3_cell_distance<<<blocks_for(n), kThreads, 0, d.stream>>>(d.view(), (const uint32_t*)d.qin.p, n, d.resolution, d.max_sqdist, (double*)d.qout.p);
+    k_dm3_cell_distance<<<blocks_for(n), kThreads, 0, d.stream>>>(d.view(), (const uint32_t*)d.qin.get(), n, d.resolution, d.max_sqdist, (double*)d.qout.get());
     d.launches[2] += 1;
     PS_TRY(cudaGetLastError());
     PS_TRY(d.record(1));
-    PS_TRY(cudaMemcpyAsync(dist, d.qout.p, (size_t)n * 8, cudaMemcpyDeviceToHost, d.stream));
+    PS_TRY(cudaMemcpyAsync(dist, d.qout.get(), (size_t)n * 8, cudaMemcpyDeviceToHost, d.stream));
     PS_TRY(d.finish(2));
     return LAMA_OK;
 }
@@ -550,7 +538,7 @@ int DistMap3Dev::read(const std::string& path)
     Dm3State s{};
     s.used = (uint32_t)f.ids.size();
     PS_TRY(cudaMemcpyAsync(d.dir, h_dir.data(), (size_t)d.ndir * 4, cudaMemcpyHostToDevice, d.stream));
-    PS_TRY(cudaMemcpyAsync(d.st, &s, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream));
+    PS_TRY(cudaMemcpyAsync(d.st.get(), &s, sizeof(Dm3State), cudaMemcpyHostToDevice, d.stream));
     PS_TRY(cudaStreamSynchronize(d.stream));
     d.h_dir = h_dir;
     d.h_st = s;

@@ -7,6 +7,7 @@
 #include <cstring>
 #include <memory>
 
+#include "cuda_owned.h"
 #include "dm_follow.h"
 #include "kernels.cuh"
 #include "render_plan.h"
@@ -20,29 +21,52 @@ namespace lama_b200 {
     } while (0)
 
 struct Engine::Impl {
-    cudaStream_t stream = nullptr;
-    bool own_stream = true;
+    // streams first, events next, buffers last: members are destroyed buffers first, then events, then streams
+    Stream stream;   // the caller's stream (EngineConfig::stream, borrowed) or one of the engine's own
+    // particle groups of the grouped step (Engine::step_groups): group g owns the particles [g * P / G, (g + 1) * P / G) and a stream of
+    // its own; an upload stream carries the scan and the predicted states.  Each group's kernels count patches into a counter block
+    // of their own (d_gcnt[g]), so that a report holds that group's work of one scan exactly; settle() folds the blocks into
+    // view.counters.  A map update on one stream is the one-group case, counting into view.counters itself.
+    // h_grep[half][g] = {status, allocated, detached, freed, free slots, ...}; with G > 1 slot G = view.counters at the step.
+    Stream gstream[kMaxGroups];
+    Stream up_stream;
+    Event ev_match, ev_sync;
+    Event ev[2];
+    Event ev_render[2];   // around one group of a following render (shift_window takes ev[0] / ev[1] between groups)
+    // timing of a map update: per report buffer {before the match, after the match, after the ray stage, after the brushfire}; read when
+    // that update is collected, so no host synchronisation is added.  evp_match: the update recorded a match (evp[half][0] is set).
+    Event evp[2][4];
+    Event ev_gmatch[kMaxGroups], ev_gdone[kMaxGroups];
+    Event ev_up, ev_fork;
+    // the store's arrays; view holds pointers into them (view.pool aligned out of pool_raw; grow_pool replaces the per-slot ones)
+    DeviceArray<char> pool_raw;
+    DeviceArray<uint32_t> fbits, kbits;
+    DeviceArray<int32_t> refcount, free_slots, freed, free_count, dirs;   // free_count: 64 B, view.free_count .. view.counters
+    DeviceArray<uint64_t> brush_spill;
+    DeviceArray<RayPullHeader> pull_hdr;
+    DeviceArray<PullEntry> pull_list;
+    DeviceArray<uint32_t> pull_hits;
+    DeviceArray<uint2> pull_tasks;
+    DeviceArray<int32_t> pull_ctrl;
     StoreView view{};
     // scan
     double* d_points = nullptr;      // current scan (points into d_scan_buf or d_staged)
-    double* d_scan_buf = nullptr;
-    double* d_staged = nullptr;
+    DeviceArray<double> d_scan_buf;
+    DeviceArray<double> d_staged;
     int staged_scans = 0, staged_beams = 0;
     ScanParams scan{};
     // per-launch staging
-    SE2* d_states = nullptr;
-    SE2* h_states = nullptr;  // pinned
-    MatchResult* d_results = nullptr;
-    MatchResult* h_results = nullptr;  // pinned
-    MapUpdateStats* d_stats = nullptr;
-    MapUpdateStats* h_stats = nullptr;  // pinned; two halves (ping-pong between consecutive map updates)
-    double* h_scan = nullptr;           // pinned staging of a host scan (step_async)
-    cudaEvent_t ev_match = nullptr, ev_sync = nullptr;
-    uint64_t* d_events = nullptr;
-    int32_t* d_idx = nullptr;
-    int32_t* h_idx = nullptr;  // pinned
-    uint32_t* h_status = nullptr;  // pinned
-    int state_cap = 0;
+    DeviceArray<SE2> d_states;
+    PinnedArray<SE2> h_states;
+    DeviceArray<MatchResult> d_results;
+    PinnedArray<MatchResult> h_results;
+    DeviceArray<MapUpdateStats> d_stats;
+    PinnedArray<MapUpdateStats> h_stats;   // two halves (ping-pong between consecutive map updates)
+    PinnedArray<double> h_scan;            // staging of a host scan (step_async)
+    DeviceArray<uint64_t> d_events;
+    DeviceArray<int32_t> d_idx;
+    PinnedArray<int32_t> h_idx;
+    PinnedArray<uint32_t> h_status;
     RayParams ray{};
     BrushParams brush{};
     int n_sms = 132;
@@ -50,65 +74,45 @@ struct Engine::Impl {
                                   // count, see launch_ray_stage); LAMA_PULL_MAX_PARTICLES overrides
     bool scan_flat = false;     // the current scan has z == 0 everywhere and a sensor that keeps z planes: every beam is planar
     bool staged_flat = false;   // the same for the staged scans
-    cudaEvent_t ev[2] = {nullptr, nullptr};
-    cudaEvent_t ev_render[2] = {nullptr, nullptr};   // around one group of a following render (shift_window takes ev[0] / ev[1] between groups)
-    void* pool_raw = nullptr;                          // the allocation view.pool was aligned out of (grow_pool replaces it)
-    // timing of a map update: per report buffer {before the match, after the match, after the ray stage, after the brushfire}; read when
-    // that update is collected, so no host synchronisation is added.  evp_match: the update recorded a match (evp[half][0] is set).
-    cudaEvent_t evp[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};
     bool evp_used[2] = {false, false}, evp_match[2] = {false, false};
-    // particle groups of the grouped step (Engine::step_groups): group g owns the particles [g * P / G, (g + 1) * P / G) and a stream of
-    // its own; an upload stream carries the scan and the predicted states.  Each group's kernels count patches into a counter block
-    // of their own (d_gcnt[g]), so that a report holds that group's work of one scan exactly; settle() folds the blocks into
-    // view.counters.  A map update on one stream is the one-group case, counting into view.counters itself.
-    // h_grep[half][g] = {status, allocated, detached, freed, free slots, ...}; with G > 1 slot G = view.counters at the step.
     int groups = 1;
-    cudaStream_t gstream[kMaxGroups] = {};
-    cudaStream_t up_stream = nullptr;
-    cudaEvent_t ev_gmatch[kMaxGroups] = {}, ev_gdone[kMaxGroups] = {};
-    cudaEvent_t ev_up = nullptr, ev_fork = nullptr;
-    uint64_t* d_gcnt = nullptr;                 // [kMaxGroups][4]
-    uint64_t* h_grep = nullptr;                 // pinned [2][kMaxGroups + 1][8]
+    DeviceArray<uint64_t> d_gcnt;               // [kMaxGroups][4]
+    PinnedArray<uint64_t> h_grep;               // [2][kMaxGroups + 1][8]
     int report_groups[2] = {0, 0};              // groups of the map update that reported into each half
     bool fork = true;                           // the group streams must wait for the launching stream before their next work
     bool groups_ran = false;                    // grouped steps since the last fold: d_gcnt and the deferred k_merge_free are pending
     int scan_half = 0;                          // half of d_scan_buf the last grouped host scan went to
     uint64_t scan_alloc = 0, prev_alloc = 0;    // patches the last booked grouped scan allocated (allocated + detached), and the sum at its booking
     // scratch for import/export/distance
-    void* d_scratch = nullptr;
-    size_t scratch_bytes = 0;
+    DeviceArray<char> d_scratch;
     // scratch of shift_window, apart from d_scratch: a following render shifts the window between groups while its scans sit in d_scratch
-    void* d_shift_scratch = nullptr;
-    size_t shift_scratch_bytes = 0;
+    DeviceArray<char> d_shift_scratch;
     // the dense directory of match_extent (Engine::extent_)
-    void* d_extent = nullptr;
-    size_t extent_bytes = 0;
+    DeviceArray<char> d_extent;
     // fleet rounds (fleet_reserve): room for fleet_cap scans of max_beams beams; the pinned staging h_fleet holds the descriptors, then
     // the points, in the layout of d_fleet; the per-block scan indices (upload_states' growth) and the sampling offsets and likelihoods
-    void* d_fleet = nullptr;
-    void* h_fleet = nullptr;
+    DeviceArray<char> d_fleet;
+    PinnedArray<char> h_fleet;
     int fleet_cap = 0, fleet_max_beams = 0;
-    int32_t* d_fleet_blocks = nullptr;
-    int32_t* h_fleet_blocks = nullptr;
-    int fleet_block_cap = 0;
-    double* d_fleet_off = nullptr;
-    double* d_fleet_lik = nullptr;
-    double* h_fleet_lik = nullptr;
+    DeviceArray<int32_t> d_fleet_blocks;
+    PinnedArray<int32_t> h_fleet_blocks;
+    DeviceArray<double> d_fleet_off;
+    DeviceArray<double> d_fleet_lik;
+    PinnedArray<double> h_fleet_lik;
     int fleet_n_off = 0;
-    FleetScan* fleet_scans() const { return (FleetScan*)d_fleet; }
-    double* fleet_points() const { return (double*)((char*)d_fleet + (size_t)fleet_cap * sizeof(FleetScan)); }
+    FleetScan* fleet_scans() const { return (FleetScan*)d_fleet.get(); }
+    double* fleet_points() const { return (double*)(d_fleet.get() + (size_t)fleet_cap * sizeof(FleetScan)); }
     // device arena of a migration round (pack_device / migration_alloc): bump allocation out of chunks that are kept between rounds, so that a resampling
     // scan costs no cudaMalloc / cudaFree once the arena has grown to its working size
-    std::vector<std::pair<char*, size_t>> mig_chunks;
+    std::vector<DeviceArray<char>> mig_chunks;
     size_t mig_chunk = 0, mig_off = 0;
-    std::vector<void*> allocs;
     // parked entries (window_shift_core.h): per set one device arena (park[set]) and the {offset, length} of every list, on the device
     // (d_park_ol[set]) and here; they change only in shift_window, resample and prune_outside
-    ParkEntry* park[2] = {nullptr, nullptr};
-    int2* d_park_ol[2] = {nullptr, nullptr};
+    DeviceArray<ParkEntry> park[2];
+    DeviceArray<int2> d_park_ol[2];
     std::vector<int2> park_ol[2];
     uint64_t shifts = 0, restored = 0;
-    ParkView pv(int set) const { return ParkView{park[set], d_park_ol[set]}; }
+    ParkView pv(int set) const { return ParkView{park[set].get(), d_park_ol[set].get()}; }
     int n_lists() const { return (int)park_ol[0].size(); }
     size_t parked(int set) const
     {
@@ -121,15 +125,14 @@ struct Engine::Impl {
         const int2 ol = park_ol[set][list];
         out.resize((size_t)ol.y);
         if (!ol.y) return cudaSuccess;
-        cudaError_t e = cudaMemcpyAsync(out.data(), park[set] + ol.x, out.size() * sizeof(ParkEntry), cudaMemcpyDeviceToHost, stream);
+        cudaError_t e = cudaMemcpyAsync(out.data(), park[set].get() + ol.x, out.size() * sizeof(ParkEntry), cudaMemcpyDeviceToHost, stream);
         return e == cudaSuccess ? cudaStreamSynchronize(stream) : e;
     }
     void drop_arena(int set)   // the stream must have passed every use of the arena
     {
-        if (park[set]) cudaFree(park[set]);
-        park[set] = nullptr;
+        park[set].reset();
         std::fill(park_ol[set].begin(), park_ol[set].end(), make_int2(0, 0));
-        cudaMemsetAsync(d_park_ol[set], 0, park_ol[set].size() * sizeof(int2), stream);
+        cudaMemsetAsync(d_park_ol[set].get(), 0, park_ol[set].size() * sizeof(int2), stream);
     }
     int launch_ray_stage(const StoreView& v, RayParams rp, const SE2* states, uint64_t* events, MapUpdateStats* stats, int count, cudaStream_t st) const;
 };
@@ -219,19 +222,17 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     const double scale = 1.0 / cfg.resolution;
     uint32_t radius = 0;
     if (!reach_fits(cfg.resolution, cfg.l2_max, &radius, err)) return nullptr;
-    Engine* e = new Engine();
+    std::unique_ptr<Engine> e(new Engine());
     e->cfg_ = cfg;
     e->max_sqdist_ = radius * radius;
     if (e->cfg_.pool_slots <= 0) e->cfg_.pool_slots = auto_pool_slots(cfg.particles);
     if (e->cfg_.pool_slots >= kDirSlotMask) {   // directory entries keep the slot in 24 bits, all ones = "not writable"
         err = "pool_slots must be below 2^24 - 1 (the slot field of a directory entry)";
-        delete e;
         return nullptr;
     }
     Impl* d = e->d_ = new Impl();
     auto bail = [&](const std::string& m) {
         err = m;
-        delete e;
         return (Engine*)nullptr;
     };
 #define CU_NEW(expr)                                                             \
@@ -240,18 +241,16 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
         if (_e != cudaSuccess) return bail(std::string(#expr) + ": " + cudaGetErrorString(_e)); \
     } while (0)
     CU_NEW(cudaSetDevice(cfg.device));
-    if (cfg.stream) {
-        d->stream = reinterpret_cast<cudaStream_t>(cfg.stream);
-        d->own_stream = false;
-    } else {
-        CU_NEW(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
-    }
-    CU_NEW(cudaEventCreate(&d->ev[0]));
-    CU_NEW(cudaEventCreate(&d->ev[1]));
-    CU_NEW(cudaEventCreate(&d->ev_render[0]));
-    CU_NEW(cudaEventCreate(&d->ev_render[1]));
+    if (cfg.stream)
+        d->stream.borrow(reinterpret_cast<cudaStream_t>(cfg.stream));
+    else
+        CU_NEW(d->stream.create());
+    CU_NEW(d->ev[0].create(cudaEventDefault));
+    CU_NEW(d->ev[1].create(cudaEventDefault));
+    CU_NEW(d->ev_render[0].create(cudaEventDefault));
+    CU_NEW(d->ev_render[1].create(cudaEventDefault));
     for (int b = 0; b < 2; ++b)
-        for (int k = 0; k < 4; ++k) CU_NEW(cudaEventCreate(&d->evp[b][k]));
+        for (int k = 0; k < 4; ++k) CU_NEW(d->evp[b][k].create(cudaEventDefault));
 
     // directory window centred on (center_x, center_y)
     const uint32_t cx = w2m(cfg.center_x, scale), cy = w2m(cfg.center_y, scale);
@@ -266,32 +265,34 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     v.kbits       = nullptr;
     v.window      = e->window_;
     const size_t dim2 = (size_t)cfg.dir_dim * cfg.dir_dim;
-    auto dalloc = [&](void** p, size_t bytes) -> cudaError_t {
-        cudaError_t r = cudaMalloc(p, bytes);
-        if (r == cudaSuccess) d->allocs.push_back(*p);
-        return r;
-    };
     // k_raycast ORs cell offsets into patch base addresses: the pool starts on a 4 KiB boundary (cudaMalloc only promises 256 B)
-    CU_NEW(dalloc(&d->pool_raw, ((size_t)v.n_slots + 1) * kPatchBytes));
-    v.pool = reinterpret_cast<uint32_t*>(((uintptr_t)d->pool_raw + (kPatchBytes - 1)) & ~(uintptr_t)(kPatchBytes - 1));
-    CU_NEW(dalloc((void**)&v.fbits, (size_t)v.n_slots * 128));
-    if (cfg.occupancy_kind == 1 || cfg.known_plane) CU_NEW(dalloc((void**)&v.kbits, (size_t)v.n_slots * 128));
-    CU_NEW(dalloc((void**)&v.refcount, (size_t)v.n_slots * 4));
-    CU_NEW(dalloc((void**)&v.free_slots, (size_t)v.n_slots * 4));
-    CU_NEW(dalloc((void**)&v.freed, (size_t)v.n_slots * 4));
-    CU_NEW(dalloc((void**)&v.free_count, 64));
+    CU_NEW(d->pool_raw.alloc(((size_t)v.n_slots + 1) * kPatchBytes));
+    v.pool = reinterpret_cast<uint32_t*>(((uintptr_t)d->pool_raw.get() + (kPatchBytes - 1)) & ~(uintptr_t)(kPatchBytes - 1));
+    CU_NEW(d->fbits.alloc((size_t)v.n_slots * 32));
+    v.fbits = d->fbits.get();
+    if (cfg.occupancy_kind == 1 || cfg.known_plane) CU_NEW(d->kbits.alloc((size_t)v.n_slots * 32));
+    v.kbits = d->kbits.get();
+    CU_NEW(d->refcount.alloc((size_t)v.n_slots));
+    CU_NEW(d->free_slots.alloc((size_t)v.n_slots));
+    CU_NEW(d->freed.alloc((size_t)v.n_slots));
+    CU_NEW(d->free_count.alloc(16));
+    v.refcount    = d->refcount.get();
+    v.free_slots  = d->free_slots.get();
+    v.freed       = d->freed.get();
+    v.free_count  = d->free_count.get();
     v.freed_count = v.free_count + 1;
     v.status      = reinterpret_cast<uint32_t*>(v.free_count + 2);
     v.counters    = reinterpret_cast<uint64_t*>(v.free_count + 4);
-    CU_NEW(dalloc((void**)&v.dirs, 2 * (size_t)cfg.particles * v.n_kinds * dim2 * 4));
+    CU_NEW(d->dirs.alloc(2 * (size_t)cfg.particles * v.n_kinds * dim2));
+    v.dirs = d->dirs.get();
     for (int set = 0; set < 2; ++set) {
         d->park_ol[set].assign((size_t)cfg.particles * v.n_kinds, make_int2(0, 0));
-        CU_NEW(dalloc((void**)&d->d_park_ol[set], d->park_ol[set].size() * sizeof(int2)));
-        CU_NEW(cudaMemset(d->d_park_ol[set], 0, d->park_ol[set].size() * sizeof(int2)));
+        CU_NEW(d->d_park_ol[set].alloc(d->park_ol[set].size()));
+        CU_NEW(cudaMemset(d->d_park_ol[set].get(), 0, d->park_ol[set].size() * sizeof(int2)));
     }
     // two halves: a grouped step uploads the next host scan into one while the other groups' ray casts may still read the other
-    CU_NEW(dalloc((void**)&d->d_scan_buf, 2 * (size_t)cfg.max_beams * 3 * 8));
-    d->d_points = d->d_scan_buf;
+    CU_NEW(d->d_scan_buf.alloc(2 * (size_t)cfg.max_beams * 3));
+    d->d_points = d->d_scan_buf.get();
 
     d->ray.log_cap   = next_pow2_host(std::max(4096, 3 * cfg.max_beams));
     d->ray.cand_cap  = 192;
@@ -330,10 +331,11 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     }
     d->brush.lower_cap = std::min(d->brush.lower_cap, d->brush.lower_total);
     d->brush.raise_cap = std::min(d->brush.raise_cap, d->brush.raise_total);
-    CU_NEW(dalloc((void**)&d->brush.lower_spill, (size_t)cfg.particles * (d->brush.lower_total + 2 + d->brush.raise_total + 2) * 8));
+    CU_NEW(d->brush_spill.alloc((size_t)cfg.particles * (d->brush.lower_total + 2 + d->brush.raise_total + 2)));
+    d->brush.lower_spill = d->brush_spill.get();
     d->brush.raise_spill = d->brush.lower_spill + (size_t)cfg.particles * (d->brush.lower_total + 2);
     d->brush.max_sqdist = e->max_sqdist_;
-    CU_NEW(dalloc((void**)&d->d_events, (size_t)cfg.particles * d->ray.event_cap * 8));
+    CU_NEW(d->d_events.alloc((size_t)cfg.particles * d->ray.event_cap));
     {   // scratch of the pull ray cast (k_ray_setup -> k_ray_pull)
         RayPullView& pv = d->ray.pull;
         pv.stride = (std::min(cfg.max_beams, kPullMaxBeams) + 31) & ~31;
@@ -341,11 +343,16 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
         int npad = 32;
         while (npad < pv.stride) npad <<= 1;
         pv.stride = npad;   // k_ray_setup writes whole sorted arrays of next_pow2(beams) entries
-        CU_NEW(dalloc((void**)&pv.hdr, (size_t)cfg.particles * sizeof(RayPullHeader)));
-        CU_NEW(dalloc((void**)&pv.list, (size_t)cfg.particles * pv.stride * sizeof(PullEntry)));
-        CU_NEW(dalloc((void**)&pv.hits, (size_t)cfg.particles * pv.stride * 4));
-        CU_NEW(dalloc((void**)&pv.tasks, (size_t)cfg.particles * dim2 * 8));
-        CU_NEW(dalloc((void**)&pv.ctrl, 64));
+        CU_NEW(d->pull_hdr.alloc((size_t)cfg.particles));
+        CU_NEW(d->pull_list.alloc((size_t)cfg.particles * pv.stride));
+        CU_NEW(d->pull_hits.alloc((size_t)cfg.particles * pv.stride));
+        CU_NEW(d->pull_tasks.alloc((size_t)cfg.particles * dim2));
+        CU_NEW(d->pull_ctrl.alloc(16));
+        pv.hdr   = d->pull_hdr.get();
+        pv.list  = d->pull_list.get();
+        pv.hits  = d->pull_hits.get();
+        pv.tasks = d->pull_tasks.get();
+        pv.ctrl  = d->pull_ctrl.get();
         CU_NEW(cudaMemset(pv.ctrl, 0, 64));
         CU_NEW(cudaMemset(pv.hdr, 0, (size_t)cfg.particles * sizeof(RayPullHeader)));
         v.ray_ctrl = pv.ctrl;
@@ -354,17 +361,17 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
         d->n_sms = sms > 0 ? sms : 132;
         if (const char* pm = std::getenv("LAMA_PULL_MAX_PARTICLES")) d->pull_max_particles = std::atoi(pm);
     }
-    CU_NEW(dalloc((void**)&d->d_stats, (size_t)cfg.particles * sizeof(MapUpdateStats)));
+    CU_NEW(d->d_stats.alloc((size_t)cfg.particles));
     const size_t idx_ints = std::max((size_t)cfg.particles, (size_t)cfg.dir_dim * cfg.dir_dim);   // resample indices / directory entries to delete
-    CU_NEW(dalloc((void**)&d->d_idx, idx_ints * 4));
-    CU_NEW(cudaMallocHost((void**)&d->h_stats, 2 * (size_t)cfg.particles * sizeof(MapUpdateStats)));
-    CU_NEW(cudaMallocHost((void**)&d->h_grep, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t)));
-    std::memset(d->h_grep, 0, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t));
-    CU_NEW(cudaMallocHost((void**)&d->h_scan, (size_t)cfg.max_beams * 24));
-    CU_NEW(cudaEventCreateWithFlags(&d->ev_match, cudaEventDisableTiming));
-    CU_NEW(cudaEventCreateWithFlags(&d->ev_sync, cudaEventDisableTiming));
-    CU_NEW(cudaMallocHost((void**)&d->h_idx, idx_ints * 4));
-    CU_NEW(cudaMallocHost((void**)&d->h_status, 64));
+    CU_NEW(d->d_idx.alloc(idx_ints));
+    CU_NEW(d->h_stats.alloc(2 * (size_t)cfg.particles));
+    CU_NEW(d->h_grep.alloc(2 * (size_t)(kMaxGroups + 1) * 8));
+    std::memset(d->h_grep.get(), 0, 2 * (size_t)(kMaxGroups + 1) * 8 * sizeof(uint64_t));
+    CU_NEW(d->h_scan.alloc((size_t)cfg.max_beams * 3));
+    CU_NEW(d->ev_match.create(cudaEventDisableTiming));
+    CU_NEW(d->ev_sync.create(cudaEventDisableTiming));
+    CU_NEW(d->h_idx.alloc(idx_ints));
+    CU_NEW(d->h_status.alloc(16));
 
     // Particle groups of step_async (DESIGN.md 7a): a scan of G groups overlaps one group's brushfire and next match with other groups'
     // ray casts.  One group when the pull ray cast may be selected (its task list is shared by every particle of a launch); otherwise
@@ -377,15 +384,15 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
         d->groups = std::max(1, std::min(std::min(g, kMaxGroups), cfg.particles));
         if (d->groups > 1) {
             for (int k = 0; k < d->groups; ++k) {
-                CU_NEW(cudaStreamCreateWithFlags(&d->gstream[k], cudaStreamNonBlocking));
-                CU_NEW(cudaEventCreateWithFlags(&d->ev_gmatch[k], cudaEventDisableTiming));
-                CU_NEW(cudaEventCreateWithFlags(&d->ev_gdone[k], cudaEventDisableTiming));
+                CU_NEW(d->gstream[k].create());
+                CU_NEW(d->ev_gmatch[k].create(cudaEventDisableTiming));
+                CU_NEW(d->ev_gdone[k].create(cudaEventDisableTiming));
             }
-            CU_NEW(cudaStreamCreateWithFlags(&d->up_stream, cudaStreamNonBlocking));
-            CU_NEW(cudaEventCreateWithFlags(&d->ev_up, cudaEventDisableTiming));
-            CU_NEW(cudaEventCreateWithFlags(&d->ev_fork, cudaEventDisableTiming));
-            CU_NEW(dalloc((void**)&d->d_gcnt, (size_t)kMaxGroups * 4 * sizeof(uint64_t)));
-            CU_NEW(cudaMemset(d->d_gcnt, 0, (size_t)kMaxGroups * 4 * sizeof(uint64_t)));
+            CU_NEW(d->up_stream.create());
+            CU_NEW(d->ev_up.create(cudaEventDisableTiming));
+            CU_NEW(d->ev_fork.create(cudaEventDisableTiming));
+            CU_NEW(d->d_gcnt.alloc((size_t)kMaxGroups * 4));
+            CU_NEW(cudaMemset(d->d_gcnt.get(), 0, (size_t)kMaxGroups * 4 * sizeof(uint64_t)));
         }
     }
 
@@ -398,53 +405,17 @@ Engine* Engine::create(const EngineConfig& cfg, std::string& err)
     CU_NEW(cudaGetLastError());
     CU_NEW(cudaStreamSynchronize(d->stream));
 #undef CU_NEW
-    return e;
+    return e.release();
 }
 
 Engine::~Engine()
 {
     if (!d_) return;
     cudaSetDevice(cfg_.device);
-    if (d_->stream) cudaStreamSynchronize(d_->stream);
-    for (int k = 0; k < kMaxGroups; ++k) {
-        if (d_->gstream[k]) { cudaStreamSynchronize(d_->gstream[k]); cudaStreamDestroy(d_->gstream[k]); }
-        for (cudaEvent_t ev : {d_->ev_gmatch[k], d_->ev_gdone[k]})
-            if (ev) cudaEventDestroy(ev);
-    }
-    if (d_->up_stream) { cudaStreamSynchronize(d_->up_stream); cudaStreamDestroy(d_->up_stream); }
-    if (d_->ev_up) cudaEventDestroy(d_->ev_up);
-    if (d_->ev_fork) cudaEventDestroy(d_->ev_fork);
-    if (d_->h_grep) cudaFreeHost(d_->h_grep);
-    for (void* p : d_->allocs) cudaFree(p);
-    for (int set = 0; set < 2; ++set)
-        if (d_->park[set]) cudaFree(d_->park[set]);
-    if (d_->d_states) cudaFree(d_->d_states);
-    if (d_->d_results) cudaFree(d_->d_results);
-    if (d_->h_states) cudaFreeHost(d_->h_states);
-    if (d_->h_results) cudaFreeHost(d_->h_results);
-    if (d_->h_stats) cudaFreeHost(d_->h_stats);
-    if (d_->h_scan) cudaFreeHost(d_->h_scan);
-    if (d_->ev_match) cudaEventDestroy(d_->ev_match);
-    if (d_->ev_sync) cudaEventDestroy(d_->ev_sync);
-    for (cudaEvent_t ev : d_->ev_render)
-        if (ev) cudaEventDestroy(ev);
-    for (auto& c : d_->mig_chunks) cudaFree(c.first);
-    if (d_->h_idx) cudaFreeHost(d_->h_idx);
-    if (d_->h_status) cudaFreeHost(d_->h_status);
-    if (d_->d_scratch) cudaFree(d_->d_scratch);
-    if (d_->d_shift_scratch) cudaFree(d_->d_shift_scratch);
-    if (d_->d_extent) cudaFree(d_->d_extent);
-    for (void* p : {d_->d_fleet, (void*)d_->d_fleet_blocks, (void*)d_->d_fleet_off, (void*)d_->d_fleet_lik})
-        if (p) cudaFree(p);
-    for (void* p : {d_->h_fleet, (void*)d_->h_fleet_blocks, (void*)d_->h_fleet_lik})
-        if (p) cudaFreeHost(p);
-    if (d_->d_staged) cudaFree(d_->d_staged);
-    for (int b = 0; b < 2; ++b)
-        for (int k = 0; k < 4; ++k)
-            if (d_->evp[b][k]) cudaEventDestroy(d_->evp[b][k]);
-    if (d_->ev[0]) cudaEventDestroy(d_->ev[0]);
-    if (d_->ev[1]) cudaEventDestroy(d_->ev[1]);
-    if (d_->stream && d_->own_stream) cudaStreamDestroy(d_->stream);
+    for (cudaStream_t s : {d_->stream.get(), d_->up_stream.get()})
+        if (s) cudaStreamSynchronize(s);
+    for (const Stream& s : d_->gstream)
+        if (s) cudaStreamSynchronize(s);
     delete d_;
 }
 
@@ -488,7 +459,7 @@ int Engine::set_scan(const double* pts, int n, const double origin[3], const dou
     if (!pts || n < 1 || n > cfg_.max_beams) return fail("set_scan: number of beams out of range", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
     set_moving(origin, quat, truncated_ray, truncated_range, n);
-    d_->d_points = d_->d_scan_buf;
+    d_->d_points = d_->d_scan_buf.get();
     d_->scan_flat = points_flat(pts, (size_t)n);
     // pageable host memory: cudaMemcpyAsync stages through the driver; the copy is small (N * 24 B)
     CU_TRY(cudaMemcpyAsync(d_->d_points, pts, (size_t)n * 3 * 8, cudaMemcpyHostToDevice, d_->stream));
@@ -502,9 +473,8 @@ int Engine::stage_scans(const double* pts, int n_scans, int n)
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
     if (!pts || n_scans < 1 || n < 1 || n > cfg_.max_beams) return fail("stage_scans: bad arguments", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
-    if (d_->d_staged) { cudaFree(d_->d_staged); d_->d_staged = nullptr; }
-    CU_TRY(cudaMalloc((void**)&d_->d_staged, (size_t)n_scans * n * 24));
-    CU_TRY(cudaMemcpyAsync(d_->d_staged, pts, (size_t)n_scans * n * 24, cudaMemcpyHostToDevice, d_->stream));
+    CU_TRY(d_->d_staged.alloc((size_t)n_scans * n * 3));
+    CU_TRY(cudaMemcpyAsync(d_->d_staged.get(), pts, (size_t)n_scans * n * 24, cudaMemcpyHostToDevice, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     d_->staged_scans = n_scans;
     d_->staged_beams = n;
@@ -514,25 +484,22 @@ int Engine::stage_scans(const double* pts, int n_scans, int n)
 
 int Engine::select_staged(int index, const double origin[3], const double quat[4], double truncated_ray, double truncated_range)
 {
-    if (!d_->d_staged || index < 0 || index >= d_->staged_scans) return fail("select_staged: no such staged scan", LAMA_ERR_ARG);
+    if (!d_->d_staged.get() || index < 0 || index >= d_->staged_scans) return fail("select_staged: no such staged scan", LAMA_ERR_ARG);
     set_moving(origin, quat, truncated_ray, truncated_range, d_->staged_beams);
-    d_->d_points = d_->d_staged + (size_t)index * d_->staged_beams * 3;
+    d_->d_points = d_->d_staged.get() + (size_t)index * d_->staged_beams * 3;
     d_->scan_flat = d_->staged_flat;
     return LAMA_OK;
 }
 
 int Engine::ensure_states(int count)
 {
-    if (count <= d_->state_cap) return LAMA_OK;
-    if (d_->d_states) { cudaFree(d_->d_states); cudaFree(d_->d_results); cudaFreeHost(d_->h_states); cudaFreeHost(d_->h_results); }
-    d_->d_states = nullptr; d_->d_results = nullptr; d_->h_states = nullptr; d_->h_results = nullptr;
-    d_->state_cap = 0;
-    const int cap = std::max(count, cfg_.particles);
-    CU_TRY(cudaMalloc((void**)&d_->d_states, (size_t)cap * sizeof(SE2)));
-    CU_TRY(cudaMalloc((void**)&d_->d_results, (size_t)cap * sizeof(MatchResult)));
-    CU_TRY(cudaMallocHost((void**)&d_->h_states, (size_t)cap * sizeof(SE2)));
-    CU_TRY(cudaMallocHost((void**)&d_->h_results, (size_t)cap * sizeof(MatchResult)));
-    d_->state_cap = cap;
+    if ((size_t)count <= d_->h_results.size()) return LAMA_OK;   // allocated last: the other three hold as many
+    d_->d_states.reset(); d_->d_results.reset(); d_->h_states.reset(); d_->h_results.reset();
+    const size_t cap = (size_t)std::max(count, cfg_.particles);
+    CU_TRY(d_->d_states.alloc(cap));
+    CU_TRY(d_->d_results.alloc(cap));
+    CU_TRY(d_->h_states.alloc(cap));
+    CU_TRY(d_->h_results.alloc(cap));
     return LAMA_OK;
 }
 
@@ -540,8 +507,8 @@ int Engine::ensure_states(int count)
 int Engine::upload_states(const SE2* states, int count, void* stream)
 {
     { int rc = ensure_states(count); if (rc != LAMA_OK) return rc; }
-    std::memcpy(d_->h_states, states, (size_t)count * sizeof(SE2));
-    CU_TRY(cudaMemcpyAsync(d_->d_states, d_->h_states, (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    std::memcpy(d_->h_states.get(), states, (size_t)count * sizeof(SE2));
+    CU_TRY(cudaMemcpyAsync(d_->d_states.get(), d_->h_states.get(), (size_t)count * sizeof(SE2), cudaMemcpyHostToDevice, (cudaStream_t)stream));
     h2d_bytes_ += (uint64_t)count * sizeof(SE2);
     return LAMA_OK;
 }
@@ -550,10 +517,10 @@ int Engine::upload_states(const SE2* states, int count, void* stream)
 // previous step returned after its match, which follows its upload.
 int Engine::upload_scan(const double* pts, int n, double* dst, void* stream)
 {
-    std::memcpy(d_->h_scan, pts, (size_t)n * 24);
+    std::memcpy(d_->h_scan.get(), pts, (size_t)n * 24);
     d_->d_points = dst;
     d_->scan_flat = points_flat(pts, (size_t)n);
-    CU_TRY(cudaMemcpyAsync(dst, d_->h_scan, (size_t)n * 24, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    CU_TRY(cudaMemcpyAsync(dst, d_->h_scan.get(), (size_t)n * 24, cudaMemcpyHostToDevice, (cudaStream_t)stream));
     h2d_bytes_ += (uint64_t)n * 24;
     return LAMA_OK;
 }
@@ -609,7 +576,7 @@ BrushParams Engine::map_update_params(int state_stride, int particle_offset, Ray
 
 int Engine::check_device_status()
 {
-    uint32_t st = *d_->h_status;
+    uint32_t st = *d_->h_status.get();
     if (!st) return LAMA_OK;
     if (st & kErrWindow) return fail("map grew outside the directory window (raise dir_dim)", LAMA_ERR_WINDOW);
     if (st & kErrPoolEmpty) return fail("patch pool exhausted (raise pool_slots)", LAMA_ERR_POOL);
@@ -628,9 +595,9 @@ uint32_t Engine::device_status()
 {
     settle(nullptr);
     cudaSetDevice(cfg_.device);
-    cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream);
+    cudaMemcpyAsync(d_->h_status.get(), d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream);
     cudaStreamSynchronize(d_->stream);
-    return *d_->h_status;
+    return *d_->h_status.get();
 }
 
 void Engine::store_counters(uint64_t out[4])
@@ -662,12 +629,12 @@ int Engine::match_sync(const SE2* states, int count, const MatchParams& mp, bool
 {
     { int rc = upload_states(states, count, d_->stream); if (rc != LAMA_OK) return rc; }
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
-    if (extent) launch_match_extent(d_->view, mp, (const int32_t*)d_->d_extent, extent_, d_->d_states, d_->d_results, count, d_->stream);
-    else launch_match(d_->view, mp, d_->d_states, d_->d_results, count, d_->stream);
+    if (extent) launch_match_extent(d_->view, mp, (const int32_t*)d_->d_extent.get(), extent_, d_->d_states.get(), d_->d_results.get(), count, d_->stream);
+    else launch_match(d_->view, mp, d_->d_states.get(), d_->d_results.get(), count, d_->stream);
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(d_->h_results, d_->d_results, (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
-    if (mp.parked_any) CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(d_->h_results.get(), d_->d_results.get(), (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
+    if (mp.parked_any) CU_TRY(cudaMemcpyAsync(d_->h_status.get(), d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     if (timing_) {
         float ms = 0;
@@ -675,9 +642,9 @@ int Engine::match_sync(const SE2* states, int count, const MatchParams& mp, bool
         times_.match_ms += ms;
     }
     times_.match_launches += 1;
-    if (mp.parked_any && *d_->h_status) return check_device_status();
+    if (mp.parked_any && *d_->h_status.get()) return check_device_status();
     static_assert(sizeof(HostMatchResult) == sizeof(MatchResult), "layout");
-    std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
+    std::memcpy(out, d_->h_results.get(), (size_t)count * sizeof(MatchResult));
     d2h_bytes_ += (uint64_t)count * sizeof(MatchResult);
     return LAMA_OK;
 }
@@ -690,8 +657,8 @@ int Engine::match_error(const SE2* states, int count, int first_particle, bool s
     if (d_->scan.n_beams < 1) return fail("match_error: no scan uploaded", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
     { int rc = upload_states(states, count, d_->stream); if (rc != LAMA_OK) return rc; }
-    double* d_out = reinterpret_cast<double*>(d_->d_results);   // count doubles fit in count MatchResults
-    launch_match_error(d_->view, d_->pv(cur_set_), cur_set_, first_particle, shared_map, d_->d_points, d_->scan, d_->d_states, count, cfg_.resolution, max_sqdist_, d_out, d_->stream);
+    double* d_out = reinterpret_cast<double*>(d_->d_results.get());   // count doubles fit in count MatchResults
+    launch_match_error(d_->view, d_->pv(cur_set_), cur_set_, first_particle, shared_map, d_->d_points, d_->scan, d_->d_states.get(), count, cfg_.resolution, max_sqdist_, d_out, d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(out, d_out, (size_t)count * 8, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
@@ -736,32 +703,32 @@ int Engine::enqueue_group(const MatchParams* mp, RayParams rp, BrushParams bp, i
     Impl* d = d_;
     cudaStream_t st = (cudaStream_t)stream;
     const int half = 1 - pending_buf_;
-    cudaEvent_t* ev = timing_ ? d->evp[half] : nullptr;
+    const Event* ev = timing_ ? d->evp[half] : nullptr;
     StoreView v = d->view;
     v.counters = counters;
-    const SE2* poses = d->d_states + lo;
+    const SE2* poses = d->d_states.get() + lo;
     if (mp) {
         MatchParams m = *mp;
         m.particle_offset += lo;
         if (ev) CU_TRY(cudaEventRecord(ev[0], st));
-        launch_match(v, m, d->d_states + lo, d->d_results + lo, cnt, st);
+        launch_match(v, m, d->d_states.get() + lo, d->d_results.get() + lo, cnt, st);
         if (ev) CU_TRY(cudaEventRecord(ev[1], st));
-        CU_TRY(cudaMemcpyAsync(d->h_results + lo, d->d_results + lo, (size_t)cnt * sizeof(MatchResult), cudaMemcpyDeviceToHost, st));
+        CU_TRY(cudaMemcpyAsync(d->h_results.get() + lo, d->d_results.get() + lo, (size_t)cnt * sizeof(MatchResult), cudaMemcpyDeviceToHost, st));
         CU_TRY(cudaEventRecord((cudaEvent_t)ev_match, st));
-        poses = reinterpret_cast<const SE2*>(d->d_results + lo);
+        poses = reinterpret_cast<const SE2*>(d->d_results.get() + lo);
         times_.match_launches += 1;
         d2h_bytes_ += (uint64_t)cnt * sizeof(MatchResult);
     } else if (ev) {
         CU_TRY(cudaEventRecord(ev[1], st));
     }
-    uint64_t* events = d->d_events + (size_t)lo * d->ray.event_cap;
+    uint64_t* events = d->d_events.get() + (size_t)lo * d->ray.event_cap;
     rp.particle_offset += lo;
-    const int ray_kernels = d->launch_ray_stage(v, rp, poses, events, d->d_stats + lo, cnt, st);
+    const int ray_kernels = d->launch_ray_stage(v, rp, poses, events, d->d_stats.get() + lo, cnt, st);
     if (ev) CU_TRY(cudaEventRecord(ev[2], st));
     bp.particle_offset += lo;
     bp.lower_spill += (size_t)lo * (d->brush.lower_total + 2);
     bp.raise_spill += (size_t)lo * (d->brush.raise_total + 2);
-    launch_brushfire(v, bp, events, d->d_stats + lo, cnt, st);
+    launch_brushfire(v, bp, events, d->d_stats.get() + lo, cnt, st);
     if (ev) {
         CU_TRY(cudaEventRecord(ev[3], st));
         d->evp_used[half]  = true;
@@ -771,8 +738,8 @@ int Engine::enqueue_group(const MatchParams* mp, RayParams rp, BrushParams bp, i
     const bool one_stream = counters == d->view.counters;
     if (one_stream) launch_merge_free(d->view, st);
     CU_TRY(cudaGetLastError());
-    uint64_t* r = d->h_grep + ((size_t)half * (kMaxGroups + 1) + g) * 8;
-    CU_TRY(cudaMemcpyAsync(d->h_stats + (size_t)half * cfg_.particles + lo, d->d_stats + lo, (size_t)cnt * sizeof(MapUpdateStats), cudaMemcpyDeviceToHost, st));
+    uint64_t* r = d->h_grep.get() + ((size_t)half * (kMaxGroups + 1) + g) * 8;
+    CU_TRY(cudaMemcpyAsync(d->h_stats.get() + (size_t)half * cfg_.particles + lo, d->d_stats.get() + lo, (size_t)cnt * sizeof(MapUpdateStats), cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaMemcpyAsync(r, d->view.status, 4, cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaMemcpyAsync(r + 1, counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     CU_TRY(cudaMemcpyAsync(r + 4, d->view.free_count, 4, cudaMemcpyDeviceToHost, st));
@@ -804,7 +771,7 @@ int Engine::step_enqueue(const double* pts, int n, const double origin[3], const
     enq_prev_buf_    = pending_buf_;
     if (pts) {
         set_moving(origin, quat, truncated_ray, truncated_range, n);
-        int rc = upload_scan(pts, n, d_->d_scan_buf, d_->stream);
+        int rc = upload_scan(pts, n, d_->d_scan_buf.get(), d_->stream);
         if (rc != LAMA_OK) return rc;
     }
     { int rc = upload_states(predicted, count, d_->stream); if (rc != LAMA_OK) return rc; }
@@ -844,7 +811,7 @@ int Engine::step_async(const double* pts, int n, const double origin[3], const d
     { int rc = step_enqueue(pts, n, origin, quat, truncated_ray, truncated_range, predicted, count, so, meas_sigma); if (rc != LAMA_OK) return rc; }
     CU_TRY(cudaEventSynchronize(d_->ev_match));
     static_assert(sizeof(HostMatchResult) == sizeof(MatchResult), "layout");
-    std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
+    std::memcpy(out, d_->h_results.get(), (size_t)count * sizeof(MatchResult));
     return collect_previous();
 }
 
@@ -884,7 +851,7 @@ int Engine::step_groups(const double* pts, int n, const double origin[3], const 
     if (pts) {
         set_moving(origin, quat, truncated_ray, truncated_range, n);
         d->scan_half ^= 1;
-        int rc = upload_scan(pts, n, d->d_scan_buf + (size_t)d->scan_half * cfg_.max_beams * 3, d->up_stream);
+        int rc = upload_scan(pts, n, d->d_scan_buf.get() + (size_t)d->scan_half * cfg_.max_beams * 3, d->up_stream);
         if (rc != LAMA_OK) return rc;
     }
     { int rc = upload_states(predicted, count, d->up_stream); if (rc != LAMA_OK) return rc; }
@@ -897,9 +864,9 @@ int Engine::step_groups(const double* pts, int n, const double origin[3], const 
         const int lo = (int)((int64_t)g * count / G), cnt = (int)((int64_t)(g + 1) * count / G) - lo;
         cudaStream_t st = d->gstream[g];
         CU_TRY(cudaStreamWaitEvent(st, d->ev_up, 0));
-        { int rc = enqueue_group(&mp, rp, bp, lo, cnt, st, d->d_gcnt + (size_t)g * 4, g, d->ev_gmatch[g]); if (rc != LAMA_OK) return rc; }
+        { int rc = enqueue_group(&mp, rp, bp, lo, cnt, st, d->d_gcnt.get() + (size_t)g * 4, g, d->ev_gmatch[g]); if (rc != LAMA_OK) return rc; }
         if (g == 0) {   // view.counters, which no kernel of a grouped step writes, into slot G of the report
-            CU_TRY(cudaMemcpyAsync(d->h_grep + ((size_t)half * (kMaxGroups + 1) + G) * 8 + 1, d->view.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+            CU_TRY(cudaMemcpyAsync(d->h_grep.get() + ((size_t)half * (kMaxGroups + 1) + G) * 8 + 1, d->view.counters, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
             d2h_bytes_ += 24;
         }
         CU_TRY(cudaEventRecord(d->ev_gdone[g], st));
@@ -911,7 +878,7 @@ int Engine::step_groups(const double* pts, int n, const double origin[3], const 
     pending_maps_ = count;
     for (int g = 0; g < G; ++g) CU_TRY(cudaEventSynchronize(d->ev_gmatch[g]));
     static_assert(sizeof(HostMatchResult) == sizeof(MatchResult), "layout");
-    std::memcpy(out, d->h_results, (size_t)count * sizeof(MatchResult));
+    std::memcpy(out, d->h_results.get(), (size_t)count * sizeof(MatchResult));
     return collect_previous();
 }
 
@@ -922,13 +889,13 @@ int Engine::fold_groups()
     Impl* d = d_;
     d->groups_ran = false;
     uint64_t g[kMaxGroups * 4], m[3];
-    CU_TRY(cudaMemcpyAsync(g, d->d_gcnt, sizeof(g), cudaMemcpyDeviceToHost, d->stream));
+    CU_TRY(cudaMemcpyAsync(g, d->d_gcnt.get(), sizeof(g), cudaMemcpyDeviceToHost, d->stream));
     CU_TRY(cudaMemcpyAsync(m, d->view.counters, sizeof(m), cudaMemcpyDeviceToHost, d->stream));
     CU_TRY(cudaStreamSynchronize(d->stream));
     for (int k = 0; k < kMaxGroups; ++k)
         for (int c = 0; c < 3; ++c) m[c] += g[k * 4 + c];
     CU_TRY(cudaMemcpyAsync(d->view.counters, m, sizeof(m), cudaMemcpyHostToDevice, d->stream));
-    CU_TRY(cudaMemsetAsync(d->d_gcnt, 0, sizeof(g), d->stream));
+    CU_TRY(cudaMemsetAsync(d->d_gcnt.get(), 0, sizeof(g), d->stream));
     launch_merge_free(d->view, d->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaStreamSynchronize(d->stream));   // `m` is on this stack
@@ -951,7 +918,7 @@ int Engine::pack_results(int count, double digest, double* d_out, void* stream)
     CU_TRY(cudaSetDevice(cfg_.device));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     CU_TRY(cudaStreamWaitEvent(st, d_->ev_match, 0));
-    launch_pack_results(d_->d_results, count, digest, d_out, st);
+    launch_pack_results(d_->d_results.get(), count, digest, d_out, st);
     CU_TRY(cudaGetLastError());
     return LAMA_OK;
 }
@@ -971,7 +938,7 @@ int Engine::settle(HostMapStats* out, bool already_complete)
     CU_TRY(cudaSetDevice(cfg_.device));
     if (!already_complete) CU_TRY(cudaStreamSynchronize(d_->stream));
     if (timing_ && d_->evp_used[half]) {   // the update's events have completed (the stream is past them, or was just synchronised)
-        const cudaEvent_t* e = d_->evp[half];
+        const Event* e = d_->evp[half];
         float m = 0, a = 0, b = 0;
         if (d_->evp_match[half]) cudaEventElapsedTime(&m, e[0], e[1]);
         cudaEventElapsedTime(&a, e[1], e[2]);
@@ -982,12 +949,12 @@ int Engine::settle(HostMapStats* out, bool already_complete)
         d_->evp_used[half] = false;
     }
     static_assert(sizeof(HostMapStats) == sizeof(MapUpdateStats), "layout");
-    const MapUpdateStats* hs = d_->h_stats + (size_t)half * cfg_.particles;
+    const MapUpdateStats* hs = d_->h_stats.get() + (size_t)half * cfg_.particles;
     last_map_stats_.assign((const HostMapStats*)hs, (const HostMapStats*)hs + count);
     if (out) std::memcpy(out, hs, (size_t)count * sizeof(MapUpdateStats));
     // view.counters plus every group's block; one group is a map update on one stream, whose block is view.counters itself
     const int G = d_->report_groups[half];
-    const uint64_t* hr = d_->h_grep + (size_t)half * (kMaxGroups + 1) * 8;
+    const uint64_t* hr = d_->h_grep.get() + (size_t)half * (kMaxGroups + 1) * 8;
     uint32_t status = 0;
     for (int c = 0; c < 3; ++c) settled_counters_[c] = G > 1 ? hr[(size_t)G * 8 + 1 + c] : 0;
     for (int g = 0; g < G; ++g) {
@@ -995,7 +962,7 @@ int Engine::settle(HostMapStats* out, bool already_complete)
         for (int c = 0; c < 3; ++c) settled_counters_[c] += hr[g * 8 + 1 + c];
     }
     settled_counters_[3] = (uint64_t)(uint32_t)hr[(G - 1) * 8 + 4];
-    *d_->h_status = status;
+    *d_->h_status.get() = status;
     if (G > 1) {
         const uint64_t alloc = settled_counters_[0] + settled_counters_[1];
         d_->scan_alloc = d_->prev_alloc && alloc > d_->prev_alloc ? alloc - d_->prev_alloc : 0;
@@ -1018,10 +985,10 @@ int Engine::share_from(int src_particle, int dst_first, int count)
         return fail("share_from: bad particle range", LAMA_ERR_ARG);
     if (has_parked()) return fail("share_from: the maps have parked entries (the window has moved); share_from builds a filter's first maps", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
-    for (int i = 0; i < count; ++i) d_->h_idx[i] = src_particle;
-    CU_TRY(cudaMemcpyAsync(d_->d_idx, d_->h_idx, (size_t)count * 4, cudaMemcpyHostToDevice, d_->stream));
+    for (int i = 0; i < count; ++i) d_->h_idx.get()[i] = src_particle;
+    CU_TRY(cudaMemcpyAsync(d_->d_idx.get(), d_->h_idx.get(), (size_t)count * 4, cudaMemcpyHostToDevice, d_->stream));
     launch_release(d_->view, cur_set_, dst_first, count, d_->stream);
-    launch_copy_dirs(d_->view, cur_set_, cur_set_, d_->d_idx, dst_first, count, d_->stream);
+    launch_copy_dirs(d_->view, cur_set_, cur_set_, d_->d_idx.get(), dst_first, count, d_->stream);
     launch_merge_free(d_->view, d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaStreamSynchronize(d_->stream));
@@ -1037,9 +1004,9 @@ int Engine::resample(const int32_t* idx)
     const int P = cfg_.particles;
     for (int i = 0; i < P; ++i) {
         if (idx[i] < -1 || idx[i] >= P) return fail("resample: index out of range", LAMA_ERR_ARG);
-        d_->h_idx[i] = idx[i];
+        d_->h_idx.get()[i] = idx[i];
     }
-    CU_TRY(cudaMemcpyAsync(d_->d_idx, d_->h_idx, (size_t)P * 4, cudaMemcpyHostToDevice, d_->stream));
+    CU_TRY(cudaMemcpyAsync(d_->d_idx.get(), d_->h_idx.get(), (size_t)P * 4, cudaMemcpyHostToDevice, d_->stream));
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
     const int other = 1 - cur_set_;
     // the offspring's parked lists: copies of their ancestors' (kinds 0 and 1, like the directories), in a new arena of the other set
@@ -1054,12 +1021,13 @@ int Engine::resample(const int32_t* idx)
                 ol[(size_t)p * nk + k] = make_int2(off, len);
                 off += len;
             }
-        if (off) CU_TRY(cudaMalloc((void**)&d_->park[other], (size_t)off * sizeof(ParkEntry)));
-        CU_TRY(cudaMemcpyAsync(d_->d_park_ol[other], ol.data(), ol.size() * sizeof(int2), cudaMemcpyHostToDevice, d_->stream));
+        if (off) CU_TRY(d_->park[other].alloc((size_t)off));
+        CU_TRY(cudaMemcpyAsync(d_->d_park_ol[other].get(), ol.data(), ol.size() * sizeof(int2), cudaMemcpyHostToDevice, d_->stream));
     }
-    launch_copy_dirs(d_->view, cur_set_, other, d_->d_idx, 0, P, d_->stream);  // share first ...
+    launch_copy_dirs(d_->view, cur_set_, other, d_->d_idx.get(), 0, P, d_->stream);  // share first ...
     if (parked && d_->park[other])
-        launch_copy_parked(d_->view, d_->park[cur_set_], d_->d_park_ol[cur_set_], d_->park[other], d_->d_park_ol[other], d_->d_idx, P, d_->stream);
+        launch_copy_parked(d_->view, d_->park[cur_set_].get(), d_->d_park_ol[cur_set_].get(), d_->park[other].get(), d_->d_park_ol[other].get(), d_->d_idx.get(), P,
+                           d_->stream);
     launch_release(d_->view, cur_set_, 0, P, d_->stream);                       // ... then drop the old set
     launch_release_parked(d_->view, d_->pv(cur_set_), 0, P, d_->stream);
     launch_merge_free(d_->view, d_->stream);
@@ -1079,18 +1047,6 @@ int Engine::resample(const int32_t* idx)
     cur_set_ = other;
     return LAMA_OK;
 }
-
-static int ensure_buffer(void** buf, size_t* cap, size_t bytes)
-{
-    if (bytes <= *cap) return 0;
-    if (*buf) cudaFree(*buf);
-    *buf = nullptr;
-    *cap = 0;
-    if (cudaMalloc(buf, bytes) != cudaSuccess) return -1;
-    *cap = bytes;
-    return 0;
-}
-static int ensure_scratch(Engine::Impl* d, size_t bytes) { return ensure_buffer(&d->d_scratch, &d->scratch_bytes, bytes); }
 
 bool Engine::has_parked(int particle) const
 {
@@ -1118,8 +1074,8 @@ int Engine::shift_window(int32_t base_px, int32_t base_py)
     // scratch: counts | new {offset, length} | enter prefixes (window_shift_core.h: the arena may have gaps after a prune)
     const size_t b_cnt = (size_t)n_lists * sizeof(int2);
     const size_t b_enter = shift_scratch_ints(reinterpret_cast<const int32_t*>(d_->park_ol[set].data()), n_lists) * 4;
-    if (ensure_buffer(&d_->d_shift_scratch, &d_->shift_scratch_bytes, 2 * b_cnt + b_enter)) return fail("shift_window: out of device memory", LAMA_ERR_CUDA);
-    int2* d_cnt = (int2*)d_->d_shift_scratch;
+    if (d_->d_shift_scratch.reserve(2 * b_cnt + b_enter) != cudaSuccess) return fail("shift_window: out of device memory", LAMA_ERR_CUDA);
+    int2* d_cnt = (int2*)d_->d_shift_scratch.get();
     int2* d_new_ol = d_cnt + n_lists;
     int32_t* d_enter = (int32_t*)(d_new_ol + n_lists);
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
@@ -1135,25 +1091,20 @@ int Engine::shift_window(int32_t base_px, int32_t base_py)
         entered += cnt[i].y;
     }
     if (total > INT32_MAX) return fail("shift_window: too many parked entries", LAMA_ERR_POOL);
-    ParkEntry* arena = nullptr;
-    if (total) CU_TRY(cudaMalloc((void**)&arena, (size_t)total * sizeof(ParkEntry)));
-    auto give_up = [&](cudaError_t e) {
-        if (arena) cudaFree(arena);
-        return fail(std::string("shift_window: ") + cudaGetErrorString(e), LAMA_ERR_CUDA);
-    };
+    DeviceArray<ParkEntry> arena;
+    if (total) CU_TRY(arena.alloc((size_t)total));
     cudaError_t e = cudaMemcpyAsync(d_new_ol, nol.data(), b_cnt, cudaMemcpyHostToDevice, d_->stream);
-    if (e == cudaSuccess) e = launch_shift_apply(d_->view, d_->pv(set), set, nw, arena, d_new_ol, d_enter, n_lists, d_->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_->d_park_ol[set], d_new_ol, b_cnt, cudaMemcpyDeviceToDevice, d_->stream);
+    if (e == cudaSuccess) e = launch_shift_apply(d_->view, d_->pv(set), set, nw, arena.get(), d_new_ol, d_enter, n_lists, d_->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_->d_park_ol[set].get(), d_new_ol, b_cnt, cudaMemcpyDeviceToDevice, d_->stream);
     if (timing_ && e == cudaSuccess) e = cudaEventRecord(d_->ev[1], d_->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(d_->stream);
-    if (e != cudaSuccess) return give_up(e);
+    if (e != cudaSuccess) return fail(std::string("shift_window: ") + cudaGetErrorString(e), LAMA_ERR_CUDA);
     if (timing_) {
         float ms = 0;
         cudaEventElapsedTime(&ms, d_->ev[0], d_->ev[1]);
         times_.shift_ms += ms;
     }
-    if (d_->park[set]) cudaFree(d_->park[set]);
-    d_->park[set] = arena;
+    d_->park[set] = std::move(arena);
     d_->park_ol[set] = nol;
     window_ = nw;
     d_->view.window = nw;
@@ -1200,8 +1151,8 @@ int Engine::render_scans(const double* pts, const int64_t* offsets, int n_scans,
     const size_t dim2 = (size_t)cfg_.dir_dim * cfg_.dir_dim;
     const size_t b_pts = up((size_t)n_pts * 24), b_off = up((size_t)(n_scans + 1) * 8), b_mov = up((size_t)n_scans * sizeof(MovingTf)),
                  b_st = up((size_t)n_scans * sizeof(SE2)), b_marks = up(dim2);
-    if (ensure_scratch(d_, b_pts + b_off + b_mov + b_st + b_marks + 16)) return fail("render_scans: out of device memory", LAMA_ERR_CUDA);
-    char* base = (char*)d_->d_scratch;
+    if (d_->d_scratch.reserve(b_pts + b_off + b_mov + b_st + b_marks + 16) != cudaSuccess) return fail("render_scans: out of device memory", LAMA_ERR_CUDA);
+    char* base = (char*)d_->d_scratch.get();
     RenderParams p;
     p.points  = (const double*)base;
     p.offsets = (const int64_t*)(base + b_pts);
@@ -1256,7 +1207,7 @@ int Engine::render_scans(const double* pts, const int64_t* offsets, int n_scans,
     }
     unsigned long long n_cells = 0;
     CU_TRY(cudaMemcpyAsync(&n_cells, p.cells, 8, cudaMemcpyDeviceToHost, d_->stream));
-    CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(d_->h_status.get(), d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     if (timed) {
         float g_ms = 0.f;
@@ -1293,24 +1244,25 @@ int Engine::grow_pool(int new_slots)
     CU_TRY(cudaStreamSynchronize(d_->stream));
     const size_t n_old = (size_t)v.n_slots, n_new = (size_t)new_slots, n_add = n_new - n_old;
     // everything is allocated before anything is changed
-    StoreView nv = v;
-    void* pool_raw = nullptr;
-    std::vector<void*> fresh;
-    auto grab = [&](void** ptr, size_t bytes) -> bool {
-        if (cudaMalloc(ptr, bytes) != cudaSuccess) return false;
-        fresh.push_back(*ptr);
-        return true;
-    };
-    bool ok = grab(&pool_raw, (n_new + 1) * kPatchBytes) && grab((void**)&nv.fbits, n_new * 128) && (!v.kbits || grab((void**)&nv.kbits, n_new * 128)) &&
-              grab((void**)&nv.refcount, n_new * 4) && grab((void**)&nv.free_slots, n_new * 4) && grab((void**)&nv.freed, n_new * 4);
-    auto give_up = [&](const std::string& why) {
+    DeviceArray<char> pool_raw;
+    DeviceArray<uint32_t> fbits, kbits;
+    DeviceArray<int32_t> refcount, free_slots, freed;
+    const bool ok = pool_raw.alloc((n_new + 1) * kPatchBytes) == cudaSuccess && fbits.alloc(n_new * 32) == cudaSuccess &&
+                    (!v.kbits || kbits.alloc(n_new * 32) == cudaSuccess) && refcount.alloc(n_new) == cudaSuccess &&
+                    free_slots.alloc(n_new) == cudaSuccess && freed.alloc(n_new) == cudaSuccess;
+    auto give_up = [&](const std::string& why) {   // the new arrays are released on return, once the stream has passed them
         cudaStreamSynchronize(d_->stream);
-        for (void* q : fresh) cudaFree(q);
         cudaGetLastError();   // a failed cudaMalloc is not sticky; clear it for the next call
         return fail("grow_pool: " + why + " (the pool keeps its " + std::to_string(n_old) + " slots)", LAMA_ERR_CUDA);
     };
     if (!ok) return give_up("out of device memory for " + std::to_string(n_new) + " slots");
-    nv.pool = reinterpret_cast<uint32_t*>(((uintptr_t)pool_raw + (kPatchBytes - 1)) & ~(uintptr_t)(kPatchBytes - 1));
+    StoreView nv = v;
+    nv.pool = reinterpret_cast<uint32_t*>(((uintptr_t)pool_raw.get() + (kPatchBytes - 1)) & ~(uintptr_t)(kPatchBytes - 1));
+    nv.fbits = fbits.get();
+    nv.kbits = kbits.get();
+    nv.refcount = refcount.get();
+    nv.free_slots = free_slots.get();
+    nv.freed = freed.get();
     nv.n_slots = new_slots;
     // slots keep their ids; the free stack gets the new slots below the old free entries, the lowest new slot deepest of them, so the
     // old free slots are handed out first, then n_old, n_old + 1, ...
@@ -1327,15 +1279,12 @@ int Engine::grow_pool(int new_slots)
     if (e == cudaSuccess) e = cudaMemcpyAsync(v.free_count, counts, 4, cudaMemcpyHostToDevice, d_->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(d_->stream);
     if (e != cudaSuccess) return give_up(cudaGetErrorString(e));   // the old arrays are untouched; only the free count is written in place, last
-    const void* old[] = {d_->pool_raw, v.fbits, v.kbits, v.refcount, v.free_slots, v.freed};
-    for (const void* q : old) {
-        if (!q) continue;
-        auto it = std::find(d_->allocs.begin(), d_->allocs.end(), q);
-        if (it != d_->allocs.end()) d_->allocs.erase(it);
-        cudaFree(const_cast<void*>(q));
-    }
-    d_->allocs.insert(d_->allocs.end(), fresh.begin(), fresh.end());
-    d_->pool_raw = pool_raw;
+    d_->pool_raw = std::move(pool_raw);
+    d_->fbits = std::move(fbits);
+    d_->kbits = std::move(kbits);
+    d_->refcount = std::move(refcount);
+    d_->free_slots = std::move(free_slots);
+    d_->freed = std::move(freed);
     v = nv;
     cfg_.pool_slots = new_slots;
     pool_growths_ += 1;
@@ -1353,7 +1302,7 @@ int Engine::prune_frequency()
     const int n_parked = d_->park_ol[cur_set_][kMapOcc].y;   // particle 0's occupancy list
     if (n_parked) launch_prune_freq_parked(d_->view, d_->pv(cur_set_), n_parked, d_->stream);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(d_->h_status.get(), d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     times_.misc_launches += n_parked ? 2 : 1;
     return check_device_status();
@@ -1411,20 +1360,20 @@ int Engine::dm_apply(int particle, const uint32_t* cells_xy, const uint8_t* is_a
         }
         MapUpdateStats st{};
         st.events = (uint32_t)m;
-        uint64_t* dev_ev = d_->d_events + (size_t)particle * cap;
+        uint64_t* dev_ev = d_->d_events.get() + (size_t)particle * cap;
         CU_TRY(cudaMemcpyAsync(dev_ev, ev.data(), (size_t)m * 8, cudaMemcpyHostToDevice, d_->stream));
-        CU_TRY(cudaMemcpyAsync(d_->d_stats + particle, &st, sizeof(st), cudaMemcpyHostToDevice, d_->stream));
+        CU_TRY(cudaMemcpyAsync(d_->d_stats.get() + particle, &st, sizeof(st), cudaMemcpyHostToDevice, d_->stream));
         const BrushParams bp = map_update_params(0, particle, nullptr);
         // block 0 of this launch must read the event list / stats of `particle`
-        launch_brushfire(d_->view, bp, dev_ev, d_->d_stats + particle, 1, d_->stream);
+        launch_brushfire(d_->view, bp, dev_ev, d_->d_stats.get() + particle, 1, d_->stream);
         launch_merge_free(d_->view, d_->stream);
         CU_TRY(cudaGetLastError());
-        CU_TRY(cudaMemcpyAsync(d_->h_stats, d_->d_stats + particle, sizeof(MapUpdateStats), cudaMemcpyDeviceToHost, d_->stream));
-        CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
+        CU_TRY(cudaMemcpyAsync(d_->h_stats.get(), d_->d_stats.get() + particle, sizeof(MapUpdateStats), cudaMemcpyDeviceToHost, d_->stream));
+        CU_TRY(cudaMemcpyAsync(d_->h_status.get(), d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
         CU_TRY(cudaStreamSynchronize(d_->stream));
         times_.brushfire_launches += 1;
         times_.misc_launches += 1;
-        total += d_->h_stats[0].dm_pops;
+        total += d_->h_stats.get()[0].dm_pops;
         done += m;
         int rc = check_device_status();
         if (rc != LAMA_OK) return rc;
@@ -1445,9 +1394,9 @@ int Engine::ensure_extent()
         return fail("match_extent: the map spans more than " + std::to_string(kExtentMaxPatches) + " patches on an axis", LAMA_ERR_WINDOW);
     if (xw.dim) {
         const size_t bytes = (size_t)xw.dim * xw.dim * 4;
-        if (ensure_buffer(&d_->d_extent, &d_->extent_bytes, bytes)) return fail("match_extent: out of device memory", LAMA_ERR_CUDA);
-        CU_TRY(cudaMemsetAsync(d_->d_extent, 0xFF, bytes, d_->stream));
-        launch_extent_dir(d_->view, d_->pv(cur_set_), cur_set_, xw, d_->park_ol[cur_set_][kMapDm].y, (int32_t*)d_->d_extent, d_->stream);
+        if (d_->d_extent.reserve(bytes) != cudaSuccess) return fail("match_extent: out of device memory", LAMA_ERR_CUDA);
+        CU_TRY(cudaMemsetAsync(d_->d_extent.get(), 0xFF, bytes, d_->stream));
+        launch_extent_dir(d_->view, d_->pv(cur_set_), cur_set_, xw, d_->park_ol[cur_set_][kMapDm].y, (int32_t*)d_->d_extent.get(), d_->stream);
         CU_TRY(cudaGetLastError());
         times_.misc_launches += 1;
     }
@@ -1474,14 +1423,14 @@ int Engine::fleet_reserve(int robots, const double* offsets_xy, int n_off)
     if (robots < 1 || n_off < 1 || !offsets_xy) return fail("fleet_reserve: bad arguments", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
     const size_t bytes = (size_t)robots * (sizeof(FleetScan) + (size_t)cfg_.max_beams * 24);
+    CU_TRY(d_->d_fleet.alloc(bytes));
+    CU_TRY(d_->h_fleet.alloc(bytes));
+    CU_TRY(d_->d_fleet_off.alloc((size_t)n_off * 2));
+    CU_TRY(d_->d_fleet_lik.alloc((size_t)robots * n_off));
+    CU_TRY(d_->h_fleet_lik.alloc((size_t)robots * n_off));
+    CU_TRY(cudaMemcpy(d_->d_fleet_off.get(), offsets_xy, (size_t)n_off * 16, cudaMemcpyHostToDevice));
     d_->fleet_cap = robots;
     d_->fleet_n_off = n_off;
-    CU_TRY(cudaMalloc(&d_->d_fleet, bytes));
-    CU_TRY(cudaMallocHost(&d_->h_fleet, bytes));
-    CU_TRY(cudaMalloc((void**)&d_->d_fleet_off, (size_t)n_off * 16));
-    CU_TRY(cudaMalloc((void**)&d_->d_fleet_lik, (size_t)robots * n_off * 8));
-    CU_TRY(cudaMallocHost((void**)&d_->h_fleet_lik, (size_t)robots * n_off * 8));
-    CU_TRY(cudaMemcpy(d_->d_fleet_off, offsets_xy, (size_t)n_off * 16, cudaMemcpyHostToDevice));
     return LAMA_OK;
 }
 
@@ -1492,8 +1441,8 @@ int Engine::fleet_scans(const double* pts, const int* n_points, int count, const
     for (int k = 0; k < count; ++k)
         if (n_points[k] < 1 || n_points[k] > cfg_.max_beams) return fail("fleet_scans: number of beams out of range", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
-    FleetScan* desc = (FleetScan*)d_->h_fleet;
-    double* hp = (double*)((char*)d_->h_fleet + (size_t)d_->fleet_cap * sizeof(FleetScan));
+    FleetScan* desc = (FleetScan*)d_->h_fleet.get();
+    double* hp = (double*)(d_->h_fleet.get() + (size_t)d_->fleet_cap * sizeof(FleetScan));
     int64_t off = 0;
     int max_n = 0;
     for (int k = 0; k < count; ++k) {
@@ -1504,7 +1453,7 @@ int Engine::fleet_scans(const double* pts, const int* n_points, int count, const
     std::memcpy(hp, pts, (size_t)off * 24);
     // descriptors and points in one copy: everything from the first descriptor to the last point
     const size_t bytes = (size_t)d_->fleet_cap * sizeof(FleetScan) + (size_t)off * 24;
-    CU_TRY(cudaMemcpyAsync(d_->d_fleet, d_->h_fleet, bytes, cudaMemcpyHostToDevice, d_->stream));
+    CU_TRY(cudaMemcpyAsync(d_->d_fleet.get(), d_->h_fleet.get(), bytes, cudaMemcpyHostToDevice, d_->stream));
     h2d_bytes_ += bytes;
     d_->fleet_max_beams = max_n;
     return LAMA_OK;
@@ -1518,23 +1467,21 @@ int Engine::match_fleet(const int32_t* scan_of_block, const SE2* states, int cou
     CU_TRY(cudaSetDevice(cfg_.device));
     const bool extent = follow_ && has_parked();
     if (extent) { int rc = ensure_extent(); if (rc != LAMA_OK) return rc; }
-    if (count > d_->fleet_block_cap) {
-        if (d_->d_fleet_blocks) { cudaFree(d_->d_fleet_blocks); cudaFreeHost(d_->h_fleet_blocks); }
-        d_->d_fleet_blocks = nullptr; d_->h_fleet_blocks = nullptr; d_->fleet_block_cap = 0;
-        CU_TRY(cudaMalloc((void**)&d_->d_fleet_blocks, (size_t)count * 4));
-        CU_TRY(cudaMallocHost((void**)&d_->h_fleet_blocks, (size_t)count * 4));
-        d_->fleet_block_cap = count;
+    if ((size_t)count > d_->h_fleet_blocks.size()) {   // h_fleet_blocks is allocated last
+        d_->d_fleet_blocks.reset(); d_->h_fleet_blocks.reset();
+        CU_TRY(d_->d_fleet_blocks.alloc((size_t)count));
+        CU_TRY(d_->h_fleet_blocks.alloc((size_t)count));
     }
-    std::memcpy(d_->h_fleet_blocks, scan_of_block, (size_t)count * 4);
-    CU_TRY(cudaMemcpyAsync(d_->d_fleet_blocks, d_->h_fleet_blocks, (size_t)count * 4, cudaMemcpyHostToDevice, d_->stream));
+    std::memcpy(d_->h_fleet_blocks.get(), scan_of_block, (size_t)count * 4);
+    CU_TRY(cudaMemcpyAsync(d_->d_fleet_blocks.get(), d_->h_fleet_blocks.get(), (size_t)count * 4, cudaMemcpyHostToDevice, d_->stream));
     { int rc = upload_states(states, count, d_->stream); if (rc != LAMA_OK) return rc; }
     MatchParams mp = match_params(so, meas_sigma, 0, true, mode);
     mp.points = d_->fleet_points();
     mp.scan.scale = 1.0 / cfg_.resolution;
     if (extent) mp.parked_any = 0;   // the dense directory holds the parked patches
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[0], d_->stream));
-    launch_match_fleet(d_->view, mp, d_->fleet_scans(), d_->d_fleet_blocks, d_->fleet_max_beams, extent ? (const int32_t*)d_->d_extent : nullptr, extent_,
-                       d_->d_states, d_->d_results, count, d_->stream);
+    launch_match_fleet(d_->view, mp, d_->fleet_scans(), d_->d_fleet_blocks.get(), d_->fleet_max_beams, extent ? (const int32_t*)d_->d_extent.get() : nullptr, extent_,
+                       d_->d_states.get(), d_->d_results.get(), count, d_->stream);
     if (timing_) CU_TRY(cudaEventRecord(d_->ev[1], d_->stream));
     CU_TRY(cudaGetLastError());
     times_.match_launches += 1;
@@ -1547,8 +1494,8 @@ int Engine::match_fleet(const int32_t* scan_of_block, const SE2* states, int cou
 int Engine::sampling_fleet()
 {
     if (fleet_count_ < 1 || fleet_count_ > d_->fleet_cap) return fail("sampling_fleet: no fleet match of at most one block per robot", LAMA_ERR_STATE);
-    launch_sampling_fleet(d_->view, d_->pv(cur_set_), cur_set_, d_->fleet_points(), d_->fleet_scans(), d_->d_fleet_blocks, d_->d_results, fleet_count_,
-                          1.0 / cfg_.resolution, d_->d_fleet_off, d_->fleet_n_off, cfg_.resolution, max_sqdist_, d_->d_fleet_lik, d_->stream);
+    launch_sampling_fleet(d_->view, d_->pv(cur_set_), cur_set_, d_->fleet_points(), d_->fleet_scans(), d_->d_fleet_blocks.get(), d_->d_results.get(), fleet_count_,
+                          1.0 / cfg_.resolution, d_->d_fleet_off.get(), d_->fleet_n_off, cfg_.resolution, max_sqdist_, d_->d_fleet_lik.get(), d_->stream);
     CU_TRY(cudaGetLastError());
     times_.misc_launches += 1;
     fleet_sampled_ = true;
@@ -1560,19 +1507,19 @@ int Engine::fleet_results(HostMatchResult* out, double* lik)
     const int count = fleet_count_;
     if (count < 1) return fail("fleet_results: no fleet match", LAMA_ERR_STATE);
     fleet_count_ = 0;
-    CU_TRY(cudaMemcpyAsync(d_->h_results, d_->d_results, (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(d_->h_results.get(), d_->d_results.get(), (size_t)count * sizeof(MatchResult), cudaMemcpyDeviceToHost, d_->stream));
     const size_t lik_n = fleet_sampled_ ? (size_t)count * d_->fleet_n_off : 0;
-    if (lik_n) CU_TRY(cudaMemcpyAsync(d_->h_fleet_lik, d_->d_fleet_lik, lik_n * 8, cudaMemcpyDeviceToHost, d_->stream));
-    if (fleet_parked_) CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
+    if (lik_n) CU_TRY(cudaMemcpyAsync(d_->h_fleet_lik.get(), d_->d_fleet_lik.get(), lik_n * 8, cudaMemcpyDeviceToHost, d_->stream));
+    if (fleet_parked_) CU_TRY(cudaMemcpyAsync(d_->h_status.get(), d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     if (timing_) {
         float ms = 0;
         cudaEventElapsedTime(&ms, d_->ev[0], d_->ev[1]);
         times_.match_ms += ms;
     }
-    if (fleet_parked_ && *d_->h_status) return check_device_status();
-    std::memcpy(out, d_->h_results, (size_t)count * sizeof(MatchResult));
-    if (lik && lik_n) std::memcpy(lik, d_->h_fleet_lik, lik_n * 8);
+    if (fleet_parked_ && *d_->h_status.get()) return check_device_status();
+    std::memcpy(out, d_->h_results.get(), (size_t)count * sizeof(MatchResult));
+    if (lik && lik_n) std::memcpy(lik, d_->h_fleet_lik.get(), lik_n * 8);
     d2h_bytes_ += (uint64_t)count * sizeof(MatchResult) + lik_n * 8;
     return LAMA_OK;
 }
@@ -1583,8 +1530,8 @@ int Engine::sampling_likelihood(int particle, const SE2& pose, const double* off
     if (particle < 0 || particle >= cfg_.particles || n < 1 || stride < 1) return fail("sampling_likelihood: bad arguments", LAMA_ERR_ARG);
     if (d_->scan.n_beams < 1) return fail("sampling_likelihood: no scan uploaded", LAMA_ERR_STATE);
     CU_TRY(cudaSetDevice(cfg_.device));
-    if (ensure_scratch(d_, (size_t)n * 24)) return fail("sampling_likelihood: out of device memory", LAMA_ERR_CUDA);
-    double* d_off = (double*)d_->d_scratch;
+    if (d_->d_scratch.reserve((size_t)n * 24) != cudaSuccess) return fail("sampling_likelihood: out of device memory", LAMA_ERR_CUDA);
+    double* d_off = (double*)d_->d_scratch.get();
     double* d_out = d_off + 2 * (size_t)n;
     CU_TRY(cudaMemcpyAsync(d_off, offsets_xy, (size_t)n * 16, cudaMemcpyHostToDevice, d_->stream));
     launch_sampling(d_->view, d_->pv(cur_set_), cur_set_, particle, d_->d_points, d_->scan, pose, d_off, n, stride, cfg_.resolution, max_sqdist_, d_out, d_->stream);
@@ -1601,8 +1548,8 @@ int Engine::dm_distance(int particle, const double* pts, int n, double* dist, do
     if (particle < 0 || particle >= cfg_.particles || n < 1) return fail("dm_distance: bad arguments", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
     const size_t bp = (size_t)n * 24, bd = (size_t)n * 8, bg = (size_t)n * 24;
-    if (ensure_scratch(d_, bp + bd + bg)) return fail("dm_distance: out of device memory", LAMA_ERR_CUDA);
-    char* base = (char*)d_->d_scratch;
+    if (d_->d_scratch.reserve(bp + bd + bg) != cudaSuccess) return fail("dm_distance: out of device memory", LAMA_ERR_CUDA);
+    char* base = (char*)d_->d_scratch.get();
     CU_TRY(cudaMemcpyAsync(base, pts, bp, cudaMemcpyHostToDevice, d_->stream));
     launch_distance(d_->view, d_->pv(cur_set_), cur_set_, particle, (const double*)base, n, cfg_.resolution, max_sqdist_, (double*)(base + bp),
                     grad ? (double*)(base + bp + bd) : nullptr, d_->stream);
@@ -1620,8 +1567,8 @@ int Engine::export_window(int particle, int kind, uint32_t x0, uint32_t y0, int 
     if (particle < 0 || particle >= cfg_.particles || kind < 0 || kind > 1 || w < 1 || h < 1) return fail("export_window: bad arguments", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
     const size_t bw = (size_t)w * h * 4, bpz = (size_t)w * h;
-    if (ensure_scratch(d_, bw + bpz)) return fail("export_window: out of device memory", LAMA_ERR_CUDA);
-    char* base = (char*)d_->d_scratch;
+    if (d_->d_scratch.reserve(bw + bpz) != cudaSuccess) return fail("export_window: out of device memory", LAMA_ERR_CUDA);
+    char* base = (char*)d_->d_scratch.get();
     launch_export(d_->view, d_->pv(cur_set_), cur_set_, particle, kind, x0, y0, w, h, (uint32_t*)base, (uint8_t*)(base + bw), d_->stream);
     CU_TRY(cudaGetLastError());
     CU_TRY(cudaMemcpyAsync(words, base, bw, cudaMemcpyDeviceToHost, d_->stream));
@@ -1639,8 +1586,8 @@ int Engine::gather_cells(int particle, int kind, const uint32_t* cells_xy, int n
     if (n == 0) return LAMA_OK;
     CU_TRY(cudaSetDevice(cfg_.device));
     const size_t bc = (size_t)n * 8, bw = (size_t)n * 4, bf = (size_t)n;
-    if (ensure_scratch(d_, bc + bw + bf)) return fail("gather_cells: out of device memory", LAMA_ERR_CUDA);
-    char* base = (char*)d_->d_scratch;
+    if (d_->d_scratch.reserve(bc + bw + bf) != cudaSuccess) return fail("gather_cells: out of device memory", LAMA_ERR_CUDA);
+    char* base = (char*)d_->d_scratch.get();
     CU_TRY(cudaMemcpyAsync(base, cells_xy, bc, cudaMemcpyHostToDevice, d_->stream));
     launch_gather_cells(d_->view, d_->pv(cur_set_), cur_set_, particle, kind, (const uint32_t*)base, n, (uint32_t*)(base + bc), (uint8_t*)(base + bc + bw), d_->stream);
     CU_TRY(cudaGetLastError());
@@ -1656,10 +1603,10 @@ int Engine::export_bits(int particle, int plane, uint32_t x0, uint32_t y0, int w
     { int rc_settle = settle(nullptr); if (rc_settle != LAMA_OK) return rc_settle; }
     if (particle < 0 || particle >= cfg_.particles || plane < 0 || plane > 1 || w < 1 || h < 1) return fail("export_bits: bad arguments", LAMA_ERR_ARG);
     CU_TRY(cudaSetDevice(cfg_.device));
-    if (ensure_scratch(d_, (size_t)w * h)) return fail("export_bits: out of device memory", LAMA_ERR_CUDA);
-    launch_export_bits(d_->view, d_->pv(cur_set_), plane, cur_set_, particle, x0, y0, w, h, (uint8_t*)d_->d_scratch, d_->stream);
+    if (d_->d_scratch.reserve((size_t)w * h) != cudaSuccess) return fail("export_bits: out of device memory", LAMA_ERR_CUDA);
+    launch_export_bits(d_->view, d_->pv(cur_set_), plane, cur_set_, particle, x0, y0, w, h, (uint8_t*)d_->d_scratch.get(), d_->stream);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(out, d_->d_scratch, (size_t)w * h, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(out, d_->d_scratch.get(), (size_t)w * h, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     times_.misc_launches += 1;
     return LAMA_OK;
@@ -1673,12 +1620,12 @@ int Engine::import_window(int particle, int kind, uint32_t x0, uint32_t y0, int 
     CU_TRY(cudaSetDevice(cfg_.device));
     extent_stale_ = true;
     const size_t bw = (size_t)w * h * 4;
-    if (ensure_scratch(d_, bw)) return fail("import_window: out of device memory", LAMA_ERR_CUDA);
-    CU_TRY(cudaMemcpyAsync(d_->d_scratch, words, bw, cudaMemcpyHostToDevice, d_->stream));
-    launch_import(d_->view, cur_set_, particle, kind, x0, y0, w, h, (const uint32_t*)d_->d_scratch, d_->stream);
+    if (d_->d_scratch.reserve(bw) != cudaSuccess) return fail("import_window: out of device memory", LAMA_ERR_CUDA);
+    CU_TRY(cudaMemcpyAsync(d_->d_scratch.get(), words, bw, cudaMemcpyHostToDevice, d_->stream));
+    launch_import(d_->view, cur_set_, particle, kind, x0, y0, w, h, (const uint32_t*)d_->d_scratch.get(), d_->stream);
     launch_merge_free(d_->view, d_->stream);
     CU_TRY(cudaGetLastError());
-    CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(d_->h_status.get(), d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     times_.misc_launches += 2;
     return check_device_status();
@@ -1707,18 +1654,18 @@ int Engine::migration_alloc(size_t bytes, void** dptr)
 {
     CU_TRY(cudaSetDevice(cfg_.device));
     const size_t need = ((bytes ? bytes : 16) + 255) & ~(size_t)255;
-    while (d_->mig_chunk < d_->mig_chunks.size() && d_->mig_off + need > d_->mig_chunks[d_->mig_chunk].second) {
+    while (d_->mig_chunk < d_->mig_chunks.size() && d_->mig_off + need > d_->mig_chunks[d_->mig_chunk].size()) {
         ++d_->mig_chunk;
         d_->mig_off = 0;
     }
     if (d_->mig_chunk == d_->mig_chunks.size()) {
         const size_t chunk = std::max(need, (size_t)64 << 20);
-        void* p = nullptr;
-        CU_TRY(cudaMalloc(&p, chunk));
-        d_->mig_chunks.push_back({(char*)p, chunk});
+        DeviceArray<char> c;
+        CU_TRY(c.alloc(chunk));
+        d_->mig_chunks.push_back(std::move(c));
         d_->mig_off = 0;
     }
-    *dptr = d_->mig_chunks[d_->mig_chunk].first + d_->mig_off;
+    *dptr = d_->mig_chunks[d_->mig_chunk].get() + d_->mig_off;
     d_->mig_off += need;
     return LAMA_OK;
 }
@@ -1795,7 +1742,7 @@ int Engine::unpack_device(int particle, const DeviceBlob& blob, bool check)
     }
     CU_TRY(cudaGetLastError());
     if (!check) return LAMA_OK;   // the caller unpacks several blobs and checks the device status after the last one
-    CU_TRY(cudaMemcpyAsync(d_->h_status, d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
+    CU_TRY(cudaMemcpyAsync(d_->h_status.get(), d_->view.status, 4, cudaMemcpyDeviceToHost, d_->stream));
     CU_TRY(cudaStreamSynchronize(d_->stream));
     return check_device_status();
 }
@@ -1880,7 +1827,7 @@ int Engine::prune_outside(int particle, const double center[2], const double hwi
         const int2 ol = d_->park_ol[cur_set_][li];
         if (ol.y == 0) continue;
         std::vector<ParkEntry> l((size_t)ol.y), keep;
-        CU_TRY(cudaMemcpyAsync(l.data(), d_->park[cur_set_] + ol.x, l.size() * sizeof(ParkEntry), cudaMemcpyDeviceToHost, d_->stream));
+        CU_TRY(cudaMemcpyAsync(l.data(), d_->park[cur_set_].get() + ol.x, l.size() * sizeof(ParkEntry), cudaMemcpyDeviceToHost, d_->stream));
         CU_TRY(cudaStreamSynchronize(d_->stream));
         for (const ParkEntry& e : l) {
             const uint32_t c0[2] = {(uint32_t)e.px << kPatchLog2, (uint32_t)e.py << kPatchLog2};
@@ -1899,9 +1846,9 @@ int Engine::prune_outside(int particle, const double center[2], const double hwi
         }
         if (keep.size() == l.size()) continue;
         if (!keep.empty())
-            CU_TRY(cudaMemcpyAsync(d_->park[cur_set_] + ol.x, keep.data(), keep.size() * sizeof(ParkEntry), cudaMemcpyHostToDevice, d_->stream));
+            CU_TRY(cudaMemcpyAsync(d_->park[cur_set_].get() + ol.x, keep.data(), keep.size() * sizeof(ParkEntry), cudaMemcpyHostToDevice, d_->stream));
         d_->park_ol[cur_set_][li].y = (int32_t)keep.size();
-        CU_TRY(cudaMemcpyAsync(d_->d_park_ol[cur_set_] + li, &d_->park_ol[cur_set_][li], sizeof(int2), cudaMemcpyHostToDevice, d_->stream));
+        CU_TRY(cudaMemcpyAsync(d_->d_park_ol[cur_set_].get() + li, &d_->park_ol[cur_set_][li], sizeof(int2), cudaMemcpyHostToDevice, d_->stream));
         CU_TRY(cudaStreamSynchronize(d_->stream));   // `keep` and the host list entry are read by the copies
     }
     std::sort(gone.begin(), gone.end());
@@ -1909,14 +1856,14 @@ int Engine::prune_outside(int particle, const double center[2], const double hwi
     if (removed) *removed = (int)(list.size() + n_gone);
     if (list.empty() && dropped.empty()) return LAMA_OK;
     if (!list.empty()) {
-        std::memcpy(d_->h_idx, list.data(), list.size() * 4);
-        CU_TRY(cudaMemcpyAsync(d_->d_idx, d_->h_idx, list.size() * 4, cudaMemcpyHostToDevice, d_->stream));
-        launch_delete_patches(d_->view, cur_set_, particle, d_->d_idx, (int)list.size(), d_->stream);
+        std::memcpy(d_->h_idx.get(), list.data(), list.size() * 4);
+        CU_TRY(cudaMemcpyAsync(d_->d_idx.get(), d_->h_idx.get(), list.size() * 4, cudaMemcpyHostToDevice, d_->stream));
+        launch_delete_patches(d_->view, cur_set_, particle, d_->d_idx.get(), (int)list.size(), d_->stream);
     }
     if (!dropped.empty()) {
-        if (ensure_scratch(d_, dropped.size() * 4)) return fail("prune_outside: out of device memory", LAMA_ERR_CUDA);
-        CU_TRY(cudaMemcpyAsync(d_->d_scratch, dropped.data(), dropped.size() * 4, cudaMemcpyHostToDevice, d_->stream));
-        launch_release_entries(d_->view, (const int32_t*)d_->d_scratch, (int)dropped.size(), d_->stream);
+        if (d_->d_scratch.reserve(dropped.size() * 4) != cudaSuccess) return fail("prune_outside: out of device memory", LAMA_ERR_CUDA);
+        CU_TRY(cudaMemcpyAsync(d_->d_scratch.get(), dropped.data(), dropped.size() * 4, cudaMemcpyHostToDevice, d_->stream));
+        launch_release_entries(d_->view, (const int32_t*)d_->d_scratch.get(), (int)dropped.size(), d_->stream);
     }
     launch_merge_free(d_->view, d_->stream);
     CU_TRY(cudaGetLastError());
@@ -2018,35 +1965,23 @@ int Engine::memory_usage(int kind, uint32_t cell_bytes, uint64_t* out)
 constexpr size_t kCkptChunk = (size_t)8 << 20;   // bytes per pinned buffer of the chunked copies (two of them)
 
 namespace {
-struct PinnedPair {   // two pinned chunk buffers and their completion events, released on every exit path
-    char* buf[2] = {nullptr, nullptr};
-    cudaEvent_t done[2] = {nullptr, nullptr};
+struct PinnedPair {   // two pinned chunk buffers and their completion events: no buffer goes while a copy may still use it
+    PinnedArray<char> buf[2];
+    Event done[2];
     cudaError_t init()
     {
         for (int b = 0; b < 2; ++b) {
-            cudaError_t e = cudaMallocHost((void**)&buf[b], kCkptChunk);
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming);
+            cudaError_t e = buf[b].alloc(kCkptChunk);
+            if (e == cudaSuccess) e = done[b].create(cudaEventDisableTiming);
             if (e != cudaSuccess) return e;
         }
         return cudaSuccess;
     }
     ~PinnedPair()
     {
-        for (int b = 0; b < 2; ++b) {
-            if (done[b]) cudaEventSynchronize(done[b]), cudaEventDestroy(done[b]);
-            if (buf[b]) cudaFreeHost(buf[b]);
-        }
+        for (const Event& d : done)
+            if (d) cudaEventSynchronize(d);
     }
-};
-struct DeviceAllocs {
-    std::vector<void*> p;
-    cudaError_t alloc(void** out, size_t bytes)
-    {
-        cudaError_t e = cudaMalloc(out, bytes ? bytes : 16);
-        if (e == cudaSuccess) p.push_back(*out);
-        return e;
-    }
-    ~DeviceAllocs() { for (void* q : p) cudaFree(q); }
 };
 double host_ms(std::chrono::steady_clock::time_point a) { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - a).count(); }
 }  // namespace
@@ -2059,17 +1994,21 @@ int Engine::snapshot(EngineImage* out, CheckpointTimes* t, int particles)
     CU_TRY(cudaSetDevice(cfg_.device));
     const StoreView& v = d_->view;
     const size_t n_slots = (size_t)v.n_slots, n_dir = (size_t)particles * v.n_kinds * cfg_.dir_dim * cfg_.dir_dim;
-    DeviceAllocs mem;
+    DeviceArray<int32_t> d_cnt, d_used, d_new_id, d_list, d_ref, d_dirs, d_parked_in, d_parked_out;
+    DeviceArray<uint32_t> d_bad;
+    DeviceArray<char> d_temp, d_stage;
     CkptScratch c{};
     c.temp_bytes = ckpt_scan_temp_bytes(v.n_slots);
-    CU_TRY(mem.alloc((void**)&c.cnt, n_slots * 4));
-    CU_TRY(mem.alloc((void**)&c.used, n_slots * 4));
-    CU_TRY(mem.alloc((void**)&c.new_id, n_slots * 4));
-    CU_TRY(mem.alloc((void**)&c.list, n_slots * 4));
-    CU_TRY(mem.alloc((void**)&c.ref, n_slots * 4));
-    CU_TRY(mem.alloc((void**)&c.dirs, n_dir * 4));
-    CU_TRY(mem.alloc((void**)&c.bad, 16));
-    CU_TRY(mem.alloc(&c.temp, c.temp_bytes));
+    CU_TRY(d_cnt.alloc(n_slots));
+    CU_TRY(d_used.alloc(n_slots));
+    CU_TRY(d_new_id.alloc(n_slots));
+    CU_TRY(d_list.alloc(n_slots));
+    CU_TRY(d_ref.alloc(n_slots));
+    CU_TRY(d_dirs.alloc(n_dir));
+    CU_TRY(d_bad.alloc(4));
+    CU_TRY(d_temp.alloc(std::max<size_t>(c.temp_bytes, 16)));
+    c.cnt = d_cnt.get(); c.used = d_used.get(); c.new_id = d_new_id.get(); c.list = d_list.get(); c.ref = d_ref.get(); c.dirs = d_dirs.get();
+    c.bad = d_bad.get(); c.temp = d_temp.get();
     // the parked entries of the saved particles, gathered list by list in (particle, kind) order; counted and remapped with the directories
     std::vector<int32_t> park_len((size_t)particles * v.n_kinds, 0);
     std::vector<ParkEntry> parked;
@@ -2085,15 +2024,14 @@ int Engine::snapshot(EngineImage* out, CheckpointTimes* t, int particles)
     c.parked = nullptr;
     c.parked_out = nullptr;
     if (c.n_parked) {
-        int32_t* pin = nullptr;
-        CU_TRY(mem.alloc((void**)&pin, c.n_parked * 4));
-        CU_TRY(mem.alloc((void**)&c.parked_out, c.n_parked * 4));
-        CU_TRY(cudaMemcpyAsync(pin, park_entries.data(), c.n_parked * 4, cudaMemcpyHostToDevice, d_->stream));
-        c.parked = pin;
+        CU_TRY(d_parked_in.alloc(c.n_parked));
+        CU_TRY(d_parked_out.alloc(c.n_parked));
+        CU_TRY(cudaMemcpyAsync(d_parked_in.get(), park_entries.data(), c.n_parked * 4, cudaMemcpyHostToDevice, d_->stream));
+        c.parked = d_parked_in.get();
+        c.parked_out = d_parked_out.get();
     }
-    cudaEvent_t ev[4] = {};
-    struct Events { cudaEvent_t* e; ~Events() { for (int k = 0; k < 4; ++k) if (e[k]) cudaEventDestroy(e[k]); } } ev_guard{ev};
-    for (int k = 0; k < 4; ++k) CU_TRY(cudaEventCreate(&ev[k]));
+    Event ev[4];
+    for (Event& x : ev) CU_TRY(x.create(cudaEventDefault));
     CU_TRY(cudaMemsetAsync(c.cnt, 0, n_slots * 4, d_->stream));
     CU_TRY(cudaMemsetAsync(c.bad, 0, 4, d_->stream));
     CU_TRY(cudaEventRecord(ev[0], d_->stream));
@@ -2126,8 +2064,8 @@ int Engine::snapshot(EngineImage* out, CheckpointTimes* t, int particles)
         img.parked = parked;
     }
     const size_t stride = img.slot_stride(), bytes = (size_t)K * stride;
-    char* stage = nullptr;
-    CU_TRY(mem.alloc((void**)&stage, bytes));
+    CU_TRY(d_stage.alloc(std::max<size_t>(bytes, 16)));
+    char* stage = d_stage.get();
     uint32_t* cells = (uint32_t*)stage;
     uint32_t* fb = (uint32_t*)(stage + (size_t)K * kPatchBytes);
     uint32_t* kb = img.has_kbits() ? (uint32_t*)(stage + (size_t)K * (kPatchBytes + 128)) : nullptr;
@@ -2154,13 +2092,13 @@ int Engine::snapshot(EngineImage* out, CheckpointTimes* t, int particles)
     for (size_t i = 0; i <= n_chunks; ++i) {
         if (i < n_chunks) {
             const size_t off = i * kCkptChunk, len = std::min(kCkptChunk, bytes - off);
-            CU_TRY(cudaMemcpyAsync(pin.buf[i & 1], stage + off, len, cudaMemcpyDeviceToHost, d_->stream));
+            CU_TRY(cudaMemcpyAsync(pin.buf[i & 1].get(), stage + off, len, cudaMemcpyDeviceToHost, d_->stream));
             CU_TRY(cudaEventRecord(pin.done[i & 1], d_->stream));
         }
         if (i > 0) {
             const size_t j = i - 1, off = j * kCkptChunk, len = std::min(kCkptChunk, bytes - off);
             CU_TRY(cudaEventSynchronize(pin.done[j & 1]));
-            std::memcpy(img.slot_store.data() + off, pin.buf[j & 1], len);
+            std::memcpy(img.slot_store.data() + off, pin.buf[j & 1].get(), len);
         }
     }
     d2h_bytes_ += bytes + n_dir * 4 + (uint64_t)K * 4;
@@ -2221,11 +2159,11 @@ Engine* Engine::restore(const EngineImage& img, int device, uint64_t stream, std
         for (size_t i = 0; i < n_chunks; ++i) {
             const size_t off = i * kCkptChunk, len = std::min(kCkptChunk, bytes - off);
             if (i >= 2 && !cu(cudaEventSynchronize(pin.done[i & 1]), "copy")) return nullptr;   // chunk i - 2 has left this buffer
-            std::memcpy(pin.buf[i & 1], img.slot_bytes + off, len);
+            std::memcpy(pin.buf[i & 1].get(), img.slot_bytes + off, len);
             size_t base = 0;
             for (const Region& r : regions) {   // the chunk may straddle the cells and the planes
                 const size_t lo = std::max(off, base), hi = std::min(off + len, base + r.len);
-                if (lo < hi && !cu(cudaMemcpyAsync(r.dst + (lo - base), pin.buf[i & 1] + (lo - off), hi - lo, cudaMemcpyHostToDevice, d->stream), "copy"))
+                if (lo < hi && !cu(cudaMemcpyAsync(r.dst + (lo - base), pin.buf[i & 1].get() + (lo - off), hi - lo, cudaMemcpyHostToDevice, d->stream), "copy"))
                     return nullptr;
                 base += r.len;
             }
@@ -2242,14 +2180,14 @@ Engine* Engine::restore(const EngineImage& img, int device, uint64_t stream, std
                 const EngineImage::SlotRef& s = img.slot_src[k];
                 const size_t plane = r == 0 ? 0 : (size_t)s.count * (kPatchBytes + (r == 2 ? 128 : 0));
                 if (fill == 0 && i >= 2 && !cu(cudaEventSynchronize(pin.done[i & 1]), "copy")) return nullptr;   // chunk i - 2 has left this buffer
-                std::memcpy(pin.buf[i & 1] + fill, s.payload + plane + (size_t)s.slot * piece, piece);
+                std::memcpy(pin.buf[i & 1].get() + fill, s.payload + plane + (size_t)s.slot * piece, piece);
                 fill += piece;
                 if (fill < kCkptChunk && !(r == last_region && k + 1 == K)) continue;
                 const size_t off = i * kCkptChunk;
                 size_t base = 0;
                 for (const Region& g : regions) {
                     const size_t lo = std::max(off, base), hi = std::min(off + fill, base + g.len);
-                    if (lo < hi && !cu(cudaMemcpyAsync(g.dst + (lo - base), pin.buf[i & 1] + (lo - off), hi - lo, cudaMemcpyHostToDevice, d->stream), "copy"))
+                    if (lo < hi && !cu(cudaMemcpyAsync(g.dst + (lo - base), pin.buf[i & 1].get() + (lo - off), hi - lo, cudaMemcpyHostToDevice, d->stream), "copy"))
                         return nullptr;
                     base += g.len;
                 }
@@ -2267,9 +2205,9 @@ Engine* Engine::restore(const EngineImage& img, int device, uint64_t stream, std
             ol[li] = make_int2(off, img.park_len[li]);
             off += img.park_len[li];
         }
-        if (!cu(cudaMalloc((void**)&d->park[0], img.parked.size() * sizeof(ParkEntry)), "parked entries") ||
-            !cu(cudaMemcpyAsync(d->park[0], img.parked.data(), img.parked.size() * sizeof(ParkEntry), cudaMemcpyHostToDevice, d->stream), "parked entries") ||
-            !cu(cudaMemcpyAsync(d->d_park_ol[0], ol.data(), ol.size() * sizeof(int2), cudaMemcpyHostToDevice, d->stream), "parked lists"))
+        if (!cu(d->park[0].alloc(img.parked.size()), "parked entries") ||
+            !cu(cudaMemcpyAsync(d->park[0].get(), img.parked.data(), img.parked.size() * sizeof(ParkEntry), cudaMemcpyHostToDevice, d->stream), "parked entries") ||
+            !cu(cudaMemcpyAsync(d->d_park_ol[0].get(), ol.data(), ol.size() * sizeof(int2), cudaMemcpyHostToDevice, d->stream), "parked lists"))
             return nullptr;
     }
     if (!cu(cudaStreamSynchronize(d->stream), "synchronize")) return nullptr;

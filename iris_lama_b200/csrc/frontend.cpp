@@ -116,14 +116,7 @@ PFSlam2D* PFSlam2D::create(const PFOptions& o, std::string& err)
 }
 PFSlam2D::~PFSlam2D()
 {
-    if (comm_) {
-        shard_comm_destroy(comm_);
-        cudaFree(d_send_);
-        cudaFree(d_recv_);
-        cudaFree(d_tab_);
-        cudaFreeHost(h_recv_);
-        cudaFreeHost(h_tab_);
-    }
+    if (comm_) shard_comm_destroy(comm_);
 }
 
 double PFSlam2D::rng_normal(double sigma)  // random::normal, src/random.cpp:69-73
@@ -456,9 +449,9 @@ int PFSlam2D::shard_connect(const uint8_t id[128])
     comm_ = shard_comm_create(id, (int)opt_.shard_rank, (int)opt_.shard_count, opt_.dev.device, e);
     if (!comm_) return fail(e, LAMA_ERR_CUDA);
     const size_t per = (size_t)(hi_ - lo_), payload = per * kShardF + 1;
-    bool ok = cudaMalloc((void**)&d_send_, payload * 8) == cudaSuccess && cudaMalloc((void**)&d_recv_, payload * 8 * opt_.shard_count) == cudaSuccess &&
-              cudaMallocHost((void**)&h_recv_, payload * 8 * opt_.shard_count) == cudaSuccess && cudaMalloc((void**)&d_tab_, (size_t)P_ * 3 * 8 * 2) == cudaSuccess &&
-              cudaMallocHost((void**)&h_tab_, (size_t)P_ * 3 * 8 * 2) == cudaSuccess;
+    bool ok = d_send_.alloc(payload) == cudaSuccess && d_recv_.alloc(payload * opt_.shard_count) == cudaSuccess &&
+              h_recv_.alloc(payload * opt_.shard_count) == cudaSuccess && d_tab_.alloc((size_t)P_ * 3 * 2) == cudaSuccess &&
+              h_tab_.alloc((size_t)P_ * 3 * 2) == cudaSuccess;
     if (!ok) return fail("shard_connect: out of memory", LAMA_ERR_CUDA);
     return LAMA_OK;
 }
@@ -489,10 +482,10 @@ int PFSlam2D::update_sharded(const double* pts, int n, const double* origin, con
                             opt_.meas_sigma);
     if (rc != LAMA_OK) return engine_fail(rc);
     const size_t payload = (size_t)nl * kShardF + 1;
-    rc = eng_->pack_results(nl, digest_, d_send_, shard_stream(comm_));   // waits for the match on the communicator's stream
+    rc = eng_->pack_results(nl, digest_, d_send_.get(), shard_stream(comm_));   // waits for the match on the communicator's stream
     if (rc != LAMA_OK) return engine_fail(rc);
-    if (shard_allgather(comm_, d_send_, d_recv_, payload * 8) != 0) return fail(shard_error(comm_), LAMA_ERR_CUDA);
-    if (cudaMemcpyAsync(h_recv_, d_recv_, payload * 8 * G, cudaMemcpyDeviceToHost, (cudaStream_t)shard_stream(comm_)) != cudaSuccess)
+    if (shard_allgather(comm_, d_send_.get(), d_recv_.get(), payload * 8) != 0) return fail(shard_error(comm_), LAMA_ERR_CUDA);
+    if (cudaMemcpyAsync(h_recv_.get(), d_recv_.get(), payload * 8 * G, cudaMemcpyDeviceToHost, (cudaStream_t)shard_stream(comm_)) != cudaSuccess)
         return fail("update_sharded: copy of the gathered results failed", LAMA_ERR_CUDA);
     if (shard_sync(comm_) != 0) return fail(shard_error(comm_), LAMA_ERR_CUDA);
     ++shard_collectives_;
@@ -506,8 +499,8 @@ int PFSlam2D::update_sharded(const double* pts, int n, const double* origin, con
     t_solve_ += ms(t1, t2);
     std::vector<double> all((size_t)P_ * 5);
     for (int r = 0; r < G; ++r) {
-        const double* src = h_recv_ + (size_t)r * payload;
-        if (src[(size_t)nl * kShardF] != h_recv_[(size_t)nl * kShardF]) return fail("the resampling decision diverged between ranks", LAMA_ERR_STATE);
+        const double* src = h_recv_.get() + (size_t)r * payload;
+        if (src[(size_t)nl * kShardF] != h_recv_.get()[(size_t)nl * kShardF]) return fail("the resampling decision diverged between ranks", LAMA_ERR_STATE);
         for (int k = 0; k < nl; ++k) {
             const double* f = src + (size_t)k * kShardF;
             double* dst = &all[((size_t)r * nl + k) * 5];
@@ -568,11 +561,11 @@ int PFSlam2D::migrate_and_apply(const std::vector<int32_t>& idx)
     cudaStream_t cs = (cudaStream_t)shard_stream(comm_);
     // the gather kernels of the packs run on the engine's stream; everything the communicator's stream does from here on (the sends) comes after them
     if (eng_->wait_for_stream(cs) != LAMA_OK) return engine_fail(LAMA_ERR_CUDA);
-    std::memcpy(h_tab_, mine.data(), mine.size() * 8);
-    int64_t* d_all = d_tab_ + (size_t)P_ * 3;
-    int64_t* h_all = h_tab_ + (size_t)P_ * 3;
-    if (cudaMemcpyAsync(d_tab_, h_tab_, mine.size() * 8, cudaMemcpyHostToDevice, cs) != cudaSuccess) return fail("migrate: size table upload failed", LAMA_ERR_CUDA);
-    if (shard_allgather(comm_, d_tab_, d_all, mine.size() * 8) != 0) return fail(shard_error(comm_), LAMA_ERR_CUDA);
+    std::memcpy(h_tab_.get(), mine.data(), mine.size() * 8);
+    int64_t* d_all = d_tab_.get() + (size_t)P_ * 3;
+    int64_t* h_all = h_tab_.get() + (size_t)P_ * 3;
+    if (cudaMemcpyAsync(d_tab_.get(), h_tab_.get(), mine.size() * 8, cudaMemcpyHostToDevice, cs) != cudaSuccess) return fail("migrate: size table upload failed", LAMA_ERR_CUDA);
+    if (shard_allgather(comm_, d_tab_.get(), d_all, mine.size() * 8) != 0) return fail(shard_error(comm_), LAMA_ERR_CUDA);
     if (cudaMemcpyAsync(h_all, d_all, (size_t)P_ * 3 * 8, cudaMemcpyDeviceToHost, cs) != cudaSuccess) return fail("migrate: size table download failed", LAMA_ERR_CUDA);
     if (shard_sync(comm_) != 0) return fail(shard_error(comm_), LAMA_ERR_CUDA);
     ++shard_collectives_;

@@ -11,6 +11,7 @@
 #include <string>
 #include <vector>
 
+#include "cuda_owned.h"
 #include "engine.h"
 #include "pgo.h"
 
@@ -152,11 +153,11 @@ private:
     std::string err_;
     bool pending_maps_ = false, counters_pending_ = false;
     struct ShardComm* comm_ = nullptr;
-    double* d_send_ = nullptr;      // device: local payload (per x kShardFields + 1 digest)
-    double* d_recv_ = nullptr;      // device: gathered payloads
-    double* h_recv_ = nullptr;      // pinned host copy
-    int64_t* d_tab_ = nullptr;      // device: blob sizes of the particles this rank serves / of all particles
-    int64_t* h_tab_ = nullptr;      // pinned
+    DeviceArray<double> d_send_;    // local payload (per x kShardFields + 1 digest)
+    DeviceArray<double> d_recv_;    // gathered payloads
+    PinnedArray<double> h_recv_;    // host copy
+    DeviceArray<int64_t> d_tab_;    // blob sizes of the particles this rank serves / of all particles
+    PinnedArray<int64_t> h_tab_;
     double digest_ = 0.0;           // of the previous scan's resampling decision, compared across ranks one scan later
     uint64_t shard_collectives_ = 0, shard_migrated_bytes_ = 0;
     int update_sharded(const double* pts, int n, const double* origin, const double* quat, const double odom_xyr[3], bool* did_update);

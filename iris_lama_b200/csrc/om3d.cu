@@ -278,6 +278,8 @@ struct OccMap3Dev::Impl : PatchStore {
     ProbParams pp{};
     Buf qin, qout, qflag, ops, changed, dops, dseg;
 
+    ~Impl() { quiesce(); }
+
     View view() const { return View{dir, (uint32_t*)cells, mask, win}; }
 };
 
@@ -332,16 +334,16 @@ int OccMap3Dev::insert_point_clouds(const double* pts, const int64_t* offsets, i
 
     const View v = d.view();
     InsertParams f{};
-    f.pts = (const double*)d.pts.p;
-    f.offsets = (const int64_t*)d.off.p;
-    f.tf = (const Affine*)d.tf.p;
+    f.pts = (const double*)d.pts.get();
+    f.offsets = (const int64_t*)d.off.get();
+    f.tf = (const Affine*)d.tf.get();
     f.n_clouds = n_clouds;
     f.p0 = 0;
     f.p1 = n_pts;
     f.scale = d.scale;
     f.full = full ? 1 : 0;
-    f.counts = (uint64_t*)d.counts.p;
-    f.offs = (const uint64_t*)d.offs.p;
+    f.counts = (uint64_t*)d.counts.get();
+    f.offs = (const uint64_t*)d.offs.get();
     f.marks = d.marks;
     f.status = d.status;
 
@@ -376,8 +378,8 @@ int OccMap3Dev::insert_point_clouds(const double* pts, const int64_t* offsets, i
             f.p0 = offsets[c0];
             f.p1 = offsets[c1];
             f.rec_base = bound[c0];
-            f.rkeys = (uint32_t*)d.rk[0].p;
-            f.rvals = (uint32_t*)d.rv[0].p;
+            f.rkeys = (uint32_t*)d.rk[0].get();
+            f.rvals = (uint32_t*)d.rv[0].get();
             k_om3_points<2><<<blocks_for((uint64_t)(f.p1 - f.p0)), kThreads, 0, d.stream>>>(f, v);
             PS_TRY(d.sort_fold<uint32_t, OpFold<false>>((int64_t)nrec, v, d.kind, d.pp, (uint8_t*)nullptr));
             d.launches[0] += 3;
@@ -429,16 +431,16 @@ int OccMap3Dev::insert_point_clouds_dm3(DistMap3Dev& dm, const double* pts, cons
     if (n_pts > 0) {
         PS_TRY(d.record(0));
         PS_TRY(d.upload_clouds(pts, offsets, n_clouds, n_pts, origins, quats));
-        f.pts = (const double*)d.pts.p;
-        f.offsets = (const int64_t*)d.off.p;
-        f.tf = (const Affine*)d.tf.p;
+        f.pts = (const double*)d.pts.get();
+        f.offsets = (const int64_t*)d.off.get();
+        f.tf = (const Affine*)d.tf.get();
         f.n_clouds = n_clouds;
         f.p0 = 0;
         f.p1 = n_pts;
         f.scale = d.scale;
         f.full = full ? 1 : 0;
-        f.counts = (uint64_t*)d.counts.p;
-        f.offs = (const uint64_t*)d.offs.p;
+        f.counts = (uint64_t*)d.counts.get();
+        f.offs = (const uint64_t*)d.offs.get();
         f.marks = d.marks;
         f.status = d.status;
         f.margin = cp.reach + 1;
@@ -471,30 +473,26 @@ int OccMap3Dev::insert_point_clouds_dm3(DistMap3Dev& dm, const double* pts, cons
     rc = dm.flush();   // queued ops first: they already sit in the reference's heaps
     if (rc != LAMA_OK) { err_ = dm.error(); return rc; }
 
-    cudaEvent_t ev[2] = {nullptr, nullptr};   // [0] distance map -> occupancy map, [1] the reverse
-    struct Events {
-        cudaEvent_t* e;
-        ~Events() { for (int k = 0; k < 2; ++k) if (e[k]) cudaEventDestroy(e[k]); }
-    } guard{ev};
-    for (int k = 0; k < 2; ++k) PS_TRY(cudaEventCreateWithFlags(&ev[k], cudaEventDisableTiming));
+    Event ev[2];   // [0] distance map -> occupancy map, [1] the reverse
+    for (Event& e : ev) PS_TRY(e.create(cudaEventDisableTiming));
     const DmView dv{cp.dir, cp.cells};
     rc = PatchStore::for_each_chunk(bound, n_clouds, [&](int c0, int c1, uint64_t nrec) -> int {
         std::vector<uint32_t> seg_end((size_t)(c1 - c0), 0);
         if (nrec > 0) {
             PS_TRY(d.record(0));
             PS_TRY(d.ensure_records<uint32_t>(nrec + 1));
-            PS_TRY(d.ensure(d.changed, (size_t)nrec));
+            PS_TRY(d.changed.reserve((size_t)nrec));
             f.p0 = offsets[c0];
             f.p1 = offsets[c1];
             f.rec_base = bound[(size_t)c0];
-            f.rkeys = (uint32_t*)d.rk[0].p;
-            f.rvals = (uint32_t*)d.rv[0].p;
-            const uint32_t* keys = (const uint32_t*)d.rk[0].p;   // record order
-            uint8_t* flags = (uint8_t*)d.changed.p;
+            f.rkeys = (uint32_t*)d.rk[0].get();
+            f.rvals = (uint32_t*)d.rv[0].get();
+            const uint32_t* keys = (const uint32_t*)d.rk[0].get();   // record order
+            uint8_t* flags = (uint8_t*)d.changed.get();
             const unsigned nb = blocks_for(nrec);
             k_om3_points<2><<<blocks_for((uint64_t)(f.p1 - f.p0)), kThreads, 0, d.stream>>>(f, v);
             PS_TRY(d.sort_records<uint32_t>((int64_t)nrec));
-            k_od3_fold<<<nb, kThreads, 0, d.stream>>>((const uint32_t*)d.rk[1].p, (const uint32_t*)d.rv[1].p, nrec, v, d.kind, d.pp, dv, flags);
+            k_od3_fold<<<nb, kThreads, 0, d.stream>>>((const uint32_t*)d.rk[1].get(), (const uint32_t*)d.rv[1].get(), nrec, v, d.kind, d.pp, dv, flags);
             PS_TRY(d.clear_marks());
             k_od3_mark<<<nb, kThreads, 0, d.stream>>>(keys, flags, nrec, d.marks);
             d.launches[0] += 4;
@@ -506,27 +504,27 @@ int OccMap3Dev::insert_point_clouds_dm3(DistMap3Dev& dm, const double* pts, cons
             if (rc != LAMA_OK) { err_ = dm.error(); return rc; }
             PS_TRY(cudaStreamWaitEvent(d.stream, ev[0], 0));
             // the sorted values are spent: rv[0] takes the push flags, rv[1] their exclusive scan (nrec + 1 entries)
-            uint32_t* push = (uint32_t*)d.rv[0].p;
-            uint32_t* pos = (uint32_t*)d.rv[1].p;
-            PS_TRY(d.ensure(d.dseg, (size_t)(c1 - c0) * 4 + 8));
-            unsigned long long* ev_count = (unsigned long long*)d.dseg.p;
-            uint32_t* dseg_end = (uint32_t*)((char*)d.dseg.p + 8);
+            uint32_t* push = (uint32_t*)d.rv[0].get();
+            uint32_t* pos = (uint32_t*)d.rv[1].get();
+            PS_TRY(d.dseg.reserve((size_t)(c1 - c0) * 4 + 8));
+            unsigned long long* ev_count = (unsigned long long*)d.dseg.get();
+            uint32_t* dseg_end = (uint32_t*)((char*)d.dseg.get() + 8);
             PS_TRY(cudaMemsetAsync(ev_count, 0, 8, d.stream));
             PS_TRY(cudaMemsetAsync(push + nrec, 0, 4, d.stream));
             k_od3_known<<<nb, kThreads, 0, d.stream>>>(keys, flags, nrec, dv, push, ev_count);
             size_t bytes = 0;
             PS_TRY(cub::DeviceScan::ExclusiveSum(nullptr, bytes, push, pos, (int64_t)nrec + 1, d.stream));
-            PS_TRY(d.ensure(d.temp, bytes));
-            PS_TRY(cub::DeviceScan::ExclusiveSum(d.temp.p, bytes, push, pos, (int64_t)nrec + 1, d.stream));
-            k_od3_segments<<<blocks_for((uint64_t)(c1 - c0)), kThreads, 0, d.stream>>>(pos, (const uint64_t*)d.bound.p, c0, c1 - c0, bound[(size_t)c0], dseg_end);
+            PS_TRY(d.temp.reserve(bytes));
+            PS_TRY(cub::DeviceScan::ExclusiveSum(d.temp.get(), bytes, push, pos, (int64_t)nrec + 1, d.stream));
+            k_od3_segments<<<blocks_for((uint64_t)(c1 - c0)), kThreads, 0, d.stream>>>(pos, (const uint64_t*)d.bound.get(), c0, c1 - c0, bound[(size_t)c0], dseg_end);
             d.launches[0] += 3;
             unsigned long long h_events = 0;
             PS_TRY(cudaMemcpyAsync(&h_events, ev_count, 8, cudaMemcpyDeviceToHost, d.stream));
             PS_TRY(cudaMemcpyAsync(seg_end.data(), dseg_end, seg_end.size() * 4, cudaMemcpyDeviceToHost, d.stream));
             PS_TRY(cudaStreamSynchronize(d.stream));
             const uint32_t n_push = seg_end.back();
-            PS_TRY(d.ensure(d.dops, (size_t)std::max<uint32_t>(n_push, 1) * kDm3OpWords * 4));
-            k_od3_ops<<<nb, kThreads, 0, d.stream>>>(keys, flags, pos, nrec, d.win, (uint32_t*)d.dops.p);
+            PS_TRY(d.dops.reserve((size_t)std::max<uint32_t>(n_push, 1) * kDm3OpWords * 4));
+            k_od3_ops<<<nb, kThreads, 0, d.stream>>>(keys, flags, pos, nrec, d.win, (uint32_t*)d.dops.get());
             d.launches[0] += 1;
             PS_TRY(cudaGetLastError());
             PS_TRY(d.record(1));
@@ -535,7 +533,7 @@ int OccMap3Dev::insert_point_clouds_dm3(DistMap3Dev& dm, const double* pts, cons
             events += h_events;
             pushes += n_push;
         }
-        rc = dm.run_segments((const uint32_t*)d.dops.p, seg_end, proc.data() + c0, nrec > 0 ? ev[1] : nullptr);
+        rc = dm.run_segments((const uint32_t*)d.dops.get(), seg_end, proc.data() + c0, nrec > 0 ? ev[1].get() : nullptr);
         if (rc != LAMA_OK) { err_ = dm.error(); return rc; }
         return LAMA_OK;
     });
@@ -556,15 +554,15 @@ int OccMap3Dev::apply(const uint32_t* cells_xyz, const uint8_t* ops, int n, uint
         if (ops[i] > kOm3SetUnknown) { err_ = "op must be 0 (setFree), 1 (setOccupied) or 2 (setUnknown)"; return LAMA_ERR_ARG; }
     PS_TRY(cudaSetDevice(d.device));
     PS_TRY(d.record(0));
-    PS_TRY(d.ensure(d.qin, (size_t)n * 12));
-    PS_TRY(d.ensure(d.ops, (size_t)n));
-    PS_TRY(d.ensure(d.changed, (size_t)n));
+    PS_TRY(d.qin.reserve((size_t)n * 12));
+    PS_TRY(d.ops.reserve((size_t)n));
+    PS_TRY(d.changed.reserve((size_t)n));
     PS_TRY(d.ensure_records<uint32_t>((uint64_t)n));
-    PS_TRY(cudaMemcpyAsync(d.qin.p, cells_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, d.stream));
-    PS_TRY(cudaMemcpyAsync(d.ops.p, ops, (size_t)n, cudaMemcpyHostToDevice, d.stream));
+    PS_TRY(cudaMemcpyAsync(d.qin.get(), cells_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, d.stream));
+    PS_TRY(cudaMemcpyAsync(d.ops.get(), ops, (size_t)n, cudaMemcpyHostToDevice, d.stream));
     PS_TRY(d.clear_marks());
-    const uint32_t* xyz = (const uint32_t*)d.qin.p;
-    const uint8_t* dops = (const uint8_t*)d.ops.p;
+    const uint32_t* xyz = (const uint32_t*)d.qin.get();
+    const uint8_t* dops = (const uint8_t*)d.ops.get();
     const View v = d.view();
     k_om3_apply<false><<<blocks_for(n), kThreads, 0, d.stream>>>(xyz, dops, n, v, d.marks, d.status, nullptr, nullptr);
     d.launches[1] += 1;
@@ -575,12 +573,12 @@ int OccMap3Dev::apply(const uint32_t* cells_xyz, const uint8_t* ops, int n, uint
     if (status & kErrWindow) { err_ = "a cell lies outside the directory window"; return LAMA_ERR_WINDOW; }
     const int rc = d.alloc_marked(marks, v, err_, d.launches[1]);
     if (rc != LAMA_OK) return rc;
-    k_om3_apply<true><<<blocks_for(n), kThreads, 0, d.stream>>>(xyz, dops, n, v, nullptr, nullptr, (uint32_t*)d.rk[0].p, (uint32_t*)d.rv[0].p);
-    PS_TRY(d.sort_fold<uint32_t, OpFold<true>>(n, v, d.kind, d.pp, (uint8_t*)d.changed.p));
+    k_om3_apply<true><<<blocks_for(n), kThreads, 0, d.stream>>>(xyz, dops, n, v, nullptr, nullptr, (uint32_t*)d.rk[0].get(), (uint32_t*)d.rv[0].get());
+    PS_TRY(d.sort_fold<uint32_t, OpFold<true>>(n, v, d.kind, d.pp, (uint8_t*)d.changed.get()));
     d.launches[1] += 3;
     PS_TRY(cudaGetLastError());
     PS_TRY(d.record(1));
-    if (changed) PS_TRY(cudaMemcpyAsync(changed, d.changed.p, (size_t)n, cudaMemcpyDeviceToHost, d.stream));
+    if (changed) PS_TRY(cudaMemcpyAsync(changed, d.changed.get(), (size_t)n, cudaMemcpyDeviceToHost, d.stream));
     PS_TRY(d.finish(1));
     return LAMA_OK;
 }
@@ -591,19 +589,19 @@ int OccMap3Dev::query(const uint32_t* cells_xyz, int n, double* prob, uint8_t* f
     if (n < 0 || (n > 0 && !cells_xyz)) { err_ = "null argument"; return LAMA_ERR_ARG; }
     if (n == 0) return LAMA_OK;
     PS_TRY(cudaSetDevice(d.device));
-    PS_TRY(d.ensure(d.qin, (size_t)n * 12));
-    PS_TRY(d.ensure(d.qout, (size_t)n * 4));
-    PS_TRY(d.ensure(d.qflag, (size_t)n));
-    PS_TRY(cudaMemcpyAsync(d.qin.p, cells_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, d.stream));
+    PS_TRY(d.qin.reserve((size_t)n * 12));
+    PS_TRY(d.qout.reserve((size_t)n * 4));
+    PS_TRY(d.qflag.reserve((size_t)n));
+    PS_TRY(cudaMemcpyAsync(d.qin.get(), cells_xyz, (size_t)n * 12, cudaMemcpyHostToDevice, d.stream));
     PS_TRY(d.record(0));
-    k_om3_gather<<<blocks_for(n), kThreads, 0, d.stream>>>((const uint32_t*)d.qin.p, n, d.view(), (uint32_t*)d.qout.p, (uint8_t*)d.qflag.p);
+    k_om3_gather<<<blocks_for(n), kThreads, 0, d.stream>>>((const uint32_t*)d.qin.get(), n, d.view(), (uint32_t*)d.qout.get(), (uint8_t*)d.qflag.get());
     d.launches[2] += 1;
     PS_TRY(d.record(1));
     PS_TRY(cudaGetLastError());
     std::vector<uint32_t> words((size_t)n);
     std::vector<uint8_t> present((size_t)n);
-    PS_TRY(cudaMemcpyAsync(words.data(), d.qout.p, (size_t)n * 4, cudaMemcpyDeviceToHost, d.stream));
-    PS_TRY(cudaMemcpyAsync(present.data(), d.qflag.p, (size_t)n, cudaMemcpyDeviceToHost, d.stream));
+    PS_TRY(cudaMemcpyAsync(words.data(), d.qout.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, d.stream));
+    PS_TRY(cudaMemcpyAsync(present.data(), d.qflag.get(), (size_t)n, cudaMemcpyDeviceToHost, d.stream));
     PS_TRY(d.finish(2));
     // getProbability takes the host's expf, as the reference's float prob() does (probabilistic_occupancy_map.cpp:38-41)
     auto prob_of = [](float l) -> float { return 1.0 - 1.0 / (1.0 + std::exp(l)); };

@@ -23,6 +23,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include "cuda_owned.h"
 #include "frontend.h"
 #include "patch_window.h"
 #include "sdm_io.h"
@@ -121,18 +122,20 @@ __global__ void __launch_bounds__(kThreads) k_fold_runs(const Word* __restrict__
 }
 
 struct PatchStore {
-    // a scratch buffer that ensure() grows; the store frees it
-    struct Buf { void* p = nullptr; size_t bytes = 0; };
+    using Buf = DeviceArray<char>;   // a scratch buffer that grows (Buf::reserve)
 
     int device = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = false, timing = false;
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    Stream stream;
+    bool timing = false;
+    Event ev[2];
     PatchWindow win{};
     int log2v = 0, ndir = 0, pool = 0, used = 0;
     int end_bit = 0;                // the bits of a record key
     std::vector<int32_t> h_dir;     // the directory, as on the device
-    int32_t* dir = nullptr;
+    DeviceArray<int32_t> dir_;
+    DeviceArray<char> cells_;
+    DeviceArray<uint32_t> mask_, status_, marks_;
+    int32_t* dir = nullptr;         // the arrays of dir_ .. marks_
     void* cells = nullptr;
     uint32_t* mask = nullptr;
     uint32_t* status = nullptr;
@@ -144,16 +147,12 @@ struct PatchStore {
     PatchStore() = default;
     PatchStore(const PatchStore&) = delete;
     PatchStore& operator=(const PatchStore&) = delete;
-    ~PatchStore()
+    ~PatchStore() { quiesce(); }
+    // selects the store's device and waits for its stream: a map's destructor calls it before its own buffers go
+    void quiesce() const
     {
         cudaSetDevice(device);
         if (stream) cudaStreamSynchronize(stream);
-        for (void* p : scratch_) cudaFree(p);
-        for (void* p : {(void*)dir, cells, (void*)mask, (void*)status, (void*)marks})
-            if (p) cudaFree(p);
-        for (cudaEvent_t e : ev)
-            if (e) cudaEventDestroy(e);
-        if (own_stream && stream) cudaStreamDestroy(stream);
     }
 
     // The window of a map's create(): resolution > 0 and patch_size 32; `window` patches per axis (dflt when null; one on z in 2-D),
@@ -202,41 +201,22 @@ struct PatchStore {
             if (_e != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(_e); return cuda_failure(); } \
         } while (0)
         PS_INIT(cudaSetDevice(dev.device));
-        if (dev.stream) {
-            stream = reinterpret_cast<cudaStream_t>(dev.stream);
-        } else {
-            PS_INIT(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-            own_stream = true;
-        }
-        PS_INIT(cudaEventCreate(&ev[0]));
-        PS_INIT(cudaEventCreate(&ev[1]));
-        PS_INIT(cudaMalloc((void**)&dir, (size_t)ndir * 4));
-        PS_INIT(cudaMalloc((void**)&marks, (size_t)ndir * 4));
-        PS_INIT(cudaMalloc(&cells, (size_t)pool * per * cell_bytes));
-        PS_INIT(cudaMalloc((void**)&mask, (size_t)pool * per / 8));
-        PS_INIT(cudaMalloc((void**)&status, 4));
+        if (dev.stream)
+            stream.borrow(reinterpret_cast<cudaStream_t>(dev.stream));
+        else
+            PS_INIT(stream.create());
+        PS_INIT(ev[0].create(cudaEventDefault));
+        PS_INIT(ev[1].create(cudaEventDefault));
+        PS_INIT(dir_.alloc((size_t)ndir));
+        PS_INIT(marks_.alloc((size_t)ndir));
+        PS_INIT(cells_.alloc((size_t)pool * per * cell_bytes));
+        PS_INIT(mask_.alloc((size_t)pool * per / 32));
+        PS_INIT(status_.alloc(1));
+        dir = dir_.get(), marks = marks_.get(), cells = cells_.get(), mask = mask_.get(), status = status_.get();
         PS_INIT(cudaMemcpyAsync(dir, h_dir.data(), (size_t)ndir * 4, cudaMemcpyHostToDevice, stream));
         PS_INIT(cudaStreamSynchronize(stream));
 #undef PS_INIT
         return LAMA_OK;
-    }
-
-    cudaError_t ensure(Buf& b, size_t bytes)
-    {
-        if (b.bytes >= bytes) return cudaSuccess;
-        if (b.p) {
-            cudaFree(b.p);
-            scratch_.erase(std::find(scratch_.begin(), scratch_.end(), b.p));
-        }
-        b = Buf{};
-        const cudaError_t e = cudaMalloc(&b.p, bytes);
-        if (e != cudaSuccess) {
-            b.p = nullptr;
-            return e;
-        }
-        b.bytes = bytes;
-        scratch_.push_back(b.p);
-        return cudaSuccess;
     }
 
     // ---- timing: kernel_times' ms[k] adds up the time from ev[0] to ev[1]; launches[k] is counted by the map -----------------------
@@ -285,16 +265,16 @@ struct PatchStore {
             std::memcpy(h_tf[k].l, m.l, sizeof(m.l));
             std::memcpy(h_tf[k].t, m.t, sizeof(m.t));
         }
-        cudaError_t e = ensure(pts, (size_t)n_pts * 24);
-        if (e == cudaSuccess) e = ensure(off, (size_t)(n_clouds + 1) * 8);
-        if (e == cudaSuccess) e = ensure(tf, (size_t)n_clouds * sizeof(Affine));
-        if (e == cudaSuccess) e = ensure(counts, (size_t)(n_pts + 1) * 8);
-        if (e == cudaSuccess) e = ensure(offs, (size_t)(n_pts + 1) * 8);
-        if (e == cudaSuccess) e = ensure(bound, (size_t)(n_clouds + 1) * 8);
-        if (e == cudaSuccess && n_pts) e = cudaMemcpyAsync(pts.p, p, (size_t)n_pts * 24, cudaMemcpyHostToDevice, stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(off.p, offsets, (size_t)(n_clouds + 1) * 8, cudaMemcpyHostToDevice, stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(tf.p, h_tf.data(), (size_t)n_clouds * sizeof(Affine), cudaMemcpyHostToDevice, stream);
-        if (e == cudaSuccess) e = cudaMemsetAsync((uint64_t*)counts.p + n_pts, 0, 8, stream);
+        cudaError_t e = pts.reserve((size_t)n_pts * 24);
+        if (e == cudaSuccess) e = off.reserve((size_t)(n_clouds + 1) * 8);
+        if (e == cudaSuccess) e = tf.reserve((size_t)n_clouds * sizeof(Affine));
+        if (e == cudaSuccess) e = counts.reserve((size_t)(n_pts + 1) * 8);
+        if (e == cudaSuccess) e = offs.reserve((size_t)(n_pts + 1) * 8);
+        if (e == cudaSuccess) e = bound.reserve((size_t)(n_clouds + 1) * 8);
+        if (e == cudaSuccess && n_pts) e = cudaMemcpyAsync(pts.get(), p, (size_t)n_pts * 24, cudaMemcpyHostToDevice, stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(off.get(), offsets, (size_t)(n_clouds + 1) * 8, cudaMemcpyHostToDevice, stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(tf.get(), h_tf.data(), (size_t)n_clouds * sizeof(Affine), cudaMemcpyHostToDevice, stream);
+        if (e == cudaSuccess) e = cudaMemsetAsync((uint64_t*)counts.get() + n_pts, 0, 8, stream);
         return e == cudaSuccess ? clear_marks() : e;
     }
 
@@ -325,11 +305,11 @@ struct PatchStore {
         if (fresh.empty()) return LAMA_OK;
         std::vector<int32_t> sl(fresh.size());
         for (size_t i = 0; i < fresh.size(); ++i) h_dir[fresh[i]] = sl[i] = used++;
-        cudaError_t e = ensure(slots, sl.size() * 4);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(slots.p, sl.data(), sl.size() * 4, cudaMemcpyHostToDevice, stream);
+        cudaError_t e = slots.reserve(sl.size() * 4);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(slots.get(), sl.data(), sl.size() * 4, cudaMemcpyHostToDevice, stream);
         if (e == cudaSuccess) e = cudaMemcpyAsync(dir, h_dir.data(), (size_t)ndir * 4, cudaMemcpyHostToDevice, stream);
         if (e != cudaSuccess) { err = std::string("patch allocation: ") + cudaGetErrorString(e); return LAMA_ERR_CUDA; }
-        k_patch_zero<<<std::min<uint64_t>(4096, blocks_for((uint64_t)sl.size() << log2v)), kThreads, 0, stream>>>((const int32_t*)slots.p,
+        k_patch_zero<<<std::min<uint64_t>(4096, blocks_for((uint64_t)sl.size() << log2v)), kThreads, 0, stream>>>((const int32_t*)slots.get(),
                                                                                                               (int)sl.size(), v);
         launch_count += 1;
         return LAMA_OK;
@@ -339,9 +319,9 @@ struct PatchStore {
     cudaError_t scan_counts(int64_t n)
     {
         size_t bytes = 0;
-        cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const uint64_t*)counts.p, (uint64_t*)offs.p, n, stream);
-        if (e == cudaSuccess) e = ensure(temp, bytes);
-        if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(temp.p, bytes, (const uint64_t*)counts.p, (uint64_t*)offs.p, n, stream);
+        cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const uint64_t*)counts.get(), (uint64_t*)offs.get(), n, stream);
+        if (e == cudaSuccess) e = temp.reserve(bytes);
+        if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(temp.get(), bytes, (const uint64_t*)counts.get(), (uint64_t*)offs.get(), n, stream);
         return e;
     }
 
@@ -351,10 +331,10 @@ struct PatchStore {
     {
         cudaError_t e = scan_counts(n_pts + 1);
         if (e != cudaSuccess) return e;
-        k_cloud_bounds<<<blocks_for(n_clouds + 1), kThreads, 0, stream>>>((const uint64_t*)offs.p, (const int64_t*)off.p, n_clouds + 1,
-                                                                           (uint64_t*)bound.p);
+        k_cloud_bounds<<<blocks_for(n_clouds + 1), kThreads, 0, stream>>>((const uint64_t*)offs.get(), (const int64_t*)off.get(), n_clouds + 1,
+                                                                           (uint64_t*)bound.get());
         h_bound.resize((size_t)n_clouds + 1);
-        e = cudaMemcpyAsync(h_bound.data(), bound.p, h_bound.size() * 8, cudaMemcpyDeviceToHost, stream);
+        e = cudaMemcpyAsync(h_bound.data(), bound.get(), h_bound.size() * 8, cudaMemcpyDeviceToHost, stream);
         return e == cudaSuccess ? cudaStreamSynchronize(stream) : e;
     }
 
@@ -379,8 +359,8 @@ struct PatchStore {
     {
         cudaError_t e = cudaSuccess;
         for (int b = 0; b < 2 && e == cudaSuccess; ++b) {
-            e = ensure(rk[b], n * sizeof(Word));
-            if (e == cudaSuccess) e = ensure(rv[b], n * sizeof(Word));
+            e = rk[b].reserve(n * sizeof(Word));
+            if (e == cudaSuccess) e = rv[b].reserve(n * sizeof(Word));
         }
         return e;
     }
@@ -391,11 +371,11 @@ struct PatchStore {
     cudaError_t sort_records(N n)
     {
         size_t bytes = 0;
-        cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const Word*)rk[0].p, (Word*)rk[1].p, (const Word*)rv[0].p, (Word*)rv[1].p, n, 0,
+        cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const Word*)rk[0].get(), (Word*)rk[1].get(), (const Word*)rv[0].get(), (Word*)rv[1].get(), n, 0,
                                                         end_bit, stream);
-        if (e == cudaSuccess) e = ensure(temp, bytes);
+        if (e == cudaSuccess) e = temp.reserve(bytes);
         if (e == cudaSuccess)
-            e = cub::DeviceRadixSort::SortPairs(temp.p, bytes, (const Word*)rk[0].p, (Word*)rk[1].p, (const Word*)rv[0].p, (Word*)rv[1].p, n, 0, end_bit,
+            e = cub::DeviceRadixSort::SortPairs(temp.get(), bytes, (const Word*)rk[0].get(), (Word*)rk[1].get(), (const Word*)rv[0].get(), (Word*)rv[1].get(), n, 0, end_bit,
                                                 stream);
         return e;
     }
@@ -406,7 +386,7 @@ struct PatchStore {
     {
         const cudaError_t e = sort_records<Word>(n);
         if (e != cudaSuccess) return e;
-        k_fold_runs<Word, Fold><<<blocks_for((uint64_t)n), kThreads, 0, stream>>>((const Word*)rk[1].p, (const Word*)rv[1].p, (uint64_t)n, v, args...);
+        k_fold_runs<Word, Fold><<<blocks_for((uint64_t)n), kThreads, 0, stream>>>((const Word*)rk[1].get(), (const Word*)rv[1].get(), (uint64_t)n, v, args...);
         return cudaSuccess;
     }
 
@@ -450,8 +430,8 @@ struct PatchStore {
         Planes out{};
         cudaError_t e = cudaSetDevice(device);
         for (int k = 0; k < Cell::kPlanes && e == cudaSuccess; ++k) {
-            e = ensure(box[k], n * Cell::kBytes[k]);
-            out.p[k] = box[k].p;
+            e = box[k].reserve(n * Cell::kBytes[k]);
+            out.p[k] = box[k].get();
         }
         if (e == cudaSuccess) {
             k_export_box<Cell><<<std::min<uint64_t>(8192, blocks_for(n)), kThreads, 0, stream>>>(v, win, dir, log2v, lo[0], lo[1], lo[2], size[0], size[1],
@@ -517,7 +497,6 @@ struct PatchStore {
     }
 
 private:
-    std::vector<void*> scratch_;   // what ensure() holds allocated
 };
 
 }  // namespace

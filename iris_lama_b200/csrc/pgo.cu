@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstdlib>
 
+#include "cuda_owned.h"
 #include "engine.h"   // status codes
 
 namespace cg = cooperative_groups;
@@ -301,15 +302,14 @@ __global__ void k_pgo_error_final(const double* __restrict__ partial, int n, dou
     }
 }
 
-struct DeviceArena {
-    std::vector<void*> blocks;
-    ~DeviceArena() { for (void* p : blocks) cudaFree(p); }
+struct DeviceArena {   // the device arrays of one solve, freed together
+    std::vector<DeviceArray<char>> blocks;
     template <typename T> T* alloc(size_t n, cudaError_t& e)
     {
-        void* p = nullptr;
-        if (e == cudaSuccess) e = cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T));
-        if (e == cudaSuccess) blocks.push_back(p);
-        return (T*)p;
+        if (e != cudaSuccess) return nullptr;
+        blocks.emplace_back();
+        e = blocks.back().alloc(std::max<size_t>(n, 1) * sizeof(T));
+        return (T*)blocks.back().get();
     }
     template <typename T> T* upload(const std::vector<T>& v, cudaError_t& e)
     {
@@ -401,15 +401,12 @@ int pgo_optimize_graph(int device, std::vector<SE2>& nodes, const std::vector<Pg
     const int err_blocks = 128;
     double* d_part = A.alloc<double>((size_t)err_blocks, ce);
     double* d_err  = A.alloc<double>(1, ce);
-    cudaStream_t st = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
-    if (ce == cudaSuccess) ce = cudaEventCreate(&e0);
-    if (ce == cudaSuccess) ce = cudaEventCreate(&e1);
+    Stream st;
+    Event e0, e1;
+    if (ce == cudaSuccess) ce = st.create();
+    if (ce == cudaSuccess) ce = e0.create(cudaEventDefault);
+    if (ce == cudaSuccess) ce = e1.create(cudaEventDefault);
     auto done = [&](int code, const std::string& what) {
-        if (st) cudaStreamDestroy(st);
-        if (e0) cudaEventDestroy(e0);
-        if (e1) cudaEventDestroy(e1);
         if (!what.empty()) err = what;
         return code;
     };

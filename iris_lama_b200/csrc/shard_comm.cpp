@@ -3,6 +3,7 @@
 
 #include <cuda_runtime.h>
 #include <dlfcn.h>
+#include "cuda_owned.h"
 #include <nccl.h>   // types and enums only: every function is resolved with dlsym
 
 #include <cstring>
@@ -59,7 +60,7 @@ Nccl* nccl(std::string& err)
 struct ShardComm {
     Nccl* n = nullptr;
     ncclComm_t comm = nullptr;
-    cudaStream_t stream = nullptr;
+    lama_b200::Stream stream;
     int rank = 0, world = 1, device = 0;
     uint64_t collectives = 0;
     std::string err;
@@ -91,7 +92,7 @@ ShardComm* shard_comm_create(const uint8_t id[128], int rank, int world, int dev
     ncclResult_t r = n->CommInitRank(&c->comm, world, u, rank);
     if (r != ncclSuccess) { err = std::string("ncclCommInitRank: ") + n->GetErrorString(r); delete c; return nullptr; }
     // its own stream: the engine's stream holds the running map update, which the exchange of the match results must not wait for
-    if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { err = "shard_comm_create: no stream"; n->CommDestroy(c->comm); delete c; return nullptr; }
+    if (c->stream.create() != cudaSuccess) { err = "shard_comm_create: no stream"; n->CommDestroy(c->comm); delete c; return nullptr; }
     return c;
 }
 
@@ -99,11 +100,12 @@ void shard_comm_destroy(ShardComm* c)
 {
     if (!c) return;
     cudaSetDevice(c->device);
-    if (c->stream) { cudaStreamSynchronize(c->stream); cudaStreamDestroy(c->stream); }
+    if (c->stream) cudaStreamSynchronize(c->stream);
+    c->stream.reset();
     if (c->comm) c->n->CommDestroy(c->comm);
     delete c;
 }
-void* shard_stream(ShardComm* c) { return c->stream; }
+void* shard_stream(ShardComm* c) { return c->stream.get(); }
 int shard_world(const ShardComm* c) { return c->world; }
 int shard_rank(const ShardComm* c) { return c->rank; }
 const std::string& shard_error(const ShardComm* c) { return c->err; }

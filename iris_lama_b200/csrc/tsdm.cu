@@ -240,6 +240,8 @@ struct TsdmDev::Impl : PatchStore {
     TsdmParams prm{};
     Buf hkeys, hval, hslot, surv, inserted, qout, list, mesh;
 
+    ~Impl() { quiesce(); }
+
     View view() const { return View{dir, (float2*)cells, mask, win, log2v}; }
 };
 
@@ -292,22 +294,22 @@ int TsdmDev::insert_point_clouds(const double* pts, const int64_t* offsets, int 
     PS_TRY(cudaSetDevice(d.device));
     PS_TRY(d.record(0));
     PS_TRY(d.upload_clouds(pts, offsets, n_clouds, n_pts, origins, quats));
-    PS_TRY(d.ensure(d.surv, std::max<size_t>(1, (size_t)n_pts)));
-    PS_TRY(d.ensure(d.inserted, (size_t)n_clouds * 4));
-    PS_TRY(cudaMemsetAsync(d.inserted.p, 0, (size_t)n_clouds * 4, d.stream));
+    PS_TRY(d.surv.reserve(std::max<size_t>(1, (size_t)n_pts)));
+    PS_TRY(d.inserted.reserve((size_t)n_clouds * 4));
+    PS_TRY(cudaMemsetAsync(d.inserted.get(), 0, (size_t)n_clouds * 4, d.stream));
 
     const View v = d.view();
     FuseParams f{};
-    f.pts = (const double*)d.pts.p;
-    f.offsets = (const int64_t*)d.off.p;
-    f.tf = (const Affine*)d.tf.p;
+    f.pts = (const double*)d.pts.get();
+    f.offsets = (const int64_t*)d.off.get();
+    f.tf = (const Affine*)d.tf.get();
     f.n_clouds = n_clouds;
     f.prm = d.prm;
-    f.surv = (uint8_t*)d.surv.p;
-    f.counts = (uint64_t*)d.counts.p;
-    f.offs = (const uint64_t*)d.offs.p;
+    f.surv = (uint8_t*)d.surv.get();
+    f.counts = (uint64_t*)d.counts.get();
+    f.offs = (const uint64_t*)d.offs.get();
     f.marks = d.marks;
-    f.inserted = (uint32_t*)d.inserted.p;
+    f.inserted = (uint32_t*)d.inserted.get();
     f.status = d.status;
 
     // 1-2. dedupe, window check, marks and counts, in passes of whole clouds
@@ -318,15 +320,15 @@ int TsdmDev::insert_point_clouds(const double* pts, const int64_t* offsets, int 
         if (np > 0) {
             uint32_t cap = 1024;
             while ((int64_t)cap < 2 * np) cap <<= 1;
-            PS_TRY(d.ensure(d.hkeys, (size_t)cap * 8));
-            PS_TRY(d.ensure(d.hval, (size_t)cap * 4));
-            PS_TRY(d.ensure(d.hslot, (size_t)np * 4));
-            PS_TRY(cudaMemsetAsync(d.hkeys.p, 0xFF, (size_t)cap * 8, d.stream));
-            PS_TRY(cudaMemsetAsync(d.hval.p, 0xFF, (size_t)cap * 4, d.stream));
-            f.hkeys = (uint64_t*)d.hkeys.p;
-            f.hval = (uint32_t*)d.hval.p;
+            PS_TRY(d.hkeys.reserve((size_t)cap * 8));
+            PS_TRY(d.hval.reserve((size_t)cap * 4));
+            PS_TRY(d.hslot.reserve((size_t)np * 4));
+            PS_TRY(cudaMemsetAsync(d.hkeys.get(), 0xFF, (size_t)cap * 8, d.stream));
+            PS_TRY(cudaMemsetAsync(d.hval.get(), 0xFF, (size_t)cap * 4, d.stream));
+            f.hkeys = (uint64_t*)d.hkeys.get();
+            f.hval = (uint32_t*)d.hval.get();
             f.hmask = cap - 1;
-            f.hslot = (uint32_t*)d.hslot.p;
+            f.hslot = (uint32_t*)d.hslot.get();
             f.p0 = offsets[c0];
             f.p1 = offsets[c1];
             f.c0 = c0;
@@ -356,8 +358,8 @@ int TsdmDev::insert_point_clouds(const double* pts, const int64_t* offsets, int 
             f.p0 = offsets[c0];
             f.p1 = offsets[c1];
             f.rec_base = bound[c0];
-            f.rkeys = (uint64_t*)d.rk[0].p;
-            f.rvals = (uint64_t*)d.rv[0].p;
+            f.rkeys = (uint64_t*)d.rk[0].get();
+            f.rvals = (uint64_t*)d.rv[0].get();
             k_tsdm_walk<true><<<blocks_for(np), kThreads, 0, d.stream>>>(f, v);
             d.launches[0] += 1;
         }
@@ -370,7 +372,7 @@ int TsdmDev::insert_point_clouds(const double* pts, const int64_t* offsets, int 
     if (rc != LAMA_OK) return rc;
     PS_TRY(cudaGetLastError());
     std::vector<uint32_t> ins((size_t)n_clouds);
-    PS_TRY(cudaMemcpyAsync(ins.data(), d.inserted.p, ins.size() * 4, cudaMemcpyDeviceToHost, d.stream));
+    PS_TRY(cudaMemcpyAsync(ins.data(), d.inserted.get(), ins.size() * 4, cudaMemcpyDeviceToHost, d.stream));
     PS_TRY(d.record(1));
     PS_TRY(d.finish(0));
     if (inserted)
@@ -384,12 +386,12 @@ int TsdmDev::distance(const double* pts, int n, double* dist, double* grad)
     if (n < 0 || (n > 0 && (!pts || !dist))) { err_ = "null argument"; return LAMA_ERR_ARG; }
     if (n == 0) return LAMA_OK;
     PS_TRY(cudaSetDevice(d.device));
-    PS_TRY(d.ensure(d.pts, (size_t)n * 24));
-    PS_TRY(d.ensure(d.qout, (size_t)n * 32));
-    PS_TRY(cudaMemcpyAsync(d.pts.p, pts, (size_t)n * 24, cudaMemcpyHostToDevice, d.stream));
-    double* dd = (double*)d.qout.p;
+    PS_TRY(d.pts.reserve((size_t)n * 24));
+    PS_TRY(d.qout.reserve((size_t)n * 32));
+    PS_TRY(cudaMemcpyAsync(d.pts.get(), pts, (size_t)n * 24, cudaMemcpyHostToDevice, d.stream));
+    double* dd = (double*)d.qout.get();
     PS_TRY(d.record(0));
-    k_tsdm_distance<<<blocks_for(n), kThreads, 0, d.stream>>>((const double*)d.pts.p, n, d.view(), d.prm, dd, dd + n);
+    k_tsdm_distance<<<blocks_for(n), kThreads, 0, d.stream>>>((const double*)d.pts.get(), n, d.view(), d.prm, dd, dd + n);
     d.launches[1] += 1;
     PS_TRY(d.record(1));
     PS_TRY(cudaGetLastError());
@@ -421,29 +423,29 @@ int TsdmDev::to_mesh(float* vertices, size_t cap, size_t* n_vertices)
     }
     PS_TRY(cudaSetDevice(d.device));
     const uint64_t total = (uint64_t)list.size() << d.log2v;
-    PS_TRY(d.ensure(d.list, list.size() * 4));
-    PS_TRY(d.ensure(d.counts, (total + 1) * 8));
-    PS_TRY(d.ensure(d.offs, (total + 1) * 8));
-    PS_TRY(cudaMemcpyAsync(d.list.p, list.data(), list.size() * 4, cudaMemcpyHostToDevice, d.stream));
-    PS_TRY(cudaMemsetAsync((uint64_t*)d.counts.p + total, 0, 8, d.stream));
+    PS_TRY(d.list.reserve(list.size() * 4));
+    PS_TRY(d.counts.reserve((total + 1) * 8));
+    PS_TRY(d.offs.reserve((total + 1) * 8));
+    PS_TRY(cudaMemcpyAsync(d.list.get(), list.data(), list.size() * 4, cudaMemcpyHostToDevice, d.stream));
+    PS_TRY(cudaMemsetAsync((uint64_t*)d.counts.get() + total, 0, 8, d.stream));
     PS_TRY(d.record(0));
     const View v = d.view();
-    k_tsdm_mesh<false><<<blocks_for(total), kThreads, 0, d.stream>>>((const int32_t*)d.list.p, (int)list.size(), v, d.prm.scale, (uint64_t*)d.counts.p,
+    k_tsdm_mesh<false><<<blocks_for(total), kThreads, 0, d.stream>>>((const int32_t*)d.list.get(), (int)list.size(), v, d.prm.scale, (uint64_t*)d.counts.get(),
                                                                      nullptr, nullptr);
     PS_TRY(d.scan_counts((int64_t)(total + 1)));
     uint64_t nv = 0;
-    PS_TRY(cudaMemcpyAsync(&nv, (uint64_t*)d.offs.p + total, 8, cudaMemcpyDeviceToHost, d.stream));
+    PS_TRY(cudaMemcpyAsync(&nv, (uint64_t*)d.offs.get() + total, 8, cudaMemcpyDeviceToHost, d.stream));
     PS_TRY(cudaStreamSynchronize(d.stream));
     d.launches[2] += 2;
     if (n_vertices) *n_vertices = (size_t)nv;
     if (!vertices || cap < nv || nv == 0) return LAMA_OK;
-    PS_TRY(d.ensure(d.mesh, (size_t)nv * 12));
-    k_tsdm_mesh<true><<<blocks_for(total), kThreads, 0, d.stream>>>((const int32_t*)d.list.p, (int)list.size(), v, d.prm.scale, nullptr,
-                                                                    (const uint64_t*)d.offs.p, (float*)d.mesh.p);
+    PS_TRY(d.mesh.reserve((size_t)nv * 12));
+    k_tsdm_mesh<true><<<blocks_for(total), kThreads, 0, d.stream>>>((const int32_t*)d.list.get(), (int)list.size(), v, d.prm.scale, nullptr,
+                                                                    (const uint64_t*)d.offs.get(), (float*)d.mesh.get());
     d.launches[2] += 1;
     PS_TRY(d.record(1));
     PS_TRY(cudaGetLastError());
-    PS_TRY(cudaMemcpyAsync(vertices, d.mesh.p, (size_t)nv * 12, cudaMemcpyDeviceToHost, d.stream));
+    PS_TRY(cudaMemcpyAsync(vertices, d.mesh.get(), (size_t)nv * 12, cudaMemcpyDeviceToHost, d.stream));
     PS_TRY(d.finish(2));
     return LAMA_OK;
 }
